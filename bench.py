@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py - KING N x N pair-dot-products/s on the BASELINE.json workload (100k samples x 1M SNPs).
+"""bench.py - KING N x N pair-dot-products/s on the BASELINE.json workload (60k samples x 1M SNPs).
 
 A "step" is one pass of the hot path (the KING pair-count kernel, CalcKing's dense loop) over one
 batch of `--batch-variants` synthetic variants for ALL sample pairs of this rank's row block; the
@@ -13,8 +13,7 @@ counts accumulate in HBM across steps exactly as in a full run (8 steps of 131,0
             fp64 kinship matrix.
   roofline= int8 tensor pipe: 5 products x 2 ops x pairs x variants / tensor-kernel time (CUDA events
             recorded by the library around the launch, on the stream it is launched on) vs the int8 rate
-            MEASURED on this GPU in the same run (pl2gpu_int8_peak: tcgen05.mma kind::i8 on all SMs
-            for >= 2 s).
+            MEASURED on this GPU in the same run (pl2gpu_int8_peak: int8 wgmma on all SMs for >= 2 s).
   cpu_baseline / --impl reference = the UNMODIFIED reference binary (oracle/_ref/plink2,
             --make-king-table, as many threads as this process may actually use) on a bounded sample.
 
@@ -23,6 +22,13 @@ equal-work blocks; each rank holds 1/G of the step's variants and the LIBRARY (N
 libpl2gpu, pl2gpu_king_add_variants_sharded) all-gathers the genotype column tile on its prep stream,
 double-buffered against the previous step's tensor kernel; outputs stay local.  Total work is fixed
 => "strong" scaling.
+
+--dump-outputs DIR writes, after the timed steps, what the timed path has computed by then (the KING counts and
+kinships a caller of the job reads back) for a fixed, seeded sample of rows, as .npy files.  Inputs depend only on
+the arguments, so two builds can be compared output for output.
+
+The 60k-sample default keeps the job's int32 accumulators (~36 GB) and staged batches resident in the 80 GB of
+one H100.
 """
 import argparse
 import json
@@ -38,10 +44,12 @@ import time
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
-FULL_N = 100_000
+FULL_N = 60_000
 FULL_M = 1_000_000
-METRIC = "KING NxN pair-dot-products/sec (100k samples x 1M SNPs)"
+METRIC = "KING NxN pair-dot-products/sec (60k samples x 1M SNPs)"
+DUMP_ROWS = 8  # rows of the pair triangle written by --dump-outputs (all pairs i < j of each row j)
 UNIT = "pair-dot-products/s (1M-SNP pairs)"
+INT8_DATASHEET_TOPS = 1979.0  # H100 SXM, dense int8, 700 W card (NVIDIA data sheet); never reached, only a yardstick
 
 
 def parse_args():
@@ -59,6 +67,7 @@ def parse_args():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-secondary", action="store_true", help="skip the short GRM / PCA / LD measurements reported under `secondary`")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write the KING counts / kinships of a seeded sample of rows as DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -227,7 +236,7 @@ def reference_arm(args):
         line = {
             "impl": "reference", "metric": METRIC, "value": val, "unit": UNIT, "n_gpus": args.gpus, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": t * 1e3, "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "u64 popcount (AVX2)", "data": "synthetic",
-            "config": {"workload": "plink2 --make-king-table, bounded sample of the 100k x 1M job", "samples": n, "variants": m, "threads": threads, "host_cpus": cores, "pair_snp_per_s": pairs * m / t},
+            "config": {"workload": f"plink2 --make-king-table, bounded sample of the {FULL_N // 1000}k x 1M job", "samples": n, "variants": m, "threads": threads, "host_cpus": cores, "pair_snp_per_s": pairs * m / t},
             "cpu_baseline": {"value": val, "unit": UNIT, "cores": threads, "host_cpus": cores, "kind": "reference", "sample": f"{n} samples x {m} variants, whole `plink2 --make-king-table --threads {threads}` run incl. .bed load"},
             "e2e": {"value": val, "unit": UNIT, "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0},
             "gpu_launches": 0,
@@ -285,12 +294,12 @@ def cpu_legs(args):
 
 
 def hbm_peak_gbs():
-    """Measured HBM copy bandwidth of this pool's B200s (driver-written MEASURED_PEAKS.json), else the profiling
-    guide's fallback."""
+    """Measured HBM copy bandwidth when a MEASURED_PEAKS.json sits beside this file, else the H100 SXM data sheet's
+    3.35 TB/s."""
     try:
         return float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"])
     except Exception:
-        return 6500.0
+        return 3350.0
 
 
 # ------------------------------------------------------------------------------------- secondary
@@ -316,9 +325,9 @@ def secondary_legs(args, torch, p, ctx, dev, peak_tops):
             g_ms = ctx.event_elapsed_ms(6, 7) / 3
         tri = n2 * (n2 + 1) // 2
         tops = 11 * 2 * tri * m2 / (g_ms * 1e-3) / 1e12
-        sec["grm"] = {"kernel": "grm_ts_kernel", "workload": f"{n2} samples x {m2} variants per add_variants call (tables + re-tiling + tensor kernel), inputs resident",
+        sec["grm"] = {"kernel": "grm_wg_kernel", "workload": f"{n2} samples x {m2} variants per add_variants call (tables + re-tiling + tensor kernel), inputs resident",
                       "ms_per_call": g_ms, "achieved": tops, "unit": "TOP/s (int8; 10 digit planes + obs = 11 products x 2 ops per pair and variant)",
-                      "peak": peak_tops, "frac": tops / peak_tops if peak_tops else None, "frac_of_nominal_4500": tops / 4500.0, "pair_snp_per_s": tri * m2 / (g_ms * 1e-3)}
+                      "peak": peak_tops, "frac": tops / peak_tops if peak_tops else None, "frac_of_datasheet": tops / INT8_DATASHEET_TOPS, "pair_snp_per_s": tri * m2 / (g_ms * 1e-3)}
         del g2
     except Exception as ex:  # reported, never faked
         sec["grm"] = {"error": str(ex)[-300:]}
@@ -463,7 +472,21 @@ def secondary_legs(args, torch, p, ctx, dev, peak_tops):
     return sec
 
 
-# ------------------------------------------------------------------------------------- B200 arm
+def dump_outputs(job, r0, r1, out_dir):
+    """KING counts (IBS0, HETHET, HET2HOM1, HET1HOM2, HOMHOM) and kinships of every pair of DUMP_ROWS rows drawn with a
+    fixed seed from [r0, r1), as float64 arrays in DIR/king_counts.npy, DIR/king_kinship.npy and DIR/king_rows.npy."""
+    import numpy as np
+
+    rows = np.sort(np.random.default_rng(12345).choice(np.arange(max(r0, 1), r1), size=min(DUMP_ROWS, r1 - max(r0, 1)), replace=False))
+    counts = [job.counts(int(j), int(j) + 1) for j in rows]
+    kin = [job.kinship(int(j), int(j) + 1) for j in rows]
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "king_rows.npy"), rows.astype(np.float64))
+    np.save(os.path.join(out_dir, "king_counts.npy"), np.concatenate(counts).astype(np.float64))
+    np.save(os.path.join(out_dir, "king_kinship.npy"), np.concatenate(kin).astype(np.float64))
+
+
+# ------------------------------------------------------------------------------------- GPU arm
 def b200_arm(args):
     import torch
     import torch.distributed as dist
@@ -542,6 +565,8 @@ def b200_arm(args):
     dev_ms = ctx.event_elapsed_ms(0, 1)
     kern_ms = job.last_kernel_ms() if algo == KING_ALGO_TENSOR_TS else dev_ms / args.steps
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(job, r0, r1, args.dump_outputs)
     wall_ms = (time.perf_counter() - t0) * 1e3
     launches = ctx.launch_count() - launches0
     clocks = sampler.stop()
@@ -610,18 +635,18 @@ def b200_arm(args):
         return
 
     # ---- measured int8 tensor peak of THIS GPU, same run (>= 2 s on all SMs, clocks sampled) ----
-    peak, peak_src, peak_detail = 4500.0, "nominal dense int8 4.5 POP/s (measurement failed)", None
+    peak, peak_src, peak_detail = INT8_DATASHEET_TOPS, "H100 SXM data sheet, dense int8 (measurement failed)", None
     try:
         del slice_dev
         torch.cuda.empty_cache()
         s2 = ClockSampler(local_rank)
         s2.start()
-        ts160, secs = ctx.int8_peak(160, 1, 2.0)
-        ss240, _ = ctx.int8_peak(240, 0, 0.5)
+        n80, secs = ctx.int8_peak(80, 1, 2.0)
+        n96, _ = ctx.int8_peak(96, 1, 0.5)
         pk = s2.stop()
-        peak = max(ts160, ss240)
-        peak_detail = {"ts_n160_tops": ts160, "ss_n240_tops": ss240, "seconds": secs, "clocks": pk}
-        peak_src = "measured in this run: pl2gpu_int8_peak (tcgen05.mma kind::i8, M=128 K=32, all SMs, >= 2 s; max of the A-in-TMEM N=160 form the kernel uses and the smem-smem N=240 form)"
+        peak = max(n80, n96)
+        peak_detail = {"n80_tops": n80, "n96_tops": n96, "seconds": secs, "clocks": pk}
+        peak_src = "measured in this run: pl2gpu_int8_peak (int8 wgmma, M=64 K=32, A in registers, all SMs, >= 2 s; max of the N=80 and N=96 shapes the KING kernels use)"
     except Exception as ex:
         peak_src += f": {ex}"
     peaks = {}
@@ -631,18 +656,13 @@ def b200_arm(args):
         pass
     ops = 5 * 2 * my_pairs * mb  # algorithmic: 5 indicator products per pair and variant, this rank's launch
     achieved = ops / (kern_ms * 1e-3) / 1e12
-    kname = {KING_ALGO_TENSOR_TS: "king_ts_kernel", KING_ALGO_TENSOR: "king_tc_kernel", KING_ALGO_POPCOUNT: "king_popc_kernel"}[algo]
+    kname = {KING_ALGO_TENSOR_TS: "king_wg_kernel<80>", KING_ALGO_TENSOR: "king_wg_kernel<96>", KING_ALGO_POPCOUNT: "king_popc_kernel"}[algo]
     acc_bytes = 2 * 20 * my_pairs  # int32 x 5 accumulators read + written once per launch (tile padding excluded)
-    # DRAM bytes of ONE king_ts_kernel launch at exactly this shape, from `ncu --metrics dram__bytes_read.sum,
-    # dram__bytes_write.sum -k regex:king_ts_kernel` on this command (profiles/r02_king_traffic_100k.csv): 609.5 GB read +
-    # 100.6 GB written.  Only quoted for the configuration it was captured on.
-    traffic = 609530605824 + 100556782336 if (n, mb, world, algo) == (FULL_N, 131072, 1, KING_ALGO_TENSOR_TS) else None
-    roofline = {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TOP/s (int8)", "frac": achieved / peak, "traffic": traffic,
+    roofline = {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TOP/s (int8)", "frac": achieved / peak,
                 "kernel": kname, "kernel_ms": kern_ms, "kernel_ms_max_over_ranks": kern_ms_max, "peak_source": peak_src, "peak_detail": peak_detail,
-                "frac_of_nominal_4500": achieved / 4500.0, "frac_of_2x_bf16_burst": achieved / (2 * peaks["bf16_tflops"]) if peaks.get("bf16_tflops") else None,
+                "frac_of_datasheet": achieved / INT8_DATASHEET_TOPS, "frac_of_2x_bf16_burst": achieved / (2 * peaks["bf16_tflops"]) if peaks.get("bf16_tflops") else None,
                 "algorithmic_ops_per_launch": ops, "algorithmic_bytes_per_launch": acc_bytes + n * mb // 2,
-                "traffic_note": "bytes per launch from one ncu capture of this kernel at this shape (profiles/r02_king_traffic_100k.csv; profiles/r02_ncu_summary.md has the --set full capture at 16,384 samples): written = the accumulators once (100.6 GB); read = accumulators once + operand tiles re-fetched when the 12x12-tile launch blocks outrun the L2 (15 % of the operand requests miss at 131,072 variants per step). 710 GB in 1.75 s is 6 % of the HBM bandwidth: the kernel is tensor-bound (pipe 82.6 % active) and the re-reads cost no time",
-                "kernel_ms_note": "CUDA events recorded by the library around the king_ts_kernel launch on its stream (last timed step); the step additionally holds the copy/all-gather, padding and row re-tiling of the next batch, overlapped on the prep stream"}
+                "kernel_ms_note": "CUDA events recorded by the library around the tensor-kernel launch on its stream (last timed step); the step additionally holds the copy/all-gather, padding and sample-major re-tiling of the next batch, overlapped on the prep stream"}
     if algo == KING_ALGO_POPCOUNT:
         roofline["note"] = "popcount kernel: int8-equivalent ops shown for comparability; its own limiter is the POPC pipe"
 
@@ -661,7 +681,7 @@ def b200_arm(args):
         "config": {"workload": f"--make-king, {n} samples x {FULL_M} SNPs in steps of {mb} variants", "samples": n, "variants_per_step": mb, "steps_per_full_job": -(-FULL_M // mb),
                    "parallelism": f"row-block x{world} ({'tile-aligned equal work' if args.row_split == 'tiles' else 'ParallelBounds'}), 1 NCCL all-gather of the genotype column tile per step inside libpl2gpu, overlapped" if world > 1 else "single GPU",
                    "algo": args.algo, "rows_rank0": [r0, r1],
-                   "l2_policy": "inputs (3.3 GB batch + 100 GB of accumulators) exceed L2; no flush needed", "pair_snp_per_s": total_pairs * mb / (step_ms * 1e-3), "wall_ms_per_step": wall_ms / args.steps},
+                   "l2_policy": f"inputs ({n * mb / 4e9:.1f} GB batch + {acc_bytes / 2e9:.0f} GB of accumulators) exceed L2; no flush needed", "pair_snp_per_s": total_pairs * mb / (step_ms * 1e-3), "wall_ms_per_step": wall_ms / args.steps},
         "roofline": roofline, "cpu_baseline": cpu_baseline, "cli_same_files": cli, "secondary": secondary, "e2e": e2e, "gpu_launches": int(launches), "clocks": clocks,
     }
     emit(line)

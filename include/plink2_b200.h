@@ -1,4 +1,4 @@
-/* plink2_b200.h - C-ABI kernel face of the B200-native pairwise-genotype path.
+/* plink2_b200.h - C-ABI kernel face of the H100-native pairwise-genotype path.
  *
  * This is the drop-in boundary (SURVEY.md 8b, "kernel face").  It is shaped like the reference's
  * only existing GPU seam, 2.0/cuda/plink2_matrix_cuda.h:23-108: plain C, extern "C", no CUDA
@@ -20,7 +20,7 @@
  *    for i in [0,j)" (:1545-1547); index 1 = smaller sample index, 2 = larger.
  *
  * There is no CPU fallback: every call fails (returns 1, message in pl2gpu_last_error()) when no
- * sm_100 device is usable.
+ * sm_90 (H100) device is usable.
  */
 #ifndef PLINK2_B200_H_
 #define PLINK2_B200_H_
@@ -87,8 +87,8 @@ typedef struct Pl2KingJob Pl2KingJob;
 enum {
   kPl2KingAlgoAuto = 0,
   kPl2KingAlgoPopcount = 1, /* bit-plane AND/XOR + __popc over smem tiles */
-  kPl2KingAlgoTensor = 2,   /* exact int8 tcgen05 contraction over {0,+-1} indicator planes (both operands via smem) */
-  kPl2KingAlgoTensorTS = 3  /* same contraction, row-side operand expanded straight into tensor memory */
+  kPl2KingAlgoTensor = 2,   /* exact int8 wgmma contraction over {0,+-1} indicator planes, 128 x 96 tiles */
+  kPl2KingAlgoTensorTS = 3  /* same contraction, 128 x 80 tiles, double-buffered staging (the default) */
 };
 
 /* Rows [row_start, row_end) of the strict lower triangle over sample_ct samples (row = larger
@@ -150,7 +150,7 @@ int pl2gpu_king_pairs_end(Pl2KingPairJob* job);
 /* ---- GRM: replaces ExpandCenteredVarmaj + the CalcGrmThread/CalcGrmPartThread dsyrk/dgemm
  * accumulation (2.0/plink2_matrix_calc.cc:3839-3886, :4285-4327) and the CalcMissingMatrix pass
  * (:4404-4553) for rows [row_start,row_end) of the lower triangle (diagonal included), one
- * TriangleFill2 slab / `--parallel` piece.  Exact int8 tcgen05 accumulation of fixed-point
+ * TriangleFill2 slab / `--parallel` piece.  Exact int8 tensor-core accumulation of fixed-point
  * (32-bit) per-variant genotype tables; see DESIGN.md for the error bound. ---- */
 typedef struct Pl2GrmJob Pl2GrmJob;
 enum {
@@ -259,18 +259,15 @@ int pl2gpu_score_get(Pl2ScoreJob* job, double* score_sums, uint64_t* named_dosag
 /* Idempotent; accepts NULL. */
 int pl2gpu_score_end(Pl2ScoreJob* job);
 
-/* ---- measured int8 tensor peak: every SM issues back-to-back tcgen05.mma kind::i8 (M = 128, N = n_cols,
- * K = 32; form 0 = both operands in shared memory, 1 = A operand in tensor memory as the KING/GRM kernels use
- * it) for at least min_seconds; *tops_out = 2*128*n_cols*32 ops x UMMAs / elapsed (CUDA events), in TOP/s.
+/* ---- measured int8 tensor peak: two warpgroups per SM issue back-to-back int8 wgmma (M = 64, N = n_cols in
+ * {80, 96}, K = 32; form 1 = A fragments in registers, B in shared memory, as the KING/GRM kernels use it) for at
+ * least min_seconds; *tops_out = 2*64*n_cols*32 ops x wgmmas / elapsed (CUDA events), in TOP/s.
  * This is the roofline denominator bench.py reports against. ---- */
 int pl2gpu_int8_peak(Pl2GpuCtx* ctx, uint32_t n_cols, int form, double min_seconds, double* tops_out, double* seconds_out);
 
-/* ---- self-test of the tcgen05 operand path (descriptor/layout probe); returns 0 iff an int8
- * UMMA over library-written shared-memory tiles reproduces a scalar device-side reference. ---- */
+/* ---- self-test of the tensor operand path (fragment / descriptor layout probe); returns 0 iff int8 wgmmas
+ * with A fragments in registers and B in the library's shared-memory layout reproduce a scalar host reference. ---- */
 int pl2gpu_selftest_umma(Pl2GpuCtx* ctx, int verbose);
-/* Debug probe used by tests to pin the operand layout: runs `k_steps` int8 UMMAs (M = 128) over the
- * given shared-memory images / descriptor fields and returns D as int32 [128][n] (host memory). */
-int pl2gpu_debug_umma(Pl2GpuCtx* ctx, const uint8_t* a_img, uint32_t a_bytes, const uint8_t* b_img, uint32_t b_bytes, uint32_t a_lbo, uint32_t a_sbo, uint32_t b_lbo, uint32_t b_sbo, uint32_t a_step_bytes, uint32_t b_step_bytes, uint32_t k_steps, uint32_t idesc, uint32_t n, int32_t* d_out_host);
 
 #ifdef __cplusplus
 }

@@ -1,4 +1,4 @@
-"""plink-ng_b200: B200-native (sm_100a) pairwise-genotype kernels behind PLINK 2.0's interfaces.
+"""plink-ng_b200: H100-native (sm_90a) pairwise-genotype kernels behind PLINK 2.0's interfaces.
 
 The product is the C-ABI shared library `libpl2gpu.so` (include/plink2_b200.h) and the `plink2_b200`
 host program built from `plink_ng_b200/csrc`.  This Python package is only the ctypes binding used by

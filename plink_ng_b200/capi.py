@@ -13,7 +13,7 @@ class Pl2Error(RuntimeError):
 if not os.path.exists(_LIB_PATH):
     raise ImportError(
         f"{_LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-        "(nvcc, sm_100a).  There is no CPU fallback."
+        "(nvcc, sm_90a).  There is no CPU fallback."
     )
 
 lib = C.CDLL(_LIB_PATH)
@@ -83,10 +83,6 @@ SIGNATURES = {
     "pl2_ld_prune_walk": (C.c_int, [C.c_uint32, vp, vp, C.c_uint32, C.c_uint32, C.c_int, vp, vp, vp, C.c_uint32, C.c_uint32, vp]),
     "pl2gpu_int8_peak": (C.c_int, [vp, C.c_uint32, C.c_int, C.c_double, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "pl2gpu_selftest_umma": (C.c_int, [vp, C.c_int]),
-    "pl2gpu_debug_umma": (
-        C.c_int,
-        [vp, vp, C.c_uint32, vp, C.c_uint32] + [C.c_uint32] * 9 + [vp],
-    ),
 }
 
 for _name, (_res, _args) in SIGNATURES.items():

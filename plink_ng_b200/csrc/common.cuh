@@ -33,8 +33,8 @@ const char* get_error();
 
 // ---- pair-tile geometry shared by every N x N kernel ----
 // Output tiles are kTileRows (larger-index samples, "sample 2") x kTileCols (smaller-index
-// samples, "sample 1").  128 rows = the UMMA M dimension / the 128 TMEM lanes; 96 columns so that
-// five 32-bit accumulators (5 * 96 = 480) fit the 512 TMEM columns of one SM.
+// samples, "sample 1").  A tensor kernel runs a tile as two CTAs of 64 rows (the wgmma M dimension), each
+// keeping its five 32-bit accumulator blocks (5 x 64 x 96 int32) in the registers of two warpgroups.
 constexpr uint32_t kTileRows = 128;
 constexpr uint32_t kTileCols = 96;
 constexpr uint32_t kKingAccs = 5;                                   // TT, TH, HT, HH, SS
@@ -64,10 +64,6 @@ struct Ctx {
 // already sits at buf + r * bytes_per_rank), and an in-place fp64 sum all-reduce, both enqueued on `stream`.
 int CommAllGatherInPlace(Ctx* ctx, void* buf, uint64_t bytes_per_rank, cudaStream_t stream);
 int CommAllReduceSumF64(Ctx* ctx, double* buf, uint64_t count, cudaStream_t stream);
-
-// 2-D uint8 tensor map over a staged block raw[rows][pitch] with box {box_bytes, box_rows} (no swizzle,
-// zero fill) for cp.async.bulk.tensor loads; cuTensorMapEncodeTiled is fetched through the runtime.
-int MakeRawTensorMap(CUtensorMap* out, void* base, uint32_t pitch, uint32_t rows, uint32_t box_bytes, uint32_t box_rows);
 
 struct TileList {
   // tiles of the strict lower triangle restricted to rows [row_start, row_end)

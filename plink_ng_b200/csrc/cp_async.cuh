@@ -1,13 +1,13 @@
-// cp_async.cuh - Ampere-style asynchronous global->shared copies used by the popcount kernels.
+// cp_async.cuh - asynchronous global->shared copies (popcount kernels, operand staging of the PCA products).
 #pragma once
 #include <cstdint>
 
-#include "umma.cuh"
+#include <cuda_runtime.h>
 
 namespace pl2 {
 
 __device__ __forceinline__ void cp_async16(void* smem_dst, const void* gmem_src) {
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(smem_u32(smem_dst)), "l"(gmem_src) : "memory");
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(static_cast<uint32_t>(__cvta_generic_to_shared(smem_dst))), "l"(gmem_src) : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 template <int N>

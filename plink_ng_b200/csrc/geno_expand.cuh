@@ -45,20 +45,13 @@ constexpr uint32_t kTabMiss = 0x01000000u;    // mu: missing indicator
 
 // A plane table as a PER-THREAD register.  PRMT needs its table operand in a vector register; a
 // compile-time constant gets hoisted into a uniform register and re-materialised with one extra
-// IMAD.U32 in front of EVERY PRMT (164 of them in king_ts_kernel, ~25 % of its issue slots).  OR-ing in
+// IMAD.U32 in front of EVERY PRMT.  OR-ing in
 // `thread_zero` - a value that is 0 at run time but that ptxas can prove neither constant nor
 // warp-uniform (callers pass threadIdx.x * (a kernel argument >> 31)) - keeps each table in one
 // vector register for the whole kernel.
 __device__ __forceinline__ uint32_t table_reg(uint32_t table, uint32_t thread_zero) { return table | thread_zero; }
 
-// MN-major, no-swizzle UMMA operand tile ("interleave" canonical layout,
-// cute/atom/mma_traits_sm100.hpp:171): 16 consecutive samples of one variant are one 16-byte row
-// of an 8-row core matrix (8 consecutive variants, 128 contiguous bytes); core matrices step by
-// kCoreBytes along the sample (M/N) direction and by `lbo` along the variant (K) direction.
+// Bytes of one no-swizzle core matrix of a wgmma operand in shared memory: 8 rows x 16 K-bytes.
 constexpr uint32_t kCoreBytes = 128;
-__host__ __device__ constexpr uint32_t operand_lbo(uint32_t samples_in_supertile) { return (samples_in_supertile / 16) * kCoreBytes; }
-__host__ __device__ constexpr uint32_t operand_offset(uint32_t k, uint32_t sample_group16, uint32_t lbo) {
-  return (k >> 3) * lbo + sample_group16 * kCoreBytes + (k & 7) * 16;
-}
 
 }  // namespace pl2

@@ -1,24 +1,16 @@
-// geno_tile.cuh - operand re-tiling for the "TS" tensor kernels (king_ts_kernel.cuh, grm_ts_kernel.cuh):
-// 128-row x 80-column pair tiles, row operand expanded into tensor memory, column operand into
-// shared memory.  Kernels are static (header is included by several translation units).
+// geno_tile.cuh - sample-major re-tiling for the tensor kernels (king_ts_kernel.cuh, grm_ts_kernel.cuh,
+// pca_ts_kernels.cuh): an 8-bit wgmma reads both operands K-major, i.e. the variants of one sample contiguous.
+// Kernels are static (header is included by several translation units).
 #pragma once
 #include "common.cuh"
 
 namespace pl2 {
 
-// 128 x 80 pair tiles.  Narrower tiles (128 x 64, eight row-operand slots instead of four) were measured and are
-// SLOWER (26.7 vs 24.2 ms per 16,384 x 65,536 batch): every k-step pays ~12 KB of tcgen05.st into tensor memory
-// (256 B/clk, ~48 clk) on top of its UMMA time whatever the tile width, so the widest tile that still leaves room
-// for a slot ring wins (profiles/r02_king_tile_width.md).
+// 128 x 80 pair tiles (the default KING tiling and the GRM tiling).
 constexpr uint32_t kTsCols = 80;
 constexpr uint32_t kTsSamplePad = 640;  // lcm(128, 80)
-constexpr uint32_t kTsKcJ = 64;         // variants per shared-memory stage (two k-steps)
-constexpr uint32_t kTsRawBoxBytes = 32; // inner extent of the TMA box over the raw block (>= 20 bytes = 80 samples, multiple of 16)
 
 // ---- operand re-tiling of the staged block raw[variant][pitch] (2-bit, variant-major) -------------
-// Both copies make every producer load of king_ts_kernel a contiguous run of bytes (the first TS
-// version read 8 bytes per lane from 32 different rows: 336 L1 wavefronts per k-step, LSU-bound).
-//
 // Row side:  raw_i[row tile rt][k-step ks][row 0..127][8 bytes]   8 bytes = 32 variants of one sample
 // One CTA = 64 variants x 64 samples through a shared-memory byte tile.
 // Only samples [s_base, s_base + 64 * gridDim.y) are written (a job re-tiles its own row tiles only);

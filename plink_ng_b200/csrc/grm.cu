@@ -27,9 +27,8 @@ struct Pl2GrmJob {
   // Double-buffered like the KING job (pl2gpu.cu): copy / all-gather, padding, genotype counts, digit tables and
   // row re-tiling of batch k+1 run on the prep stream while the tensor kernel of batch k runs.
   GenoStage stage[2];
-  uint8_t* d_raw_i[2] = {nullptr, nullptr};  // row-side re-tiled copy of the job's own row tiles (geno_tile.cuh)
-  CUtensorMap tmap[2];                       // tensor maps over stage[b].d_raw for the column-side TMA loads
-  uint32_t* d_tab[2] = {nullptr, nullptr};
+  uint8_t* d_raw_i[2] = {nullptr, nullptr};  // sample-major copy of the staged block (geno_tile.cuh)
+  uint8_t* d_tab[2] = {nullptr, nullptr};    // digit tables (grm_tables_kernel)
   double* d_lvals[2] = {nullptr, nullptr};
   uint32_t* d_counts[2] = {nullptr, nullptr};
   double* h_lvals[2] = {nullptr, nullptr};     // pinned
@@ -58,7 +57,7 @@ int pl2gpu_grm_begin(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start, uin
     return 1;
   }
   PL2_CUDA_OK(cudaSetDevice(ctx->c.device));
-  PL2_CUDA_OK(cudaFuncSetAttribute(grm_ts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kGtsSmemBytes));
+  PL2_CUDA_OK(cudaFuncSetAttribute(grm_wg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kGwSmemBytes));
   Pl2GrmJob* job = new Pl2GrmJob();
   job->ctx = ctx;
   job->sample_ct = sample_ct;
@@ -76,13 +75,12 @@ int pl2gpu_grm_begin(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start, uin
   for (int b = 0; b < 2 && ok; ++b) {
     if (StageAlloc(sample_ct, kMaxStageVariants, &job->stage[b], kGrmSamplePad)) return fail();
     const uint64_t cap = job->stage[b].variant_cap;
-    const uint64_t raw_i_bytes = static_cast<uint64_t>(job->tiles.row_tile_ct) * kTileRows * (cap / 4);
-    ok = cudaMalloc(&job->d_raw_i[b], raw_i_bytes ? raw_i_bytes : 16) == cudaSuccess && cudaMalloc(&job->d_tab[b], cap * kGrmTabPlanes * 4) == cudaSuccess &&
+    const uint64_t raw_i_bytes = static_cast<uint64_t>(job->stage[b].sample_ct_padded) * (cap / 4);
+    ok = cudaMalloc(&job->d_raw_i[b], raw_i_bytes ? raw_i_bytes : 16) == cudaSuccess && cudaMalloc(&job->d_tab[b], cap / 16 * kGrmTabChunkBytes) == cudaSuccess &&
          cudaMalloc(&job->d_lvals[b], cap * 6 * 8) == cudaSuccess && cudaMalloc(&job->d_counts[b], cap * 16) == cudaSuccess &&
          cudaHostAlloc(reinterpret_cast<void**>(&job->h_lvals[b]), cap * 6 * 8, cudaHostAllocDefault) == cudaSuccess &&
          cudaHostAlloc(reinterpret_cast<void**>(&job->h_counts[b]), cap * 16, cudaHostAllocDefault) == cudaSuccess &&
          cudaEventCreateWithFlags(&job->ev_prep_done[b], cudaEventDisableTiming) == cudaSuccess && cudaEventCreateWithFlags(&job->ev_kernel_done[b], cudaEventDisableTiming) == cudaSuccess;
-    if (ok && MakeRawTensorMap(&job->tmap[b], job->stage[b].d_raw, job->stage[b].pitch, job->stage[b].variant_cap, kTsRawBoxBytes, kGrmKc)) return fail();
   }
   if (!ok || cudaMalloc(&job->d_acc_g, words * 8 + 8) != cudaSuccess || cudaMalloc(&job->d_acc_obs, words * 4 + 4) != cudaSuccess || cudaMalloc(&job->d_out_stage, job->out_stage_bytes) != cudaSuccess) {
     cudaGetLastError();
@@ -178,12 +176,12 @@ static int GrmPrepAndLaunch(Pl2GrmJob* job, uint32_t b, uint32_t cur, bool pad_v
   grm_tables_kernel<<<DivUpU32(padded, 128), 128, 0, prep>>>(job->d_lvals[b], cur, padded, scale, job->d_tab[b]);
   c->launches++;
   if (job->tiles.tile_ct) {
-    geno_tile_rows_kernel<<<dim3(padded / 64, job->tiles.row_tile_ct * (kTileRows / 64)), 256, 0, prep>>>(st.d_raw, st.pitch, padded / 32, job->tiles.row_tile_first * kTileRows, job->d_raw_i[b]);
+    geno_tile_rows_kernel<<<dim3(padded / 64, st.sample_ct_padded / 64), 256, 0, prep>>>(st.d_raw, st.pitch, padded / 32, 0, job->d_raw_i[b]);
     c->launches++;
     PL2_CUDA_OK(cudaGetLastError());
     PL2_CUDA_OK(cudaEventRecord(job->ev_prep_done[b], prep));
     PL2_CUDA_OK(cudaStreamWaitEvent(c->stream, job->ev_prep_done[b], 0));
-    grm_ts_kernel<<<job->tiles.tile_ct, kGtsThreads, kGtsSmemBytes, c->stream>>>(job->tmap[b], job->d_raw_i[b], job->tiles.row_tile_first, padded, job->d_tab[b], inv_scale, job->tiles.d_tile_order, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->d_acc_g, job->d_acc_obs);
+    grm_wg_kernel<<<2 * job->tiles.tile_ct, kGwThreads, kGwSmemBytes, c->stream>>>(job->d_raw_i[b], padded, job->d_tab[b], inv_scale, job->tiles.d_tile_order, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->d_acc_g, job->d_acc_obs);
     c->launches++;
     PL2_CUDA_OK(cudaGetLastError());
     PL2_CUDA_OK(cudaEventRecord(job->ev_kernel_done[b], c->stream));

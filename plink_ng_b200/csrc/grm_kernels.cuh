@@ -1,7 +1,7 @@
 // grm_kernels.cuh - device kernels of the GRM path (CalcGrm, 2.0/plink2_matrix_calc.cc:4555).
 //
 // Replaces ExpandCenteredVarmaj + the dsyrk/dgemm accumulation (CalcGrmThread / CalcGrmPartThread,
-// :4285-4327) and the CalcMissingMatrix popcount pass (:4404-4553) with ONE exact int8 tcgen05
+// :4285-4327) and the CalcMissingMatrix popcount pass (:4404-4553) with ONE exact int8 tensor-core
 // contraction per variant batch:
 //
 //   G_ij * obs_ij = sum_v z_iv z_jv,   z_v(g) = intercept_v + g * slope_v (0 for missing)   [PopulateRescaledDosage]
@@ -15,13 +15,11 @@
 // so the only error is the 2^-(F+1) rounding of each table entry: 40 significant bits relative to
 // the largest |L| of the batch (DESIGN.md has the bound; measured < 1e-10 absolute on G).
 //
-// Tile = 128 rows (I side: planes g, m) x 80 cols (J side: 10 digit planes + m).  TMEM columns:
-// [0,400) digit accumulators D_0..D_4, [400,480) obs counts.  The kernel itself is grm_ts_kernel.cuh
-// (an earlier smem x smem form of it lived here; see DESIGN.md section 4 for why it was replaced).
+// Tile = 128 rows (I side: planes g, m) x 80 cols (J side: 10 digit planes + m); accumulators D_0..D_4 and the
+// obs counts.  The kernel itself is grm_ts_kernel.cuh.
 #pragma once
 #include "common.cuh"
 #include "geno_expand.cuh"
-#include "umma.cuh"
 
 namespace pl2 {
 
@@ -31,42 +29,34 @@ constexpr uint32_t kGrmLimbs = 5;
 constexpr uint32_t kGrmFixedBits = 38;          // |L| * 2^F < 2^38
 constexpr uint32_t kGrmPlanesJ = 2 * kGrmLimbs + 1;
 constexpr uint32_t kGrmGroupsJ = kGrmTileCols / 16;  // 16-sample groups per J plane
-constexpr uint32_t kGrmTabPlanes = 12;          // uint32 tables per variant (11 used)
-constexpr uint32_t kGrmKc = 64;                 // variants per stage = two UMMA k-steps
 constexpr uint32_t kGrmTileWords = kTileRows * kGrmTileCols;  // per-tile accumulator entries
-static_assert((kGrmLimbs + 1) * kGrmTileCols <= 512, "GRM accumulators exceed TMEM");
 
-// ---- per-variant digit tables, byte c of a table = digit of that plane for genotype code c.
-// planes 0..4 = L1 digits (least significant first), 5..9 = L2 digits, 10 = m (constant), 11 unused.
-// Layout: tab[variant / 64][plane][variant % 64], so the 32 lanes of a column-side warp (consecutive
-// variants of one stage, same plane) read one contiguous 128-byte line per plane.
+// ---- per-variant digit tables, in the form the column-side expansion of grm_ts_kernel.cuh reads: for every chunk of
+// 16 variants, digit plane p (0..4 = L1 digits, least significant first, 5..9 = L2 digits) and genotype code
+// g (0..2) one 16-byte vector holding that digit of each variant of the chunk, variant v at byte SampleToPos(v % 16)
+// (the K order of the operand rows).  Missing genotypes select no vector and give 0.  The m plane is constant.
 // lvals[v] = {L1(0), L1(1), L1(2), L2(0), L2(1), L2(2)} as doubles (host-prepared, grm.cu).
-__host__ __device__ constexpr uint64_t grm_tab_index(uint32_t v, uint32_t plane) { return static_cast<uint64_t>(v >> 6) * (kGrmTabPlanes * 64) + plane * 64 + (v & 63); }
+constexpr uint32_t kGrmTabChunkBytes = 2 * kGrmLimbs * 3 * 16;  // 480 bytes per 16 variants
+__host__ __device__ constexpr uint64_t grm_tab_offset(uint32_t v, uint32_t plane, uint32_t code) {
+  return (static_cast<uint64_t>(v >> 4) * (2 * kGrmLimbs) + plane) * 48 + code * 16 + SampleToPos(v & 15u);
+}
 
-__global__ void grm_tables_kernel(const double* __restrict__ lvals, uint32_t variant_ct, uint32_t variant_ct_padded, double scale, uint32_t* __restrict__ tab) {
+__global__ void grm_tables_kernel(const double* __restrict__ lvals, uint32_t variant_ct, uint32_t variant_ct_padded, double scale, uint8_t* __restrict__ tabk) {
   const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
   if (v >= variant_ct_padded) return;
-  uint32_t out[kGrmTabPlanes];
 #pragma unroll
-  for (uint32_t p = 0; p < kGrmTabPlanes; ++p) out[p] = 0;
-  out[2 * kGrmLimbs] = kTabNonmiss;
-  if (v < variant_ct) {
+  for (uint32_t which = 0; which < 2; ++which) {
 #pragma unroll
-    for (uint32_t which = 0; which < 2; ++which) {
+    for (uint32_t g = 0; g < 3; ++g) {
+      long long x = (v < variant_ct) ? __double2ll_rn(lvals[6ull * v + 3 * which + g] * scale) : 0;
 #pragma unroll
-      for (uint32_t g = 0; g < 3; ++g) {
-        long long x = __double2ll_rn(lvals[6ull * v + 3 * which + g] * scale);
-#pragma unroll
-        for (uint32_t k = 0; k < kGrmLimbs; ++k) {
-          const long long d = ((x + 128) & 255) - 128;  // balanced base-256 digit in [-128, 127]
-          x = (x - d) >> 8;
-          out[kGrmLimbs * which + k] |= (static_cast<uint32_t>(d) & 0xFFu) << (8 * g);
-        }
+      for (uint32_t k = 0; k < kGrmLimbs; ++k) {
+        const long long d = ((x + 128) & 255) - 128;  // balanced base-256 digit in [-128, 127]
+        x = (x - d) >> 8;
+        tabk[grm_tab_offset(v, kGrmLimbs * which + k, g)] = static_cast<uint8_t>(d & 0xFF);
       }
     }
   }
-#pragma unroll
-  for (uint32_t p = 0; p < kGrmTabPlanes; ++p) tab[grm_tab_index(v, p)] = out[p];
 }
 
 // ---- finalisation: rows [r0, r1) of the lower triangle INCLUDING the diagonal into the reference's

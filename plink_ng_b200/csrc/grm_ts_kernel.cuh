@@ -1,323 +1,224 @@
-// grm_ts_kernel.cuh - GRM contraction, "TS" form: the row-side operand (planes g, m) is expanded from
-// the sample-major re-tiled copy straight into tensor memory, only the column side (10 digit planes
-// + m) goes through shared memory.  Same math, tables and accumulator semantics as grm_kernels.cuh
-// (which documents the fixed-point digit decomposition); that SS form moved 56 KB of operands through
-// shared memory per 440 tensor clocks (127 B/clk of the 128 B/clk available) and sat at 45 % of the
-// tensor pipe.
+// grm_ts_kernel.cuh - GRM contraction on the int8 tensor pipe (wgmma, sm_90a).  Same math, digit tables and
+// accumulator semantics as grm_kernels.cuh, which documents the fixed-point digit decomposition:
+//   D_l += g_I x d1_l,J + m_I x d2_l,J   (l = 0..4),   obs += m_I x m_J.
 //
-// Tile = 128 rows x 80 cols.  TMEM columns: [0,400) digit accumulators D_0..D_4, [400,480) obs counts,
-// [480,512) two A slots of 16 columns (planes g, m; 8 columns = 32 K-bytes per lane).
-// Per 32 variants (6 UMMAs, 440 tensor clk):  m x [d2_0 d2_1], m x [d2_2 d2_3], m x [d2_4 | m] (N = 160,
-// lands on D_4 and obs), g x [d1_0 d1_1], g x [d1_2 d1_3], g x d1_4.  The m products are issued first so
-// that on the very first k-step they zero-initialise every accumulator (accumulate = 0) and the g
-// products always accumulate.
+// One CTA = 64 rows (half of a 128-row tile) x 80 columns, two warpgroups with int32 accumulators in registers:
+//   warpgroup 0: D_0, D_1, D_2;  warpgroup 1: D_3, D_4, obs (+ g x a zero plane, so that both warpgroups issue
+//   the same six wgmmas per k32 step: a wgmma under a branch is serialised).
+// Row side (A): planes g, m expanded by each thread straight into its fragment registers from the sample-major
+// copy (wgmma.cuh).  Column side (B): 11 planes of the 80 column samples in the K-major no-swizzle layout in shared
+// memory, one 64-variant stage ahead (double buffer).  A K-major row holds 16 variants of one sample, each with its
+// own digit table, so a byte cannot come from one PRMT table as on the row side: the stage's tables are kept as
+// three 16-byte vectors per (16-variant chunk, plane) - the digit for genotype 0, 1, 2 of each variant, in the K
+// order of the fragments - and a row is (t0 & mask0) | (t1 & mask1) | (t2 & mask2) with byte masks of the codes.
 #pragma once
-#include <cuda.h>
 
 #include "common.cuh"
 #include "geno_expand.cuh"
 #include "geno_tile.cuh"
 #include "grm_kernels.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace pl2 {
 
-static_assert(kGrmTileCols == kTsCols && kGrmSamplePad == kTsSamplePad && kGrmKc == kTsKcJ, "GRM TS kernel shares the KING TS tiling");
-constexpr uint32_t kGtsAccCols = (kGrmLimbs + 1) * kGrmTileCols;          // 480
-constexpr uint32_t kGtsASlots = 2;
-constexpr uint32_t kGtsASlotCols = 16;
-constexpr uint32_t kGtsStagesJ = 3;
-constexpr uint32_t kGtsLboJ = kGrmPlanesJ * kGrmGroupsJ * kCoreBytes + 64;  // 7104: +64 keeps the K-permuted rows bank-conflict free
-constexpr uint32_t kGtsStageBytesJ = (kGrmKc / 8) * kGtsLboJ;               // 56832
-// Operand staging as in king_ts_kernel.cuh: one producer warp keeps three shared-memory rings full with the TMA
-// unit - raw column boxes read in place from the variant-major block through a tensor map (UTMALDG), row-side
-// k-steps of the sample-major copy, and the per-variant digit tables (both UBLKCP).
-constexpr uint32_t kGtsRawJSlots = 4;
-constexpr uint32_t kGtsRawJBytes = kGrmKc * kTsRawBoxBytes;                 // 2048
-constexpr uint32_t kGtsRawISlots = 2;                                       // four row-side k-steps per 4 KB copy
-constexpr uint32_t kGtsRawIBytes = 4 * kTileRows * 8;                       // 4096
-constexpr uint32_t kGtsTabSlots = 4;
-constexpr uint32_t kGtsTabBytes = kGrmTabPlanes * kGrmKc * 4;               // 3072
-constexpr uint32_t kGtsSmemOffRawJ = kGtsStagesJ * kGtsStageBytesJ;         // 170496 (multiple of 128)
-constexpr uint32_t kGtsSmemOffRawI = kGtsSmemOffRawJ + kGtsRawJSlots * kGtsRawJBytes;
-constexpr uint32_t kGtsSmemOffTab = kGtsSmemOffRawI + kGtsRawISlots * kGtsRawIBytes;
-constexpr uint32_t kGtsSmemBytes = kGtsSmemOffTab + kGtsTabSlots * kGtsTabBytes + 1024;
-constexpr uint32_t kGtsRowWarps = 8;
-constexpr uint32_t kGtsColWarps = 10;                                       // 5 words x 64 variants per stage
-constexpr uint32_t kGtsIssuerWarp = kGtsRowWarps + kGtsColWarps;
-constexpr uint32_t kGtsThreads = 32 * (kGtsRowWarps + kGtsColWarps + 2);    // + UMMA issuer + TMA producer
-static_assert(kGtsSmemOffRawJ % 128 == 0, "TMA destination alignment (128 bytes without swizzle)");
-static_assert(kGtsSmemBytes <= 232448, "GRM TS pipeline exceeds the 227 KB shared-memory opt-in limit");
-static_assert(kGtsAccCols + kGtsASlots * kGtsASlotCols <= 512, "GRM TS accumulators + A slots exceed TMEM");
+static_assert(kGrmTileCols == kTsCols && kGrmSamplePad == kTsSamplePad, "GRM shares the KING tiling");
+constexpr uint32_t kGwKs = 2;                                        // k32 steps per stage (64 variants)
+constexpr uint32_t kGwThreads = 256;
+constexpr uint32_t kGwSbo = 2 * kGwKs * kCoreBytes;                  // 512: next group of 8 B rows
+constexpr uint32_t kGwZeroPlane = kGrmPlanesJ;                       // plane 11: zeros
+constexpr uint32_t kGwRowsB = (kGrmPlanesJ + 1) * kGrmTileCols;      // 960 B rows: planes 0..11 stacked along N
+constexpr uint32_t kGwBBytes = kGwRowsB * 32 * kGwKs;                // 61440
+constexpr uint32_t kGwABytes = kGwKs * 64 * 8;                       // 1024
+constexpr uint32_t kGwTabBytes = (32 * kGwKs / 16) * kGrmTabChunkBytes;  // 1920
+constexpr uint32_t kGwStageBytes = kGwBBytes + kGwABytes + kGwTabBytes;
+constexpr uint32_t kGwSmemBytes = 2 * kGwStageBytes + 128;
+constexpr uint32_t kGwItems = kGrmTileCols * 2 * kGwKs;              // (column sample, 16-variant chunk) per stage
+static_assert(kGwSmemBytes <= 232448, "exceeds the 227 KB shared-memory opt-in limit");
+static_assert(kGwTabBytes % 16 == 0, "staging granularity");
 
-__global__ void __launch_bounds__(kGtsThreads, 1)
-grm_ts_kernel(const __grid_constant__ CUtensorMap tmap_raw, const uint8_t* __restrict__ raw_i, uint32_t row_tile_first, uint32_t variant_ct_padded /* multiple of 256 */, const uint32_t* __restrict__ tab, double inv_scale, const uint32_t* __restrict__ tile_order, const uint32_t* __restrict__ tile_rt, const uint32_t* __restrict__ tile_tc, double* __restrict__ acc_g, int32_t* __restrict__ acc_obs) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ __align__(8) uint64_t bar_full_a[kGtsASlots];
-  __shared__ __align__(8) uint64_t bar_empty_a[kGtsASlots];
-  __shared__ __align__(8) uint64_t bar_full_b[kGtsStagesJ];
-  __shared__ __align__(8) uint64_t bar_empty_b[kGtsStagesJ];
-  __shared__ __align__(8) uint64_t bar_full_rj[kGtsRawJSlots];   // raw column box + its table slot (same ring index)
-  __shared__ __align__(8) uint64_t bar_empty_rj[kGtsRawJSlots];
-  __shared__ __align__(8) uint64_t bar_full_ri[kGtsRawISlots];
-  __shared__ __align__(8) uint64_t bar_empty_ri[kGtsRawISlots];
-  __shared__ __align__(8) uint64_t bar_acc;
-  __shared__ uint32_t tmem_base_slot;
+template <int N>
+__device__ __forceinline__ void grm_acc_zero(int32_t (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) d[i] = 0;
+}
 
-  const uint32_t tid = threadIdx.x;
-  const uint32_t warp = uniform_warp_idx();
-  const uint32_t lane = tid & 31;
-  const uint32_t tile = tile_order[blockIdx.x];
-  const uint32_t rt = tile_rt[tile];
-  const uint32_t ct = tile_tc[tile];
-  const uint32_t stage_iters = variant_ct_padded / kGrmKc;
-  const uint32_t smem_base = (smem_u32(smem) + 1023u) & ~1023u;
+// raw_t: sample-major copy of the whole padded block; tabk: grm_tables_kernel output.  Grid: 2 CTAs per tile.
+__global__ void __launch_bounds__(kGwThreads, 1)
+grm_wg_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* multiple of 256 */, const uint8_t* __restrict__ tabk, double inv_scale, const uint32_t* __restrict__ tile_order, const uint32_t* __restrict__ tile_rt, const uint32_t* __restrict__ tile_tc, double* __restrict__ acc_g, int32_t* __restrict__ acc_obs) {
+  extern __shared__ __align__(128) uint8_t smem_dyn[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 127) & ~static_cast<uintptr_t>(127));
+  const uint32_t smem_base = static_cast<uint32_t>(__cvta_generic_to_shared(smem));
+  const uint32_t tid = threadIdx.x, wg = tid >> 7, warp4 = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, c = lane & 3;
+  const uint32_t tile = tile_order[blockIdx.x >> 1];
+  const uint32_t half = blockIdx.x & 1;
+  const uint32_t rt = tile_rt[tile], ct = tile_tc[tile];
+  const uint32_t kstep_ct = variant_ct_padded / 32;
+  const uint32_t stage_ct = kstep_ct / kGwKs;
+  const uint32_t thread_zero = tid * (variant_ct_padded >> 31);
+  const uint32_t tab_g = table_reg(kTabDosage, thread_zero), tab_m = table_reg(kTabNonmiss, thread_zero);
+  const uint32_t mask0 = table_reg(0x000000FFu, thread_zero), mask1 = table_reg(0x0000FF00u, thread_zero), mask2 = table_reg(0x00FF0000u, thread_zero);
 
-  if (tid == 0) {
-    for (uint32_t s = 0; s < kGtsASlots; ++s) {
-      mbar_init(&bar_full_a[s], 4);  // one arrival per row-side warp of the owning group
-      mbar_init(&bar_empty_a[s], 1);
+  // ---- staging of one stage: column words (registers), row words and tables (16-byte pieces)
+  constexpr uint32_t kItemsPerThread = (kGwItems + kGwThreads - 1) / kGwThreads;
+  struct Pre {
+    uint32_t w[kItemsPerThread];
+    uint2 a;
+    uint4 t[(kGwTabBytes / 16 + kGwThreads - 1) / kGwThreads];
+  };
+  auto load_stage = [&](uint32_t st) -> Pre {
+    Pre p;
+#pragma unroll
+    for (uint32_t q = 0; q < kItemsPerThread; ++q) {
+      const uint32_t i = tid + q * kGwThreads;
+      p.w[q] = 0xFFFFFFFFu;
+      if (i < kGwItems) {
+        const uint32_t n = i % kGrmTileCols, kc = i / kGrmTileCols;  // a warp shares its chunk: broadcast table reads
+        const uint32_t s = kGrmTileCols * ct + n, ks = st * kGwKs + (kc >> 1);
+        p.w[q] = __ldg(reinterpret_cast<const uint32_t*>(raw_t + (static_cast<uint64_t>(s >> 7) * kstep_ct + ks) * 1024 + (s & 127) * 8 + 4 * (kc & 1)));
+      }
     }
-    for (uint32_t s = 0; s < kGtsStagesJ; ++s) {
-      mbar_init(&bar_full_b[s], kGtsColWarps);
-      mbar_init(&bar_empty_b[s], 1);
+    {  // row words: [k-step][64 rows][8 B]; thread = (k-step, row)
+      const uint32_t ks = st * kGwKs + (tid >> 7), row = 64 * half + (tid & 63);
+      p.a = (tid & 64) ? make_uint2(0, 0) : __ldg(reinterpret_cast<const uint2*>(raw_t + (static_cast<uint64_t>(rt) * kstep_ct + ks) * 1024 + row * 8));
     }
-    for (uint32_t s = 0; s < kGtsRawJSlots; ++s) {
-      mbar_init(&bar_full_rj[s], 1);
-      mbar_init(&bar_empty_rj[s], kGtsColWarps);
+#pragma unroll
+    for (uint32_t q = 0; q < sizeof(p.t) / 16; ++q) {
+      const uint32_t i = tid + q * kGwThreads;
+      if (i < kGwTabBytes / 16) p.t[q] = __ldg(reinterpret_cast<const uint4*>(tabk + static_cast<uint64_t>(st) * kGwTabBytes) + i);
     }
-    for (uint32_t s = 0; s < kGtsRawISlots; ++s) {
-      mbar_init(&bar_full_ri[s], 1);
-      mbar_init(&bar_empty_ri[s], kGtsRowWarps);
+    return p;
+  };
+  auto sts128 = [](uint32_t addr, const uint4& v) { asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory"); };
+  auto lds128 = [](uint32_t addr) -> uint4 {
+    uint4 v;
+    asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(addr) : "memory");
+    return v;
+  };
+  // part 1: row words and tables into shared memory (the tables feed part 2 of the same stage)
+  auto store_stage_raw = [&](const Pre& p, uint32_t buf) {
+    const uint32_t base = smem_base + buf * kGwStageBytes;
+    if (!(tid & 64)) asm volatile("st.shared.v2.b32 [%0], {%1,%2};" ::"r"(base + kGwBBytes + (tid >> 7) * 512 + (tid & 63) * 8), "r"(p.a.x), "r"(p.a.y) : "memory");
+#pragma unroll
+    for (uint32_t q = 0; q < sizeof(p.t) / 16; ++q) {
+      const uint32_t i = tid + q * kGwThreads;
+      if (i < kGwTabBytes / 16) sts128(base + kGwBBytes + kGwABytes + 16 * i, p.t[q]);
     }
-    mbar_init(&bar_acc, 1);
-    mbar_fence_init();
+  };
+  // part 2: column words -> 11 planes (needs the stage's tables in shared memory)
+  auto store_stage_b = [&](const Pre& p, uint32_t buf) {
+    const uint32_t base = smem_base + buf * kGwStageBytes;
+    const uint32_t tabs = base + kGwBBytes + kGwABytes;
+#pragma unroll
+    for (uint32_t q = 0; q < kItemsPerThread; ++q) {
+      const uint32_t i = tid + q * kGwThreads;
+      if (i < kGwItems) {
+        const uint32_t n = i % kGrmTileCols, kc = i / kGrmTileCols;
+        const Sel4 sel = make_selectors(p.w[q]);
+        const uint4 m0 = expand16(mask0, sel), m1 = expand16(mask1, sel), m2 = expand16(mask2, sel);
+        const uint32_t dst = base + kc * kCoreBytes + (n & 7) * 16;
+#pragma unroll
+        for (uint32_t pl = 0; pl < 2 * kGrmLimbs; ++pl) {
+          const uint32_t t = tabs + (kc * 2 * kGrmLimbs + pl) * 48;
+          const uint4 t0 = lds128(t), t1 = lds128(t + 16), t2 = lds128(t + 32);
+          uint4 v;
+          v.x = (t0.x & m0.x) | (t1.x & m1.x) | (t2.x & m2.x);
+          v.y = (t0.y & m0.y) | (t1.y & m1.y) | (t2.y & m2.y);
+          v.z = (t0.z & m0.z) | (t1.z & m1.z) | (t2.z & m2.z);
+          v.w = (t0.w & m0.w) | (t1.w & m1.w) | (t2.w & m2.w);
+          const uint32_t row = pl * kGrmTileCols + n;
+          sts128(dst + (row >> 3) * kGwSbo, v);
+        }
+        sts128(dst + ((2 * kGrmLimbs * kGrmTileCols + n) >> 3) * kGwSbo, expand16(tab_m, sel));  // plane 10: m
+      }
+    }
+  };
+
+  // warpgroup 0: D_0..D_2; warpgroup 1: D_3, D_4, obs
+  int32_t da[kGrmTileCols / 2], db[kGrmTileCols / 2], dc[kGrmTileCols / 2];
+  grm_acc_zero(da);
+  grm_acc_zero(db);
+  grm_acc_zero(dc);
+  const uint32_t r_lo = 16 * warp4 + g;
+  constexpr uint32_t kPlaneStep = (kGrmTileCols / 8) * kGwSbo;  // 5120 bytes between planes
+  const uint32_t l0 = wg ? 3 : 0;                                // first digit of this warpgroup
+
+  {
+    constexpr uint32_t kZeroBytes = kGrmTileCols * 32 * kGwKs;
+    for (uint32_t i = tid; i < 2 * kZeroBytes / 16; i += kGwThreads) {
+      const uint32_t buf = i / (kZeroBytes / 16);
+      sts128(smem_base + buf * kGwStageBytes + kGwZeroPlane * kZeroBytes + 16 * (i % (kZeroBytes / 16)), make_uint4(0, 0, 0, 0));
+    }
+    const Pre p0 = load_stage(0);
+    store_stage_raw(p0, 0);
+    __syncthreads();
+    store_stage_b(p0, 0);
   }
-  if (warp == kGtsIssuerWarp) tmem_alloc<512>(&tmem_base_slot);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_base_slot;
-
-  if (warp < kGtsRowWarps) {
-    // ---------------- row-side producers: 2-bit words -> registers -> tensor memory ----------------
-    // Group g = warp / 4 owns k-steps ks = 2 n + g and A slot g.  Thread = TMEM lane = sample.
-    const uint32_t grp = warp >> 2;
-    const uint32_t lq = warp & 3;
-    const uint32_t row = 32 * lq + lane;
-    const uint32_t thread_zero = tid * (variant_ct_padded >> 31);  // 0; keeps the tables in vector registers (geno_expand.cuh)
-    const uint32_t tab_g = table_reg(kTabDosage, thread_zero), tab_m = table_reg(kTabNonmiss, thread_zero);
-    const uint32_t ring_i = smem_base + kGtsSmemOffRawI + row * 8;
-    const uint32_t ta = tmem_base + ((32u * lq) << 16) + kGtsAccCols + grp * kGtsASlotCols;
-    struct ExpI {
-      uint32_t v[2][8];
-    };
-    auto expand_i = [&](const uint2& w) -> ExpI {
-      ExpI e;
-      const Sel4 s0 = make_selectors(w.x), s1 = make_selectors(w.y);
-      const uint32_t tabs[2] = {tab_g, tab_m};
-#pragma unroll
-      for (int p = 0; p < 2; ++p) {
-        const uint4 a = expand16(tabs[p], s0), b = expand16(tabs[p], s1);
-        e.v[p][0] = a.x; e.v[p][1] = a.y; e.v[p][2] = a.z; e.v[p][3] = a.w;
-        e.v[p][4] = b.x; e.v[p][5] = b.y; e.v[p][6] = b.z; e.v[p][7] = b.w;
-      }
-      return e;
-    };
-    // ring slot = k-steps 4 q .. 4 q + 3; this group needs 4 q + grp and 4 q + grp + 2 (see king_ts_kernel.cuh)
-    struct Words {
-      uint2 w[2];
-    };
-    auto load_slot = [&](uint32_t q) -> Words {
-      const uint32_t si = q % kGtsRawISlots;
-      mbar_wait(&bar_full_ri[si], (q / kGtsRawISlots) & 1);
-      Words r;
-      r.w[0] = lds64(ring_i + si * kGtsRawIBytes + grp * (kTileRows * 8));
-      r.w[1] = lds64(ring_i + si * kGtsRawIBytes + (grp + 2) * (kTileRows * 8));
-      return r;  // released after both words went through tcgen05.st (king_ts_kernel.cuh explains why)
-    };
-    const uint32_t slot_iters = stage_iters / 2;  // stage_iters is a multiple of 4 (variant pad 256)
-    Words words = load_slot(0);
-    ExpI cur = expand_i(words.w[0]);
-    for (uint32_t q = 0; q < slot_iters; ++q) {
-#pragma unroll
-      for (uint32_t h = 0; h < 2; ++h) {
-        const uint32_t n = 2 * q + h;  // k-step 2 n + grp
-        mbar_wait(&bar_empty_a[grp], (n & 1) ^ 1);
-        tc_fence_after_sync();
-        tmem_st8(ta, cur.v[0]);
-        tmem_st8(ta + 8, cur.v[1]);
-        tmem_st_wait();
-        tc_fence_before_sync();
-        mbar_arrive_warp(&bar_full_a[grp], lane);
-        if (h == 0) {
-          cur = expand_i(words.w[1]);
-        } else {
-          mbar_arrive_warp(&bar_empty_ri[q % kGtsRawISlots], lane);
-          if (q + 1 < slot_iters) {
-            words = load_slot(q + 1);
-            cur = expand_i(words.w[0]);
-          }
-        }
-      }
-    }
-  } else if (warp < kGtsRowWarps + kGtsColWarps) {
-    // ---------------- column-side producers: 2-bit words -> 11 int8 planes in shared memory ----------------
-    // Thread = (word w of the 20-byte row, variant k of the 64-variant stage); the per-variant digit
-    // tables come from grm_tables_kernel.
-    const uint32_t t = tid - 32 * kGtsRowWarps;  // 0..319
-    const uint32_t combo = t >> 3;               // (k group of 8) * 5 + word: see king_ts_kernel.cuh
-    const uint32_t k = 8 * (combo / 5) + (t & 7);
-    const uint32_t w = combo % 5;
-    const uint32_t ring_j = smem_base + kGtsSmemOffRawJ + k * kTsRawBoxBytes + ((ct * (kGrmTileCols / 4)) & 15u) + 4 * w;  // box starts 16-byte aligned
-    const uint32_t ring_t = smem_base + kGtsSmemOffTab + 4 * k;  // tab[slot][plane][64 variants] (grm_tab_index)
-    const uint32_t kpos = (k & ~15u) + SampleToPos(k & 15u);  // K rows in the PRMT position order of the row side
-    const uint32_t dst_k = (kpos >> 3) * kGtsLboJ + (kpos & 7) * 16 + w * kCoreBytes;
-    struct RowJ {
-      uint32_t w;
-      uint32_t t[kGrmPlanesJ];  // tables of planes 0..10
-    };
-    auto fetch = [&](uint32_t it) -> RowJ {
-      const uint32_t sj = it % kGtsRawJSlots;
-      mbar_wait(&bar_full_rj[sj], (it / kGtsRawJSlots) & 1);
-      RowJ r;
-      r.w = lds32(ring_j + sj * kGtsRawJBytes);
-#pragma unroll
-      for (uint32_t p = 0; p < kGrmPlanesJ; ++p) r.t[p] = lds32(ring_t + sj * kGtsTabBytes + p * (kGrmKc * 4));
-      return r;
-    };
-    auto sts16 = [](uint32_t addr, const uint4& v) { asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory"); };
-    constexpr uint32_t kPlane = kGrmGroupsJ * kCoreBytes;  // 640 bytes between planes inside a k-group
-    RowJ cur = fetch(0);
-    uint32_t sb = 0, ph = 0;
-    for (uint32_t it = 0; it < stage_iters; ++it) {
-      const Sel4 sel = make_selectors(cur.w);
-      mbar_wait(&bar_empty_b[sb], ph ^ 1);
-      const uint32_t a0 = smem_base + sb * kGtsStageBytesJ + dst_k;
-#pragma unroll
-      for (uint32_t p = 0; p < kGrmPlanesJ; ++p) sts16(a0 + p * kPlane, expand16(cur.t[p], sel));
-      // every lane has consumed its ring words (they fed the PRMTs above): release the raw / table slot
-      mbar_arrive_warp(&bar_empty_rj[it % kGtsRawJSlots], lane);
-      fence_proxy_async_smem();
-      mbar_arrive_warp(&bar_full_b[sb], lane);
-      if (it + 1 < stage_iters) cur = fetch(it + 1);
-      if (++sb == kGtsStagesJ) {
-        sb = 0;
-        ph ^= 1;
-      }
-    }
-  } else if (warp == kGtsIssuerWarp) {
-    // ---------------- UMMA issuer: whole warp loops, one elected lane issues (umma.cuh) ----------------
-    constexpr uint32_t idesc_n160 = make_idesc_i8(128, 2 * kGrmTileCols, false, true);
-    constexpr uint32_t idesc_n80 = make_idesc_i8(128, kGrmTileCols, false, true);
-    constexpr uint32_t kPlaneStep = (kGrmGroupsJ * kCoreBytes) >> 4;  // plane step in descriptor units
-    const uint32_t tmem_u = uniform_u32(tmem_base);
-    const uint64_t desc0 = make_smem_desc(smem_base, kGtsLboJ, kCoreBytes);
-    uint32_t sb = 0, ph = 0;
-    for (uint32_t it = 0; it < stage_iters; ++it) {
-      mbar_wait(&bar_full_b[sb], ph);
-#pragma unroll
-      for (uint32_t kk = 0; kk < 2; ++kk) {
-        // k-step ks = 2 it + kk lives in A slot kk, round it
-        mbar_wait(&bar_full_a[kk], it & 1);
-        tc_fence_after_sync();
-        if (elect_one_sync()) {
-          const uint32_t acc = (it | kk) ? 1u : 0u;  // 0 only on the very first k-step
-          const uint64_t bj = desc0 + ((sb * kGtsStageBytesJ + kk * 4 * kGtsLboJ) >> 4);
-          const uint32_t a_g = tmem_u + kGtsAccCols + kk * kGtsASlotCols;
-          const uint32_t a_m = a_g + 8;
-          umma_i8_ts(tmem_u + 0, a_m, bj + 5 * kPlaneStep, idesc_n160, acc);                    // m x [d2_0 d2_1]
-          umma_i8_ts(tmem_u + 2 * kGrmTileCols, a_m, bj + 7 * kPlaneStep, idesc_n160, acc);     // m x [d2_2 d2_3]
-          umma_i8_ts(tmem_u + 4 * kGrmTileCols, a_m, bj + 9 * kPlaneStep, idesc_n160, acc);     // m x [d2_4 | m] -> D_4, obs
-          umma_i8_ts(tmem_u + 0, a_g, bj, idesc_n160, 1u);                                        // g x [d1_0 d1_1]
-          umma_i8_ts(tmem_u + 2 * kGrmTileCols, a_g, bj + 2 * kPlaneStep, idesc_n160, 1u);        // g x [d1_2 d1_3]
-          umma_i8_ts(tmem_u + 4 * kGrmTileCols, a_g, bj + 4 * kPlaneStep, idesc_n80, 1u);         // g x d1_4
-          umma_commit(&bar_empty_a[kk]);
-          if (kk == 1) umma_commit(&bar_empty_b[sb]);
-        }
-        __syncwarp();
-      }
-      if (++sb == kGtsStagesJ) {
-        sb = 0;
-        ph ^= 1;
-      }
-    }
-    if (elect_one_sync()) umma_commit(&bar_acc);
-    __syncwarp();
-  } else {
-    // ---------------- TMA producer: one elected lane keeps the raw / table rings full ----------------
-    if (elect_one_sync()) {
-      const uint8_t* src_i = raw_i + static_cast<uint64_t>(rt - row_tile_first) * (2 * stage_iters) * (kTileRows * 8);
-      const uint32_t ring_j = smem_base + kGtsSmemOffRawJ, ring_i = smem_base + kGtsSmemOffRawI, ring_t = smem_base + kGtsSmemOffTab;
-      const int32_t c0 = static_cast<int32_t>((ct * (kGrmTileCols / 4)) & ~15u);
-      for (uint32_t it = 0; it < stage_iters; ++it) {
-        if (!(it & 1)) {
-          const uint32_t q = it >> 1, si = q % kGtsRawISlots;
-          mbar_wait(&bar_empty_ri[si], ((q / kGtsRawISlots) & 1) ^ 1);
-          mbar_expect_tx(&bar_full_ri[si], kGtsRawIBytes);
-          bulk_load_1d(ring_i + si * kGtsRawIBytes, src_i + static_cast<uint64_t>(q) * kGtsRawIBytes, kGtsRawIBytes, &bar_full_ri[si]);
-        }
-        const uint32_t sj = it % kGtsRawJSlots;
-        mbar_wait(&bar_empty_rj[sj], ((it / kGtsRawJSlots) & 1) ^ 1);
-        mbar_expect_tx(&bar_full_rj[sj], kGtsRawJBytes + kGtsTabBytes);
-        tma_load_2d(ring_j + sj * kGtsRawJBytes, &tmap_raw, c0, static_cast<int32_t>(it * kGrmKc), &bar_full_rj[sj]);
-        bulk_load_1d(ring_t + sj * kGtsTabBytes, tab + static_cast<uint64_t>(it) * (kGrmTabPlanes * kGrmKc), kGtsTabBytes, &bar_full_rj[sj]);
-      }
-    }
-    __syncwarp();
-  }
-
-  if (warp < kGtsRowWarps) {
-    // ---------------- epilogue: digits -> fp64 in shared memory -> bulk reduce-add into the HBM accumulators ----------------
-    // As in king_ts_kernel.cuh: the tile's fp64 sums (80 KB) and observation counts (40 KB) are staged in the idle
-    // operand stages and added to the accumulators by two cp.reduce.async.bulk operations (.add.f64 / .add.s32) at
-    // the L2, instead of a latency-bound load-add-store per element.  One add per element and launch: bit-identical
-    // to the in-register `+=`.
-    mbar_wait(&bar_acc, 0);
-    tc_fence_after_sync();
-    constexpr uint32_t kStageG = kGrmTileCols * kTileRows * 8, kStageO = kGrmTileCols * kTileRows * 4;  // 81920 + 40960
-    static_assert(kStageG + kStageO <= kGtsSmemOffRawJ, "epilogue staging must fit the operand stages");
-    const uint32_t lane_grp = warp & 3;
-    const uint32_t rsample = 32 * lane_grp + lane;  // rows are in natural sample order here
-    const uint32_t stage_g = smem_base + rsample * 8, stage_o = smem_base + kStageG + rsample * 4;
-    const uint32_t taddr = tmem_base + ((32u * lane_grp) << 16);
-    // 5 column groups of 16: warps 0-3 take groups {0,2,4}, warps 4-7 take {1,3}
-#pragma unroll 1
-    for (uint32_t grp = warp >> 2; grp < kGrmGroupsJ; grp += 2) {
-      const uint32_t c0 = grp * 16;
-      uint32_t d0[16], d1[16], d2[16], d3[16], d4[16], nn[16];
-      tmem_ld16(taddr + c0, d0);
-      tmem_ld16(taddr + kGrmTileCols + c0, d1);
-      tmem_ld16(taddr + 2 * kGrmTileCols + c0, d2);
-      tmem_ld16(taddr + 3 * kGrmTileCols + c0, d3);
-      tmem_ld16(taddr + 4 * kGrmTileCols + c0, d4);
-      tmem_ld16(taddr + 5 * kGrmTileCols + c0, nn);
-      tmem_ld_wait();
-#pragma unroll
-      for (uint32_t c = 0; c < 16; ++c) {
-        const uint32_t csample = c0 + PosToSample(c);
-        const long long tot = static_cast<long long>(static_cast<int32_t>(d0[c])) + (static_cast<long long>(static_cast<int32_t>(d1[c])) << 8) +
-                              (static_cast<long long>(static_cast<int32_t>(d2[c])) << 16) + (static_cast<long long>(static_cast<int32_t>(d3[c])) << 24) +
-                              (static_cast<long long>(static_cast<int32_t>(d4[c])) << 32);
-        sts64(stage_g + csample * (kTileRows * 8), static_cast<double>(tot) * inv_scale);
-        sts32(stage_o + csample * (kTileRows * 4), nn[c]);
-      }
-    }
+  for (uint32_t st = 0; st < stage_ct; ++st) {
+    const uint32_t buf = st & 1;
+    const bool more = st + 1 < stage_ct;
+    Pre next;
+    if (more) next = load_stage(st + 1);
     fence_proxy_async_smem();
-    tc_fence_before_sync();
-    named_bar_sync<2, 32 * kGtsRowWarps>();
-    if (tid == 0) {
-      bulk_reduce_add_f64(acc_g + static_cast<uint64_t>(tile) * kGrmTileWords, smem_base, kStageG);
-      bulk_reduce_add_s32(acc_obs + static_cast<uint64_t>(tile) * kGrmTileWords, smem_base + kStageG, kStageO);
-      bulk_commit_group();
+    __syncthreads();  // stage st in shared memory; the other buffer's wgmmas have retired
+    if (more) store_stage_raw(next, buf ^ 1);
+    const uint32_t base = smem_base + buf * kGwStageBytes;
+    const uint64_t desc = make_wg_desc(base, kCoreBytes, kGwSbo);
+#pragma unroll
+    for (uint32_t ks = 0; ks < kGwKs; ++ks) {
+      uint2 w_lo, w_hi;
+      asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w_lo.x), "=r"(w_lo.y) : "r"(base + kGwBBytes + ks * 512 + r_lo * 8) : "memory");
+      asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w_hi.x), "=r"(w_hi.y) : "r"(base + kGwBBytes + ks * 512 + (r_lo + 8) * 8) : "memory");
+      const ASel sel = make_asel(w_lo, w_hi, c);
+      uint32_t fg[4], fm[4];
+      afrag(tab_g, sel, fg);
+      afrag(tab_m, sel, fm);
+      const uint64_t dk = desc + ((ks * 2 * kCoreBytes) >> 4);
+      auto plane = [&](uint32_t pl) { return dk + ((pl * kPlaneStep) >> 4); };
+      wgmma_fence();
+      wgmma_s8_rs<kGrmTileCols>(da, fg, plane(l0));
+      wgmma_s8_rs<kGrmTileCols>(da, fm, plane(kGrmLimbs + l0));
+      wgmma_s8_rs<kGrmTileCols>(db, fg, plane(l0 + 1));
+      wgmma_s8_rs<kGrmTileCols>(db, fm, plane(kGrmLimbs + l0 + 1));
+      wgmma_s8_rs<kGrmTileCols>(dc, fg, plane(wg ? kGwZeroPlane : 2));
+      wgmma_s8_rs<kGrmTileCols>(dc, fm, plane(wg ? 2 * kGrmLimbs : kGrmLimbs + 2));  // warpgroup 1: obs = m x m
+      wgmma_commit();
+      wgmma_wait<1>();
     }
+    if (more) {
+      __syncthreads();  // the next stage's tables are in shared memory
+      store_stage_b(next, buf ^ 1);
+    }
+    wgmma_wait<0>();
+  }
+
+  // ---- epilogue: D = D_0 + 2^8 D_1 + ... + 2^32 D_4 in int64 (warpgroup 1 hands 2^24 D_3 + 2^32 D_4 over through
+  // shared memory), then one fp64 add into acc_g and one int32 add into acc_obs per element
+  __syncthreads();  // operand buffers are free
+  long long* part = reinterpret_cast<long long*>(smem);  // [64 rows][80 columns]
+  const uint32_t r = 64 * half + r_lo;
+  if (wg == 1) {
+#pragma unroll
+    for (uint32_t j = 0; j < kGrmTileCols / 8; ++j)
+#pragma unroll
+      for (uint32_t i = 0; i < 4; ++i) {
+        const uint32_t col = 8 * j + 2 * c + (i & 1), row = r_lo + 8 * (i >> 1);
+        part[row * kGrmTileCols + col] = (static_cast<long long>(da[4 * j + i]) << 24) + (static_cast<long long>(db[4 * j + i]) << 32);
+        int32_t* o = acc_obs + static_cast<uint64_t>(tile) * kGrmTileWords + static_cast<uint64_t>(col) * kTileRows + r + 8 * (i >> 1);
+        *o += dc[4 * j + i];
+      }
   }
   __syncthreads();
-  if (warp == kGtsIssuerWarp) {
-    tc_fence_after_sync();
-    tmem_dealloc<512>(tmem_base);
+  if (wg == 0) {
+#pragma unroll
+    for (uint32_t j = 0; j < kGrmTileCols / 8; ++j)
+#pragma unroll
+      for (uint32_t i = 0; i < 4; ++i) {
+        const uint32_t col = 8 * j + 2 * c + (i & 1), row = r_lo + 8 * (i >> 1);
+        const long long tot = static_cast<long long>(da[4 * j + i]) + (static_cast<long long>(db[4 * j + i]) << 8) + (static_cast<long long>(dc[4 * j + i]) << 16) + part[row * kGrmTileCols + col];
+        double* o = acc_g + static_cast<uint64_t>(tile) * kGrmTileWords + static_cast<uint64_t>(col) * kTileRows + r + 8 * (i >> 1);
+        *o += static_cast<double>(tot) * inv_scale;
+      }
   }
-  if (tid == 0) bulk_wait_group_read<0>();  // shared memory must outlive the reductions' reads
 }
 
 }  // namespace pl2

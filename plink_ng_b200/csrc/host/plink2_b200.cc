@@ -3957,7 +3957,7 @@ int main(int argc, char** argv) {
   for (int i = 1; i + 1 < argc; ++i)
     if (!strcmp(argv[i], "--out")) c.out = argv[i + 1];
   g_log = fopen((c.out + ".log").c_str(), "w");
-  logprintf("plink2_b200: B200-native KING / GRM / PCA / --indep-pairwise (plink2 command-line face)\n");
+  logprintf("plink2_b200: H100-native KING / GRM / PCA / --indep-pairwise (plink2 command-line face)\n");
   {
     std::string opts = "Options in effect:\n";
     for (int i = 1; i < argc; ++i) {

@@ -9,11 +9,10 @@
 // with T = het indicator, H = hom indicator, S = +1 hom-REF / -1 hom-ALT:
 //   TT = HETHET, TH = (row het, col hom) = HET2HOM1, HT = HET1HOM2, HH = HOMHOM,
 //   SS = HH - 2*IBS0  (so IBS0 = (HH - SS) / 2, always an exact integer).
-// Both algorithms (popcount and int8 tcgen05) accumulate into the same layout, bit-identically.
+// Both algorithms (popcount and int8 wgmma) accumulate into the same layout, bit-identically.
 #pragma once
 #include "common.cuh"
 #include "geno_expand.cuh"
-#include "umma.cuh"
 #include "cp_async.cuh"
 
 namespace pl2 {
@@ -190,200 +189,9 @@ king_popc_kernel(const uint32_t* __restrict__ planes, uint32_t sample_ct_padded,
 }
 
 // ---------------------------------------------------------------------------------------------
-// Tensor path: the same five counts as an exact int8 contraction on tcgen05.
-//   D[r][c] += sum_v A_plane[r][v] * B_plane[c][v],  planes in {T, H, S}, int32 accumulators in TMEM.
-// One CTA per pair tile.  Warps 0-7 expand 2-bit genotypes into MN-major int8 operand tiles in
-// shared memory (geno_expand.cuh), warp 8 lane 0 issues the UMMAs, and at the end of the variant
-// loop warps 0-7 drain TMEM into the raw accumulators.
-//   per 32-variant k-step:  T_I x [T_J;H_J] (N=192) -> cols [0,192)    = TT | TH
-//                           H_I x [T_J;H_J] (N=192) -> cols [192,384)  = HT | HH
-//                           S_I x  S_J      (N=96)  -> cols [384,480)  = SS
-// Algorithmic work: 5 * 128 * 96 * variants MACs per tile.
+// Tensor path: the same five counts as an exact int8 contraction on the tensor pipe,
+// king_wg_kernel<kTileCols> (king_ts_kernel.cuh).
 // ---------------------------------------------------------------------------------------------
-constexpr uint32_t kTcKc = 64;       // variants per pipeline stage (two K=32 UMMA steps)
-constexpr uint32_t kTcStages = 4;
-constexpr uint32_t kTcLookahead = 4; // register-prefetched stages (per producer group) of raw genotype rows
-constexpr uint32_t kTcSuperI = 3 * kTileRows;  // 384 "samples" (3 planes x 128)
-constexpr uint32_t kTcSuperJ = 3 * kTileCols;  // 288
-constexpr uint32_t kTcLboI = operand_lbo(kTcSuperI);  // 3072
-constexpr uint32_t kTcLboJ = operand_lbo(kTcSuperJ);  // 2304
-constexpr uint32_t kTcStageBytesI = kTcSuperI * kTcKc;  // 24576
-constexpr uint32_t kTcStageBytesJ = kTcSuperJ * kTcKc;  // 18432
-constexpr uint32_t kTcStageBytes = kTcStageBytesI + kTcStageBytesJ;
-constexpr uint32_t kTcSmemBytes = kTcStages * kTcStageBytes + 1024;
-constexpr uint32_t kTcProducerThreads = 256;
-constexpr uint32_t kTcGroupThreads = 128;  // two producer groups alternate stages
-constexpr uint32_t kTcThreads = kTcProducerThreads + 32;
-
-__device__ __forceinline__ void sts16(uint32_t addr, const uint4& v) {
-  asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-
-__global__ void __launch_bounds__(kTcThreads, 1)
-king_tc_kernel(const uint8_t* __restrict__ raw, uint32_t pitch, uint32_t variant_ct_padded /* multiple of kTcKc */, const uint32_t* __restrict__ tile_order, const uint32_t* __restrict__ tile_rt, const uint32_t* __restrict__ tile_tc, int32_t* __restrict__ raw_acc) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ __align__(8) uint64_t bar_full[kTcStages];
-  __shared__ __align__(8) uint64_t bar_empty[kTcStages];
-  __shared__ __align__(8) uint64_t bar_acc;
-  __shared__ uint32_t tmem_base_slot;
-
-  const uint32_t tid = threadIdx.x;
-  const uint32_t warp = uniform_warp_idx();
-  const uint32_t lane = tid & 31;
-  const uint32_t tile = tile_order[blockIdx.x];
-  const uint32_t i0 = tile_rt[tile] * kTileRows;
-  const uint32_t j0 = tile_tc[tile] * kTileCols;
-  const uint32_t stage_iters = variant_ct_padded / kTcKc;
-  const uint32_t smem_base = (smem_u32(smem) + 1023u) & ~1023u;
-
-  if (tid == 0) {
-    for (uint32_t s = 0; s < kTcStages; ++s) {
-      mbar_init(&bar_full[s], kTcGroupThreads / 32);
-      mbar_init(&bar_empty[s], 1);
-    }
-    mbar_init(&bar_acc, 1);
-    mbar_fence_init();
-  }
-  if (warp == 8) {
-    tmem_alloc<512>(&tmem_base_slot);
-  }
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_base_slot;
-
-  if (warp < 8) {
-    // ---------------- producers ----------------
-    // Group g = warp / 4 owns stages it = 2 j + g.  Within a group, thread u < 64 expands the
-    // 128 row-side samples of variant k = u (one 32-byte sector), thread u >= 64 the 96 col-side
-    // samples of variant k = u - 64 (24 bytes): every global sector is requested exactly once.
-    const uint32_t group = tid >> 7;
-    const uint32_t u = tid & 127;
-    const bool is_i = u < 64;
-    const uint32_t k = u & 63;
-    const uint8_t* src = raw + static_cast<uint64_t>(k) * pitch + (is_i ? (i0 / 4) : (j0 / 4));
-    const uint64_t stage_stride = static_cast<uint64_t>(kTcKc) * pitch;
-    const uint32_t lbo = is_i ? kTcLboI : kTcLboJ;
-    const uint32_t groups_per_plane = is_i ? 8u : 6u;
-    const uint32_t dst_k = operand_offset(k, 0, lbo) + (is_i ? 0u : kTcStageBytesI);
-
-    struct Row {
-      uint32_t w[8];
-    };
-    auto load_row = [&](uint32_t it) -> Row {
-      Row r;
-#pragma unroll
-      for (uint32_t q = 0; q < 8; ++q) r.w[q] = 0xFFFFFFFFu;
-      if (it < stage_iters) {
-        const uint8_t* p = src + it * stage_stride;
-        if (is_i) {
-          const uint4 a = __ldg(reinterpret_cast<const uint4*>(p));
-          const uint4 b = __ldg(reinterpret_cast<const uint4*>(p) + 1);
-          r.w[0] = a.x; r.w[1] = a.y; r.w[2] = a.z; r.w[3] = a.w;
-          r.w[4] = b.x; r.w[5] = b.y; r.w[6] = b.z; r.w[7] = b.w;
-        } else {
-          const uint2 a = __ldg(reinterpret_cast<const uint2*>(p));
-          const uint2 b = __ldg(reinterpret_cast<const uint2*>(p) + 1);
-          const uint2 c = __ldg(reinterpret_cast<const uint2*>(p) + 2);
-          r.w[0] = a.x; r.w[1] = a.y; r.w[2] = b.x; r.w[3] = b.y; r.w[4] = c.x; r.w[5] = c.y;
-        }
-      }
-      return r;
-    };
-
-    Row pre[kTcLookahead];
-#pragma unroll
-    for (uint32_t d = 0; d < kTcLookahead; ++d) pre[d] = load_row(2 * d + group);
-
-    for (uint32_t j0s = 0; 2 * j0s + group < stage_iters; j0s += kTcLookahead) {
-#pragma unroll
-      for (uint32_t d = 0; d < kTcLookahead; ++d) {
-        const uint32_t it = 2 * (j0s + d) + group;
-        if (it < stage_iters) {
-          const uint32_t s = it % kTcStages;
-          const uint32_t ph = (it / kTcStages) & 1;
-          const Row cur = pre[d];
-          pre[d] = load_row(it + 2 * kTcLookahead);
-          mbar_wait(&bar_empty[s], ph ^ 1);
-          const uint32_t dst = smem_base + s * kTcStageBytes + dst_k;
-#pragma unroll
-          for (uint32_t q = 0; q < 8; ++q) {
-            if (q < groups_per_plane) {
-              const Sel4 sel = make_selectors(cur.w[q]);
-              const uint32_t a0 = dst + q * kCoreBytes;
-              sts16(a0, expand16(kTabHet, sel));
-              sts16(a0 + groups_per_plane * kCoreBytes, expand16(kTabHom, sel));
-              sts16(a0 + 2 * groups_per_plane * kCoreBytes, expand16(kTabSgn, sel));
-            }
-          }
-          fence_proxy_async_smem();
-          mbar_arrive_warp(&bar_full[s], lane);
-        }
-      }
-    }
-
-    // ---------------- epilogue: TMEM -> raw accumulators (+=) ----------------
-    mbar_wait(&bar_acc, 0);
-    tc_fence_after_sync();
-    const uint32_t lane_grp = warp & 3;
-    const uint32_t col_half = warp >> 2;
-    const uint32_t rpos = 32 * lane_grp + lane;
-    const uint32_t rsample = (rpos & ~15u) + PosToSample(rpos & 15u);
-    int32_t* acc_tile = raw_acc + static_cast<uint64_t>(tile) * kKingTileAccWords + rsample;
-#pragma unroll 1
-    for (uint32_t chunk = 0; chunk < 15; ++chunk) {
-      const uint32_t col0 = col_half * 240 + chunk * 16;
-      uint32_t v[16];
-      tmem_ld16(tmem_base + ((32u * lane_grp) << 16) + col0, v);
-      tmem_ld_wait();
-      const uint32_t grp = col0 / 16;         // 16-column group
-      const uint32_t q = grp / 6;             // accumulator
-      const uint32_t cgrp = grp % 6;          // 16-sample group within the 96 columns
-      int32_t* base = acc_tile + static_cast<uint64_t>(q * kTileCols + cgrp * 16) * kTileRows;
-#pragma unroll
-      for (uint32_t c = 0; c < 16; ++c) {
-        int32_t* p = base + PosToSample(c) * kTileRows;
-        *p += static_cast<int32_t>(v[c]);
-      }
-    }
-    tc_fence_before_sync();
-  } else {
-    // ---------------- UMMA issuer (warp 8): whole warp loops, one elected lane issues (umma.cuh) ----------------
-    constexpr uint32_t idesc_n192 = make_idesc_i8(128, 192, true, true);
-    constexpr uint32_t idesc_n96 = make_idesc_i8(128, 96, true, true);
-    const uint32_t tmem_u = uniform_u32(tmem_base);
-    const uint64_t desc_i = make_smem_desc(smem_base, kTcLboI, kCoreBytes);
-    const uint64_t desc_j = make_smem_desc(smem_base + kTcStageBytesI, kTcLboJ, kCoreBytes);
-    for (uint32_t it0 = 0; it0 < stage_iters; it0 += kTcStages) {  // stage_iters is a multiple of kTcStages (variant pad 256)
-      const uint32_t ph = (it0 / kTcStages) & 1;
-#pragma unroll
-      for (uint32_t s = 0; s < kTcStages; ++s) {
-        mbar_wait(&bar_full[s], ph);
-        tc_fence_after_sync();
-        if (elect_one_sync()) {
-#pragma unroll
-          for (uint32_t kk = 0; kk < kTcKc / 32; ++kk) {
-            const uint32_t acc = (it0 | s | kk) ? 1u : 0u;
-            const uint64_t a_t = desc_i + ((s * kTcStageBytes + kk * 4 * kTcLboI) >> 4);
-            const uint64_t b_th = desc_j + ((s * kTcStageBytes + kk * 4 * kTcLboJ) >> 4);
-            umma_i8_ss(tmem_u + 0, a_t, b_th, idesc_n192, acc);
-            umma_i8_ss(tmem_u + 192, a_t + ((8 * kCoreBytes) >> 4), b_th, idesc_n192, acc);
-            umma_i8_ss(tmem_u + 384, a_t + ((16 * kCoreBytes) >> 4), b_th + ((12 * kCoreBytes) >> 4), idesc_n96, acc);
-          }
-          umma_commit(&bar_empty[s]);
-        }
-        __syncwarp();
-      }
-    }
-    if (elect_one_sync()) umma_commit(&bar_acc);
-    __syncwarp();
-  }
-  __syncthreads();
-  if (warp == 8) {
-    tc_fence_after_sync();
-    tmem_dealloc<512>(tmem_base);
-  }
-}
 
 // ---------------------------------------------------------------------------------------------
 // Finalisation: raw tiles -> the reference's in-memory results for rows [out_row_start, out_row_end).

@@ -1,353 +1,191 @@
-// king_ts_kernel.cuh - KING pair counts, "TS" tensor kernel: the row-side (A) operand is expanded
-// from a SAMPLE-major copy of the genotype block straight into tensor memory (tcgen05.st), so only
-// the column-side (B) operand goes through shared memory.  In the SS kernel (king_kernels.cuh) every
-// operand byte is written to and read back from shared memory (~200 B/clk wanted vs 128 B/clk
-// available, profiles/r01_ncu_king_v1.md); here shared-memory traffic drops to ~100 B/clk and the
-// tensor pipe becomes the limiter.
+// king_ts_kernel.cuh - KING pair counts on the int8 tensor pipe (wgmma, sm_90a).
 //
-// Tile = 128 rows x 80 cols.  TMEM columns: [0,400) accumulators TT|TH, HT|HH, SS (int32),
-// [400,496) four A slots of 24 columns (planes T, H, S; 8 columns = 32 K-bytes per lane).
-// Same products and the same raw accumulator semantics as king_tc_kernel (tile width 80).
+//   D[r][c] += sum_v A_plane[r][v] * B_plane[c][v],  planes T (het), H (hom), S (+1 hom-REF / -1 hom-ALT),
+// exact int32 sums, the raw accumulator semantics of king_kernels.cuh.  One CTA = 64 rows (half of a 128-row
+// pair tile) x kCols columns, two warpgroups:
+//   warpgroup 0:  T_I x T_J -> TT,  T_I x H_J -> TH,  S_I x S_J, columns [0, kS)
+//   warpgroup 1:  H_I x T_J -> HT,  H_I x H_J -> HH,  S_I x S_J, columns [kCols - kS, kCols)
+// so that each thread keeps ~100-120 int32 accumulators in registers for the whole variant loop (the 64 x 5 kCols
+// accumulators of a half tile are 100-120 KB; a whole 128-row tile would not fit the register file).  Both
+// warpgroups issue the same shapes (ptxas serialises a wgmma under a branch), so for 80 columns the S x S halves
+// overlap by 16 columns and warpgroup 1 stores only its last 32.
 //
-// Operand staging (round 2): one producer warp feeds two shared-memory rings with the TMA unit,
-//   * column side: the RAW variant-major 2-bit block is read in place through a 2-D tensor map
-//     (cp.async.bulk.tensor, SASS UTMALDG): box = 64 variants x 32 bytes at byte column 20 * ct (the
-//     tile's 80 samples are the first 20 bytes of each box row) - no column re-tiling pass, no copy;
-//   * row side: 1 KB bulk copies (UBLKCP) of the sample-major k-steps written by
-//     geno_tile_rows_kernel (the bit transpose CalcKing also needs, TransposeBitblock
-//     2.0/include/plink2_bits.cc:2065), restricted to the job's own row tiles.
-// The expansion warps read their words from shared memory (LDS) instead of issuing global loads.
+// Both operands come from the sample-major copy of the staged block written by geno_tile_rows_kernel
+// (raw_t[sample / 128][k-step][sample % 128][8 bytes = 32 variants]): K-major, which is what an 8-bit wgmma
+// reads.  Row side (A): each thread expands only its own fragment bytes straight into registers (wgmma.cuh).
+// Column side (B): all 256 threads expand the 3 planes of the kCols column samples into the K-major no-swizzle
+// layout in shared memory, one 256-variant stage ahead of the tensor pipe (double buffer, one __syncthreads per
+// stage); the row-side words of the stage are copied next to it.
 #pragma once
-#include <cuda.h>
 
 #include "common.cuh"
 #include "geno_expand.cuh"
 #include "geno_tile.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace pl2 {
 
-constexpr uint32_t kTsGroupsJ = kTsCols / 16;
 constexpr uint32_t kTsAccCols = 5 * kTsCols;   // 400
 constexpr uint32_t kTsTileAccWords = kTsAccCols * kTileRows;
-constexpr uint32_t kTsASlots = 4;
-constexpr uint32_t kTsASlotCols = 24;
-constexpr uint32_t kTsStagesJ = 4;
-constexpr uint32_t kTsLboJ = (3 * kTsCols / 16) * kCoreBytes + 64;  // 1984: +64 keeps the K-permuted rows bank-conflict free
-constexpr uint32_t kTsStageBytesJ = (kTsKcJ / 8) * kTsLboJ;         // 15872
-// Both rings move 4 KB per copy (= 4 k-steps): the single producer lane spends ~3 mbarrier / TMA operations per
-// copy, and at one copy per k-step (first version: 34.2 ms vs 24.4 ms per 16,384 x 65,536 batch) it, not the
-// tensor pipe, set the pace.
-constexpr uint32_t kTsRawJSlots = 4;                                // TMA ring: raw column boxes (128 variants x 32 B = two stages)
-constexpr uint32_t kTsRawJBytes = 2 * kTsKcJ * kTsRawBoxBytes;      // 4096
-constexpr uint32_t kTsRawISlots = 4;                                // bulk-copy ring: four row-side k-steps (128 samples x 8 B each)
-constexpr uint32_t kTsRawIBytes = 4 * kTileRows * 8;                // 4096
-constexpr uint32_t kTsSmemOffRawJ = kTsStagesJ * kTsStageBytesJ;    // 63488 (multiple of 1024)
-constexpr uint32_t kTsSmemOffRawI = kTsSmemOffRawJ + kTsRawJSlots * kTsRawJBytes;
-constexpr uint32_t kTsSmemBytes = kTsSmemOffRawI + kTsRawISlots * kTsRawIBytes + 1024;
-constexpr uint32_t kTsRowWarps = 8;
-constexpr uint32_t kTsColWarps = 10;           // 5 words x 64 variants per stage
-constexpr uint32_t kTsIssuerWarp = kTsRowWarps + kTsColWarps;
-constexpr uint32_t kTsLoaderWarp = kTsIssuerWarp + 1;
-constexpr uint32_t kTsThreads = 32 * (kTsRowWarps + kTsColWarps + 2);  // + the UMMA issuer warp + the TMA producer warp
-static_assert(kTsSmemOffRawJ % 1024 == 0, "TMA destination alignment");
 
-__global__ void __launch_bounds__(kTsThreads, 1)
-king_ts_kernel(const __grid_constant__ CUtensorMap tmap_raw, const uint8_t* __restrict__ raw_i, uint32_t row_tile_first, uint32_t variant_ct_padded /* multiple of 256 */, const uint32_t* __restrict__ tile_order, const uint32_t* __restrict__ tile_rt, const uint32_t* __restrict__ tile_tc, int32_t* __restrict__ raw_acc) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ __align__(8) uint64_t bar_full_a[kTsASlots];
-  __shared__ __align__(8) uint64_t bar_empty_a[kTsASlots];
-  __shared__ __align__(8) uint64_t bar_full_b[kTsStagesJ];
-  __shared__ __align__(8) uint64_t bar_empty_b[kTsStagesJ];
-  __shared__ __align__(8) uint64_t bar_full_rj[kTsRawJSlots];
-  __shared__ __align__(8) uint64_t bar_empty_rj[kTsRawJSlots];
-  __shared__ __align__(8) uint64_t bar_full_ri[kTsRawISlots];
-  __shared__ __align__(8) uint64_t bar_empty_ri[kTsRawISlots];
-  __shared__ __align__(8) uint64_t bar_acc;
-  __shared__ uint32_t tmem_base_slot;
+constexpr uint32_t kKwKs = 8;                    // k32 steps per shared-memory stage (256 variants)
+constexpr uint32_t kKwThreads = 256;             // two warpgroups
+constexpr uint32_t kKwChunkBytes = 128;          // LBO: next 16-variant chunk (core matrix) of the same 8 samples
+constexpr uint32_t kKwSbo = 2 * kKwKs * kKwChunkBytes;  // 2048: next group of 8 samples
+constexpr uint32_t kKwABytes = kKwKs * 64 * 8;   // row-side words of one stage: [k-step][64 rows][8 B]
 
+template <uint32_t kCols>
+struct KingWgShape {
+  static constexpr uint32_t kBBytes = 3 * kCols * 32 * kKwKs;  // planes T | H | S stacked along N
+  static constexpr uint32_t kStageBytes = kBBytes + kKwABytes;
+  static constexpr uint32_t kSmemBytes = 2 * kStageBytes + 128;
+  static constexpr uint32_t kS = (kCols / 2 + 15) / 16 * 16;  // S x S columns per warpgroup (wgmma N: multiple of 16)
+  static constexpr uint32_t kItems = kCols * kKwKs;             // (column sample, k-step) words per stage
+  static constexpr uint32_t kItemsPerThread = (kItems + kKwThreads - 1) / kKwThreads;
+  static_assert(kCols % 16 == 0 && 2 * kS >= kCols, "wgmma N");
+  static_assert(kSmemBytes <= 232448, "exceeds the 227 KB shared-memory opt-in limit");
+};
+
+template <int N>
+__device__ __forceinline__ void king_acc_add(int32_t* base, const int32_t (&d)[N / 2], uint32_t r, uint32_t c, int j0 = 0) {
+  // base -> accumulator column 0 of this block, row 0 of the tile; fragment (j, i): column 8 j + 2 c + (i & 1),
+  // row r + 8 (i >> 1); column groups j < j0 are skipped
+#pragma unroll
+  for (int j = 0; j < N / 8; ++j) {
+    if (j < j0) continue;
+#pragma unroll
+    for (int i = 0; i < 4; ++i) {
+      int32_t* p = base + static_cast<uint64_t>(8 * j + 2 * c + (i & 1)) * kTileRows + r + 8 * (i >> 1);
+      *p += d[4 * j + i];
+    }
+  }
+}
+
+// raw_t: sample-major copy of the whole padded block (sample 0 at row tile 0); kstep_ct = variant_ct_padded / 32.
+// Grid: 2 CTAs per tile (blockIdx.x & 1 = row half).
+template <uint32_t kCols>
+__global__ void __launch_bounds__(kKwThreads, 1)
+king_wg_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* multiple of 256 */, const uint32_t* __restrict__ tile_order, const uint32_t* __restrict__ tile_rt, const uint32_t* __restrict__ tile_tc, int32_t* __restrict__ raw_acc) {
+  using S = KingWgShape<kCols>;
+  extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t tid = threadIdx.x;
-  const uint32_t warp = uniform_warp_idx();
+  const uint32_t wg = tid >> 7;
+  const uint32_t warp4 = (tid >> 5) & 3;
   const uint32_t lane = tid & 31;
-  const uint32_t tile = tile_order[blockIdx.x];
+  const uint32_t g = lane >> 2, c = lane & 3;
+  const uint32_t tile = tile_order[blockIdx.x >> 1];
+  const uint32_t half = blockIdx.x & 1;
   const uint32_t rt = tile_rt[tile];
   const uint32_t ct = tile_tc[tile];
-  const uint32_t stage_iters = variant_ct_padded / kTsKcJ;
-  const uint32_t smem_base = (smem_u32(smem) + 1023u) & ~1023u;
+  const uint32_t kstep_ct = variant_ct_padded / 32;
+  const uint32_t stage_ct = kstep_ct / kKwKs;
+  const uint32_t smem_base = (static_cast<uint32_t>(__cvta_generic_to_shared(smem)) + 127u) & ~127u;
 
-  if (tid == 0) {
-    for (uint32_t s = 0; s < kTsASlots; ++s) {
-      mbar_init(&bar_full_a[s], 4);             // one arrival per row-side warp of the owning group
-      mbar_init(&bar_empty_a[s], 1);
-    }
-    for (uint32_t s = 0; s < kTsStagesJ; ++s) {
-      mbar_init(&bar_full_b[s], kTsColWarps);
-      mbar_init(&bar_empty_b[s], 1);
-    }
-    for (uint32_t s = 0; s < kTsRawJSlots; ++s) {
-      mbar_init(&bar_full_rj[s], 1);            // the producer's expect_tx arrival
-      mbar_init(&bar_empty_rj[s], kTsColWarps);
-    }
-    for (uint32_t s = 0; s < kTsRawISlots; ++s) {
-      mbar_init(&bar_full_ri[s], 1);
-      mbar_init(&bar_empty_ri[s], kTsRowWarps); // every row warp reads two of the slot's four k-steps
-    }
-    mbar_init(&bar_acc, 1);
-    mbar_fence_init();
-  }
-  __syncthreads();  // barriers initialised
-  // Tensor memory is needed by the row warps and the issuer only.  The allocation blocks while the previous CTA on
-  // this SM still holds its 512 columns (two CTAs fit an SM otherwise), so the TMA producer and the column warps do
-  // NOT wait for it: rings and B stages of this tile fill up behind the previous tile's epilogue.
-  uint32_t tmem_base = 0;
-  if (warp == kTsIssuerWarp) tmem_alloc<512>(&tmem_base_slot);
-  if (warp < kTsRowWarps || warp == kTsIssuerWarp) {
-    tc_fence_before_sync();
-    named_bar_sync<1, 32 * (kTsRowWarps + 1)>();
-    tc_fence_after_sync();
-    tmem_base = tmem_base_slot;
-  }
-
-  const uint32_t thread_zero = tid * (variant_ct_padded >> 31);  // 0 (a batch never has 2^31 variants)
+  const uint32_t thread_zero = tid * (variant_ct_padded >> 31);  // 0; keeps the plane tables in vector registers
   const uint32_t tab_t = table_reg(kTabHet, thread_zero), tab_h = table_reg(kTabHom, thread_zero), tab_s = table_reg(kTabSgn, thread_zero);
 
-  if (warp < kTsRowWarps) {
-    // ---------------- row-side producers: 2-bit words -> registers -> tensor memory ----------------
-    // Two groups of four warps (group = warp / 4); group g owns k-steps ks = 2 n + g and the A slots
-    // ks % 4 in {g, g + 2}.  Thread = TMEM lane = sample 128 rt + 32 (warp % 4) + lane.  The words of
-    // the next k-step are expanded while the UMMAs of the previous ones run.
-    const uint32_t grp = warp >> 2;
-    const uint32_t lq = warp & 3;
-    const uint32_t row = 32 * lq + lane;
-    const uint32_t ring_i = smem_base + kTsSmemOffRawI + row * 8;
-    const uint32_t taddr_lane = tmem_base + ((32u * lq) << 16) + kTsAccCols;
-    struct ExpI {
-      uint32_t v[3][8];
-    };
-    auto expand_i = [&](const uint2& w) -> ExpI {
-      ExpI e;
-      const Sel4 s0 = make_selectors(w.x), s1 = make_selectors(w.y);
-      const uint32_t tabs[3] = {tab_t, tab_h, tab_s};
+  // ---- staging: this thread's share of a stage (column-side words + one 16-byte piece of the row-side words)
+  const uint8_t* a_src = raw_t + static_cast<uint64_t>(rt) * kstep_ct * 1024 + half * 512 + (tid >> 5) * 1024 + (tid & 31) * 16;
+  // tid / 32 = k-step of the stage, (tid % 32) * 16 = byte of the 512-byte half row block
+  struct Pre {
+    uint2 w[S::kItemsPerThread];
+    uint4 a;
+  };
+  auto load_stage = [&](uint32_t st) -> Pre {
+    Pre p;
 #pragma unroll
-      for (int p = 0; p < 3; ++p) {
-        const uint4 a = expand16(tabs[p], s0), b = expand16(tabs[p], s1);
-        e.v[p][0] = a.x; e.v[p][1] = a.y; e.v[p][2] = a.z; e.v[p][3] = a.w;
-        e.v[p][4] = b.x; e.v[p][5] = b.y; e.v[p][6] = b.z; e.v[p][7] = b.w;
+    for (uint32_t q = 0; q < S::kItemsPerThread; ++q) {
+      const uint32_t i = tid + q * kKwThreads;
+      p.w[q] = make_uint2(0xFFFFFFFFu, 0xFFFFFFFFu);
+      if (i < S::kItems) {
+        const uint32_t n = (i & 7) | (((i >> 3) % (kCols / 8)) << 3);
+        const uint32_t ks = st * kKwKs + (i >> 3) / (kCols / 8);
+        const uint32_t s = kCols * ct + n;
+        p.w[q] = __ldg(reinterpret_cast<const uint2*>(raw_t + (static_cast<uint64_t>(s >> 7) * kstep_ct + ks) * 1024 + (s & 127) * 8));
       }
-      return e;
-    };
-    // One ring slot = k-steps 4 q .. 4 q + 3; this group needs 4 q + grp and 4 q + grp + 2.  Both words are read
-    // (and the slot released) up front, expanded one k-step ahead of the tensor-memory store.
-    struct Words {
-      uint2 w[2];
-    };
-    auto load_slot = [&](uint32_t q) -> Words {
-      const uint32_t si = q % kTsRawISlots;
-      mbar_wait(&bar_full_ri[si], (q / kTsRawISlots) & 1);
-      Words r;
-      r.w[0] = lds64(ring_i + si * kTsRawIBytes + grp * (kTileRows * 8));
-      r.w[1] = lds64(ring_i + si * kTsRawIBytes + (grp + 2) * (kTileRows * 8));
-      return r;  // the slot is released only after both words have gone through tcgen05.st (see below)
-    };
-    const uint32_t slot_iters = stage_iters / 2;  // stage_iters is a multiple of 4
-    Words words = load_slot(0);
-    ExpI cur = expand_i(words.w[0]);
-    for (uint32_t q = 0; q < slot_iters; ++q) {
+    }
+    p.a = __ldg(reinterpret_cast<const uint4*>(a_src + static_cast<uint64_t>(st) * kKwKs * 1024));
+    return p;
+  };
+  auto store_stage = [&](const Pre& p, uint32_t buf) {
+    const uint32_t base = smem_base + buf * S::kStageBytes;
 #pragma unroll
-      for (uint32_t h = 0; h < 2; ++h) {
-        const uint32_t ks = 4 * q + grp + 2 * h;
-        const uint32_t slot = ks % kTsASlots;
-        mbar_wait(&bar_empty_a[slot], ((ks / kTsASlots) & 1) ^ 1);
-        tc_fence_after_sync();
-        const uint32_t ta = taddr_lane + slot * kTsASlotCols;
-        tmem_st8(ta, cur.v[0]);
-        tmem_st8(ta + 8, cur.v[1]);
-        tmem_st8(ta + 16, cur.v[2]);
-        tmem_st_wait();
-        tc_fence_before_sync();
-        mbar_arrive_warp(&bar_full_a[slot], lane);
-        if (h == 0) {
-          cur = expand_i(words.w[1]);
-        } else {
-          // Release the ring slot HERE: the warp-collective tcgen05.st above could only issue once every lane's
-          // expanded registers - hence both ld.shared results - were complete.  (Releasing right after the loads
-          // is a race: the arrive can overtake a queued ld.shared, the producer refills the slot, and half a
-          // warp reads the next revolution's words - seen as 16-sample groups with slightly wrong counts.)
-          mbar_arrive_warp(&bar_empty_ri[q % kTsRawISlots], lane);
-          if (q + 1 < slot_iters) {
-            words = load_slot(q + 1);
-            cur = expand_i(words.w[0]);
+    for (uint32_t q = 0; q < S::kItemsPerThread; ++q) {
+      const uint32_t i = tid + q * kKwThreads;
+      if (i < S::kItems) {
+        const uint32_t n = (i & 7) | (((i >> 3) % (kCols / 8)) << 3);
+        const uint32_t ks = (i >> 3) / (kCols / 8);
+        const uint32_t tabs[3] = {tab_t, tab_h, tab_s};
+#pragma unroll
+        for (uint32_t h = 0; h < 2; ++h) {
+          const Sel4 sel = make_selectors(h ? p.w[q].y : p.w[q].x);
+#pragma unroll
+          for (uint32_t pl = 0; pl < 3; ++pl) {
+            const uint32_t row = pl * kCols + n;
+            const uint32_t addr = base + (row >> 3) * kKwSbo + (2 * ks + h) * kKwChunkBytes + (row & 7) * 16;
+            const uint4 v = expand16(tabs[pl], sel);
+            asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
           }
         }
       }
     }
-  } else if (warp < kTsIssuerWarp) {
-    // ---------------- column-side producers: 2-bit words -> int8 planes in shared memory ----------------
-    // Thread = (word w of the 20-byte tile row, variant k of the 64-variant stage).  A quarter-warp is
-    // one (8-variant group, word) combination: conflict-free st.shared.v4 (the 8 K rows of a phase land in
-    // 8 different 16-byte bank groups) and 2-way ld.shared.b32 from the 32-byte-pitch TMA box.
-    const uint32_t t = tid - 32 * kTsRowWarps;     // 0..319
-    const uint32_t combo = t >> 3;                 // 0..39 = (k group of 8) * 5 + word
-    const uint32_t k = 8 * (combo / 5) + (t & 7);
-    const uint32_t w = combo % 5;
-    // the box starts at the 16-byte boundary at or below byte column 20 * ct (TMA-friendly start address)
-    const uint32_t ring_j = smem_base + kTsSmemOffRawJ + k * kTsRawBoxBytes + ((ct * (kTsCols / 4)) & 15u) + 4 * w;
-    // K rows are stored in the PRMT position order of the row side (geno_expand.cuh): variant k of a
-    // 16-variant group sits at row SampleToPos(k % 16)
-    const uint32_t kpos = (k & ~15u) + SampleToPos(k & 15u);
-    const uint32_t dst_k = (kpos >> 3) * kTsLboJ + (kpos & 7) * 16 + w * kCoreBytes;
-    struct ExpJ {
-      uint4 vt, vh, vs;
-    };
-    auto expand_j = [&](uint32_t word) -> ExpJ {
-      const Sel4 sel = make_selectors(word);
-      ExpJ e;
-      e.vt = expand16(tab_t, sel);
-      e.vh = expand16(tab_h, sel);
-      e.vs = expand16(tab_s, sel);
-      return e;
-    };
-    // One ring slot = 128 variants = stages 2 q and 2 q + 1; variant k of either stage is this thread's.
-    auto load_slot = [&](uint32_t q) -> uint2 {
-      const uint32_t sj = q % kTsRawJSlots;
-      mbar_wait(&bar_full_rj[sj], (q / kTsRawJSlots) & 1);
-      uint2 r;
-      r.x = lds32(ring_j + sj * kTsRawJBytes);
-      r.y = lds32(ring_j + sj * kTsRawJBytes + kTsKcJ * kTsRawBoxBytes);
-      return r;  // released after the second word has been stored (st.shared needs the loaded value)
-    };
-    const uint32_t slot_iters = stage_iters / 2;
-    uint2 words = load_slot(0);
-    ExpJ cur = expand_j(words.x);
-    for (uint32_t q = 0; q < slot_iters; ++q) {
+    const uint32_t a_addr = base + S::kBBytes + tid * 16;
+    asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(a_addr), "r"(p.a.x), "r"(p.a.y), "r"(p.a.z), "r"(p.a.w) : "memory");
+  };
+
+  int32_t acc_x[kCols / 2], acc_y[kCols / 2], acc_s[S::kS / 2];
 #pragma unroll
-      for (uint32_t h = 0; h < 2; ++h) {
-        const uint32_t it = 2 * q + h;
-        const uint32_t sb = it % kTsStagesJ;
-        mbar_wait(&bar_empty_b[sb], ((it / kTsStagesJ) & 1) ^ 1);
-        const uint32_t a0 = smem_base + sb * kTsStageBytesJ + dst_k;
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(a0), "r"(cur.vt.x), "r"(cur.vt.y), "r"(cur.vt.z), "r"(cur.vt.w) : "memory");
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(a0 + kTsGroupsJ * kCoreBytes), "r"(cur.vh.x), "r"(cur.vh.y), "r"(cur.vh.z), "r"(cur.vh.w) : "memory");
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(a0 + 2 * kTsGroupsJ * kCoreBytes), "r"(cur.vs.x), "r"(cur.vs.y), "r"(cur.vs.z), "r"(cur.vs.w) : "memory");
-        fence_proxy_async_smem();
-        mbar_arrive_warp(&bar_full_b[sb], lane);
-        if (h == 0) {
-          cur = expand_j(words.y);
-        } else {
-          mbar_arrive_warp(&bar_empty_rj[q % kTsRawJSlots], lane);  // both words consumed by the st.shared above
-          if (q + 1 < slot_iters) {
-            words = load_slot(q + 1);
-            cur = expand_j(words.x);
-          }
-        }
-      }
-    }
-  } else if (warp == kTsIssuerWarp) {
-    // ---------------- UMMA issuer: whole warp loops, one elected lane issues (umma.cuh) ----------------
-    // One outer iteration = the 4 shared-memory stages = 8 k-steps = two rounds of the 4 A slots, so
-    // every slot index, A parity and descriptor offset is a compile-time constant.
-    static_assert(kTsStagesJ == 4 && kTsASlots == 4, "issuer unrolling assumes 4 stages / 4 slots");
-    constexpr uint32_t idesc_n160 = make_idesc_i8(128, 2 * kTsCols, false, true);
-    constexpr uint32_t idesc_n80 = make_idesc_i8(128, kTsCols, false, true);
-    const uint32_t tmem_u = uniform_u32(tmem_base);
-    const uint64_t desc0 = make_smem_desc(smem_base, kTsLboJ, kCoreBytes);
-    for (uint32_t it0 = 0; it0 < stage_iters; it0 += kTsStagesJ) {
-      const uint32_t ph_b = (it0 / kTsStagesJ) & 1;
+  for (uint32_t i = 0; i < kCols / 2; ++i) acc_x[i] = acc_y[i] = 0;
 #pragma unroll
-      for (uint32_t sb = 0; sb < kTsStagesJ; ++sb) {
-        mbar_wait(&bar_full_b[sb], ph_b);
+  for (uint32_t i = 0; i < S::kS / 2; ++i) acc_s[i] = 0;
+  const uint32_t s_first = wg ? kCols - S::kS : 0;  // first S x S column of this warpgroup
+
+  const uint32_t tab_a = wg ? tab_h : tab_t;
+  const uint32_t r_lo = 16 * warp4 + g;  // this thread's fragment rows r_lo, r_lo + 8 of the 64-row half
+
+  {
+    const Pre p0 = load_stage(0);
+    store_stage(p0, 0);
+  }
+  for (uint32_t st = 0; st < stage_ct; ++st) {
+    const uint32_t buf = st & 1;
+    Pre next;
+    const bool more = st + 1 < stage_ct;
+    if (more) next = load_stage(st + 1);
+    fence_proxy_async_smem();
+    __syncthreads();  // stage st complete in shared memory; every wgmma of stage st - 1 (other buffer) has retired
+    const uint32_t base = smem_base + buf * S::kStageBytes;
+    const uint64_t desc_t = make_wg_desc(base, kKwChunkBytes, kKwSbo);
+    constexpr uint32_t kPlaneStep = (kCols / 8) * kKwSbo;
 #pragma unroll
-        for (uint32_t kk = 0; kk < 2; ++kk) {
-          const uint32_t kq = 2 * sb + kk;            // k-step inside the outer iteration
-          const uint32_t slot = kq % kTsASlots;
-          mbar_wait(&bar_full_a[slot], (kq / kTsASlots) & 1);
-          tc_fence_after_sync();
-          if (elect_one_sync()) {
-            const uint32_t acc = (it0 | kq) ? 1u : 0u;
-            const uint64_t b_th = desc0 + ((sb * kTsStageBytesJ + kk * 4 * kTsLboJ) >> 4);
-            const uint64_t b_s = b_th + ((2 * kTsGroupsJ * kCoreBytes) >> 4);
-            const uint32_t ta = tmem_u + kTsAccCols + slot * kTsASlotCols;
-            umma_i8_ts(tmem_u + 0, ta, b_th, idesc_n160, acc);
-            umma_i8_ts(tmem_u + 2 * kTsCols, ta + 8, b_th, idesc_n160, acc);
-            umma_i8_ts(tmem_u + 4 * kTsCols, ta + 16, b_s, idesc_n80, acc);
-            umma_commit(&bar_empty_a[slot]);
-            if (kk == 1) umma_commit(&bar_empty_b[sb]);
-          }
-          __syncwarp();
-        }
-      }
+    for (uint32_t ks = 0; ks < kKwKs; ++ks) {
+      const uint32_t a_row = base + S::kBBytes + ks * 512;
+      uint2 w_lo, w_hi;
+      asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w_lo.x), "=r"(w_lo.y) : "r"(a_row + r_lo * 8) : "memory");
+      asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w_hi.x), "=r"(w_hi.y) : "r"(a_row + (r_lo + 8) * 8) : "memory");
+      const ASel sel = make_asel(w_lo, w_hi, c);
+      uint32_t fa[4], fs[4];
+      afrag(tab_a, sel, fa);
+      afrag(tab_s, sel, fs);
+      const uint64_t dk = desc_t + ((ks * 2 * kKwChunkBytes) >> 4);
+      wgmma_fence();
+      wgmma_s8_rs<kCols>(acc_x, fa, dk);                                   // x T_J
+      wgmma_s8_rs<kCols>(acc_y, fa, dk + (kPlaneStep >> 4));               // x H_J
+      wgmma_s8_rs<S::kS>(acc_s, fs, dk + ((2 * kPlaneStep + (s_first / 8) * kKwSbo) >> 4));
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (ks == kKwKs / 2 && more) store_stage(next, buf ^ 1);  // the other buffer: its wgmmas retired before the barrier
     }
-    if (elect_one_sync()) umma_commit(&bar_acc);
-    __syncwarp();
-  } else {
-    // ---------------- TMA producer: one elected lane keeps both raw rings full ----------------
-    if (elect_one_sync()) {
-      const uint8_t* src_i = raw_i + static_cast<uint64_t>(rt - row_tile_first) * (2 * stage_iters) * (kTileRows * 8);
-      const uint32_t ring_j = smem_base + kTsSmemOffRawJ, ring_i = smem_base + kTsSmemOffRawI;
-      const int32_t c0 = static_cast<int32_t>((ct * (kTsCols / 4)) & ~15u);  // 20 bytes at offset 0/4/8/12 of a 32-byte box
-      for (uint32_t q = 0; q < stage_iters / 2; ++q) {
-        const uint32_t si = q % kTsRawISlots;
-        mbar_wait(&bar_empty_ri[si], ((q / kTsRawISlots) & 1) ^ 1);
-        mbar_expect_tx(&bar_full_ri[si], kTsRawIBytes);
-        bulk_load_1d(ring_i + si * kTsRawIBytes, src_i + static_cast<uint64_t>(q) * kTsRawIBytes, kTsRawIBytes, &bar_full_ri[si]);
-        const uint32_t sj = q % kTsRawJSlots;
-        mbar_wait(&bar_empty_rj[sj], ((q / kTsRawJSlots) & 1) ^ 1);
-        mbar_expect_tx(&bar_full_rj[sj], kTsRawJBytes);
-        tma_load_2d(ring_j + sj * kTsRawJBytes, &tmap_raw, c0, static_cast<int32_t>(q * 2 * kTsKcJ), &bar_full_rj[sj]);
-      }
-    }
-    __syncwarp();
+    wgmma_wait<0>();
   }
 
-  if (warp < kTsRowWarps) {
-    // ---------------- epilogue: TMEM -> shared memory -> bulk reduce-add into the HBM accumulators ----------------
-    // The accumulators of a tile are one contiguous int32 [5 x 80 columns][128 rows] block.  Instead of a
-    // load-add-store per element from registers (latency-bound: ~16 KB in flight per SM, ~45 us per tile, i.e. >10 %
-    // of the tile), each accumulator plane (80 columns = 40 KB) is staged in shared memory - the operand stages and
-    // rings are idle now - and handed to the TMA unit as ONE cp.reduce.async.bulk .add.s32: the addition happens at
-    // the L2, nothing is read back, and tensor memory is released as soon as the last tcgen05.ld has returned.
-    mbar_wait(&bar_acc, 0);
-    tc_fence_after_sync();
-    constexpr uint32_t kPlaneBytes = kTsCols * kTileRows * 4;  // 40960
-    static_assert(2 * kPlaneBytes <= kTsSmemBytes - 1024, "two staging planes must fit the dynamic shared memory");
-    const uint32_t lq = warp & 3, half = warp >> 2;
-    const uint32_t rsample = 32 * lq + lane;  // rows are in natural sample order here
-    int32_t* acc_tile = raw_acc + static_cast<uint64_t>(tile) * kTsTileAccWords;
-#pragma unroll 1
-    for (uint32_t q = 0; q < 5; ++q) {  // accumulator planes TT, TH, HT, HH, SS
-      const uint32_t stage = smem_base + (q & 1) * kPlaneBytes + rsample * 4;
-      if (q >= 2) {
-        // plane q - 2 used this staging buffer: its bulk reduction must have finished READING shared memory
-        if (tid == 0) bulk_wait_group_read<1>();
-        named_bar_sync<2, 32 * kTsRowWarps>();
-      }
-      // 5 chunks of 16 columns per plane and lane quarter: half 0 takes chunks 0, 2, 4, half 1 takes 1, 3
-#pragma unroll 1
-      for (uint32_t cgrp = half; cgrp < kTsGroupsJ; cgrp += 2) {
-        uint32_t v[16];
-        tmem_ld16(tmem_base + ((32u * lq) << 16) + 16 * (q * kTsGroupsJ + cgrp), v);
-        tmem_ld_wait();
-#pragma unroll
-        for (uint32_t c = 0; c < 16; ++c) sts32(stage + (cgrp * 16 + PosToSample(c)) * (kTileRows * 4), v[c]);
-      }
-      fence_proxy_async_smem();
-      if (q == 4) tc_fence_before_sync();  // last tcgen05.ld of this warp is complete
-      named_bar_sync<2, 32 * kTsRowWarps>();
-      if (tid == 0) {
-        bulk_reduce_add_s32(acc_tile + static_cast<uint64_t>(q) * (kTsCols * kTileRows), smem_base + (q & 1) * kPlaneBytes, kPlaneBytes);
-        bulk_commit_group();
-      }
-    }
-  }
-  if (warp < kTsRowWarps || warp == kTsIssuerWarp) {
-    // all tensor-memory reads are done: hand the columns to the next CTA before the reductions have drained
-    named_bar_sync<1, 32 * (kTsRowWarps + 1)>();
-    if (warp == kTsIssuerWarp) {
-      tc_fence_after_sync();
-      tmem_dealloc<512>(tmem_base);
-    }
-  }
-  if (tid == 0) bulk_wait_group_read<0>();  // shared memory must outlive the reductions' reads
+  // ---- epilogue: registers -> raw accumulators (+=); rows are in natural sample order
+  int32_t* acc_tile = raw_acc + static_cast<uint64_t>(tile) * (5ull * kCols * kTileRows);
+  const uint32_t r = 64 * half + r_lo;
+  king_acc_add<kCols>(acc_tile + static_cast<uint64_t>((wg ? 2 : 0) * kCols) * kTileRows, acc_x, r, c);  // TT | HT
+  king_acc_add<kCols>(acc_tile + static_cast<uint64_t>((wg ? 3 : 1) * kCols) * kTileRows, acc_y, r, c);  // TH | HH
+  // warpgroup 1 skips the columns warpgroup 0 already covers
+  king_acc_add<S::kS>(acc_tile + static_cast<uint64_t>(4 * kCols + s_first) * kTileRows, acc_s, r, c, wg ? static_cast<int>((2 * S::kS - kCols) / 8) : 0);
 }
 
 }  // namespace pl2

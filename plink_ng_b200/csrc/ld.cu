@@ -89,12 +89,10 @@ int pl2gpu_ld_band_flags(Pl2GpuCtx* ctx, const void* genovecs, uint64_t variant_
   // through two pinned-size device buffers in the same rhythm
   GenoStage st[2];
   DevBuf d_planes, d_flags[2];
-  CUtensorMap tmap_a[2], tmap_b[2];
   cudaEvent_t ev_copied[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr};
   int rc = 0;
   for (int b = 0; b < 2 && !rc; ++b) {
     rc = StageAlloc(founder_ct, rows_cap, &st[b], use_popc ? kSamplePad : 64) || d_flags[b].alloc(static_cast<uint64_t>(kLdChunkVariants) * band);
-    if (!rc && !use_popc) rc = MakeRawTensorMap(&tmap_a[b], st[b].d_raw, st[b].pitch, st[b].variant_cap, kLdtBoxBytes, kLdtRows) || MakeRawTensorMap(&tmap_b[b], st[b].d_raw, st[b].pitch, st[b].variant_cap, kLdtBoxBytes, kLdtCols);
     if (!rc && (cudaEventCreateWithFlags(&ev_copied[b], cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&ev_done[b], cudaEventDisableTiming) != cudaSuccess)) {
       set_error("pl2gpu_ld_band_flags: cudaEventCreate failed");
       rc = 1;
@@ -144,7 +142,7 @@ int pl2gpu_ld_band_flags(Pl2GpuCtx* ctx, const void* genovecs, uint64_t variant_
       ld_band_kernel<<<dim3(DivUpU32(a1 - a0, 64), band_r / 64 + 1), 256, 0, c->stream>>>(static_cast<const uint32_t*>(d_planes.p), word_ct, padded, lo, a0, a1, band, prune_ld_thresh, static_cast<uint8_t*>(d_flags[b].p));
       c->launches++;
     } else {
-      ld_ts_kernel<<<dim3(DivUpU32(a1 - a0, kLdtRows), band_r / kLdtCols + 2), kLdtThreads, kLdtSmemBytes, c->stream>>>(tmap_a[b], tmap_b[b], st[b].sample_ct_padded, lo, a0, a1, band, prune_ld_thresh, static_cast<uint8_t*>(d_flags[b].p));
+      ld_ts_kernel<<<dim3(DivUpU32(a1 - a0, kLdtRows), (kLdtRows - kLdtCols + band_r) / kLdtCols + 1), kLdtThreads, kLdtSmemBytes, c->stream>>>(st[b].d_raw, st[b].pitch, st[b].sample_ct_padded, lo, a0, a1, band, prune_ld_thresh, static_cast<uint8_t*>(d_flags[b].p));
       c->launches++;
     }
     if (cudaGetLastError() != cudaSuccess) {

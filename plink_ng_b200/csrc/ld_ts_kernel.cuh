@@ -1,4 +1,4 @@
-// ld_ts_kernel.cuh - --indep-pairwise pair decisions on the int8 tensor pipe.
+// ld_ts_kernel.cuh - --indep-pairwise pair decisions on the int8 tensor pipe (wgmma, sm_90a).
 //
 // For every (second = a, first = b) variant pair within `band` positions the reference evaluates six exact
 // integer sums over the founders (ComputeIndepPairwiseR2Components, 2.0/plink2_ld.cc:699-723: DotprodWords
@@ -8,299 +8,159 @@
 //   nm12 = nm_a.nm_b   dot = x_a.x_b   ssq_b = nm_a.hom_b   sum_b = nm_a.x_b   ssq_a = hom_a.nm_b   sum_a = x_a.nm_b
 // i.e. a banded (variants x variants) contraction over SAMPLES - the same shape as the KING kernel with the
 // roles of the axes swapped, and here BOTH operands come straight from the variant-major 2-bit block: a
-// variant's samples are contiguous in its PgrGet row, which is K-major for both UMMA operands.  No bit-plane
-// split, no transpose, no re-tiling pass (the popcount kernel in ld_kernels.cuh needs ld_split_kernel).
+// variant's samples are contiguous in its PgrGet row, which is K-major for both wgmma operands.
 //
-// Tile = 128 "second" variants (rows = TMEM lanes) x 64 "first" variants (columns); k-step = 32 founders.
-// TMEM columns: [0,192) nm_a x [hom_b | nm_b | x_b], [192,256) hom_a x nm_b, [256,384) x_a x [nm_b | x_b],
-// [384,504) five A slots of 24 columns (planes nm, hom, x).  Three UMMAs (N = 192, 64, 128) = 192 tensor clk per
-// k-step.  All founders are contracted inside one CTA, so nothing is accumulated in HBM: the epilogue turns the
-// six int32 sums of each pair into the 1-byte decision the host-side greedy walk looks up.
-//
-// Staging: one producer warp issues 2-D TMA loads (UTMALDG) of raw boxes (variants x 16 bytes = 64 founders =
-// two k-steps) for both operands; row warps expand their word pairs into tensor memory (tcgen05.st), column
-// warps into the K-major no-swizzle canonical layout in shared memory.
+// One CTA = 64 "second" variants (rows) x 64 "first" variants (columns), k-step = 32 founders, two warpgroups
+// over the B planes [hom_b | nm_b | x_b] (N = 192), issuing the same shapes (ptxas serialises a wgmma under a
+// branch):
+//   warpgroup 0:  nm_a x [hom_b | nm_b] -> ssq_b, nm12 (N = 128);   nm_a x x_b  -> sum_b (N = 64)
+//   warpgroup 1:  x_a  x [nm_b | x_b]   -> sum_a, dot  (N = 128);   hom_a x nm_b -> ssq_a (N = 64)
+// 96 int32 accumulators per thread.  All founders are contracted inside one CTA, so nothing is accumulated in
+// HBM: warpgroup 1 hands its three sums over through shared memory and warpgroup 0 turns the six sums of each
+// pair into the 1-byte decision the host-side greedy walk looks up.
 #pragma once
-#include <cuda.h>
 
 #include "common.cuh"
 #include "geno_expand.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace pl2 {
 
-constexpr uint32_t kLdtRows = 128;                 // second variants per tile
-constexpr uint32_t kLdtCols = 64;                  // first variants per tile
-constexpr uint32_t kLdtBoxBytes = 16;              // 64 founders = one stage = two k-steps
-constexpr uint32_t kLdtAccCols = 6 * kLdtCols;     // 384
-constexpr uint32_t kLdtASlots = 5;                 // 384 + 5 x 24 = 504 columns; the slot hand-off (~750 clk) must stay below (slots - 1) x 192 clk
-constexpr uint32_t kLdtASlotCols = 24;
-constexpr uint32_t kLdtStagesB = 4;
-constexpr uint32_t kLdtPlaneBytes = kLdtCols * 64; // one plane of one stage: 64 variants x 64 K-bytes = 4096
-constexpr uint32_t kLdtStageBytesB = 3 * kLdtPlaneBytes;  // 12288
-constexpr uint32_t kLdtLbo = 128;                  // K direction: next 16-founder chunk of the same 8 variants
-constexpr uint32_t kLdtSbo = 512;                  // N direction: next group of 8 variants (4 chunks x 128 B)
-constexpr uint32_t kLdtRawASlots = 8;              // ring of raw row boxes (128 variants x 16 B)
-constexpr uint32_t kLdtRawABytes = kLdtRows * kLdtBoxBytes;  // 2048
-constexpr uint32_t kLdtRawBSlots = 8;              // ring of raw column boxes (64 variants x 16 B)
-constexpr uint32_t kLdtRawBBytes = kLdtCols * kLdtBoxBytes;  // 1024
-constexpr uint32_t kLdtSmemOffRawA = kLdtStagesB * kLdtStageBytesB;  // 49152
-constexpr uint32_t kLdtSmemOffRawB = kLdtSmemOffRawA + kLdtRawASlots * kLdtRawABytes;
-constexpr uint32_t kLdtSmemBytes = kLdtSmemOffRawB + kLdtRawBSlots * kLdtRawBBytes + 1024;
-constexpr uint32_t kLdtRowWarps = 8;
-constexpr uint32_t kLdtColWarps = 8;               // 64 variants x 4 words per stage = 256 threads
-constexpr uint32_t kLdtIssuerWarp = kLdtRowWarps + kLdtColWarps;
-constexpr uint32_t kLdtThreads = 32 * (kLdtRowWarps + kLdtColWarps + 3);  // + UMMA issuer + one TMA producer warp per operand ring
-static_assert(kLdtAccCols + kLdtASlots * kLdtASlotCols <= 512, "LD accumulators + A slots exceed TMEM");
+constexpr uint32_t kLdtRows = 64;                  // second variants per CTA
+constexpr uint32_t kLdtCols = 64;                  // first variants per CTA
+constexpr uint32_t kLdtThreads = 256;
+constexpr uint32_t kLdtKs = 2;                     // k32 steps per stage (64 founders: the stage's sample padding)
+constexpr uint32_t kLdtSbo = 2 * kLdtKs * kCoreBytes;   // 512: next group of 8 B rows
+constexpr uint32_t kLdtBBytes = 3 * kLdtCols * 32 * kLdtKs;  // 12288
+constexpr uint32_t kLdtABytes = kLdtRows * 8 * kLdtKs;       // 1024: [row][16 B]
+constexpr uint32_t kLdtStageBytes = kLdtBBytes + kLdtABytes;
+constexpr uint32_t kLdtXBytes = 3 * kLdtRows * kLdtCols * 4;  // warpgroup 1's sums for the epilogue
+constexpr uint32_t kLdtSmemBytes = (2 * kLdtStageBytes > kLdtXBytes ? 2 * kLdtStageBytes : kLdtXBytes) + 128;
 
-// variants_in_chunk: rows of the staged block (multiple of 64, >= every row a box touches is zero-filled by TMA
-// beyond it and decodes to "hom-REF everywhere", which only ever reaches pairs that are masked out below).
-// sample_ct_padded: multiple of 64; padding founders are coded missing (all planes 0).
+// raw: the staged block [row][pitch], row r = variant chunk_lo + r (rows are padded to a multiple of 64 with
+// "missing"); sample_ct_padded: multiple of 64, padding founders coded missing (all planes 0).
 // flags[(a - a_out0) * band + (a - b - 1)] = (cov12^2 > thresh * var1 * var2) for 0 < a - b <= band,
-// a in [a_out0, a_out1), b >= chunk_lo; a, b are global variant indices, row r of the block is variant chunk_lo + r.
+// a in [a_out0, a_out1), b >= chunk_lo; a, b are global variant indices.
 static __global__ void __launch_bounds__(kLdtThreads, 1)
-ld_ts_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, uint32_t sample_ct_padded, uint32_t chunk_lo, uint32_t a_out0, uint32_t a_out1, uint32_t band, double thresh, uint8_t* __restrict__ flags) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ __align__(8) uint64_t bar_full_a[kLdtASlots];
-  __shared__ __align__(8) uint64_t bar_empty_a[kLdtASlots];
-  __shared__ __align__(8) uint64_t bar_full_b[kLdtStagesB];
-  __shared__ __align__(8) uint64_t bar_empty_b[kLdtStagesB];
-  __shared__ __align__(8) uint64_t bar_full_ra[kLdtRawASlots];
-  __shared__ __align__(8) uint64_t bar_empty_ra[kLdtRawASlots];
-  __shared__ __align__(8) uint64_t bar_full_rb[kLdtRawBSlots];
-  __shared__ __align__(8) uint64_t bar_empty_rb[kLdtRawBSlots];
-  __shared__ __align__(8) uint64_t bar_acc;
-  __shared__ uint32_t tmem_base_slot;
-
-  // tile geometry (uniform per CTA); tiles without an in-band pair exit before touching TMEM
+ld_ts_kernel(const uint8_t* __restrict__ raw, uint32_t pitch, uint32_t sample_ct_padded, uint32_t chunk_lo, uint32_t a_out0, uint32_t a_out1, uint32_t band, double thresh, uint8_t* __restrict__ flags) {
+  // tile geometry (uniform per CTA); tiles without an in-band pair exit at once
   const uint32_t a_start = a_out0 + blockIdx.x * kLdtRows;                              // multiple of 64 (a_out0 is)
   const int64_t b_start_s = static_cast<int64_t>(a_start) + kLdtRows - kLdtCols - static_cast<int64_t>(kLdtCols) * blockIdx.y;
   if (b_start_s < static_cast<int64_t>(chunk_lo)) return;
   const uint32_t b_start = static_cast<uint32_t>(b_start_s);
-  // closest pair of the tile: a = a_start, b = b_start + 63 (when b_start + 63 < a_start); farthest is irrelevant
   if (a_start > b_start + (kLdtCols - 1) && a_start - (b_start + kLdtCols - 1) > band) return;
   if (b_start >= a_start + kLdtRows - 1) return;                                        // no b < a in this tile
 
-  const uint32_t tid = threadIdx.x;
-  const uint32_t warp = uniform_warp_idx();
-  const uint32_t lane = tid & 31;
-  const uint32_t stage_iters = sample_ct_padded / 64;   // stages of two k-steps
-  const uint32_t smem_base = (smem_u32(smem) + 1023u) & ~1023u;
-
-  if (tid == 0) {
-    for (uint32_t s = 0; s < kLdtASlots; ++s) {
-      mbar_init(&bar_full_a[s], 4);
-      mbar_init(&bar_empty_a[s], 1);
-    }
-    for (uint32_t s = 0; s < kLdtStagesB; ++s) {
-      mbar_init(&bar_full_b[s], kLdtColWarps);
-      mbar_init(&bar_empty_b[s], 1);
-    }
-    for (uint32_t s = 0; s < kLdtRawASlots; ++s) {
-      mbar_init(&bar_full_ra[s], 1);
-      mbar_init(&bar_empty_ra[s], kLdtRowWarps);   // both k-step groups read every row box
-    }
-    for (uint32_t s = 0; s < kLdtRawBSlots; ++s) {
-      mbar_init(&bar_full_rb[s], 1);
-      mbar_init(&bar_empty_rb[s], kLdtColWarps);
-    }
-    mbar_init(&bar_acc, 1);
-    mbar_fence_init();
-  }
-  if (warp == kLdtIssuerWarp) tmem_alloc<512>(&tmem_base_slot);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_base_slot;
-
+  extern __shared__ __align__(128) uint8_t smem_dyn[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 127) & ~static_cast<uintptr_t>(127));
+  const uint32_t smem_base = static_cast<uint32_t>(__cvta_generic_to_shared(smem));
+  const uint32_t tid = threadIdx.x, wg = tid >> 7, warp4 = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, c = lane & 3;
+  const uint32_t stage_ct = sample_ct_padded / (32 * kLdtKs);
   const uint32_t thread_zero = tid * (sample_ct_padded >> 31);  // 0; keeps the plane tables in vector registers
   const uint32_t tab_nm = table_reg(kTabNonmiss, thread_zero), tab_hom = table_reg(kTabHom, thread_zero), tab_x = table_reg(kTabSgn, thread_zero);
 
-  if (warp < kLdtRowWarps) {
-    // ---------------- row side: the "second" variants; lane = variant, 8 bytes = 32 founders per k-step ----------------
-    // group g = warp / 4 owns k-steps ks = 2 n + g, i.e. the g-th half of raw box n.
-    const uint32_t grp = warp >> 2;
-    const uint32_t lq = warp & 3;
-    const uint32_t row = 32 * lq + lane;
-    const uint32_t ring_a = smem_base + kLdtSmemOffRawA + row * kLdtBoxBytes + 8 * grp;
-    const uint32_t taddr_lane = tmem_base + ((32u * lq) << 16) + kLdtAccCols;
-    struct ExpI {
-      uint32_t v[3][8];
-    };
-    auto fetch = [&](uint32_t n) -> uint2 {
-      const uint32_t sa = n % kLdtRawASlots;
-      mbar_wait(&bar_full_ra[sa], (n / kLdtRawASlots) & 1);
-      return lds64(ring_a + sa * kLdtRawABytes);  // the ring slot is released after the tcgen05.st of the expansion (see king_ts_kernel.cuh)
-    };
-    auto expand_i = [&](const uint2& w) -> ExpI {
-      ExpI e;
-      const Sel4 s0 = make_selectors(w.x), s1 = make_selectors(w.y);
-      const uint32_t tabs[3] = {tab_nm, tab_hom, tab_x};
+  // staging: thread = (column variant, 16-founder word) of the stage; threads 0..63 also copy one row's 16 bytes
+  const uint32_t bv = tid >> 2, bw = tid & 3;
+  const uint8_t* b_src = raw + static_cast<uint64_t>(b_start - chunk_lo + bv) * pitch + 4 * bw;
+  const uint8_t* a_src = raw + static_cast<uint64_t>(a_start - chunk_lo + (tid & 63)) * pitch;
+  struct Pre {
+    uint32_t w;
+    uint4 a;
+  };
+  auto load_stage = [&](uint32_t st) -> Pre {
+    Pre p;
+    p.w = __ldg(reinterpret_cast<const uint32_t*>(b_src + st * 16));
+    p.a = (tid < kLdtRows) ? __ldg(reinterpret_cast<const uint4*>(a_src + st * 16)) : make_uint4(0, 0, 0, 0);
+    return p;
+  };
+  auto store_stage = [&](const Pre& p, uint32_t buf) {
+    const uint32_t base = smem_base + buf * kLdtStageBytes;
+    const Sel4 sel = make_selectors(p.w);
+    const uint32_t tabs[3] = {tab_hom, tab_nm, tab_x};
 #pragma unroll
-      for (int p = 0; p < 3; ++p) {
-        const uint4 a = expand16(tabs[p], s0), b = expand16(tabs[p], s1);
-        e.v[p][0] = a.x; e.v[p][1] = a.y; e.v[p][2] = a.z; e.v[p][3] = a.w;
-        e.v[p][4] = b.x; e.v[p][5] = b.y; e.v[p][6] = b.z; e.v[p][7] = b.w;
-      }
-      return e;
-    };
-    // the next box is fetched and expanded while this k-step's tensor-memory stores are in flight (the
-    // tcgen05.st -> wait::st round trip, ~300 clk, would otherwise bound each group to one k-step per round trip)
-    uint2 w = fetch(0);
-    for (uint32_t n = 0; n < stage_iters; ++n) {
-      const uint32_t ks = 2 * n + grp;
-      const uint32_t slot = ks % kLdtASlots;
-      const ExpI cur = expand_i(w);
-      mbar_wait(&bar_empty_a[slot], ((ks / kLdtASlots) & 1) ^ 1);
-      tc_fence_after_sync();
-      const uint32_t ta = taddr_lane + slot * kLdtASlotCols;
-      tmem_st8(ta, cur.v[0]);
-      tmem_st8(ta + 8, cur.v[1]);
-      tmem_st8(ta + 16, cur.v[2]);
-      mbar_arrive_warp(&bar_empty_ra[n % kLdtRawASlots], lane);  // box n consumed: its words went through tcgen05.st
-      if (n + 1 < stage_iters) w = fetch(n + 1);
-      tmem_st_wait();
-      tc_fence_before_sync();
-      mbar_arrive_warp(&bar_full_a[slot], lane);
+    for (uint32_t pl = 0; pl < 3; ++pl) {
+      const uint32_t row = pl * kLdtCols + bv;
+      const uint4 v = expand16(tabs[pl], sel);
+      asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(base + (row >> 3) * kLdtSbo + bw * kCoreBytes + (row & 7) * 16), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
     }
-  } else if (warp < kLdtIssuerWarp) {
-    // ---------------- column side: the "first" variants; thread = (variant, 16-founder word of the stage) ----------------
-    // K-major no-swizzle canonical layout: 8 variants x 16 K-bytes per 128-byte core matrix; a quarter-warp writes one
-    // core matrix (conflict-free st.shared.v4), a warp reads 32 consecutive words of the raw box.
-    const uint32_t t = tid - 32 * kLdtRowWarps;    // 0..255
-    const uint32_t b = (t & 7) | ((t >> 5) << 3);  // variant 0..63 of the tile
-    const uint32_t w = (t >> 3) & 3;               // 16-founder chunk 0..3 of the 64-founder stage
-    const uint32_t ring_b = smem_base + kLdtSmemOffRawB + b * kLdtBoxBytes + 4 * w;
-    const uint32_t dst = (b >> 3) * kLdtSbo + w * kLdtLbo + (b & 7) * 16;
-    struct ExpJ {
-      uint4 v_hom, v_nm, v_x;
-    };
-    auto fetch = [&](uint32_t it) -> ExpJ {
-      const uint32_t sb = it % kLdtRawBSlots;
-      mbar_wait(&bar_full_rb[sb], (it / kLdtRawBSlots) & 1);
-      const Sel4 sel = make_selectors(lds32(ring_b + sb * kLdtRawBBytes));
-      ExpJ e;
-      e.v_hom = expand16(tab_hom, sel);
-      e.v_nm = expand16(tab_nm, sel);
-      e.v_x = expand16(tab_x, sel);
-      return e;  // slot released after the st.shared of these registers
-    };
-    ExpJ cur = fetch(0);
-    for (uint32_t it = 0; it < stage_iters; ++it) {
-      const uint32_t sb = it % kLdtStagesB;
-      mbar_wait(&bar_empty_b[sb], ((it / kLdtStagesB) & 1) ^ 1);
-      const uint32_t a0 = smem_base + sb * kLdtStageBytesB + dst;
-      asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(a0), "r"(cur.v_hom.x), "r"(cur.v_hom.y), "r"(cur.v_hom.z), "r"(cur.v_hom.w) : "memory");
-      asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(a0 + kLdtPlaneBytes), "r"(cur.v_nm.x), "r"(cur.v_nm.y), "r"(cur.v_nm.z), "r"(cur.v_nm.w) : "memory");
-      asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(a0 + 2 * kLdtPlaneBytes), "r"(cur.v_x.x), "r"(cur.v_x.y), "r"(cur.v_x.z), "r"(cur.v_x.w) : "memory");
-      mbar_arrive_warp(&bar_empty_rb[it % kLdtRawBSlots], lane);
-      fence_proxy_async_smem();
-      mbar_arrive_warp(&bar_full_b[sb], lane);
-      if (it + 1 < stage_iters) cur = fetch(it + 1);
-    }
-  } else if (warp == kLdtIssuerWarp) {
-    // ---------------- UMMA issuer ----------------
-    constexpr uint32_t idesc_n192 = make_idesc_i8(128, 3 * kLdtCols, false, false);
-    constexpr uint32_t idesc_n128 = make_idesc_i8(128, 2 * kLdtCols, false, false);
-    constexpr uint32_t idesc_n64 = make_idesc_i8(128, kLdtCols, false, false);
-    const uint32_t tmem_u = uniform_u32(tmem_base);
-    const uint64_t desc0 = make_smem_desc(smem_base, kLdtLbo, kLdtSbo);
-    for (uint32_t it = 0; it < stage_iters; ++it) {
-      const uint32_t sb = it % kLdtStagesB;
-      mbar_wait(&bar_full_b[sb], (it / kLdtStagesB) & 1);
+    if (tid < kLdtRows)
+      asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(base + kLdtBBytes + tid * 16), "r"(p.a.x), "r"(p.a.y), "r"(p.a.z), "r"(p.a.w) : "memory");
+  };
+
+  int32_t d128[64], d64[32];
 #pragma unroll
-      for (uint32_t kk = 0; kk < 2; ++kk) {
-        const uint32_t ks = 2 * it + kk;
-        const uint32_t slot = ks % kLdtASlots;
-        mbar_wait(&bar_full_a[slot], (ks / kLdtASlots) & 1);
-        tc_fence_after_sync();
-        if (elect_one_sync()) {
-          const uint32_t acc = ks ? 1u : 0u;
-          // k-step kk = K chunks {2 kk, 2 kk + 1} of the stage: start address advances by two LBO steps
-          const uint64_t b_all = desc0 + ((sb * kLdtStageBytesB + kk * 2 * kLdtLbo) >> 4);   // planes hom | nm | x
-          const uint64_t b_nm = b_all + (kLdtPlaneBytes >> 4);                                  // planes nm | x
-          const uint32_t ta = tmem_u + kLdtAccCols + slot * kLdtASlotCols;
-          umma_i8_ts(tmem_u + 0, ta, b_all, idesc_n192, acc);                 // nm_a  x [hom_b | nm_b | x_b]
-          umma_i8_ts(tmem_u + 3 * kLdtCols, ta + 8, b_nm, idesc_n64, acc);    // hom_a x nm_b
-          umma_i8_ts(tmem_u + 4 * kLdtCols, ta + 16, b_nm, idesc_n128, acc);  // x_a   x [nm_b | x_b]
-          umma_commit(&bar_empty_a[slot]);
-          if (kk == 1) umma_commit(&bar_empty_b[sb]);
-        }
-        __syncwarp();
-      }
+  for (uint32_t i = 0; i < 64; ++i) d128[i] = 0;
+#pragma unroll
+  for (uint32_t i = 0; i < 32; ++i) d64[i] = 0;
+  const uint32_t tab_1 = wg ? tab_x : tab_nm, tab_2 = wg ? tab_hom : tab_nm;  // A planes of the N = 128 / N = 64 products
+  const uint32_t off_1 = wg ? kLdtCols : 0, off_2 = wg ? kLdtCols : 2 * kLdtCols;  // first B row of each product
+  const uint32_t r_lo = 16 * warp4 + g;
+
+  {
+    const Pre p0 = load_stage(0);
+    store_stage(p0, 0);
+  }
+  for (uint32_t st = 0; st < stage_ct; ++st) {
+    const uint32_t buf = st & 1;
+    const bool more = st + 1 < stage_ct;
+    Pre next;
+    if (more) next = load_stage(st + 1);
+    fence_proxy_async_smem();
+    __syncthreads();  // stage st in shared memory; the other buffer's wgmmas have retired
+    const uint32_t base = smem_base + buf * kLdtStageBytes;
+    const uint64_t desc = make_wg_desc(base, kCoreBytes, kLdtSbo);
+#pragma unroll
+    for (uint32_t ks = 0; ks < kLdtKs; ++ks) {
+      uint2 w_lo, w_hi;
+      asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w_lo.x), "=r"(w_lo.y) : "r"(base + kLdtBBytes + r_lo * 16 + ks * 8) : "memory");
+      asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w_hi.x), "=r"(w_hi.y) : "r"(base + kLdtBBytes + (r_lo + 8) * 16 + ks * 8) : "memory");
+      const ASel sel = make_asel(w_lo, w_hi, c);
+      uint32_t f1[4], f2[4];
+      afrag(tab_1, sel, f1);
+      afrag(tab_2, sel, f2);
+      const uint64_t dk = desc + ((ks * 2 * kCoreBytes) >> 4);
+      wgmma_fence();
+      wgmma_s8_rs<128>(d128, f1, dk + (((off_1 / 8) * kLdtSbo) >> 4));
+      wgmma_s8_rs<64>(d64, f2, dk + (((off_2 / 8) * kLdtSbo) >> 4));
+      wgmma_commit();
+      wgmma_wait<1>();
     }
-    if (elect_one_sync()) umma_commit(&bar_acc);
-    __syncwarp();
-  } else {
-    // ---------------- TMA producers: one elected lane per operand ring (a single lane feeding both rings spends
-    // ~6 mbarrier / TMA operations per 384-clk stage and becomes the limiter, cf. king_ts_kernel.cuh) ----------------
-    if (elect_one_sync()) {
-      if (warp == kLdtIssuerWarp + 1) {
-        const uint32_t ring_a = smem_base + kLdtSmemOffRawA;
-        const int32_t row_a = static_cast<int32_t>(a_start - chunk_lo);
-        for (uint32_t it = 0; it < stage_iters; ++it) {
-          const uint32_t sa = it % kLdtRawASlots;
-          mbar_wait(&bar_empty_ra[sa], ((it / kLdtRawASlots) & 1) ^ 1);
-          mbar_expect_tx(&bar_full_ra[sa], kLdtRawABytes);
-          tma_load_2d(ring_a + sa * kLdtRawABytes, &tmap_a, static_cast<int32_t>(it * kLdtBoxBytes), row_a, &bar_full_ra[sa]);
-        }
-      } else {
-        const uint32_t ring_b = smem_base + kLdtSmemOffRawB;
-        const int32_t row_b = static_cast<int32_t>(b_start - chunk_lo);
-        for (uint32_t it = 0; it < stage_iters; ++it) {
-          const uint32_t sb = it % kLdtRawBSlots;
-          mbar_wait(&bar_empty_rb[sb], ((it / kLdtRawBSlots) & 1) ^ 1);
-          mbar_expect_tx(&bar_full_rb[sb], kLdtRawBBytes);
-          tma_load_2d(ring_b + sb * kLdtRawBBytes, &tmap_b, static_cast<int32_t>(it * kLdtBoxBytes), row_b, &bar_full_rb[sb]);
-        }
-      }
-    }
-    __syncwarp();
+    if (more) store_stage(next, buf ^ 1);
+    wgmma_wait<0>();
   }
 
-  if (warp < kLdtRowWarps) {
-    // ---------------- epilogue: six sums per pair -> the r^2 decision byte ----------------
-    // warps 0-3 take columns [0,32), warps 4-7 columns [32,64) of their lane quarter.
-    mbar_wait(&bar_acc, 0);
-    tc_fence_after_sync();
-    const uint32_t lq = warp & 3;
-    const uint32_t a = a_start + 32 * lq + lane;
-    const uint32_t taddr = tmem_base + ((32u * lq) << 16);
-    const uint32_t col_begin = (warp < 4) ? 0u : 32u;
-#pragma unroll 1
-    for (uint32_t c0 = col_begin; c0 < col_begin + 32; c0 += 8) {
-      uint32_t qb[8], nm[8], sb_[8], qa[8], sa_[8], dt[8];
-      tmem_ld8(taddr + c0, qb);
-      tmem_ld8(taddr + kLdtCols + c0, nm);
-      tmem_ld8(taddr + 2 * kLdtCols + c0, sb_);
-      tmem_ld8(taddr + 3 * kLdtCols + c0, qa);
-      tmem_ld8(taddr + 4 * kLdtCols + c0, sa_);
-      tmem_ld8(taddr + 5 * kLdtCols + c0, dt);
-      tmem_ld_wait();
-      if (a < a_out1) {
+  // ---- epilogue: six sums per pair -> the r^2 decision byte
+  __syncthreads();  // operand buffers are free
+  int32_t* xs = reinterpret_cast<int32_t*>(smem);  // [3][64 rows][64 columns]: sum_a, dot, ssq_a
+  if (wg == 1) {
 #pragma unroll
-        for (uint32_t c = 0; c < 8; ++c) {
-          const uint32_t b = b_start + c0 + c;
-          if (b >= a || a - b > band) continue;
-          const int64_t n12 = static_cast<int32_t>(nm[c]);
-          const int64_t dot = static_cast<int32_t>(dt[c]);
-          const int64_t q_b = static_cast<int32_t>(qb[c]), s_b = static_cast<int32_t>(sb_[c]);  // first
-          const int64_t q_a = static_cast<int32_t>(qa[c]), s_a = static_cast<int32_t>(sa_[c]);  // second
-          // plink2_ld.cc:1085-1090; int64 -> double casts, unfused left-to-right multiplies
-          const double cov12 = static_cast<double>(dot * n12 - s_b * s_a);
-          const double var1 = static_cast<double>(q_b * n12 - s_b * s_b);
-          const double var2 = static_cast<double>(q_a * n12 - s_a * s_a);
-          const bool over = __dmul_rn(cov12, cov12) > __dmul_rn(__dmul_rn(thresh, var1), var2);
-          flags[static_cast<uint64_t>(a - a_out0) * band + (a - b - 1)] = over ? 1 : 0;
-        }
+    for (uint32_t j = 0; j < 8; ++j)
+#pragma unroll
+      for (uint32_t i = 0; i < 4; ++i) {
+        const uint32_t col = 8 * j + 2 * c + (i & 1), row = r_lo + 8 * (i >> 1);
+        xs[row * kLdtCols + col] = d128[4 * j + i];                               // sum_a = x_a . nm_b
+        xs[kLdtRows * kLdtCols + row * kLdtCols + col] = d128[4 * (8 + j) + i];   // dot = x_a . x_b
+        xs[2 * kLdtRows * kLdtCols + row * kLdtCols + col] = d64[4 * j + i];      // ssq_a = hom_a . nm_b
       }
-    }
-    tc_fence_before_sync();
   }
   __syncthreads();
-  if (warp == kLdtIssuerWarp) {
-    tc_fence_after_sync();
-    tmem_dealloc<512>(tmem_base);
+  if (wg == 0) {
+#pragma unroll
+    for (uint32_t j = 0; j < 8; ++j)
+#pragma unroll
+      for (uint32_t i = 0; i < 4; ++i) {
+        const uint32_t col = 8 * j + 2 * c + (i & 1), row = r_lo + 8 * (i >> 1);
+        const uint32_t a = a_start + row, b = b_start + col;
+        if (a >= a_out1 || b >= a || a - b > band) continue;
+        const int64_t q_b = d128[4 * j + i], n12 = d128[4 * (8 + j) + i], s_b = d64[4 * j + i];  // first
+        const int64_t s_a = xs[row * kLdtCols + col], dot = xs[kLdtRows * kLdtCols + row * kLdtCols + col], q_a = xs[2 * kLdtRows * kLdtCols + row * kLdtCols + col];
+        // plink2_ld.cc:1085-1090; int64 -> double casts, unfused left-to-right multiplies
+        const double cov12 = static_cast<double>(dot * n12 - s_b * s_a);
+        const double var1 = static_cast<double>(q_b * n12 - s_b * s_b);
+        const double var2 = static_cast<double>(q_a * n12 - s_a * s_a);
+        const bool over = __dmul_rn(cov12, cov12) > __dmul_rn(__dmul_rn(thresh, var1), var2);
+        flags[static_cast<uint64_t>(a - a_out0) * band + (a - b - 1)] = over ? 1 : 0;
+      }
   }
 }
 

@@ -39,7 +39,6 @@ struct Pl2PcaJob {
   double* d_icpt = nullptr;     // per variant: -2 alt_freq inv_stdev
   double* d_twof = nullptr;     // per variant: 2 alt_freq (the mean-imputation value of --variant-score)
   std::vector<double> h_slope, h_icpt, h_twof;
-  CUtensorMap tmap_raw;         // box {16 B, 128 variants} over d_raw
   uint32_t retiled_to = 0;      // variants [0, retiled_to) are in d_raw_i (multiple of 64)
 };
 
@@ -85,9 +84,8 @@ static int PcaBeginImpl(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t variant_ct_
   }
   if (job->tensor) {
     if (cudaMemsetAsync(job->d_slope, 0, 8ull * job->variant_cap, ctx->c.stream) != cudaSuccess || cudaMemsetAsync(job->d_icpt, 0, 8ull * job->variant_cap, ctx->c.stream) != cudaSuccess ||
-        MakeRawTensorMap(&job->tmap_raw, job->d_raw, job->pitch, job->variant_cap, 16, 128) ||
-        cudaFuncSetAttribute(pca_xa_ts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPxaSmemBytes) != cudaSuccess ||
-        cudaFuncSetAttribute(pca_xtb_ts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPxtSmemBytes) != cudaSuccess) {
+        cudaFuncSetAttribute(pca_xa_wg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPxaSmemBytes) != cudaSuccess ||
+        cudaFuncSetAttribute(pca_xtb_wg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPxtSmemBytes) != cudaSuccess) {
       if (!*get_error()) set_error("pl2gpu_pca_begin: %s", cudaGetErrorString(cudaGetLastError()));
       pl2gpu_pca_end(job);
       return 1;
@@ -204,7 +202,7 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
   double *d_scale = nullptr, *d_inv_scale = nullptr, *d_partial = nullptr;
   unsigned long long* d_colmax = nullptr;
   const uint32_t kstep_total = job->variant_cap / 32;
-  const uint32_t tiles2 = DivUpU32(npad / 128, 2);
+  const uint32_t tiles2 = npad / 128;
   uint32_t splits = std::max(1u, std::min(DivUpU32(2 * static_cast<uint32_t>(c->sm_count), tiles2), kstep_total / 64));
   const uint32_t ksteps_per_split = RoundUpU32(DivUpU32(kstep_total, splits), 4);
   splits = DivUpU32(kstep_total, ksteps_per_split);
@@ -240,11 +238,11 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
   constexpr int kPasses = 2;
   auto launch_xa_ts = [&](const double* g, uint32_t g_ld, double* hout, uint64_t h_ld, uint32_t hcol0, uint32_t cols_total) {
     for (uint32_t cc = 0; cc < cols_total; cc += kPcaCgMax) {
-      const uint32_t valid = std::min(kPcaCgMax, cols_total - cc), cg = RoundUpU32(valid, 4);
+      const uint32_t valid = std::min(kPcaCgMax, cols_total - cc), cg = kPcaCgMax;
       group_scales(g + cc, g_ld, 1, npad, valid, nullptr, nullptr);
       for (int pass = 0; pass < kPasses; ++pass) {
         pca_digits_kernel<<<npad / 64, 256, 0, c->stream>>>(g + cc, g_ld, 1, npad, cg, valid, nullptr, nullptr, d_scale, d_gdig, nullptr, pass);
-        pca_xa_ts_kernel<<<job->variant_cap / 128, kPxaThreads, kPxaSmemBytes, c->stream>>>(job->tmap_raw, npad, m, d_gdig, cg, valid, job->d_slope, job->d_icpt, d_inv_scale, hout + static_cast<uint64_t>(hcol0 + cc) * h_ld, h_ld,
+        pca_xa_wg_kernel<<<job->variant_cap / 128, kPcaThreads, kPxaSmemBytes, c->stream>>>(job->d_raw, job->pitch, npad, m, d_gdig, valid, job->d_slope, job->d_icpt, d_inv_scale, hout + static_cast<uint64_t>(hcol0 + cc) * h_ld, h_ld,
                                                                                           pass ? 1.0 / kPcaPass1Scale : 1.0, pass);
         c->launches += 2;
       }
@@ -252,13 +250,13 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
   };
   auto launch_xtb_ts = [&](const double* hin, uint64_t h_ld, uint32_t hcol0, uint32_t cols_total, double* out, uint64_t out_rs, uint64_t out_cs) {
     for (uint32_t cc = 0; cc < cols_total; cc += kPcaCgMax) {
-      const uint32_t valid = std::min(kPcaCgMax, cols_total - cc), cg = RoundUpU32(valid, 4);
+      const uint32_t valid = std::min(kPcaCgMax, cols_total - cc), cg = kPcaCgMax;
       const double* src = hin + static_cast<uint64_t>(hcol0 + cc) * h_ld;
       group_scales(src, 1, h_ld, m, valid, job->d_slope, job->d_icpt);
       for (int pass = 0; pass < kPasses; ++pass) {
         pca_digits_kernel<<<job->variant_cap / 64, 256, 0, c->stream>>>(src, 1, h_ld, m, cg, valid, job->d_slope, job->d_icpt, d_scale, d_hs, d_hi, pass);
         if (cudaMemsetAsync(d_partial, 0, static_cast<uint64_t>(splits) * npad * cg * 8, c->stream) != cudaSuccess) ts_rc = 1;
-        pca_xtb_ts_kernel<<<dim3(tiles2, splits), kPxtThreads, kPxtSmemBytes, c->stream>>>(job->d_raw_i, kstep_total, ksteps_per_split, n, d_hs, d_hi, cg, d_inv_scale, d_partial, npad);
+        pca_xtb_wg_kernel<<<dim3(tiles2, splits), kPcaThreads, kPxtSmemBytes, c->stream>>>(job->d_raw_i, kstep_total, ksteps_per_split, n, d_hs, d_hi, d_inv_scale, d_partial, npad);
         pca_xtb_reduce_kernel<<<static_cast<uint32_t>(DivUpU64(static_cast<uint64_t>(n) * cg, 256)), 256, 0, c->stream>>>(d_partial, splits, n, npad, cg, valid, pass ? 1.0 / kPcaPass1Scale : 1.0, out + static_cast<uint64_t>(cc) * out_cs, out_rs, out_cs);
         c->launches += 3;
       }
@@ -332,11 +330,10 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
     // from dgesvd; only their span enters B = Y^T Q and everything after it).
     //   Default: block classical Gram-Schmidt over the k + 1 Krylov blocks, three projection passes per block (the
     //   blocks span 35 orders of magnitude - two passes are not enough), each followed by a Jacobi SVD of the M x 2k
-    //   residual whose unit left singular vectors replace the block.  O(M q^2) once instead of per Jacobi sweep:
-    //   0.36 s instead of 7.9 s at 65,536 x 840 (profiles/r02_pca_timing.txt).
+    //   residual whose unit left singular vectors replace the block.  O(M q^2) once instead of per Jacobi sweep.
     //   PL2_PCA_BASIS=jacobi: one-sided Jacobi SVD of the whole M x q matrix (jacobi.cuh), the round-1 form.
     //   Both give the structure PCs to 1e-13 of the LAPACK-based restatement and differ from it by 1e-4..1e-3 in the
-    //   noise-level eigenvalues (profiles/r02_pca_basis_compare.txt): the Krylov matrix is numerically rank deficient
+    //   noise-level eigenvalues (tests/harness/pca_basis_compare.py): the Krylov matrix is numerically rank deficient
     //   and every method completes the basis differently there.
     std::vector<double> s(q);
     const char* err = nullptr;
@@ -545,14 +542,14 @@ int pl2gpu_pca_vscore(Pl2PcaJob* job, const double* weights_host, uint32_t cols,
     if (job->variant_cap > m && LaunchPadGenotypes(c, job->d_raw + static_cast<uint64_t>(m) * job->pitch, job->pitch, job->sample_ct, 0, job->variant_cap - m)) break;
     bool ok = true;
     for (uint32_t cc = 0; ok && cc < cols; cc += kPcaCgMax) {
-      const uint32_t valid = std::min(kPcaCgMax, cols - cc), cg = RoundUpU32(valid, 4);
+      const uint32_t valid = std::min(kPcaCgMax, cols - cc), cg = kPcaCgMax;
       ok = cudaMemsetAsync(d_colmax, 0, 8 * kPcaCgMax, c->stream) == cudaSuccess;
       pca_colmax_kernel<<<dim3(valid, std::min<uint32_t>(64, DivUpU32(npad, 256))), 256, 0, c->stream>>>(d_w + cc, cols, 1, npad, nullptr, nullptr, d_colmax);
       pca_scales_kernel<<<1, 64, 0, c->stream>>>(d_colmax, kPcaCgMax, d_scale, d_inv_scale);
       c->launches += 2;
       for (int pass = 0; pass < 2; ++pass) {
         pca_digits_kernel<<<npad / 64, 256, 0, c->stream>>>(d_w + cc, cols, 1, npad, cg, valid, nullptr, nullptr, d_scale, d_gdig, nullptr, pass);
-        pca_xa_ts_kernel<<<job->variant_cap / 128, kPxaThreads, kPxaSmemBytes, c->stream>>>(job->tmap_raw, npad, m, d_gdig, cg, valid, job->d_slope, job->d_icpt, d_inv_scale, d_h + static_cast<uint64_t>(cc) * m, m,
+        pca_xa_wg_kernel<<<job->variant_cap / 128, kPcaThreads, kPxaSmemBytes, c->stream>>>(job->d_raw, job->pitch, npad, m, d_gdig, valid, job->d_slope, job->d_icpt, d_inv_scale, d_h + static_cast<uint64_t>(cc) * m, m,
                                                                                           pass ? 1.0 / kPcaPass1Scale : 1.0, pass);
         c->launches += 2;
       }

@@ -1,6 +1,6 @@
 // pca_ts_kernels.cuh - the two skinny products of `--pca approx` (CalcPca approx branch,
 // 2.0/plink2_matrix_calc.cc:5697-5941: CalcPcaXaThread :5243 / CalcPcaXtxaThread :5210 / CalcPcaXtbThread :5272)
-// on the int8 tensor pipe - the same tile path as the KING / GRM / LD kernels.
+// on the int8 tensor pipe (wgmma, sm_90a).
 //
 // Y is the M x N standardised genotype matrix (ExpandCenteredVarmaj, missing -> 0): y_vs = slope_v g_vs + icpt_v m_vs
 // with g the ALT dosage (0/1/2, missing 0) and m the non-missing indicator - exact small integers.  The dense
@@ -9,35 +9,36 @@
 // 2^-31-relative quantisation of the dense operand (the power iteration needs ~1e-6):
 //
 //   XA :  H[v][c]  = slope_v sum_s g_vs G[s][c] + icpt_v sum_s m_vs G[s][c]          (contract over samples)
-//         A = {g, m} planes of 128 variants, read straight from the variant-major block (K-major, as ld_ts_kernel);
-//         B = digit planes of G;  2 UMMAs (N = 4 cg) per 32 samples;  epilogue recombines digits in int64.
+//         A = {g, m} planes of 128 variants, read straight from the variant-major block (a variant's samples are
+//         contiguous: K-major); B = digit planes of G;  2 wgmmas (N = 4 cg) per 32 samples;  epilogue recombines
+//         digits in int64.
 //   XtB:  O[s][c] += sum_v g_vs (slope_v H[v][c]) + m_vs (icpt_v H[v][c])           (contract over variants)
-//         A = {g, m} planes of TWO 128-sample tiles from the sample-major copy (as king_ts_kernel's row side);
-//         B = digit planes of slope.H and of icpt.H (common per-column scale, so both UMMAs add into one
-//         accumulator); 4 UMMAs per 32 variants share the two B blocks (32 B/clk of L2->SM traffic instead of 64).
+//         A = {g, m} planes of a 128-sample tile from the sample-major copy (as king_ts_kernel's row side);
+//         B = digit planes of slope.H and of icpt.H (common per-column scale, so both wgmmas add into one
+//         accumulator).
 //
-// The B operand needs no expansion warps: pca_digits_kernel writes it ONCE per pass in the MN-major no-swizzle
-// canonical layout, one contiguous 32 N-byte block per k-step, and the producer lane brings it in with plain
-// cp.async.bulk copies.  K rows are stored in the PRMT position order of the A side (geno_expand.cuh).
+// The B operand needs no expansion: pca_digits_kernel writes it ONCE per pass in the K-major no-swizzle layout
+// (8 columns x 16 K-bytes per core matrix), one contiguous 32 N-byte block per k-step, and the kernels stage it
+// with cp.async.  K bytes are stored in the PRMT position order of the A side (geno_expand.cuh, wgmma.cuh).
+// A thread holds accumulator columns 2 c, 2 c + 1 (mod 8) only, so the four digits d cg + col of a column meet in
+// one thread when cg is a multiple of 8: every launch uses cg = kPcaCgMax (columns beyond the valid ones are 0).
 #pragma once
-#include <cuda.h>
-
 #include "common.cuh"
+#include "cp_async.cuh"
 #include "geno_expand.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace pl2 {
 
 constexpr uint32_t kPcaDigits = 4;
-constexpr uint32_t kPcaCgMax = 48;                      // columns per launch (multiple of 4): N = 4 cg <= 192
-constexpr uint32_t kPcaNMax = kPcaDigits * kPcaCgMax;   // 192
+constexpr uint32_t kPcaCgMax = 32;                      // columns per launch: N = 4 cg = 128 int32 accumulators per row
+constexpr uint32_t kPcaNMax = kPcaDigits * kPcaCgMax;   // 128
 constexpr uint32_t kPcaFixedBits = 30;                  // |x| 2^F <= 2^30 < the balanced 4-digit range (~2^31)
-constexpr uint32_t kPcaBlockBytesMax = 32 * kPcaNMax;   // one k-step of B: 6144
 
 __host__ __device__ constexpr uint32_t pca_block_bytes(uint32_t n) { return 32 * n; }
-// byte offset of (K row k of the k-step, column n) inside a k-step block (MN-major, SBO = 128, LBO = (n_total / 16) * 128)
-__host__ __device__ constexpr uint32_t pca_b_offset(uint32_t k, uint32_t n, uint32_t n_total) {
-  return ((((k & ~15u) + SampleToPos(k & 15u)) >> 3) * (n_total / 16) * kCoreBytes) + (n >> 4) * kCoreBytes + ((((k & ~15u) + SampleToPos(k & 15u)) & 7) * 16) + (n & 15);
+// byte offset of (K byte k of the k-step, column n) inside a k-step block (K-major, LBO = 128, SBO = 256)
+__host__ __device__ constexpr uint32_t pca_b_offset(uint32_t k, uint32_t n) {
+  return (n >> 3) * 256 + (k >> 4) * kCoreBytes + (n & 7) * 16 + SampleToPos(k & 15u);
 }
 
 // ---- per-column scale: colmax[c] = max_r |src(r, c) * mul(r)| over one or two row multipliers -------------------
@@ -101,394 +102,204 @@ static __global__ void __launch_bounds__(256) pca_digits_kernel(const double* __
       for (uint32_t d = 0; d < kPcaDigits; ++d) {
         const long long dig = ((v + 128) & 255) - 128;  // balanced digit in [-128, 127]
         v = (v - dig) >> 8;
-        out[base + pca_b_offset(k, d * cg + c, n_total)] = static_cast<uint8_t>(static_cast<int8_t>(dig));
+        out[base + pca_b_offset(k, d * cg + c)] = static_cast<uint8_t>(static_cast<int8_t>(dig));
       }
     }
   }
 }
 
 // ================================================================================================================
-// XA: H[v][col0 + c] for 128 variants per CTA.  TMEM: D_g [0, N), D_m [N, 2N), A slots of 16 columns (planes g, m)
-// from column 2 N.  Warps: 8 row (2 groups x 4 lane quarters; group g owns k-steps = g mod 2), issuer, producer.
+// Both products: 2 warpgroups x 64 rows, N = kPcaNMax, one stage = 4 k-steps staged with cp.async into a double
+// buffer [row words][B blocks], one __syncthreads per stage.
 // ================================================================================================================
-constexpr uint32_t kPxaStagesB = 4;                    // stages of two k-steps
-constexpr uint32_t kPxaRawASlots = 8;                  // raw boxes: 128 variants x 16 B (64 samples = two k-steps)
-constexpr uint32_t kPxaRawABytes = 128 * 16;
-constexpr uint32_t kPxaSmemOffRawA = kPxaStagesB * 2 * kPcaBlockBytesMax;  // 49152
-constexpr uint32_t kPxaSmemBytes = kPxaSmemOffRawA + kPxaRawASlots * kPxaRawABytes + 1024;
-constexpr uint32_t kPxaRowWarps = 8;
-constexpr uint32_t kPxaIssuerWarp = kPxaRowWarps;
-constexpr uint32_t kPxaThreads = 32 * (kPxaRowWarps + 2);
+constexpr uint32_t kPcaThreads = 256;
+constexpr uint32_t kPcaStageK = 4;                          // k-steps per stage
+constexpr uint32_t kPcaABytes = kPcaStageK * 128 * 8;       // 4096: 128 rows x 4 k-steps x 8 B
+constexpr uint32_t kPcaBlk = pca_block_bytes(kPcaNMax);     // 4096
 
-static __global__ void __launch_bounds__(kPxaThreads, 1)
-pca_xa_ts_kernel(const __grid_constant__ CUtensorMap tmap_raw /* box {16 B, 128 variants} */, uint32_t sample_ct_padded /* multiple of 64 */, uint32_t variant_ct, const uint8_t* __restrict__ gdig /* [samples / 32][32 N] */, uint32_t cg, uint32_t cols_valid,
-                 const double* __restrict__ slope, const double* __restrict__ icpt, const double* __restrict__ inv_scale /* [cg] */, double* __restrict__ h /* column-major, ld = h_ld, first column = this group's */, uint64_t h_ld,
+// selectors of this thread's A fragment rows (r, r + 8) for one k-step; word (row, k-step j) at
+// a_words + row * row_stride + j * ks_stride
+__device__ __forceinline__ ASel pca_asel(uint32_t a_words, uint32_t row_stride, uint32_t ks_stride, uint32_t j, uint32_t r, uint32_t c) {
+  uint2 w_lo, w_hi;
+  asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w_lo.x), "=r"(w_lo.y) : "r"(a_words + r * row_stride + j * ks_stride) : "memory");
+  asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w_hi.x), "=r"(w_hi.y) : "r"(a_words + (r + 8) * row_stride + j * ks_stride) : "memory");
+  return make_asel(w_lo, w_hi, c);
+}
+
+// ================================================================================================================
+// XA: H[v][c] for 128 variants per CTA (warpgroup w: variants v0 + 64 w ..), accumulators D_g, D_m in registers.
+// Row words come from the variant-major block: a stage is 32 contiguous bytes (128 samples) of each variant.
+// ================================================================================================================
+constexpr uint32_t kPxaStage = kPcaABytes + kPcaStageK * kPcaBlk;
+constexpr uint32_t kPxaSmemBytes = 2 * kPxaStage + 128;
+
+static __global__ void __launch_bounds__(kPcaThreads, 1)
+pca_xa_wg_kernel(const uint8_t* __restrict__ raw /* [variant][pitch] */, uint32_t pitch, uint32_t sample_ct_padded /* multiple of 128 */, uint32_t variant_ct, const uint8_t* __restrict__ gdig /* [samples / 32][32 N] */, uint32_t cols_valid,
+                 const double* __restrict__ slope, const double* __restrict__ icpt, const double* __restrict__ inv_scale /* [kPcaCgMax] */, double* __restrict__ h /* column-major, ld = h_ld, first column = this group's */, uint64_t h_ld,
                  double post_scale /* 1, or 2^-30 for the residual pass */, int accumulate /* add to h instead of overwriting */) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ __align__(8) uint64_t bar_full_a[16];
-  __shared__ __align__(8) uint64_t bar_empty_a[16];
-  __shared__ __align__(8) uint64_t bar_full_b[kPxaStagesB];
-  __shared__ __align__(8) uint64_t bar_empty_b[kPxaStagesB];
-  __shared__ __align__(8) uint64_t bar_full_ra[kPxaRawASlots];
-  __shared__ __align__(8) uint64_t bar_empty_ra[kPxaRawASlots];
-  __shared__ __align__(8) uint64_t bar_acc;
-  __shared__ uint32_t tmem_base_slot;
-
-  const uint32_t tid = threadIdx.x;
-  const uint32_t warp = uniform_warp_idx();
-  const uint32_t lane = tid & 31;
-  const uint32_t n_total = kPcaDigits * cg;
-  const uint32_t blk = pca_block_bytes(n_total);
-  const uint32_t a_slots = min(16u, (512u - 2 * n_total) / 16u);   // >= 8 for N <= 192
-  const uint32_t stage_iters = sample_ct_padded / 64;
+  extern __shared__ __align__(128) uint8_t smem_dyn[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 127) & ~static_cast<uintptr_t>(127));
+  const uint32_t smem_base = static_cast<uint32_t>(__cvta_generic_to_shared(smem));
+  const uint32_t tid = threadIdx.x, wg = tid >> 7, warp4 = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, c = lane & 3;
   const uint32_t v0 = blockIdx.x * 128;
-  const uint32_t smem_base = (smem_u32(smem) + 1023u) & ~1023u;
+  const uint32_t stage_ct = sample_ct_padded / (32 * kPcaStageK);
+  const uint32_t thread_zero = tid * (sample_ct_padded >> 31);
+  const uint32_t tab_g = table_reg(kTabDosage, thread_zero), tab_m = table_reg(kTabNonmiss, thread_zero);
+  auto issue = [&](uint32_t st) {
+    uint8_t* dst = smem + (st & 1) * kPxaStage;
+    {  // row words: [variant][32 B]; thread = (variant, 16-byte half)
+      const uint32_t v = tid >> 1, hf = tid & 1;
+      cp_async16(dst + v * 32 + 16 * hf, raw + static_cast<uint64_t>(v0 + v) * pitch + st * (kPcaStageK * 8) + 16 * hf);
+    }
+    const uint8_t* src = gdig + static_cast<uint64_t>(st) * kPcaStageK * kPcaBlk;
+    for (uint32_t i = tid; i < kPcaStageK * kPcaBlk / 16; i += kPcaThreads) cp_async16(dst + kPcaABytes + 16 * i, src + 16 * i);
+    cp_async_commit();
+  };
 
-  if (tid == 0) {
-    for (uint32_t s = 0; s < 16; ++s) {
-      mbar_init(&bar_full_a[s], 4);
-      mbar_init(&bar_empty_a[s], 1);
-    }
-    for (uint32_t s = 0; s < kPxaStagesB; ++s) {
-      mbar_init(&bar_full_b[s], 1);
-      mbar_init(&bar_empty_b[s], 1);
-    }
-    for (uint32_t s = 0; s < kPxaRawASlots; ++s) {
-      mbar_init(&bar_full_ra[s], 1);
-      mbar_init(&bar_empty_ra[s], kPxaRowWarps);
-    }
-    mbar_init(&bar_acc, 1);
-    mbar_fence_init();
-  }
-  if (warp == kPxaIssuerWarp) tmem_alloc<512>(&tmem_base_slot);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_base_slot;
-
-  if (warp < kPxaRowWarps) {
-    // ---------------- row side: lane = variant; 8 bytes = 32 samples per k-step; planes g, m -> tensor memory ----------------
-    const uint32_t grp = warp >> 2, lq = warp & 3;
-    const uint32_t thread_zero = tid * (sample_ct_padded >> 31);
-    const uint32_t tab_g = table_reg(kTabDosage, thread_zero), tab_m = table_reg(kTabNonmiss, thread_zero);
-    const uint32_t ring_a = smem_base + kPxaSmemOffRawA + (32 * lq + lane) * 16 + 8 * grp;
-    const uint32_t ta0 = tmem_base + ((32u * lq) << 16) + 2 * n_total;
-    auto fetch = [&](uint32_t n) -> uint2 {
-      const uint32_t sa = n % kPxaRawASlots;
-      mbar_wait(&bar_full_ra[sa], (n / kPxaRawASlots) & 1);
-      return lds64(ring_a + sa * kPxaRawABytes);
-    };
-    uint2 w = fetch(0);
-    for (uint32_t n = 0; n < stage_iters; ++n) {
-      const uint32_t ks = 2 * n + grp;
-      const uint32_t slot = ks % a_slots;
-      const Sel4 s0 = make_selectors(w.x), s1 = make_selectors(w.y);
-      uint32_t eg[8], em[8];
-      {
-        const uint4 a = expand16(tab_g, s0), b = expand16(tab_g, s1);
-        eg[0] = a.x; eg[1] = a.y; eg[2] = a.z; eg[3] = a.w; eg[4] = b.x; eg[5] = b.y; eg[6] = b.z; eg[7] = b.w;
-        const uint4 c = expand16(tab_m, s0), d = expand16(tab_m, s1);
-        em[0] = c.x; em[1] = c.y; em[2] = c.z; em[3] = c.w; em[4] = d.x; em[5] = d.y; em[6] = d.z; em[7] = d.w;
-      }
-      mbar_wait(&bar_empty_a[slot], ((ks / a_slots) & 1) ^ 1);
-      tc_fence_after_sync();
-      tmem_st8(ta0 + slot * 16, eg);
-      tmem_st8(ta0 + slot * 16 + 8, em);
-      mbar_arrive_warp(&bar_empty_ra[n % kPxaRawASlots], lane);  // the box's words went through tcgen05.st
-      if (n + 1 < stage_iters) w = fetch(n + 1);
-      tmem_st_wait();
-      tc_fence_before_sync();
-      mbar_arrive_warp(&bar_full_a[slot], lane);
-    }
-  } else if (warp == kPxaIssuerWarp) {
-    // ---------------- UMMA issuer ----------------
-    const uint32_t idesc = make_idesc_i8(128, n_total, false, true);
-    const uint32_t tmem_u = uniform_u32(tmem_base);
-    const uint32_t lbo = (n_total / 16) * kCoreBytes;
-    const uint64_t desc0 = make_smem_desc(smem_base, lbo, kCoreBytes);
-    for (uint32_t it = 0; it < stage_iters; ++it) {
-      const uint32_t sb = it % kPxaStagesB;
-      mbar_wait(&bar_full_b[sb], (it / kPxaStagesB) & 1);
+  int32_t dg[kPcaNMax / 2], dm[kPcaNMax / 2];
 #pragma unroll
-      for (uint32_t kk = 0; kk < 2; ++kk) {
-        const uint32_t ks = 2 * it + kk;
-        const uint32_t slot = ks % a_slots;
-        mbar_wait(&bar_full_a[slot], (ks / a_slots) & 1);
-        tc_fence_after_sync();
-        if (elect_one_sync()) {
-          const uint32_t acc = ks ? 1u : 0u;
-          const uint64_t b = desc0 + ((sb * 2 * kPcaBlockBytesMax + kk * blk) >> 4);
-          const uint32_t ta = tmem_u + 2 * n_total + slot * 16;
-          umma_i8_ts(tmem_u + 0, ta, b, idesc, acc);            // sum_s g G
-          umma_i8_ts(tmem_u + n_total, ta + 8, b, idesc, acc);  // sum_s m G
-          umma_commit(&bar_empty_a[slot]);
-          if (kk == 1) umma_commit(&bar_empty_b[sb]);
+  for (uint32_t i = 0; i < kPcaNMax / 2; ++i) dg[i] = dm[i] = 0;
+  const uint32_t r = 64 * wg + 16 * warp4 + g;
+  issue(0);
+  for (uint32_t st = 0; st < stage_ct; ++st) {
+    if (st + 1 < stage_ct) {
+      issue(st + 1);  // the other buffer: its wgmmas retired (wait<0>) before the barrier that ended stage st - 1
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    fence_proxy_async_smem();
+    __syncthreads();
+    const uint32_t base = smem_base + (st & 1) * kPxaStage;
+    const uint64_t desc = make_wg_desc(base + kPcaABytes, kCoreBytes, 256);
+#pragma unroll
+    for (uint32_t j = 0; j < kPcaStageK; ++j) {
+      const ASel sel = pca_asel(base, 32, 8, j, r, c);
+      uint32_t fg[4], fm[4];
+      afrag(tab_g, sel, fg);
+      afrag(tab_m, sel, fm);
+      const uint64_t dj = desc + ((j * kPcaBlk) >> 4);
+      wgmma_fence();
+      wgmma_s8_rs<kPcaNMax>(dg, fg, dj);  // sum_s g G
+      wgmma_s8_rs<kPcaNMax>(dm, fm, dj);  // sum_s m G
+      wgmma_commit();
+      wgmma_wait<1>();
+    }
+    wgmma_wait<0>();
+    __syncthreads();  // every warpgroup is done with this buffer before the next stage's copies into it
+  }
+
+  // ---- epilogue: digits -> int64 -> fp64, H[v][col] = (slope_v S_g + icpt_v S_m) 2^-F_col
+#pragma unroll
+  for (uint32_t rh = 0; rh < 2; ++rh) {
+    const uint32_t v = v0 + r + 8 * rh;
+    if (v >= variant_ct) continue;
+    const double sl = slope[v], ic = icpt[v];
+#pragma unroll
+    for (uint32_t j = 0; j < kPcaCgMax / 8; ++j) {  // column col = 8 j + 2 c + e, digit d at accumulator column d cg + col
+#pragma unroll
+      for (uint32_t e = 0; e < 2; ++e) {
+        long long sg = 0, sm = 0;
+#pragma unroll
+        for (int d = kPcaDigits - 1; d >= 0; --d) {
+          const uint32_t reg = 4 * (d * (kPcaCgMax / 8) + j) + 2 * rh + e;
+          sg = sg * 256 + dg[reg];
+          sm = sm * 256 + dm[reg];
         }
-        __syncwarp();
-      }
-    }
-    if (elect_one_sync()) umma_commit(&bar_acc);
-    __syncwarp();
-  } else {
-    // ---------------- producer: raw boxes (TMA tensor map) + digit blocks (bulk copies), two k-steps at a time ----------------
-    if (elect_one_sync()) {
-      const uint32_t ring_a = smem_base + kPxaSmemOffRawA;
-      for (uint32_t it = 0; it < stage_iters; ++it) {
-        const uint32_t sa = it % kPxaRawASlots;
-        mbar_wait(&bar_empty_ra[sa], ((it / kPxaRawASlots) & 1) ^ 1);
-        mbar_expect_tx(&bar_full_ra[sa], kPxaRawABytes);
-        tma_load_2d(ring_a + sa * kPxaRawABytes, &tmap_raw, static_cast<int32_t>(it * 16), static_cast<int32_t>(v0), &bar_full_ra[sa]);
-        const uint32_t sb = it % kPxaStagesB;
-        mbar_wait(&bar_empty_b[sb], ((it / kPxaStagesB) & 1) ^ 1);
-        mbar_expect_tx(&bar_full_b[sb], 2 * blk);
-        bulk_load_1d(smem_base + sb * 2 * kPcaBlockBytesMax, gdig + static_cast<uint64_t>(2 * it) * blk, 2 * blk, &bar_full_b[sb]);
-      }
-    }
-    __syncwarp();
-  }
-
-  if (warp < kPxaRowWarps) {
-    // ---------------- epilogue: digits -> int64 -> fp64, H[v][c] = (slope_v S_g + icpt_v S_m) 2^-F_c ----------------
-    mbar_wait(&bar_acc, 0);
-    tc_fence_after_sync();
-    const uint32_t lq = warp & 3, half = warp >> 2;
-    const uint32_t v = v0 + 32 * lq + lane;
-    const double sl = (v < variant_ct) ? slope[v] : 0.0, ic = (v < variant_ct) ? icpt[v] : 0.0;
-    const uint32_t taddr = tmem_base + ((32u * lq) << 16);
-    // columns in chunks of 4 (cg is a multiple of 4); the two groups alternate chunks
-#pragma unroll 1
-    for (uint32_t c0 = 4 * half; c0 < cg; c0 += 8) {
-      uint32_t dg[kPcaDigits][4], dm[kPcaDigits][4];
-#pragma unroll
-      for (uint32_t d = 0; d < kPcaDigits; ++d) {
-        tmem_ld4(taddr + d * cg + c0, dg[d]);
-        tmem_ld4(taddr + n_total + d * cg + c0, dm[d]);
-      }
-      tmem_ld_wait();
-      if (v < variant_ct) {
-#pragma unroll
-        for (uint32_t c = 0; c < 4; ++c) {
-          long long sg = 0, sm = 0;
-#pragma unroll
-          for (int d = kPcaDigits - 1; d >= 0; --d) {
-            sg = sg * 256 + static_cast<int32_t>(dg[d][c]);
-            sm = sm * 256 + static_cast<int32_t>(dm[d][c]);
-          }
-          if (c0 + c < cols_valid) {
-            double* dst = &h[static_cast<uint64_t>(c0 + c) * h_ld + v];
-            const double val = (sl * static_cast<double>(sg) + ic * static_cast<double>(sm)) * (inv_scale[c0 + c] * post_scale);
-            *dst = accumulate ? (*dst + val) : val;
-          }
+        const uint32_t col = 8 * j + 2 * c + e;
+        if (col < cols_valid) {
+          double* dst = &h[static_cast<uint64_t>(col) * h_ld + v];
+          const double val = (sl * static_cast<double>(sg) + ic * static_cast<double>(sm)) * (inv_scale[col] * post_scale);
+          *dst = accumulate ? (*dst + val) : val;
         }
       }
     }
-    tc_fence_before_sync();
-  }
-  __syncthreads();
-  if (warp == kPxaIssuerWarp) {
-    tc_fence_after_sync();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 
 // ================================================================================================================
-// XtB: partial[split][s][c] = sum over this CTA's variants of g (slope H) + m (icpt H) for 256 samples per CTA.
-// TMEM: D0 [0, N) (samples 0-127), D1 [N, 2N) (samples 128-255), A slots of 32 columns (tile0 g, m, tile1 g, m).
-// Warps: 8 row (warp = tile * 4 + lane quarter; every warp handles every k-step, two per tcgen05.wait::st),
-// issuer, producer.
+// XtB: partial[split][s][c] = sum over this CTA's variants of g (slope H) + m (icpt H) for 128 samples per CTA
+// (warpgroup w: samples 64 w ..).  Row words: the sample-major copy ([row tile][k-step][128][8 B]).
 // ================================================================================================================
-constexpr uint32_t kPxtStagesB = 3;                    // stages of two k-steps x two blocks (slope.H, icpt.H)
-constexpr uint32_t kPxtRawISlots = 3;                  // per tile: four k-steps (4 KB) per slot
-constexpr uint32_t kPxtSmemOffRawI = kPxtStagesB * 4 * kPcaBlockBytesMax;  // 73728
-constexpr uint32_t kPxtSmemBytes = kPxtSmemOffRawI + 2 * kPxtRawISlots * 4096 + 1024;
-constexpr uint32_t kPxtRowWarps = 8;
-constexpr uint32_t kPxtIssuerWarp = kPxtRowWarps;
-constexpr uint32_t kPxtThreads = 32 * (kPxtRowWarps + 2);
+constexpr uint32_t kPxtStage = kPcaABytes + 2 * kPcaStageK * kPcaBlk;   // [row words][slope.H blocks][icpt.H blocks]
+constexpr uint32_t kPxtSmemBytes = 2 * kPxtStage + 128;
 
-static __global__ void __launch_bounds__(kPxtThreads, 1)
-pca_xtb_ts_kernel(const uint8_t* __restrict__ raw_i /* [row tile][kstep_total][128][8 B] */, uint32_t kstep_total, uint32_t ksteps_per_split /* multiple of 4 */, uint32_t sample_ct, const uint8_t* __restrict__ hs_dig, const uint8_t* __restrict__ hi_dig /* [variants / 32][32 N] */,
-                  uint32_t cg, const double* __restrict__ inv_scale /* [cg] */, double* __restrict__ partial /* [split][sample_ct_padded][cg] */, uint32_t sample_ct_padded) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ __align__(8) uint64_t bar_full_a[8];
-  __shared__ __align__(8) uint64_t bar_empty_a[8];
-  __shared__ __align__(8) uint64_t bar_full_b[kPxtStagesB];
-  __shared__ __align__(8) uint64_t bar_empty_b[kPxtStagesB];
-  __shared__ __align__(8) uint64_t bar_full_ri[kPxtRawISlots];
-  __shared__ __align__(8) uint64_t bar_empty_ri[kPxtRawISlots];
-  __shared__ __align__(8) uint64_t bar_acc;
-  __shared__ uint32_t tmem_base_slot;
-
-  const uint32_t tid = threadIdx.x;
-  const uint32_t warp = uniform_warp_idx();
-  const uint32_t lane = tid & 31;
-  const uint32_t n_total = kPcaDigits * cg;
-  const uint32_t blk = pca_block_bytes(n_total);
-  const uint32_t a_slots = min(8u, (512u - 2 * n_total) / 32u);   // 4 for N = 192, 6 for N = 160 -> use 4..8
+static __global__ void __launch_bounds__(kPcaThreads, 1)
+pca_xtb_wg_kernel(const uint8_t* __restrict__ raw_i /* [row tile][kstep_total][128][8 B] */, uint32_t kstep_total, uint32_t ksteps_per_split /* multiple of 4 */, uint32_t sample_ct, const uint8_t* __restrict__ hs_dig, const uint8_t* __restrict__ hi_dig /* [variants / 32][32 N] */,
+                  const double* __restrict__ inv_scale /* [kPcaCgMax] */, double* __restrict__ partial /* [split][sample_ct_padded][kPcaCgMax] */, uint32_t sample_ct_padded) {
+  extern __shared__ __align__(128) uint8_t smem_dyn[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_dyn) + 127) & ~static_cast<uintptr_t>(127));
+  const uint32_t smem_base = static_cast<uint32_t>(__cvta_generic_to_shared(smem));
+  const uint32_t tid = threadIdx.x, wg = tid >> 7, warp4 = (tid >> 5) & 3, lane = tid & 31, g = lane >> 2, c = lane & 3;
+  const uint32_t rt = blockIdx.x;
   const uint32_t ks_begin = blockIdx.y * ksteps_per_split;
   const uint32_t ks_end = min(kstep_total, ks_begin + ksteps_per_split);
-  const uint32_t ks_ct = ks_end > ks_begin ? ks_end - ks_begin : 0;   // multiple of 4 (kstep_total is)
-  const uint32_t quad_iters = ks_ct / 4;
-  const uint32_t rt0 = 2 * blockIdx.x;                                // first of the CTA's two 128-sample tiles
-  const uint32_t rt_ct = sample_ct_padded / 128;
-  const uint32_t smem_base = (smem_u32(smem) + 1023u) & ~1023u;
+  const uint32_t stage_ct = ks_end > ks_begin ? (ks_end - ks_begin) / kPcaStageK : 0;  // kstep_total is a multiple of 4
+  const uint32_t thread_zero = tid * (kstep_total >> 31);
+  const uint32_t tab_g = table_reg(kTabDosage, thread_zero), tab_m = table_reg(kTabNonmiss, thread_zero);
+  auto issue = [&](uint32_t st) {
+    uint8_t* dst = smem + (st & 1) * kPxtStage;
+    const uint64_t ks0 = ks_begin + st * kPcaStageK;
+    const uint8_t* a_src = raw_i + (static_cast<uint64_t>(rt) * kstep_total + ks0) * 1024;
+    cp_async16(dst + 16 * tid, a_src + 16 * tid);  // 4 KB = 256 x 16 B
+    for (uint32_t i = tid; i < 2 * kPcaStageK * kPcaBlk / 16; i += kPcaThreads) {
+      const uint32_t which = i / (kPcaStageK * kPcaBlk / 16), o = 16 * (i % (kPcaStageK * kPcaBlk / 16));
+      cp_async16(dst + kPcaABytes + which * (kPcaStageK * kPcaBlk) + o, (which ? hi_dig : hs_dig) + ks0 * kPcaBlk + o);
+    }
+    cp_async_commit();
+  };
 
-  if (tid == 0) {
-    for (uint32_t s = 0; s < 8; ++s) {
-      mbar_init(&bar_full_a[s], kPxtRowWarps);
-      mbar_init(&bar_empty_a[s], 1);
-    }
-    for (uint32_t s = 0; s < kPxtStagesB; ++s) {
-      mbar_init(&bar_full_b[s], 1);
-      mbar_init(&bar_empty_b[s], 1);
-    }
-    for (uint32_t s = 0; s < kPxtRawISlots; ++s) {
-      mbar_init(&bar_full_ri[s], 1);
-      mbar_init(&bar_empty_ri[s], kPxtRowWarps);
-    }
-    mbar_init(&bar_acc, 1);
-    mbar_fence_init();
-  }
-  if (warp == kPxtIssuerWarp) tmem_alloc<512>(&tmem_base_slot);
-  tc_fence_before_sync();
-  __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = tmem_base_slot;
-
-  if (warp < kPxtRowWarps) {
-    // ---------------- row side: lane = sample of tile (warp / 4); 8 bytes = 32 variants per k-step ----------------
-    const uint32_t tile = warp >> 2, lq = warp & 3;
-    const uint32_t thread_zero = tid * (kstep_total >> 31);
-    const uint32_t tab_g = table_reg(kTabDosage, thread_zero), tab_m = table_reg(kTabNonmiss, thread_zero);
-    const uint32_t ring_i = smem_base + kPxtSmemOffRawI + tile * (kPxtRawISlots * 4096) + (32 * lq + lane) * 8;
-    const uint32_t ta0 = tmem_base + ((32u * lq) << 16) + 2 * n_total + tile * 16;
-    for (uint32_t q = 0; q < quad_iters; ++q) {
-      const uint32_t si = q % kPxtRawISlots;
-      mbar_wait(&bar_full_ri[si], (q / kPxtRawISlots) & 1);
-      uint2 w[4];
+  int32_t acc[kPcaNMax / 2];
 #pragma unroll
-      for (uint32_t j = 0; j < 4; ++j) w[j] = lds64(ring_i + si * 4096 + j * 1024);
-#pragma unroll
-      for (uint32_t pair = 0; pair < 2; ++pair) {
-        // two k-steps per tcgen05.wait::st
-        uint32_t slots[2];
-#pragma unroll
-        for (uint32_t j = 0; j < 2; ++j) {
-          const uint32_t ks = 4 * q + 2 * pair + j;
-          const uint32_t slot = ks % a_slots;
-          slots[j] = slot;
-          const Sel4 s0 = make_selectors(w[2 * pair + j].x), s1 = make_selectors(w[2 * pair + j].y);
-          uint32_t eg[8], em[8];
-          const uint4 a = expand16(tab_g, s0), b = expand16(tab_g, s1);
-          eg[0] = a.x; eg[1] = a.y; eg[2] = a.z; eg[3] = a.w; eg[4] = b.x; eg[5] = b.y; eg[6] = b.z; eg[7] = b.w;
-          const uint4 c = expand16(tab_m, s0), d = expand16(tab_m, s1);
-          em[0] = c.x; em[1] = c.y; em[2] = c.z; em[3] = c.w; em[4] = d.x; em[5] = d.y; em[6] = d.z; em[7] = d.w;
-          mbar_wait(&bar_empty_a[slot], ((ks / a_slots) & 1) ^ 1);
-          tc_fence_after_sync();
-          tmem_st8(ta0 + slot * 32, eg);
-          tmem_st8(ta0 + slot * 32 + 8, em);
-        }
-        if (pair == 1) mbar_arrive_warp(&bar_empty_ri[si], lane);  // all four words went through tcgen05.st
-        tmem_st_wait();
-        tc_fence_before_sync();
-        mbar_arrive_warp(&bar_full_a[slots[0]], lane);
-        mbar_arrive_warp(&bar_full_a[slots[1]], lane);
-      }
+  for (uint32_t i = 0; i < kPcaNMax / 2; ++i) acc[i] = 0;
+  const uint32_t r = 64 * wg + 16 * warp4 + g;
+  if (stage_ct) issue(0);
+  for (uint32_t st = 0; st < stage_ct; ++st) {
+    if (st + 1 < stage_ct) {
+      issue(st + 1);
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
     }
-  } else if (warp == kPxtIssuerWarp) {
-    // ---------------- UMMA issuer ----------------
-    const uint32_t idesc = make_idesc_i8(128, n_total, false, true);
-    const uint32_t tmem_u = uniform_u32(tmem_base);
-    const uint32_t lbo = (n_total / 16) * kCoreBytes;
-    const uint64_t desc0 = make_smem_desc(smem_base, lbo, kCoreBytes);
-    const uint32_t stage_iters = ks_ct / 2;
-    for (uint32_t it = 0; it < stage_iters; ++it) {
-      const uint32_t sb = it % kPxtStagesB;
-      mbar_wait(&bar_full_b[sb], (it / kPxtStagesB) & 1);
+    fence_proxy_async_smem();
+    __syncthreads();
+    const uint32_t base = smem_base + (st & 1) * kPxtStage;
+    const uint64_t desc_s = make_wg_desc(base + kPcaABytes, kCoreBytes, 256);
+    const uint64_t desc_i = desc_s + ((kPcaStageK * kPcaBlk) >> 4);
 #pragma unroll
-      for (uint32_t kk = 0; kk < 2; ++kk) {
-        const uint32_t ks = 2 * it + kk;
-        const uint32_t slot = ks % a_slots;
-        mbar_wait(&bar_full_a[slot], (ks / a_slots) & 1);
-        tc_fence_after_sync();
-        if (elect_one_sync()) {
-          const uint32_t acc = ks ? 1u : 0u;
-          // stage layout: [k-step kk][block 0 = slope.H, block 1 = icpt.H]
-          const uint64_t bs = desc0 + ((sb * 4 * kPcaBlockBytesMax + (2 * kk) * blk) >> 4);
-          const uint64_t bi = bs + (blk >> 4);
-          const uint32_t ta = tmem_u + 2 * n_total + slot * 32;
-          umma_i8_ts(tmem_u + 0, ta, bs, idesc, acc);             // tile 0: g x slope.H
-          umma_i8_ts(tmem_u + 0, ta + 8, bi, idesc, 1u);          // tile 0: m x icpt.H
-          umma_i8_ts(tmem_u + n_total, ta + 16, bs, idesc, acc);  // tile 1
-          umma_i8_ts(tmem_u + n_total, ta + 24, bi, idesc, 1u);
-          umma_commit(&bar_empty_a[slot]);
-          if (kk == 1) umma_commit(&bar_empty_b[sb]);
-        }
-        __syncwarp();
-      }
+    for (uint32_t j = 0; j < kPcaStageK; ++j) {
+      const ASel sel = pca_asel(base, 8, 1024, j, r, c);
+      uint32_t fg[4], fm[4];
+      afrag(tab_g, sel, fg);
+      afrag(tab_m, sel, fm);
+      wgmma_fence();
+      wgmma_s8_rs<kPcaNMax>(acc, fg, desc_s + ((j * kPcaBlk) >> 4));  // g x slope.H
+      wgmma_s8_rs<kPcaNMax>(acc, fm, desc_i + ((j * kPcaBlk) >> 4));  // m x icpt.H
+      wgmma_commit();
+      wgmma_wait<1>();
     }
-    if (elect_one_sync()) umma_commit(&bar_acc);
-    __syncwarp();
-  } else {
-    // ---------------- producer ----------------
-    if (elect_one_sync()) {
-      const uint32_t ring_i = smem_base + kPxtSmemOffRawI;
-      const uint32_t stage_iters = ks_ct / 2;
-      for (uint32_t it = 0; it < stage_iters; ++it) {
-        if (!(it & 1)) {
-          const uint32_t q = it >> 1, si = q % kPxtRawISlots;
-          mbar_wait(&bar_empty_ri[si], ((q / kPxtRawISlots) & 1) ^ 1);
-          mbar_expect_tx(&bar_full_ri[si], 2 * 4096);
-#pragma unroll
-          for (uint32_t t = 0; t < 2; ++t) {
-            // a tile beyond the padded sample range re-reads the last tile (its rows are masked in the epilogue)
-            const uint32_t rt = min(rt0 + t, rt_ct - 1);
-            bulk_load_1d(ring_i + t * (kPxtRawISlots * 4096) + si * 4096, raw_i + (static_cast<uint64_t>(rt) * kstep_total + ks_begin + 4 * q) * 1024, 4096, &bar_full_ri[si]);
-          }
-        }
-        const uint32_t sb = it % kPxtStagesB;
-        mbar_wait(&bar_empty_b[sb], ((it / kPxtStagesB) & 1) ^ 1);
-        mbar_expect_tx(&bar_full_b[sb], 4 * blk);
-        const uint64_t ks0 = ks_begin + 2 * it;
-#pragma unroll
-        for (uint32_t kk = 0; kk < 2; ++kk) {
-          bulk_load_1d(smem_base + sb * 4 * kPcaBlockBytesMax + (2 * kk) * blk, hs_dig + (ks0 + kk) * blk, blk, &bar_full_b[sb]);
-          bulk_load_1d(smem_base + sb * 4 * kPcaBlockBytesMax + (2 * kk + 1) * blk, hi_dig + (ks0 + kk) * blk, blk, &bar_full_b[sb]);
-        }
-      }
-    }
-    __syncwarp();
+    wgmma_wait<0>();
+    __syncthreads();
   }
 
-  if (warp < kPxtRowWarps) {
-    // ---------------- epilogue: digits -> fp64 partial sums ----------------
-    mbar_wait(&bar_acc, 0);
-    tc_fence_after_sync();
-    const uint32_t tile = warp >> 2, lq = warp & 3;
-    const uint32_t s = (rt0 + tile) * 128 + 32 * lq + lane;
-    const uint32_t taddr = tmem_base + ((32u * lq) << 16) + tile * n_total;
-    double* out = partial + (static_cast<uint64_t>(blockIdx.y) * sample_ct_padded + s) * cg;
-#pragma unroll 1
-    for (uint32_t c0 = 0; c0 < cg; c0 += 4) {
-      uint32_t dd[kPcaDigits][4];
+  // ---- epilogue: digits -> fp64 partial sums
+  if (!stage_ct) return;
 #pragma unroll
-      for (uint32_t d = 0; d < kPcaDigits; ++d) tmem_ld4(taddr + d * cg + c0, dd[d]);
-      tmem_ld_wait();
-      if (s < sample_ct_padded && ks_ct) {
+  for (uint32_t rh = 0; rh < 2; ++rh) {
+    const uint32_t s = 128 * rt + r + 8 * rh;
+    if (s >= sample_ct_padded) continue;
+    double* out = partial + (static_cast<uint64_t>(blockIdx.y) * sample_ct_padded + s) * kPcaCgMax;
 #pragma unroll
-        for (uint32_t c = 0; c < 4; ++c) {
-          long long sum = 0;
+    for (uint32_t j = 0; j < kPcaCgMax / 8; ++j) {
 #pragma unroll
-          for (int d = kPcaDigits - 1; d >= 0; --d) sum = sum * 256 + static_cast<int32_t>(dd[d][c]);
-          out[c0 + c] = (s < sample_ct) ? static_cast<double>(sum) * inv_scale[c0 + c] : 0.0;
-        }
+      for (uint32_t e = 0; e < 2; ++e) {
+        long long sum = 0;
+#pragma unroll
+        for (int d = kPcaDigits - 1; d >= 0; --d) sum = sum * 256 + acc[4 * (d * (kPcaCgMax / 8) + j) + 2 * rh + e];
+        const uint32_t col = 8 * j + 2 * c + e;
+        out[col] = (s < sample_ct) ? static_cast<double>(sum) * inv_scale[col] : 0.0;
       }
     }
-    tc_fence_before_sync();
-  }
-  __syncthreads();
-  if (warp == kPxtIssuerWarp) {
-    tc_fence_after_sync();
-    tmem_dealloc<512>(tmem_base);
   }
 }
 

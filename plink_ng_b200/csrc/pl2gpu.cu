@@ -13,7 +13,7 @@
 #include "king_kernels.cuh"
 #include "king_ts_kernel.cuh"
 #include "king_pairs_kernel.cuh"
-#include "umma_probe.cuh"
+#include "wgmma_probe.cuh"
 
 namespace pl2 {
 
@@ -99,32 +99,6 @@ void FreeTileList(TileList* tl) {
   cudaFree(tl->d_tile_order);
   tl->d_tile_order = nullptr;
   tl->d_tile_rt = tl->d_tile_tc = tl->d_rowtile_offset = nullptr;
-}
-
-// ---- TMA tensor maps ----
-int MakeRawTensorMap(CUtensorMap* out, void* base, uint32_t pitch, uint32_t rows, uint32_t box_bytes, uint32_t box_rows) {
-  typedef CUresult (*EncodeFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-  static EncodeFn encode = nullptr;
-  if (!encode) {
-    void* fn = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &fn, cudaEnableDefault, &qres) != cudaSuccess || qres != cudaDriverEntryPointSuccess || !fn) {
-      cudaGetLastError();
-      set_error("cuTensorMapEncodeTiled is not available from this driver");
-      return 1;
-    }
-    encode = reinterpret_cast<EncodeFn>(fn);
-  }
-  const cuuint64_t dims[2] = {pitch, rows};
-  const cuuint64_t strides[1] = {pitch};  // bytes, dimension 1
-  const cuuint32_t box[2] = {box_bytes, box_rows};
-  const cuuint32_t elem_strides[2] = {1, 1};
-  const CUresult r = encode(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, base, dims, strides, box, elem_strides, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) {
-    set_error("cuTensorMapEncodeTiled failed (%d) for a %u x %u-byte block", static_cast<int>(r), rows, pitch);
-    return 1;
-  }
-  return 0;
 }
 
 // ---- NCCL, loaded on first use: the library has no link-time dependency on it, and inside a process that
@@ -250,8 +224,7 @@ struct Pl2KingJob {
   // row re-tiling of batch k+1 (prep stream) overlap the tensor kernel of batch k (compute stream).
   // The other algorithms use buffer 0 on the compute stream only.
   GenoStage stage[2];
-  uint8_t* d_raw_t[2] = {nullptr, nullptr};  // TS path: row-side re-tiled copy of the job's own row tiles (geno_tile.cuh)
-  CUtensorMap tmap[2];                       // TS path: 2-D tensor maps over stage[b].d_raw for the column-side TMA loads
+  uint8_t* d_raw_t[2] = {nullptr, nullptr};  // tensor paths: sample-major copy of the staged block (geno_tile.cuh)
   cudaEvent_t ev_prep_done[2] = {nullptr, nullptr};
   cudaEvent_t ev_kernel_start[2] = {nullptr, nullptr};  // timing-enabled pair around the tensor kernel (pl2gpu_king_last_kernel_ms)
   cudaEvent_t ev_kernel_done[2] = {nullptr, nullptr};
@@ -293,8 +266,8 @@ int pl2gpu_ctx_create(int device_idx, Pl2GpuCtx** ctx_ptr) {
   }
   cudaDeviceProp prop;
   PL2_CUDA_OK(cudaGetDeviceProperties(&prop, device_idx));
-  if (prop.major != 10) {
-    set_error("pl2gpu_ctx_create: device %d is sm_%d%d; this library contains sm_100a code only", device_idx, prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("pl2gpu_ctx_create: device %d is sm_%d%d; this library contains sm_90a code only", device_idx, prop.major, prop.minor);
     return 1;
   }
   PL2_CUDA_OK(cudaSetDevice(device_idx));
@@ -309,10 +282,8 @@ int pl2gpu_ctx_create(int device_idx, Pl2GpuCtx** ctx_ptr) {
     PL2_CUDA_OK(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
     PL2_CUDA_OK(cudaStreamCreateWithPriority(&ctx->c.copy_stream, cudaStreamNonBlocking, prio_hi));
   }
-  PL2_CUDA_OK(cudaFuncSetAttribute(king_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTcSmemBytes));
-  PL2_CUDA_OK(cudaFuncSetAttribute(umma_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kProbeSmemBytes));
-  PL2_CUDA_OK(cudaFuncSetAttribute(umma_probe_ts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kProbeSmemBytes));
-  PL2_CUDA_OK(cudaFuncSetAttribute(king_ts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kTsSmemBytes));
+  PL2_CUDA_OK(cudaFuncSetAttribute(king_wg_kernel<kTileCols>, cudaFuncAttributeMaxDynamicSharedMemorySize, KingWgShape<kTileCols>::kSmemBytes));
+  PL2_CUDA_OK(cudaFuncSetAttribute(king_wg_kernel<kTsCols>, cudaFuncAttributeMaxDynamicSharedMemorySize, KingWgShape<kTsCols>::kSmemBytes));
   *ctx_ptr = ctx;
   return 0;
 }
@@ -456,15 +427,14 @@ uint64_t pl2gpu_king_mem_required(uint32_t sample_ct, uint32_t row_start, uint32
   // re-layouts + tile lists + the output staging buffer, plus slack for allocator granularity.
   const uint64_t cap = ClampStageCap(max_variants_per_add);
   const uint64_t slack = 128ull << 20;
-  // SS tensor / popcount: 128 x 96 tiles, raw block + 3 bit planes (popcount only)
+  // 128 x 96 tiles (tensor / popcount): raw block + its sample-major copy (tensor) or 3 bit planes (popcount)
   const uint64_t tiles = CountTiles(row_start, row_end, false);
   const uint64_t npad = RoundUpU32(sample_ct, kSamplePad);
   const uint64_t need_ss = tiles * kKingTileAccWords * 4 + cap * (npad / 4) + 3ull * (cap / 32) * npad * 4 + tiles * 16;
-  // TS tensor (the default): 128 x 64 tiles, two raw blocks + two row-side re-tiled copies of the job's row tiles
+  // 128 x 80 tiles (the default): two raw blocks + two sample-major copies
   const uint64_t tiles_ts = CountTiles(row_start, row_end, false, kTsCols);
   const uint64_t npad_ts = RoundUpU32(sample_ct, kTsSamplePad);
-  const uint64_t row_tiles = row_end > row_start ? (DivUpU32(row_end, kTileRows) - row_start / kTileRows) : 0;
-  const uint64_t need_ts = tiles_ts * kTsTileAccWords * 4 + 2 * cap * (npad_ts / 4) + 2 * row_tiles * kTileRows * (cap / 4) + tiles_ts * 16;
+  const uint64_t need_ts = tiles_ts * kTsTileAccWords * 4 + 4 * cap * (npad_ts / 4) + tiles_ts * 16;
   return (need_ss > need_ts ? need_ss : need_ts) + kKingOutStageBytes + slack;
 }
 
@@ -512,14 +482,13 @@ int pl2gpu_king_begin_ex(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start,
   if (BuildTileList(row_start, row_end, false, &job->tiles, job->tile_cols)) return fail();
   for (int b = 0; b < (ts ? 2 : 1); ++b) {
     if (StageAlloc(sample_ct, cap, &job->stage[b], ts ? kTsSamplePad : kSamplePad)) return fail();
-    if (ts) {
-      const uint64_t raw_t_bytes = static_cast<uint64_t>(job->tiles.row_tile_ct) * kTileRows * (job->stage[b].variant_cap / 4);
-      if (cudaMalloc(&job->d_raw_t[b], raw_t_bytes ? raw_t_bytes : 16) != cudaSuccess) {
+    if (algo != kPl2KingAlgoPopcount) {
+      const uint64_t raw_t_bytes = static_cast<uint64_t>(job->stage[b].sample_ct_padded) * (job->stage[b].variant_cap / 4);
+      if (cudaMalloc(&job->d_raw_t[b], raw_t_bytes) != cudaSuccess) {
         cudaGetLastError();
-        set_error("pl2gpu_king_begin: insufficient device memory for the row-side re-tiled genotype copy");
+        set_error("pl2gpu_king_begin: insufficient device memory for the sample-major genotype copy");
         return fail();
       }
-      if (MakeRawTensorMap(&job->tmap[b], job->stage[b].d_raw, job->stage[b].pitch, job->stage[b].variant_cap, kTsRawBoxBytes, 2 * kTsKcJ)) return fail();
     }
   }
   const uint64_t acc_bytes = static_cast<uint64_t>(job->tiles.tile_ct) * (5ull * job->tile_cols * kTileRows) * sizeof(int32_t);
@@ -550,8 +519,8 @@ int pl2gpu_king_begin_ex(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start,
   return 0;
 }
 
-// TS path: the staged block stage[b] holds `cur` variants (rows [0, cur)); pad it, re-tile the job's row
-// tiles and queue the tensor kernel.  Everything up to the kernel runs on the prep stream.
+// TS path: the staged block stage[b] holds `cur` variants (rows [0, cur)); pad it, write its sample-major copy
+// and queue the tensor kernel.  Everything up to the kernel runs on the prep stream.
 static int KingTsPrepAndLaunch(Pl2KingJob* job, uint32_t b, uint32_t cur, bool pad_valid_rows) {
   Ctx* c = &job->ctx->c;
   cudaStream_t prep = c->copy_stream;
@@ -568,13 +537,13 @@ static int KingTsPrepAndLaunch(Pl2KingJob* job, uint32_t b, uint32_t cur, bool p
     job->kernel_pending[b] = true;
     return 0;
   }
-  geno_tile_rows_kernel<<<dim3(padded / 64, job->tiles.row_tile_ct * (kTileRows / 64)), 256, 0, prep>>>(st.d_raw, st.pitch, padded / 32, job->tiles.row_tile_first * kTileRows, job->d_raw_t[b]);
+  geno_tile_rows_kernel<<<dim3(padded / 64, st.sample_ct_padded / 64), 256, 0, prep>>>(st.d_raw, st.pitch, padded / 32, 0, job->d_raw_t[b]);
   c->launches++;
   PL2_CUDA_OK(cudaGetLastError());
   PL2_CUDA_OK(cudaEventRecord(job->ev_prep_done[b], prep));
   PL2_CUDA_OK(cudaStreamWaitEvent(c->stream, job->ev_prep_done[b], 0));
   PL2_CUDA_OK(cudaEventRecord(job->ev_kernel_start[b], c->stream));
-  king_ts_kernel<<<job->tiles.tile_ct, kTsThreads, kTsSmemBytes, c->stream>>>(job->tmap[b], job->d_raw_t[b], job->tiles.row_tile_first, padded, job->tiles.d_tile_order, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->d_raw_acc);
+  king_wg_kernel<kTsCols><<<2 * job->tiles.tile_ct, kKwThreads, KingWgShape<kTsCols>::kSmemBytes, c->stream>>>(job->d_raw_t[b], padded, job->tiles.d_tile_order, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->d_raw_acc);
   c->launches++;
   PL2_CUDA_OK(cudaGetLastError());
   PL2_CUDA_OK(cudaEventRecord(job->ev_kernel_done[b], c->stream));
@@ -631,7 +600,10 @@ int pl2gpu_king_add_variants(Pl2KingJob* job, const void* genovecs, uint64_t var
           king_popc_kernel<<<job->tiles.tile_ct * 2, 256, 0, c->stream>>>(job->d_planes, job->stage[0].sample_ct_padded, word_ct, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->d_raw_acc);
           c->launches++;
         } else {
-          king_tc_kernel<<<job->tiles.tile_ct, kTcThreads, kTcSmemBytes, c->stream>>>(job->stage[0].d_raw, job->stage[0].pitch, padded, job->tiles.d_tile_order, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->d_raw_acc);
+          const GenoStage& st = job->stage[0];
+          geno_tile_rows_kernel<<<dim3(padded / 64, st.sample_ct_padded / 64), 256, 0, c->stream>>>(st.d_raw, st.pitch, padded / 32, 0, job->d_raw_t[0]);
+          c->launches++;
+          king_wg_kernel<kTileCols><<<2 * job->tiles.tile_ct, kKwThreads, KingWgShape<kTileCols>::kSmemBytes, c->stream>>>(job->d_raw_t[0], padded, job->tiles.d_tile_order, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->d_raw_acc);
           c->launches++;
         }
         PL2_CUDA_OK(cudaGetLastError());
@@ -979,27 +951,32 @@ int pl2gpu_king_pairs_end(Pl2KingPairJob* job) {
 // ------------------------------------------------------------------------------------------ probe
 
 int pl2gpu_int8_peak(Pl2GpuCtx* ctx, uint32_t n_cols, int form, double min_seconds, double* tops_out, double* seconds_out) {
-  if (!ctx || !tops_out || n_cols < 16 || n_cols > 240 || (n_cols & 15) || (form != 0 && form != 1)) {
-    set_error("pl2gpu_int8_peak: bad arguments (n_cols must be a multiple of 16 in [16,240])");
+  if (!ctx || !tops_out || (n_cols != 80 && n_cols != 96) || form != 1) {
+    set_error("pl2gpu_int8_peak: bad arguments (n_cols must be 80 or 96, form 1 = A in registers)");
     return 1;
   }
   Ctx* c = &ctx->c;
   PL2_CUDA_OK(cudaSetDevice(c->device));
-  PL2_CUDA_OK(cudaFuncSetAttribute(umma_peak_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kProbeSmemBytes));
+  int32_t* d_sink = nullptr;
+  PL2_CUDA_OK(cudaMalloc(&d_sink, 256 * sizeof(int32_t)));
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   PL2_CUDA_OK(cudaEventCreate(&e0));
   PL2_CUDA_OK(cudaEventCreate(&e1));
-  const uint32_t blocks = 4096;  // x 32 UMMAs x 2 issuer warps: ~15-35 ms per launch
-  const double ops_per_launch = 2.0 * 128 * n_cols * 32 * 32.0 * 2 * blocks * c->sm_count;
-  umma_peak_kernel<<<c->sm_count, 128, kProbeSmemBytes, c->stream>>>(n_cols, blocks, static_cast<uint32_t>(form));  // warm-up
-  c->launches++;
+  const uint32_t blocks = 4096;  // x 32 wgmmas x 2 warpgroups per SM
+  const double ops_per_launch = 2.0 * 64 * n_cols * 32 * 32.0 * 2 * blocks * c->sm_count;
+  auto launch = [&]() {
+    if (n_cols == 80) wgmma_peak_kernel<80><<<c->sm_count, 256, 0, c->stream>>>(blocks, d_sink);
+    else wgmma_peak_kernel<96><<<c->sm_count, 256, 0, c->stream>>>(blocks, d_sink);
+    c->launches++;
+  };
+  launch();  // warm-up
   PL2_CUDA_OK(cudaStreamSynchronize(c->stream));
+  PL2_CUDA_OK(cudaGetLastError());
   double total_s = 0, total_ops = 0;
-  uint32_t per_batch = 8;
+  const uint32_t per_batch = 8;
   while (total_s < min_seconds) {
     PL2_CUDA_OK(cudaEventRecord(e0, c->stream));
-    for (uint32_t k = 0; k < per_batch; ++k) umma_peak_kernel<<<c->sm_count, 128, kProbeSmemBytes, c->stream>>>(n_cols, blocks, static_cast<uint32_t>(form));
-    c->launches += per_batch;
+    for (uint32_t k = 0; k < per_batch; ++k) launch();
     PL2_CUDA_OK(cudaEventRecord(e1, c->stream));
     PL2_CUDA_OK(cudaEventSynchronize(e1));
     PL2_CUDA_OK(cudaGetLastError());
@@ -1011,105 +988,51 @@ int pl2gpu_int8_peak(Pl2GpuCtx* ctx, uint32_t n_cols, int form, double min_secon
   }
   cudaEventDestroy(e0);
   cudaEventDestroy(e1);
+  cudaFree(d_sink);
   *tops_out = total_ops / total_s / 1e12;
   if (seconds_out) *seconds_out = total_s;
   return 0;
 }
 
-
-
-int pl2gpu_debug_umma(Pl2GpuCtx* ctx, const uint8_t* a_img, uint32_t a_bytes, const uint8_t* b_img, uint32_t b_bytes, uint32_t a_lbo, uint32_t a_sbo, uint32_t b_lbo, uint32_t b_sbo, uint32_t a_step_bytes, uint32_t b_step_bytes, uint32_t k_steps, uint32_t idesc, uint32_t n, int32_t* d_out_host) {
+// The int8 wgmma form of every tensor kernel (A fragments in registers, B K-major in shared memory) against a
+// scalar product on the host: M = 64, N = 80, K = 64 (two k-steps).
+int pl2gpu_selftest_umma(Pl2GpuCtx* ctx, int verbose) {
   if (!ctx) {
-    set_error("pl2gpu_debug_umma: null context");
+    set_error("pl2gpu_selftest_umma: null context");
     return 1;
   }
   Ctx* c = &ctx->c;
   PL2_CUDA_OK(cudaSetDevice(c->device));
-  UmmaProbeParams prm;
-  prm.a_bytes = a_bytes;
-  prm.b_bytes = b_bytes;
-  prm.b_smem_off = RoundUpU32(a_bytes, 1024);
-  if (prm.b_smem_off + b_bytes + 1024 > kProbeSmemBytes || n > 256 || (n & 15)) {
-    set_error("pl2gpu_debug_umma: images too large or bad n");
-    return 1;
-  }
-  prm.a_lbo = a_lbo;
-  prm.a_sbo = a_sbo;
-  prm.b_lbo = b_lbo;
-  prm.b_sbo = b_sbo;
-  prm.a_step_bytes = a_step_bytes;
-  prm.b_step_bytes = b_step_bytes;
-  prm.k_steps = k_steps;
-  prm.idesc = idesc;
-  prm.n = n;
-  uint8_t *d_a = nullptr, *d_b = nullptr;
+  const uint32_t M = 64, N = kProbeN, K = kProbeK;
+  std::vector<int8_t> a(M * K), b(N * K);
+  uint32_t seed = 12345;
+  auto rnd = [&]() {
+    seed = seed * 1664525u + 1013904223u;
+    return static_cast<int8_t>(static_cast<int>((seed >> 24) % 255) - 127);
+  };
+  for (auto& v : a) v = rnd();
+  for (auto& v : b) v = rnd();
+  int8_t *d_a = nullptr, *d_b = nullptr;
   int32_t* d_d = nullptr;
-  PL2_CUDA_OK(cudaMalloc(&d_a, a_bytes));
-  PL2_CUDA_OK(cudaMalloc(&d_b, b_bytes));
-  PL2_CUDA_OK(cudaMalloc(&d_d, 128ull * n * 4));
-  PL2_CUDA_OK(cudaMemcpyAsync(d_a, a_img, a_bytes, cudaMemcpyHostToDevice, c->stream));
-  PL2_CUDA_OK(cudaMemcpyAsync(d_b, b_img, b_bytes, cudaMemcpyHostToDevice, c->stream));
-  umma_probe_kernel<<<1, 128, kProbeSmemBytes, c->stream>>>(d_a, d_b, prm, d_d);
+  std::vector<int32_t> d(M * N);
+  PL2_CUDA_OK(cudaMalloc(&d_a, M * K));
+  PL2_CUDA_OK(cudaMalloc(&d_b, N * K));
+  PL2_CUDA_OK(cudaMalloc(&d_d, 4ull * M * N));
+  PL2_CUDA_OK(cudaMemcpyAsync(d_a, a.data(), M * K, cudaMemcpyHostToDevice, c->stream));
+  PL2_CUDA_OK(cudaMemcpyAsync(d_b, b.data(), N * K, cudaMemcpyHostToDevice, c->stream));
+  wgmma_probe_kernel<<<1, 128, 0, c->stream>>>(d_a, d_b, d_d);
   c->launches++;
   PL2_CUDA_OK(cudaGetLastError());
-  PL2_CUDA_OK(cudaMemcpyAsync(d_out_host, d_d, 128ull * n * 4, cudaMemcpyDeviceToHost, c->stream));
+  PL2_CUDA_OK(cudaMemcpyAsync(d.data(), d_d, 4ull * M * N, cudaMemcpyDeviceToHost, c->stream));
   PL2_CUDA_OK(cudaStreamSynchronize(c->stream));
   cudaFree(d_a);
   cudaFree(d_b);
   cudaFree(d_d);
-  return 0;
-}
-
-int pl2gpu_selftest_umma(Pl2GpuCtx* ctx, int verbose) {
-  if (getenv("PL2_UMMA_BENCH")) {  // diagnostic: tcgen05.mma issue / execution rate (umma_probe.cuh)
-    Ctx* c = &ctx->c;
-    long long* d_out = nullptr;
-    PL2_CUDA_OK(cudaMalloc(&d_out, 64));
-    PL2_CUDA_OK(cudaFuncSetAttribute(umma_issue_bench_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kProbeSmemBytes));
-    const uint32_t reps = 512;
-    for (uint32_t mode = 0; mode < 4; ++mode)
-      for (uint32_t issuers = 1; issuers <= 2; ++issuers)
-        for (uint32_t n : {80u, 160u, 224u})
-          for (uint32_t ce : {0u, 1u}) {
-            if (n * issuers > 448) continue;
-            umma_issue_bench_kernel<<<1, 128, kProbeSmemBytes, c->stream>>>(n, reps, mode, issuers, ce, d_out);
-            long long h[8] = {0};
-            PL2_CUDA_OK(cudaMemcpyAsync(h, d_out, 64, cudaMemcpyDeviceToHost, c->stream));
-            PL2_CUDA_OK(cudaStreamSynchronize(c->stream));
-            printf("umma_bench style=%s mode=%s issuers=%u n=%3u commit_every=%u: issue %.1f clk/mma, complete %.1f clk/mma (floor %.0f)\n", (mode >> 1) ? "elect" : "lane0", (mode & 1) ? "TS" : "SS", issuers, n, ce, double(h[0]) / reps, double(h[1]) / reps, n / 2.0 * issuers);
-          }
-    cudaFree(d_out);
-  }
-  // Production operand layout (geno_expand.cuh operand_offset), M=128, N=96, K=64 (two k-steps).
-  const uint32_t M = 128, N = 96, K = 64;
-  const uint32_t lbo_a = operand_lbo(M), lbo_b = operand_lbo(N);
-  std::vector<uint8_t> a(M * K), b(N * K);
-  std::vector<int8_t> av(M * K), bv(N * K);
-  uint32_t seed = 12345;
-  auto rnd = [&]() {
-    seed = seed * 1664525u + 1013904223u;
-    return static_cast<int8_t>((seed >> 24) % 7) - 3;
-  };
-  for (uint32_t m = 0; m < M; ++m)
-    for (uint32_t k = 0; k < K; ++k) {
-      const int8_t v = rnd();
-      av[m * K + k] = v;
-      a[operand_offset(k, m / 16, lbo_a) + (m % 16)] = static_cast<uint8_t>(v);
-    }
-  for (uint32_t n = 0; n < N; ++n)
-    for (uint32_t k = 0; k < K; ++k) {
-      const int8_t v = rnd();
-      bv[n * K + k] = v;
-      b[operand_offset(k, n / 16, lbo_b) + (n % 16)] = static_cast<uint8_t>(v);
-    }
-  std::vector<int32_t> d(128 * N);
-  const uint32_t idesc = make_idesc_i8(M, N, true, true);
-  PL2_TRY(pl2gpu_debug_umma(ctx, a.data(), M * K, b.data(), N * K, lbo_a, kCoreBytes, lbo_b, kCoreBytes, 4 * lbo_a, 4 * lbo_b, K / 32, idesc, N, d.data()));
   uint32_t bad = 0;
   for (uint32_t m = 0; m < M; ++m)
     for (uint32_t n = 0; n < N; ++n) {
       int32_t ref = 0;
-      for (uint32_t k = 0; k < K; ++k) ref += static_cast<int32_t>(av[m * K + k]) * bv[n * K + k];
+      for (uint32_t k = 0; k < K; ++k) ref += static_cast<int32_t>(a[m * K + k]) * b[n * K + k];
       if (ref != d[m * N + n]) {
         if (verbose && bad < 8) fprintf(stderr, "selftest_umma mismatch m=%u n=%u got=%d want=%d\n", m, n, d[m * N + n], ref);
         ++bad;
@@ -1118,50 +1041,6 @@ int pl2gpu_selftest_umma(Pl2GpuCtx* ctx, int verbose) {
   if (bad) {
     set_error("pl2gpu_selftest_umma: %u of %u accumulator entries differ from the scalar reference", bad, M * N);
     return 1;
-  }
-  // TS form: same B image, A rows written to tensor memory with tcgen05.st (K-major, 4 K-bytes per column)
-  {
-    Ctx* c = &ctx->c;
-    std::vector<uint8_t> a_rows(M * K);
-    for (uint32_t m = 0; m < M; ++m)
-      for (uint32_t k = 0; k < K; ++k) a_rows[m * K + k] = static_cast<uint8_t>(av[m * K + k]);
-    UmmaProbeParams prm{};
-    prm.b_bytes = N * K;
-    prm.b_lbo = lbo_b;
-    prm.b_sbo = kCoreBytes;
-    prm.b_step_bytes = 4 * lbo_b;
-    prm.k_steps = K / 32;
-    prm.idesc = make_idesc_i8(M, N, false, true);
-    prm.n = N;
-    uint8_t *d_a = nullptr, *d_b = nullptr;
-    int32_t* d_d = nullptr;
-    PL2_CUDA_OK(cudaMalloc(&d_a, M * K));
-    PL2_CUDA_OK(cudaMalloc(&d_b, N * K));
-    PL2_CUDA_OK(cudaMalloc(&d_d, 128ull * N * 4));
-    PL2_CUDA_OK(cudaMemcpyAsync(d_a, a_rows.data(), M * K, cudaMemcpyHostToDevice, c->stream));
-    PL2_CUDA_OK(cudaMemcpyAsync(d_b, b.data(), N * K, cudaMemcpyHostToDevice, c->stream));
-    umma_probe_ts_kernel<<<1, 128, kProbeSmemBytes, c->stream>>>(d_a, d_b, prm, d_d);
-    c->launches++;
-    PL2_CUDA_OK(cudaGetLastError());
-    PL2_CUDA_OK(cudaMemcpyAsync(d.data(), d_d, 128ull * N * 4, cudaMemcpyDeviceToHost, c->stream));
-    PL2_CUDA_OK(cudaStreamSynchronize(c->stream));
-    cudaFree(d_a);
-    cudaFree(d_b);
-    cudaFree(d_d);
-    bad = 0;
-    for (uint32_t m = 0; m < M; ++m)
-      for (uint32_t n = 0; n < N; ++n) {
-        int32_t ref = 0;
-        for (uint32_t k = 0; k < K; ++k) ref += static_cast<int32_t>(av[m * K + k]) * bv[n * K + k];
-        if (ref != d[m * N + n]) {
-          if (verbose && bad < 8) fprintf(stderr, "selftest_umma(TS) mismatch m=%u n=%u got=%d want=%d\n", m, n, d[m * N + n], ref);
-          ++bad;
-        }
-      }
-    if (bad) {
-      set_error("pl2gpu_selftest_umma: TS form: %u of %u accumulator entries differ from the scalar reference", bad, M * N);
-      return 3;
-    }
   }
   return 0;
 }

@@ -82,8 +82,8 @@ class GpuContext:
     def stream(self) -> int:
         return int(lib.pl2gpu_ctx_stream(self._h) or 0)
 
-    def int8_peak(self, n_cols: int = 160, form: int = 1, min_seconds: float = 2.0):
-        """Measured chip-wide tcgen05 kind::i8 rate (TOP/s, seconds): the roofline denominator."""
+    def int8_peak(self, n_cols: int = 96, form: int = 1, min_seconds: float = 2.0):
+        """Measured chip-wide int8 wgmma rate (TOP/s, seconds): the roofline denominator."""
         tops, secs = C.c_double(), C.c_double()
         check(lib.pl2gpu_int8_peak(self._h, n_cols, form, min_seconds, C.byref(tops), C.byref(secs)), "pl2gpu_int8_peak")
         return float(tops.value), float(secs.value)

@@ -10,7 +10,7 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu on a machine that has one)")
     # built artefacts are not in git: build them once if this is a fresh checkout
     pkg = os.path.join(ROOT, "plink_ng_b200")
     if not (os.path.exists(os.path.join(pkg, "libpl2gpu.so")) and os.path.exists(os.path.join(pkg, "plink2_b200"))):
@@ -38,7 +38,7 @@ def gpu_ctx():
     import plink_ng_b200 as p
 
     if p.lib.pl2gpu_device_count() <= 0:
-        pytest.fail("no CUDA device visible: -m gpu tests need a B200 (there is no CPU fallback)")
+        pytest.fail("no CUDA device visible: -m gpu tests need an H100 (there is no CPU fallback)")
     ctx = p.GpuContext(0)
     yield ctx
     ctx.close()

@@ -139,7 +139,7 @@ $P --bfile x --keep x_keep1.txt x_keep2.txt --mind 0.05 --geno 0.05 --missing --
 # relatedness prune from a table, then --make-bed on the survivors
 $P --bfile a --king-cutoff-table $T/in.kin0 0.02 --make-bed --threads 2 --out $T/a_kctb > /dev/null
 cp $T/a_kctb.fam a_kctb.fam; cp $T/a_kctb.bed a_kctb.bed
-# the same filters / prune chaining through the device commands (tests/test_filters_gpu.py, tools/check_r2s.py)
+# the same filters / prune chaining through the device commands (tests/test_filters_gpu.py)
 XF="--keep x_keep1.txt x_keep2.txt --remove x_remove.txt --extract x_extract.txt --exclude x_exclude.txt"
 $P --bfile x $XF --make-king-table --threads 2 --out $T/g1 > /dev/null; gzip -9 -n -c $T/g1.kin0 > g_xfilt.kin0.gz
 $P --bfile x $XF --indep-pairwise 50 5 0.2 --threads 2 --out $T/g2 > /dev/null; cp $T/g2.prune.in g_xfilt.prune.in

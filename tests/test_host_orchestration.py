@@ -253,7 +253,7 @@ def test_grm_driver_and_writers_replayed_on_the_cpu(mock_so, tmp_path):
 
 def test_exact_pca_driver_and_prune_chaining_replayed_on_the_cpu(mock_so, tmp_path):
     """Exact --pca on the stand-in's eigen-solver (eigenvalues + eigenvectors up to sign vs the reference), then the two
-    chained forms checked on the B200 as well: --king-cutoff -> --make-grm-bin and --king-cutoff-table -> --pca, both with
+    chained forms also checked through the device (tests/test_filters_gpu.py): --king-cutoff -> --make-grm-bin and --king-cutoff-table -> --pca, both with
     the pre-prune allele frequencies."""
     import numpy as np
 

@@ -126,7 +126,7 @@ def test_approx_pca_k20_tensor_path_matches_oracle(gpu_ctx):
     assert np.allclose(_align(vecs[:top], want_vecs[:top]), want_vecs[:top], atol=1e-5 * np.abs(want_vecs[:top]).max())
     # The 13 noise-level eigenvalues are Ritz values over a numerically rank-deficient Krylov space (its singular
     # values span 1e35 .. 1e-4): LAPACK's SVD in the restatement, one-sided Jacobi and block Gram-Schmidt each complete
-    # the basis differently there, and the values move by 1e-4 .. 1e-3 (profiles/r02_pca_basis_compare.txt; the
+    # the basis differently there, and the values move by 1e-4 .. 1e-3 (tests/harness/pca_basis_compare.py; the
     # reference's own comparison against PLINK 1.9 allows 9e-3, 2.0/Tests/TEST_PHASED_VCF/run_tests.sh:76-99).
     assert np.allclose(vals[top:], want_vals[top:], rtol=3e-3)
 

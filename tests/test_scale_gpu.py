@@ -1,15 +1,18 @@
-"""GPU: parity AT SCALE, through the product (the plink2_b200 host program), against the UNMODIFIED reference
-binary run on this box on the same files (oracle/_ref/plink2[_lapack], built by oracle/build_ref.sh; it
-travels to the GPU box with the snapshot).  Inputs come from the reference's own generator
-(`--dummy`, 2.0/plink2_import.cc:16326-16460) so both programs read identical bytes.
+"""GPU: parity AT SCALE, through the product (the plink2_b200 host program), against what the UNMODIFIED reference
+binary (oracle/_ref/plink2[_lapack]) wrote for the same seeded filesets (oracle/synth.py).  The reference's
+outputs are stored under tests/golden/ by oracle/make_scale_golden.py: SHA-256 digests of every byte-exact file
+and a seeded sample of the fp32 GRM.
 
 Sizes are the ones SURVEY.md 8(c) names for the smoke set: 4,096 samples x 65,536 variants (32 row tiles x
 up to 52 column tiles, two 32,768-variant batches for GRM / several for KING), plus a 20,000-sample KING
 run (157 row tiles) that pins tile placement and orientation pair by pair, and a forced multipass run.
 """
+import hashlib
+import json
 import os
 import re
 import subprocess
+import sys
 
 import numpy as np
 import pytest
@@ -17,10 +20,10 @@ import pytest
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 BIN = os.path.join(ROOT, "plink_ng_b200", "plink2_b200")
-REF = os.path.join(ROOT, "oracle", "_ref", "plink2")
-REF_LAPACK = os.path.join(ROOT, "oracle", "_ref", "plink2_lapack")
 ENV = dict(os.environ, CUDA_VISIBLE_DEVICES=os.environ.get("CUDA_VISIBLE_DEVICES", "0").split(",")[0])
-THREADS = str(max(1, min(32, len(os.sched_getaffinity(0)))))
+GOLD = json.load(open(os.path.join(ROOT, "tests", "golden", "scale_reference.json")))
+sys.path.insert(0, ROOT)
+from oracle.synth import write_bed  # noqa: E402
 
 
 def sh(cmd, env=None, ok=(0,)):
@@ -29,84 +32,63 @@ def sh(cmd, env=None, ok=(0,)):
     return r
 
 
-def need(path):
-    if not os.path.exists(path):
-        pytest.fail(f"{path} is missing: run oracle/build_ref.sh where /root/reference exists (it travels with the snapshot)")
+def sha256(path):
+    h = hashlib.sha256()
+    with open(path, "rb") as f:
+        for chunk in iter(lambda: f.read(1 << 24), b""):
+            h.update(chunk)
+    return h.hexdigest()
 
 
-def same_file(a, b, chunk=1 << 26):
-    if os.path.getsize(a) != os.path.getsize(b):
-        return False
-    with open(a, "rb") as fa, open(b, "rb") as fb:
-        while True:
-            x, y = fa.read(chunk), fb.read(chunk)
-            if x != y:
-                return False
-            if not x:
-                return True
+def assert_same_as_reference(prefix, digests):
+    """Every file prefix + ext byte-identical to the reference's (SHA-256 of the reference's file)."""
+    bad = [ext for ext, want in digests.items() if sha256(prefix + ext) != want]
+    assert not bad, f"differ from the reference's output: {', '.join(prefix + e for e in bad)}"
 
 
-def assert_same_text(ref, got):
-    """Byte-identical text files; on mismatch say where (line counts, first differing line)."""
-    if same_file(ref, got):
-        return
-    a, b = open(ref, "rb").read().split(b"\n"), open(got, "rb").read().split(b"\n")
-    k = next((i for i, (x, y) in enumerate(zip(a, b)) if x != y), min(len(a), len(b)))
-    ndiff = sum(1 for x, y in zip(a, b) if x != y)
-    raise AssertionError(f"{got} differs from {ref}: {len(a)} vs {len(b)} lines, {ndiff} differing among the common ones, first at line {k + 1}:\n"
-                         f"  ref: {a[k][:200] if k < len(a) else None}\n  got: {b[k][:200] if k < len(b) else None}\n"
-                         f"  ref prev: {a[k - 1][:200] if k else None}\n  ref next: {a[k + 1][:200] if k + 1 < len(a) else None}\n  got next: {b[k + 1][:200] if k + 1 < len(b) else None}")
+def fileset(tmp_path, name):
+    pre = str(tmp_path / name)
+    write_bed(pre, *GOLD["sets"][name])
+    return pre
 
 
 @pytest.fixture(scope="module")
 def dummy4k(tmp_path_factory):
-    need(REF)
-    d = tmp_path_factory.mktemp("scale4k")
-    pre = str(d / "d")
-    sh([REF, "--dummy", "4096", "65536", "0.01", "--seed", "1", "--threads", "4", "--make-bed", "--out", pre])
-    return pre
+    return fileset(tmp_path_factory.mktemp("scale4k"), "d4k")
 
 
 def test_king_table_and_matrix_4096x65536_byte_identical(dummy4k, tmp_path):
     """Every .kin0 count column (NSNP HETHET IBS0 HET1_HOM2 HET2_HOM1 IBS KINSHIP) on a NON-EMPTY filtered table
-    (>= 1e5 rows) plus the whole fp32 kinship triangle, byte for byte."""
-    ref, out = str(tmp_path / "ref"), str(tmp_path / "b200")
-    sh([REF, "--bfile", dummy4k, "--make-king", "bin4", "triangle", "--threads", THREADS, "--out", ref])
-    kin = np.fromfile(ref + ".king.bin", dtype=np.float32)
-    assert kin.size == 4096 * 4095 // 2
-    thr = repr(float(np.quantile(kin.astype(np.float64), 0.97)))
-    flags = ["--make-king-table", "counts", "cols=+ibs1,+ibs", "--king-table-filter", thr]
-    sh([REF, "--bfile", dummy4k] + flags + ["--threads", THREADS, "--out", ref])
+    (>= 1e5 rows; the filter is the 97 % quantile of the reference's kinships) plus the whole fp32 kinship triangle,
+    byte for byte."""
+    gold = GOLD["king4k"]
+    out = str(tmp_path / "b200")
+    flags = ["--make-king-table", "counts", "cols=+ibs1,+ibs", "--king-table-filter", gold["filter"]]
     sh([BIN, "--bfile", dummy4k] + flags + ["--make-king", "bin4", "triangle", "--out", out], env=ENV)
-    rows = sum(1 for _ in open(ref + ".kin0")) - 1
-    assert rows >= 100_000, rows
-    assert same_file(ref + ".king.bin", out + ".king.bin")
-    assert same_file(ref + ".king.id", out + ".king.id")
-    assert_same_text(ref + ".kin0", out + ".kin0")
+    assert gold["kin0_rows"] >= 100_000
+    assert os.path.getsize(out + ".king.bin") == 4 * (4096 * 4095 // 2)
+    rows = sum(1 for _ in open(out + ".kin0")) - 1
+    assert rows == gold["kin0_rows"], rows
+    assert_same_as_reference(out, gold["sha256"])
 
 
 def test_king_matrix_20000_samples_pairwise(tmp_path):
     """157 row tiles x up to 250 column tiles: the whole 2e8-pair fp32 kinship triangle against the reference's, so a
     tile-placement or orientation error anywhere in the triangle fails (the marginal-sum test cannot see those)."""
-    need(REF)
-    pre, ref, out = str(tmp_path / "d"), str(tmp_path / "ref"), str(tmp_path / "b200")
-    sh([REF, "--dummy", "20000", "2048", "0.02", "--seed", "5", "--threads", "4", "--make-bed", "--out", pre])
-    sh([REF, "--bfile", pre, "--make-king", "bin4", "triangle", "--threads", THREADS, "--out", ref])
+    pre, out = fileset(tmp_path, "d20k"), str(tmp_path / "b200")
     sh([BIN, "--bfile", pre, "--make-king", "bin4", "triangle", "--out", out], env=ENV)
-    assert os.path.getsize(ref + ".king.bin") == 4 * (20000 * 19999 // 2)
-    assert same_file(ref + ".king.bin", out + ".king.bin")
+    assert os.path.getsize(out + ".king.bin") == 4 * (20000 * 19999 // 2)
+    assert_same_as_reference(out, GOLD["king20k"]["sha256"])
 
 
 def test_king_forced_multipass_matches_single_pass(tmp_path):
     """--gpu-memory caps the device budget so RunKing needs >= 3 row-block passes (the reference's
     CountTrianglePasses behaviour, 2.0/plink2_matrix_calc.cc:216-255); outputs must not change."""
-    need(REF)
-    pre, ref, one = str(tmp_path / "d"), str(tmp_path / "ref"), str(tmp_path / "one")
-    sh([REF, "--dummy", "3000", "4096", "0.02", "--seed", "9", "--threads", "4", "--make-bed", "--out", pre])
+    pre, one = fileset(tmp_path, "d3k"), str(tmp_path / "one")
+    digests = GOLD["king3k"]["sha256"]
     flags = ["--make-king", "bin", "triangle", "--make-king-table", "counts", "--king-table-filter", "-0.05"]
-    sh([REF, "--bfile", pre] + flags + ["--threads", THREADS, "--out", ref])
     sh([BIN, "--bfile", pre] + flags + ["--out", one], env=ENV)
-    assert same_file(ref + ".king.bin", one + ".king.bin") and same_file(ref + ".kin0", one + ".kin0")
+    assert_same_as_reference(one, digests)
     passes = 0
     for mib in (640, 560, 500, 470, 450, 435, 425, 415):
         multi = str(tmp_path / f"multi{mib}")
@@ -115,36 +97,32 @@ def test_king_forced_multipass_matches_single_pass(tmp_path):
             break  # below the fixed staging buffers: nothing smaller can work
         m = re.search(r"(\d+) passes over the variants", r.stdout)
         passes = int(m.group(1)) if m else 1
-        assert same_file(ref + ".king.bin", multi + ".king.bin"), mib
-        assert same_file(ref + ".kin0", multi + ".kin0"), mib
+        assert_same_as_reference(multi, digests)
         if passes >= 3:
             break
     assert passes >= 3, f"no --gpu-memory value produced >= 3 passes (last: {passes})"
 
 
 def test_grm_4096x65536_vs_reference_blas(dummy4k, tmp_path):
-    """.grm.bin against the LAPACK build of the reference (threaded OpenBLAS dsyrk in fp64) within 1e-5 relative,
-    .grm.N.bin (per-pair observation counts) and .grm.id exactly."""
-    need(REF_LAPACK)
-    ref, out = str(tmp_path / "ref"), str(tmp_path / "b200")
-    sh([REF_LAPACK, "--bfile", dummy4k, "--make-grm-bin", "--threads", THREADS, "--out", ref])
+    """.grm.bin against the LAPACK build of the reference (threaded OpenBLAS dsyrk in fp64) within 1e-5 relative on a
+    seeded sample of 20,000 entries, .grm.N.bin (per-pair observation counts) and .grm.id exactly."""
+    gold = GOLD["grm4k"]
+    out = str(tmp_path / "b200")
     sh([BIN, "--bfile", dummy4k, "--make-grm-bin", "--out", out], env=ENV)
-    a = np.fromfile(ref + ".grm.bin", dtype=np.float32).astype(np.float64)
     b = np.fromfile(out + ".grm.bin", dtype=np.float32).astype(np.float64)
-    assert a.size == b.size == 4096 * 4097 // 2
+    assert b.size == gold["entries"] == 4096 * 4097 // 2
+    idx = np.sort(np.random.default_rng(gold["sample_seed"]).choice(b.size, gold["sample"], replace=False))
+    a = np.load(os.path.join(ROOT, "tests", "golden", "scale_grm_sample.npy")).astype(np.float64)
     # fp32 payload: half an ulp of the stored value (6e-8 relative) on top of the 1e-5 relative contract
-    assert np.allclose(b, a, rtol=1e-5, atol=2e-8), float(np.max(np.abs(a - b)))
-    assert same_file(ref + ".grm.N.bin", out + ".grm.N.bin")
-    assert same_file(ref + ".grm.id", out + ".grm.id")
+    assert np.allclose(b[idx], a, rtol=1e-5, atol=2e-8), float(np.max(np.abs(a - b[idx])))
+    assert_same_as_reference(out, gold["sha256"])
 
 
 def test_indep_pairwise_500_50_02_keep_list_4096x65536(dummy4k, tmp_path):
     """The BASELINE config-4 command on the 65,536-variant set: .prune.in / .prune.out byte-identical."""
-    ref, out = str(tmp_path / "ref"), str(tmp_path / "b200")
-    flags = ["--indep-pairwise", "500", "50", "0.2"]
-    sh([REF, "--bfile", dummy4k] + flags + ["--threads", THREADS, "--out", ref])
-    sh([BIN, "--bfile", dummy4k] + flags + ["--out", out], env=ENV)
-    kept = sum(1 for _ in open(ref + ".prune.in"))
-    assert 10_000 < kept < 60_000, kept
-    assert same_file(ref + ".prune.in", out + ".prune.in")
-    assert same_file(ref + ".prune.out", out + ".prune.out")
+    gold = GOLD["prune4k"]
+    out = str(tmp_path / "b200")
+    sh([BIN, "--bfile", dummy4k, "--indep-pairwise", "500", "50", "0.2", "--out", out], env=ENV)
+    assert 10_000 < gold["kept"] < 60_000, gold["kept"]
+    assert sum(1 for _ in open(out + ".prune.in")) == gold["kept"]
+    assert_same_as_reference(out, gold["sha256"])
