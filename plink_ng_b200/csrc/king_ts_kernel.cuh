@@ -2,20 +2,24 @@
 //
 //   D[r][c] += sum_v A_plane[r][v] * B_plane[c][v],  planes T (het), H (hom), S (+1 hom-REF / -1 hom-ALT),
 // exact int32 sums, the raw accumulator semantics of king_kernels.cuh.  One CTA = 64 rows (half of a 128-row
-// pair tile) x kCols columns, two warpgroups:
-//   warpgroup 0:  T_I x T_J -> TT,  T_I x H_J -> TH,  S_I x S_J, columns [0, kS)
-//   warpgroup 1:  H_I x T_J -> HT,  H_I x H_J -> HH,  S_I x S_J, columns [kCols - kS, kCols)
-// so that each thread keeps ~100-120 int32 accumulators in registers for the whole variant loop (the 64 x 5 kCols
-// accumulators of a half tile are 100-120 KB; a whole 128-row tile would not fit the register file).  Both
-// warpgroups issue the same shapes (ptxas serialises a wgmma under a branch), so for 80 columns the S x S halves
-// overlap by 16 columns and warpgroup 1 stores only its last 32.
+// pair tile) x kCols columns, three warpgroups:
+//   warpgroup 0:  producer - stages the operands of the variant loop in a ring of shared-memory stages
+//   warpgroup 1:  T_I x T_J -> TT,  T_I x H_J -> TH,  S_I x S_J, columns [0, kS)
+//   warpgroup 2:  H_I x T_J -> HT,  H_I x H_J -> HH,  S_I x S_J, columns [kCols - kS, kCols)
+// so that each consumer thread keeps ~100-120 int32 accumulators in registers for the whole variant loop (the
+// 64 x 5 kCols accumulators of a half tile are 100-120 KB; a whole 128-row tile would not fit the register file).
+// Both consumers issue the same shapes (ptxas serialises a wgmma under a branch), so for 80 columns the S x S
+// halves overlap by 16 columns and warpgroup 2 stores only its last 32.
 //
 // Both operands come from the sample-major copy of the staged block written by geno_tile_rows_kernel
 // (raw_t[sample / 128][k-step][sample % 128][8 bytes = 32 variants]): K-major, which is what an 8-bit wgmma
-// reads.  Row side (A): each thread expands only its own fragment bytes straight into registers (wgmma.cuh).
-// Column side (B): all 256 threads expand the 3 planes of the kCols column samples into the K-major no-swizzle
-// layout in shared memory, one 256-variant stage ahead of the tensor pipe (double buffer, one __syncthreads per
-// stage); the row-side words of the stage are copied next to it.
+// reads.  Column side (B): the producer loads the words of the kCols column samples one stage ahead in registers
+// and expands them into the 3 planes, K-major no-swizzle layout; it copies the stage's row-side words next to
+// them.  Row side (A): each consumer thread expands only its own fragment bytes from those words straight into
+// registers (wgmma.cuh).  Each stage has a `full` mbarrier (the producer's 128 threads arrive after their
+// stores) and an `empty` one (the consumers' 256 threads arrive once every wgmma reading the stage has
+// retired), so the staging runs on its own warps while the consumers keep one wgmma group in flight across
+// stage boundaries; nothing in the variant loop waits for the whole CTA.
 #pragma once
 
 #include "common.cuh"
@@ -28,22 +32,32 @@ namespace pl2 {
 constexpr uint32_t kTsAccCols = 5 * kTsCols;   // 400
 constexpr uint32_t kTsTileAccWords = kTsAccCols * kTileRows;
 
-constexpr uint32_t kKwKs = 8;                    // k32 steps per shared-memory stage (256 variants)
-constexpr uint32_t kKwThreads = 256;             // two warpgroups
-constexpr uint32_t kKwChunkBytes = 128;          // LBO: next 16-variant chunk (core matrix) of the same 8 samples
-constexpr uint32_t kKwSbo = 2 * kKwKs * kKwChunkBytes;  // 2048: next group of 8 samples
-constexpr uint32_t kKwABytes = kKwKs * 64 * 8;   // row-side words of one stage: [k-step][64 rows][8 B]
+constexpr uint32_t kKwProducerThreads = 128;  // warpgroup 0
+constexpr uint32_t kKwConsumerThreads = 256;  // warpgroups 1, 2
+constexpr uint32_t kKwThreads = kKwProducerThreads + kKwConsumerThreads;
+constexpr uint32_t kKwChunkBytes = 128;       // LBO: next 16-variant chunk (core matrix) of the same 8 samples
+constexpr uint32_t kKwSmemLimit = 232448;     // the 227 KB shared-memory opt-in
 
 template <uint32_t kCols>
 struct KingWgShape {
-  static constexpr uint32_t kBBytes = 3 * kCols * 32 * kKwKs;  // planes T | H | S stacked along N
-  static constexpr uint32_t kStageBytes = kBBytes + kKwABytes;
-  static constexpr uint32_t kSmemBytes = 2 * kStageBytes + 128;
-  static constexpr uint32_t kS = (kCols / 2 + 15) / 16 * 16;  // S x S columns per warpgroup (wgmma N: multiple of 16)
-  static constexpr uint32_t kItems = kCols * kKwKs;             // (column sample, k-step) words per stage
-  static constexpr uint32_t kItemsPerThread = (kItems + kKwThreads - 1) / kKwThreads;
+  // k32 steps per stage: 8 (256 variants) where three such stages fit the opt-in, else 4; both divide the
+  // 256-variant padding unit
+  static constexpr uint32_t stage_bytes(uint32_t ks) { return 3 * kCols * 32 * ks + ks * 64 * 8; }
+  static constexpr uint32_t kKs = 3 * stage_bytes(8) + 256 <= kKwSmemLimit ? 8 : 4;
+  static constexpr uint32_t kSbo = 2 * kKs * kKwChunkBytes;          // next group of 8 samples
+  static constexpr uint32_t kBBytes = 3 * kCols * 32 * kKs;          // planes T | H | S stacked along N
+  static constexpr uint32_t kABytes = kKs * 64 * 8;                  // row-side words: [k-step][64 rows][8 B]
+  static constexpr uint32_t kStageBytes = kBBytes + kABytes;
+  static constexpr uint32_t kStages = (kKwSmemLimit - 256) / kStageBytes < 4 ? (kKwSmemLimit - 256) / kStageBytes : 4;
+  static constexpr uint32_t kSmemBytes = kStages * kStageBytes + 128 + 2 * kStages * 8;  // + alignment + mbarriers
+  static constexpr uint32_t kS = (kCols / 2 + 15) / 16 * 16;  // S x S columns per consumer (wgmma N: multiple of 16)
+  static constexpr uint32_t kItems = kCols * kKs;              // (column sample, k-step) words per stage
+  static constexpr uint32_t kItemsPerThread = (kItems + kKwProducerThreads - 1) / kKwProducerThreads;
+  static constexpr uint32_t kAPerThread = kABytes / 16 / kKwProducerThreads;  // 16-byte pieces of the row-side words
   static_assert(kCols % 16 == 0 && 2 * kS >= kCols, "wgmma N");
-  static_assert(kSmemBytes <= 232448, "exceeds the 227 KB shared-memory opt-in limit");
+  static_assert(kStages >= 3, "the ring needs at least three stages");
+  static_assert(kABytes % (16 * kKwProducerThreads) == 0, "row-side copy");
+  static_assert(kSmemBytes <= kKwSmemLimit, "exceeds the 227 KB shared-memory opt-in limit");
 };
 
 template <int N>
@@ -70,95 +84,128 @@ king_wg_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t tid = threadIdx.x;
   const uint32_t wg = tid >> 7;
-  const uint32_t warp4 = (tid >> 5) & 3;
-  const uint32_t lane = tid & 31;
-  const uint32_t g = lane >> 2, c = lane & 3;
   const uint32_t tile = tile_order[blockIdx.x >> 1];
   const uint32_t half = blockIdx.x & 1;
   const uint32_t rt = tile_rt[tile];
   const uint32_t ct = tile_tc[tile];
   const uint32_t kstep_ct = variant_ct_padded / 32;
-  const uint32_t stage_ct = kstep_ct / kKwKs;
+  const uint32_t stage_ct = kstep_ct / S::kKs;
   const uint32_t smem_base = (static_cast<uint32_t>(__cvta_generic_to_shared(smem)) + 127u) & ~127u;
+  const uint32_t bar_full = smem_base + S::kStages * S::kStageBytes;  // full[s] = bar_full + 8 s
+  const uint32_t bar_empty = bar_full + S::kStages * 8;               // empty[s] = bar_empty + 8 s
+  if (tid == 0) {
+    for (uint32_t s = 0; s < S::kStages; ++s) {
+      mbar_init(bar_full + 8 * s, kKwProducerThreads);
+      mbar_init(bar_empty + 8 * s, kKwConsumerThreads);
+    }
+  }
+  __syncthreads();
 
   const uint32_t thread_zero = tid * (variant_ct_padded >> 31);  // 0; keeps the plane tables in vector registers
   const uint32_t tab_t = table_reg(kTabHet, thread_zero), tab_h = table_reg(kTabHom, thread_zero), tab_s = table_reg(kTabSgn, thread_zero);
 
-  // ---- staging: this thread's share of a stage (column-side words + one 16-byte piece of the row-side words)
-  const uint8_t* a_src = raw_t + static_cast<uint64_t>(rt) * kstep_ct * 1024 + half * 512 + (tid >> 5) * 1024 + (tid & 31) * 16;
-  // tid / 32 = k-step of the stage, (tid % 32) * 16 = byte of the 512-byte half row block
-  struct Pre {
-    uint2 w[S::kItemsPerThread];
-    uint4 a;
-  };
-  auto load_stage = [&](uint32_t st) -> Pre {
-    Pre p;
+  if (wg == 0) {
+    // ---- producer: this thread's share of a stage (column-side words + 16-byte pieces of the row-side words)
+    // Item i of a stage = (column sample n, k-step ks); its global word and its shared-memory rows move by a
+    // whole stage from one stage to the next, so both offsets are computed once.
+    const uint8_t* w_src[S::kItemsPerThread];
+    uint32_t w_dst[S::kItemsPerThread];  // plane T, first 16 variants; H and S follow kCols rows apart
 #pragma unroll
     for (uint32_t q = 0; q < S::kItemsPerThread; ++q) {
-      const uint32_t i = tid + q * kKwThreads;
-      p.w[q] = make_uint2(0xFFFFFFFFu, 0xFFFFFFFFu);
-      if (i < S::kItems) {
-        const uint32_t n = (i & 7) | (((i >> 3) % (kCols / 8)) << 3);
-        const uint32_t ks = st * kKwKs + (i >> 3) / (kCols / 8);
-        const uint32_t s = kCols * ct + n;
-        p.w[q] = __ldg(reinterpret_cast<const uint2*>(raw_t + (static_cast<uint64_t>(s >> 7) * kstep_ct + ks) * 1024 + (s & 127) * 8));
-      }
+      const uint32_t i = tid + q * kKwProducerThreads;
+      const uint32_t n = (i & 7) | (((i >> 3) % (kCols / 8)) << 3);
+      const uint32_t ks = (i >> 3) / (kCols / 8);
+      const uint32_t s = kCols * ct + n;
+      w_src[q] = raw_t + (static_cast<uint64_t>(s >> 7) * kstep_ct + ks) * 1024 + (s & 127) * 8;
+      w_dst[q] = (n >> 3) * S::kSbo + 2 * ks * kKwChunkBytes + (n & 7) * 16;
     }
-    p.a = __ldg(reinterpret_cast<const uint4*>(a_src + static_cast<uint64_t>(st) * kKwKs * 1024));
-    return p;
-  };
-  auto store_stage = [&](const Pre& p, uint32_t buf) {
-    const uint32_t base = smem_base + buf * S::kStageBytes;
+    auto has_item = [&](uint32_t q) { return S::kItems % kKwProducerThreads == 0 || tid + q * kKwProducerThreads < S::kItems; };
+    const uint8_t* a_src = raw_t + static_cast<uint64_t>(rt) * kstep_ct * 1024 + half * 512;
+    struct Pre {
+      uint2 w[S::kItemsPerThread];
+      uint4 a[S::kAPerThread];
+    };
+    auto load_stage = [&](uint32_t st) -> Pre {
+      Pre p;
+      const uint64_t stage_off = static_cast<uint64_t>(st) * S::kKs * 1024;
 #pragma unroll
-    for (uint32_t q = 0; q < S::kItemsPerThread; ++q) {
-      const uint32_t i = tid + q * kKwThreads;
-      if (i < S::kItems) {
-        const uint32_t n = (i & 7) | (((i >> 3) % (kCols / 8)) << 3);
-        const uint32_t ks = (i >> 3) / (kCols / 8);
-        const uint32_t tabs[3] = {tab_t, tab_h, tab_s};
+      for (uint32_t q = 0; q < S::kItemsPerThread; ++q) {
+        p.w[q] = make_uint2(0xFFFFFFFFu, 0xFFFFFFFFu);
+        if (has_item(q)) p.w[q] = __ldg(reinterpret_cast<const uint2*>(w_src[q] + stage_off));
+      }
 #pragma unroll
-        for (uint32_t h = 0; h < 2; ++h) {
-          const Sel4 sel = make_selectors(h ? p.w[q].y : p.w[q].x);
+      for (uint32_t q = 0; q < S::kAPerThread; ++q) {
+        const uint32_t i = tid + q * kKwProducerThreads;  // i / 32 = k-step of the stage, (i % 32) * 16 = byte of the 512-byte half row block
+        p.a[q] = __ldg(reinterpret_cast<const uint4*>(a_src + stage_off + (i >> 5) * 1024 + (i & 31) * 16));
+      }
+      return p;
+    };
+    auto store_stage = [&](const Pre& p, uint32_t base) {
+      const uint32_t tabs[3] = {tab_t, tab_h, tab_s};
 #pragma unroll
-          for (uint32_t pl = 0; pl < 3; ++pl) {
-            const uint32_t row = pl * kCols + n;
-            const uint32_t addr = base + (row >> 3) * kKwSbo + (2 * ks + h) * kKwChunkBytes + (row & 7) * 16;
-            const uint4 v = expand16(tabs[pl], sel);
-            asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+      for (uint32_t q = 0; q < S::kItemsPerThread; ++q) {
+        if (has_item(q)) {
+          const uint32_t addr = base + w_dst[q];
+#pragma unroll
+          for (uint32_t h = 0; h < 2; ++h) {
+            const Sel4 sel = make_selectors(h ? p.w[q].y : p.w[q].x);
+#pragma unroll
+            for (uint32_t pl = 0; pl < 3; ++pl) {
+              const uint4 v = expand16(tabs[pl], sel);
+              asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + pl * (kCols / 8) * S::kSbo + h * kKwChunkBytes), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
+            }
           }
         }
       }
-    }
-    const uint32_t a_addr = base + S::kBBytes + tid * 16;
-    asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(a_addr), "r"(p.a.x), "r"(p.a.y), "r"(p.a.z), "r"(p.a.w) : "memory");
-  };
+#pragma unroll
+      for (uint32_t q = 0; q < S::kAPerThread; ++q) {
+        const uint32_t a_addr = base + S::kBBytes + (tid + q * kKwProducerThreads) * 16;
+        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(a_addr), "r"(p.a[q].x), "r"(p.a[q].y), "r"(p.a[q].z), "r"(p.a[q].w) : "memory");
+      }
+    };
 
+    // Words are loaded two stages ahead and issued after the previous stage's hand-off: the proxy fence (a
+    // MEMBAR.ALL.CTA in SASS) waits for every memory access of this thread in flight, so loads issued just before
+    // it would hold up the hand-off.  Near the end the last stage is loaded again; it is never stored twice.
+    const uint32_t last = stage_ct - 1;
+    Pre cur = load_stage(0), next = load_stage(last ? 1 : 0);
+    uint32_t slot = 0, phase = 0;
+    for (uint32_t st = 0; st < stage_ct; ++st) {
+      // the first pass over the ring finds every slot free: parity 1 is the phase before a fresh barrier's first
+      mbar_wait(bar_empty + 8 * slot, phase ^ 1);
+      store_stage(cur, smem_base + slot * S::kStageBytes);
+      fence_proxy_async_smem();  // this thread's st.shared -> visible to the consumers' wgmma operand fetch
+      mbar_arrive(bar_full + 8 * slot);
+      cur = next;
+      next = load_stage(st + 2 < last ? st + 2 : last);
+      if (++slot == S::kStages) slot = 0, phase ^= 1;
+    }
+    return;
+  }
+
+  // ---- consumers
+  const uint32_t cw = wg - 1;  // 0: T_I rows, 1: H_I rows
+  const uint32_t warp4 = (tid >> 5) & 3;
+  const uint32_t lane = tid & 31;
+  const uint32_t g = lane >> 2, c = lane & 3;
   int32_t acc_x[kCols / 2], acc_y[kCols / 2], acc_s[S::kS / 2];
 #pragma unroll
   for (uint32_t i = 0; i < kCols / 2; ++i) acc_x[i] = acc_y[i] = 0;
 #pragma unroll
   for (uint32_t i = 0; i < S::kS / 2; ++i) acc_s[i] = 0;
-  const uint32_t s_first = wg ? kCols - S::kS : 0;  // first S x S column of this warpgroup
+  const uint32_t s_first = cw ? kCols - S::kS : 0;  // first S x S column of this warpgroup
 
-  const uint32_t tab_a = wg ? tab_h : tab_t;
+  const uint32_t tab_a = cw ? tab_h : tab_t;
   const uint32_t r_lo = 16 * warp4 + g;  // this thread's fragment rows r_lo, r_lo + 8 of the 64-row half
 
-  {
-    const Pre p0 = load_stage(0);
-    store_stage(p0, 0);
-  }
+  uint32_t slot = 0, phase = 0, prev_slot = 0;
   for (uint32_t st = 0; st < stage_ct; ++st) {
-    const uint32_t buf = st & 1;
-    Pre next;
-    const bool more = st + 1 < stage_ct;
-    if (more) next = load_stage(st + 1);
-    fence_proxy_async_smem();
-    __syncthreads();  // stage st complete in shared memory; every wgmma of stage st - 1 (other buffer) has retired
-    const uint32_t base = smem_base + buf * S::kStageBytes;
-    const uint64_t desc_t = make_wg_desc(base, kKwChunkBytes, kKwSbo);
-    constexpr uint32_t kPlaneStep = (kCols / 8) * kKwSbo;
+    mbar_wait(bar_full + 8 * slot, phase);
+    const uint32_t base = smem_base + slot * S::kStageBytes;
+    const uint64_t desc_t = make_wg_desc(base, kKwChunkBytes, S::kSbo);
+    constexpr uint32_t kPlaneStep = (kCols / 8) * S::kSbo;
 #pragma unroll
-    for (uint32_t ks = 0; ks < kKwKs; ++ks) {
+    for (uint32_t ks = 0; ks < S::kKs; ++ks) {
       const uint32_t a_row = base + S::kBBytes + ks * 512;
       uint2 w_lo, w_hi;
       asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w_lo.x), "=r"(w_lo.y) : "r"(a_row + r_lo * 8) : "memory");
@@ -171,21 +218,24 @@ king_wg_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
       wgmma_fence();
       wgmma_s8_rs<kCols>(acc_x, fa, dk);                                   // x T_J
       wgmma_s8_rs<kCols>(acc_y, fa, dk + (kPlaneStep >> 4));               // x H_J
-      wgmma_s8_rs<S::kS>(acc_s, fs, dk + ((2 * kPlaneStep + (s_first / 8) * kKwSbo) >> 4));
+      wgmma_s8_rs<S::kS>(acc_s, fs, dk + ((2 * kPlaneStep + (s_first / 8) * S::kSbo) >> 4));
       wgmma_commit();
       wgmma_wait<1>();
-      if (ks == kKwKs / 2 && more) store_stage(next, buf ^ 1);  // the other buffer: its wgmmas retired before the barrier
+      // every group but the one just issued has retired, the previous stage's last one included: hand that slot back
+      if (ks == 0 && st > 0) mbar_arrive(bar_empty + 8 * prev_slot);
     }
-    wgmma_wait<0>();
+    prev_slot = slot;
+    if (++slot == S::kStages) slot = 0, phase ^= 1;
   }
+  wgmma_wait<0>();
 
   // ---- epilogue: registers -> raw accumulators (+=); rows are in natural sample order
   int32_t* acc_tile = raw_acc + static_cast<uint64_t>(tile) * (5ull * kCols * kTileRows);
   const uint32_t r = 64 * half + r_lo;
-  king_acc_add<kCols>(acc_tile + static_cast<uint64_t>((wg ? 2 : 0) * kCols) * kTileRows, acc_x, r, c);  // TT | HT
-  king_acc_add<kCols>(acc_tile + static_cast<uint64_t>((wg ? 3 : 1) * kCols) * kTileRows, acc_y, r, c);  // TH | HH
-  // warpgroup 1 skips the columns warpgroup 0 already covers
-  king_acc_add<S::kS>(acc_tile + static_cast<uint64_t>(4 * kCols + s_first) * kTileRows, acc_s, r, c, wg ? static_cast<int>((2 * S::kS - kCols) / 8) : 0);
+  king_acc_add<kCols>(acc_tile + static_cast<uint64_t>((cw ? 2 : 0) * kCols) * kTileRows, acc_x, r, c);  // TT | HT
+  king_acc_add<kCols>(acc_tile + static_cast<uint64_t>((cw ? 3 : 1) * kCols) * kTileRows, acc_y, r, c);  // TH | HH
+  // warpgroup 2 skips the columns warpgroup 1 already covers
+  king_acc_add<S::kS>(acc_tile + static_cast<uint64_t>(4 * kCols + s_first) * kTileRows, acc_s, r, c, cw ? static_cast<int>((2 * S::kS - kCols) / 8) : 0);
 }
 
 }  // namespace pl2

@@ -28,6 +28,31 @@ __device__ __forceinline__ void wgmma_wait() {
 // generic-proxy st.shared -> visible to the async proxy (wgmma operand fetch)
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
+// Shared-memory mbarriers (CTA scope) for producer / consumer rings.  `bar` is a shared-window address, 8-byte
+// aligned; arrive releases and a successful try_wait acquires, so stores before an arrive are visible after the wait.
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("{\n\t.reg .b64 state;\n\tmbarrier.arrive.shared::cta.b64 state, [%0];\n\t}" ::"r"(bar) : "memory");
+}
+// true once the phase of the given parity has completed (parity = 1 on a fresh barrier: the phase before its first)
+__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
+  uint32_t done;
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+      "selp.u32 %0, 1, 0, p;\n\t}"
+      : "=r"(done)
+      : "r"(bar), "r"(parity)
+      : "memory");
+  return done != 0;
+}
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+  while (!mbar_try_wait(bar, parity)) {
+  }
+}
+
 // A fragment of one k32 step (m64nNk32, 8-bit): thread (warp w of the warpgroup, lane = 4 g + c) holds rows
 // 16 w + g and 16 w + g + 8, K bytes 4 c .. 4 c + 3 (regs 0, 1) and 16 + 4 c .. 16 + 4 c + 3 (regs 2, 3).
 // From the sample-major 2-bit words of its two rows (8 bytes = 32 variants each) the thread expands only its
