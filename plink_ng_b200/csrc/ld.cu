@@ -2,7 +2,6 @@
 // host-side greedy window walk (function face of LdPrune/IndepPairwise, 2.0/plink2_ld.cc:2530, :1116).
 #include <algorithm>
 #include <cmath>
-#include <cstring>
 #include <vector>
 
 #include "../../include/plink2_b200.h"
@@ -79,28 +78,22 @@ int pl2gpu_ld_band_flags(Pl2GpuCtx* ctx, const void* genovecs, uint64_t variant_
   }
   Ctx* c = &ctx->c;
   PL2_CUDA_OK(cudaSetDevice(c->device));
-  // PL2_LD_ALGO=popcount selects the bit-plane popcount kernel (ld_kernels.cuh), kept as an independent cross-check
-  // of the default tensor kernel (ld_ts_kernel.cuh); both produce the same exact integer sums.
-  const char* algo_env = getenv("PL2_LD_ALGO");
-  const bool use_popc = algo_env && !strcmp(algo_env, "popcount");
   const uint32_t band_r = RoundUpU32(band, 64);
   const uint32_t rows_cap = kLdChunkVariants + band_r;
   // two staged chunks: the copy of chunk k+1 (prep stream) overlaps the pair kernel of chunk k; flags come back
   // through two pinned-size device buffers in the same rhythm
   GenoStage st[2];
-  DevBuf d_planes, d_flags[2];
-  cudaEvent_t ev_copied[2] = {nullptr, nullptr}, ev_done[2] = {nullptr, nullptr};
+  DevBuf d_flags[2];
+  cudaEvent_t ev_copied[2] = {nullptr, nullptr};
   int rc = 0;
   for (int b = 0; b < 2 && !rc; ++b) {
-    rc = StageAlloc(founder_ct, rows_cap, &st[b], use_popc ? kSamplePad : 64) || d_flags[b].alloc(static_cast<uint64_t>(kLdChunkVariants) * band);
-    if (!rc && (cudaEventCreateWithFlags(&ev_copied[b], cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&ev_done[b], cudaEventDisableTiming) != cudaSuccess)) {
+    rc = StageAlloc(founder_ct, rows_cap, &st[b], 64) || d_flags[b].alloc(static_cast<uint64_t>(kLdChunkVariants) * band);
+    if (!rc && cudaEventCreateWithFlags(&ev_copied[b], cudaEventDisableTiming) != cudaSuccess) {
       set_error("pl2gpu_ld_band_flags: cudaEventCreate failed");
       rc = 1;
     }
   }
-  const uint32_t word_ct = st[0].sample_ct_padded / 32;
-  if (!rc && use_popc) rc = d_planes.alloc(3ull * word_ct * rows_cap * 4);
-  if (!rc && !use_popc && cudaFuncSetAttribute(ld_ts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kLdtSmemBytes) != cudaSuccess) {
+  if (!rc && cudaFuncSetAttribute(ld_ts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kLdtSmemBytes) != cudaSuccess) {
     set_error("pl2gpu_ld_band_flags: %s", cudaGetErrorString(cudaGetLastError()));
     rc = 1;
   }
@@ -136,15 +129,8 @@ int pl2gpu_ld_band_flags(Pl2GpuCtx* ctx, const void* genovecs, uint64_t variant_
     if (rc) break;
     cudaEventRecord(ev_copied[b], c->copy_stream);
     cudaStreamWaitEvent(c->stream, ev_copied[b], 0);
-    if (use_popc) {
-      ld_split_kernel<<<dim3(padded / 32, DivUpU32(word_ct, 32)), 1024, 0, c->stream>>>(st[b].d_raw, st[b].pitch, word_ct, padded, static_cast<uint32_t*>(d_planes.p));
-      c->launches++;
-      ld_band_kernel<<<dim3(DivUpU32(a1 - a0, 64), band_r / 64 + 1), 256, 0, c->stream>>>(static_cast<const uint32_t*>(d_planes.p), word_ct, padded, lo, a0, a1, band, prune_ld_thresh, static_cast<uint8_t*>(d_flags[b].p));
-      c->launches++;
-    } else {
-      ld_ts_kernel<<<dim3(DivUpU32(a1 - a0, kLdtRows), (kLdtRows - kLdtCols + band_r) / kLdtCols + 1), kLdtThreads, kLdtSmemBytes, c->stream>>>(st[b].d_raw, st[b].pitch, st[b].sample_ct_padded, lo, a0, a1, band, prune_ld_thresh, static_cast<uint8_t*>(d_flags[b].p));
-      c->launches++;
-    }
+    ld_ts_kernel<<<dim3(DivUpU32(a1 - a0, kLdtRows), (kLdtRows - kLdtCols + band_r) / kLdtCols + 1), kLdtThreads, kLdtSmemBytes, c->stream>>>(st[b].d_raw, st[b].pitch, st[b].sample_ct_padded, lo, a0, a1, band, prune_ld_thresh, static_cast<uint8_t*>(d_flags[b].p));
+    c->launches++;
     if (cudaGetLastError() != cudaSuccess) {
       set_error("pl2gpu_ld_band_flags: %s", cudaGetErrorString(cudaGetLastError()));
       rc = 1;
@@ -168,7 +154,6 @@ int pl2gpu_ld_band_flags(Pl2GpuCtx* ctx, const void* genovecs, uint64_t variant_
   for (int b = 0; b < 2; ++b) {
     StageFree(&st[b]);
     if (ev_copied[b]) cudaEventDestroy(ev_copied[b]);
-    if (ev_done[b]) cudaEventDestroy(ev_done[b]);
   }
   return rc;
 }

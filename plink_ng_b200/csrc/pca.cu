@@ -4,14 +4,12 @@
 // reproduces the reference's SFMT / Box-Muller stream, host/sfmt.cc).
 #include <algorithm>
 #include <cmath>
-#include <cstring>
 #include <vector>
 
 #include "../../include/plink2_b200.h"
 #include "common.cuh"
 #include "ld_kernels.cuh"    // geno_counts_kernel
 #include "geno_tile.cuh"
-#include "pca_kernels.cuh"
 #include "pca_ts_kernels.cuh"
 #include "jacobi.cuh"
 #include "dense_fp64.cuh"
@@ -28,12 +26,8 @@ struct Pl2PcaJob {
   uint32_t sample_ct = 0, sample_ct_padded = 0, pitch = 0;
   uint32_t variant_cap = 0, variant_ct = 0, pc_ct = 0;
   uint8_t* d_raw = nullptr;
-  double* d_ztab = nullptr;
   uint32_t* d_counts = nullptr;
-  std::vector<double> h_ztab;
   std::vector<uint32_t> h_counts;
-  // tensor path (default; PL2_PCA_ALGO=fp64 selects the CUDA-core kernels of pca_kernels.cuh as a cross-check)
-  bool tensor = true;
   uint8_t* d_raw_i = nullptr;   // sample-major copy [row tile][k-step][128][8 B] of the whole matrix (geno_tile.cuh)
   double* d_slope = nullptr;    // per variant: inv_stdev (0 for skipped variants)
   double* d_icpt = nullptr;     // per variant: -2 alt_freq inv_stdev
@@ -69,27 +63,20 @@ static int PcaBeginImpl(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t variant_ct_
   job->pitch = job->sample_ct_padded / 4;
   job->variant_cap = RoundUpU32(variant_ct_total, 128);
   job->pc_ct = pc_ct;
-  {
-    const char* algo = getenv("PL2_PCA_ALGO");
-    job->tensor = !(algo && !strcmp(algo, "fp64"));
-  }
-  if (cudaMalloc(&job->d_raw, static_cast<uint64_t>(job->variant_cap) * job->pitch) != cudaSuccess || cudaMalloc(&job->d_ztab, static_cast<uint64_t>(job->variant_cap) * 32) != cudaSuccess ||
-      cudaMalloc(&job->d_counts, 16ull * 65536) != cudaSuccess ||
-      (job->tensor && (cudaMalloc(&job->d_raw_i, static_cast<uint64_t>(job->sample_ct_padded) * (job->variant_cap / 4)) != cudaSuccess || cudaMalloc(&job->d_slope, 8ull * job->variant_cap) != cudaSuccess ||
-                       cudaMalloc(&job->d_icpt, 8ull * job->variant_cap) != cudaSuccess || cudaMalloc(&job->d_twof, 8ull * job->variant_cap) != cudaSuccess))) {
+  if (cudaMalloc(&job->d_raw, static_cast<uint64_t>(job->variant_cap) * job->pitch) != cudaSuccess || cudaMalloc(&job->d_counts, 16ull * 65536) != cudaSuccess ||
+      cudaMalloc(&job->d_raw_i, static_cast<uint64_t>(job->sample_ct_padded) * (job->variant_cap / 4)) != cudaSuccess || cudaMalloc(&job->d_slope, 8ull * job->variant_cap) != cudaSuccess ||
+      cudaMalloc(&job->d_icpt, 8ull * job->variant_cap) != cudaSuccess || cudaMalloc(&job->d_twof, 8ull * job->variant_cap) != cudaSuccess) {
     cudaGetLastError();
     set_error("pl2gpu_pca_begin: insufficient device memory to keep %u x %u genotypes resident", variant_ct_total, sample_ct);
     pl2gpu_pca_end(job);
     return 1;
   }
-  if (job->tensor) {
-    if (cudaMemsetAsync(job->d_slope, 0, 8ull * job->variant_cap, ctx->c.stream) != cudaSuccess || cudaMemsetAsync(job->d_icpt, 0, 8ull * job->variant_cap, ctx->c.stream) != cudaSuccess ||
-        cudaFuncSetAttribute(pca_xa_wg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPxaSmemBytes) != cudaSuccess ||
-        cudaFuncSetAttribute(pca_xtb_wg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPxtSmemBytes) != cudaSuccess) {
-      if (!*get_error()) set_error("pl2gpu_pca_begin: %s", cudaGetErrorString(cudaGetLastError()));
-      pl2gpu_pca_end(job);
-      return 1;
-    }
+  if (cudaMemsetAsync(job->d_slope, 0, 8ull * job->variant_cap, ctx->c.stream) != cudaSuccess || cudaMemsetAsync(job->d_icpt, 0, 8ull * job->variant_cap, ctx->c.stream) != cudaSuccess ||
+      cudaFuncSetAttribute(pca_xa_wg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPxaSmemBytes) != cudaSuccess ||
+      cudaFuncSetAttribute(pca_xtb_wg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPxtSmemBytes) != cudaSuccess) {
+    if (!*get_error()) set_error("pl2gpu_pca_begin: %s", cudaGetErrorString(cudaGetLastError()));
+    pl2gpu_pca_end(job);
+    return 1;
   }
   *job_ptr = job;
   return 0;
@@ -116,7 +103,6 @@ int pl2gpu_pca_add_variants(Pl2PcaJob* job, const void* genovecs, uint64_t varia
     job->h_counts.resize(4ull * cur);
     PL2_CUDA_OK(cudaMemcpyAsync(job->h_counts.data(), job->d_counts, 16ull * cur, cudaMemcpyDeviceToHost, c->stream));
     PL2_CUDA_OK(cudaStreamSynchronize(c->stream));
-    job->h_ztab.assign(4ull * cur, 0.0);
     job->h_slope.assign(cur, 0.0);
     job->h_icpt.assign(cur, 0.0);
     job->h_twof.assign(cur, 0.0);
@@ -144,20 +130,12 @@ int pl2gpu_pca_add_variants(Pl2PcaJob* job, const void* genovecs, uint64_t varia
         continue;
       }
       const double inv_stdev = 1.0 / sqrt(variance);
-      const double intercept = -2 * alt_freq * inv_stdev;
-      double* z = &job->h_ztab[4ull * v];
-      z[0] = intercept;
-      z[1] = intercept + inv_stdev;
-      z[2] = intercept + 2 * inv_stdev;
       job->h_slope[v] = inv_stdev;
-      job->h_icpt[v] = intercept;
+      job->h_icpt[v] = -2 * alt_freq * inv_stdev;
     }
-    PL2_CUDA_OK(cudaMemcpyAsync(job->d_ztab + 4ull * job->variant_ct, job->h_ztab.data(), 32ull * cur, cudaMemcpyHostToDevice, c->stream));
-    if (job->tensor) {
-      PL2_CUDA_OK(cudaMemcpyAsync(job->d_slope + job->variant_ct, job->h_slope.data(), 8ull * cur, cudaMemcpyHostToDevice, c->stream));
-      PL2_CUDA_OK(cudaMemcpyAsync(job->d_icpt + job->variant_ct, job->h_icpt.data(), 8ull * cur, cudaMemcpyHostToDevice, c->stream));
-      PL2_CUDA_OK(cudaMemcpyAsync(job->d_twof + job->variant_ct, job->h_twof.data(), 8ull * cur, cudaMemcpyHostToDevice, c->stream));
-    }
+    PL2_CUDA_OK(cudaMemcpyAsync(job->d_slope + job->variant_ct, job->h_slope.data(), 8ull * cur, cudaMemcpyHostToDevice, c->stream));
+    PL2_CUDA_OK(cudaMemcpyAsync(job->d_icpt + job->variant_ct, job->h_icpt.data(), 8ull * cur, cudaMemcpyHostToDevice, c->stream));
+    PL2_CUDA_OK(cudaMemcpyAsync(job->d_twof + job->variant_ct, job->h_twof.data(), 8ull * cur, cudaMemcpyHostToDevice, c->stream));
     PL2_CUDA_OK(cudaStreamSynchronize(c->stream));
     job->variant_ct += cur;
     done += cur;
@@ -184,8 +162,8 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
   const uint32_t c2 = 2 * k;
   const uint64_t q = static_cast<uint64_t>(c2) * (k + 1);
   const uint32_t world = sharded ? static_cast<uint32_t>(c->comm_world) : 1, rank = sharded ? static_cast<uint32_t>(c->comm_rank) : 0;
-  if (sharded && (!c->comm || !job->tensor || !m)) {
-    set_error("pl2gpu_pca_run_sharded: needs a communicator on the context, the tensor path and a non-empty shard");
+  if (sharded && (!c->comm || !m)) {
+    set_error("pl2gpu_pca_run_sharded: needs a communicator on the context and a non-empty shard");
     return 1;
   }
   if (!sharded) total_variant_ct = m;
@@ -196,8 +174,7 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
   double *d_qq = nullptr, *d_u = nullptr, *d_g1 = nullptr, *d_g2 = nullptr, *d_b = nullptr, *d_gram = nullptr, *d_gram_u = nullptr, *d_gram_partial = nullptr, *d_colscale = nullptr;
   int rc = 1;
   const double m_recip = 1.0 / static_cast<double>(total_variant_ct);
-  // ---- tensor path scratch (pca_ts_kernels.cuh): digit planes, per-column scales, split-K partial sums ----
-  const bool tensor = job->tensor;
+  // ---- tensor pass scratch (pca_ts_kernels.cuh): digit planes, per-column scales, split-K partial sums ----
   uint8_t *d_gdig = nullptr, *d_hs = nullptr, *d_hi = nullptr;
   double *d_scale = nullptr, *d_inv_scale = nullptr, *d_partial = nullptr;
   unsigned long long* d_colmax = nullptr;
@@ -207,23 +184,21 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
   const uint32_t ksteps_per_split = RoundUpU32(DivUpU32(kstep_total, splits), 4);
   splits = DivUpU32(kstep_total, ksteps_per_split);
   int ts_rc = 0;
-  if (tensor) {
-    if (cudaMalloc(&d_gdig, static_cast<uint64_t>(npad) * kPcaNMax) != cudaSuccess || cudaMalloc(&d_hs, static_cast<uint64_t>(job->variant_cap) * kPcaNMax) != cudaSuccess ||
-        cudaMalloc(&d_hi, static_cast<uint64_t>(job->variant_cap) * kPcaNMax) != cudaSuccess || cudaMalloc(&d_scale, 8 * kPcaCgMax) != cudaSuccess || cudaMalloc(&d_inv_scale, 8 * kPcaCgMax) != cudaSuccess ||
-        cudaMalloc(&d_colmax, 8 * kPcaCgMax) != cudaSuccess || cudaMalloc(&d_partial, static_cast<uint64_t>(splits) * npad * kPcaCgMax * 8) != cudaSuccess) {
-      cudaGetLastError();
-      set_error("pl2gpu_pca_run: insufficient device memory for the digit planes");
-      cudaFree(d_gdig); cudaFree(d_hs); cudaFree(d_hi); cudaFree(d_scale); cudaFree(d_inv_scale); cudaFree(d_colmax); cudaFree(d_partial);
-      return 1;
-    }
-    // rows [variant_ct, variant_cap) must decode to "missing" in both layouts; finish the sample-major copy
-    if (job->variant_cap > m) PL2_TRY(LaunchPadGenotypes(c, job->d_raw + static_cast<uint64_t>(m) * job->pitch, job->pitch, job->sample_ct, 0, job->variant_cap - m));
-    if (job->retiled_to < job->variant_cap) {
-      const uint32_t from = job->retiled_to;
-      geno_tile_rows_kernel<<<dim3((job->variant_cap - from) / 64, npad / 64), 256, 0, c->stream>>>(job->d_raw + static_cast<uint64_t>(from) * job->pitch, job->pitch, kstep_total, 0, job->d_raw_i + static_cast<uint64_t>(from / 32) * 1024);
-      c->launches++;
-      job->retiled_to = job->variant_cap;
-    }
+  if (cudaMalloc(&d_gdig, static_cast<uint64_t>(npad) * kPcaNMax) != cudaSuccess || cudaMalloc(&d_hs, static_cast<uint64_t>(job->variant_cap) * kPcaNMax) != cudaSuccess ||
+      cudaMalloc(&d_hi, static_cast<uint64_t>(job->variant_cap) * kPcaNMax) != cudaSuccess || cudaMalloc(&d_scale, 8 * kPcaCgMax) != cudaSuccess || cudaMalloc(&d_inv_scale, 8 * kPcaCgMax) != cudaSuccess ||
+      cudaMalloc(&d_colmax, 8 * kPcaCgMax) != cudaSuccess || cudaMalloc(&d_partial, static_cast<uint64_t>(splits) * npad * kPcaCgMax * 8) != cudaSuccess) {
+    cudaGetLastError();
+    set_error("pl2gpu_pca_run: insufficient device memory for the digit planes");
+    cudaFree(d_gdig); cudaFree(d_hs); cudaFree(d_hi); cudaFree(d_scale); cudaFree(d_inv_scale); cudaFree(d_colmax); cudaFree(d_partial);
+    return 1;
+  }
+  // rows [variant_ct, variant_cap) must decode to "missing" in both layouts; finish the sample-major copy
+  if (job->variant_cap > m) PL2_TRY(LaunchPadGenotypes(c, job->d_raw + static_cast<uint64_t>(m) * job->pitch, job->pitch, job->sample_ct, 0, job->variant_cap - m));
+  if (job->retiled_to < job->variant_cap) {
+    const uint32_t from = job->retiled_to;
+    geno_tile_rows_kernel<<<dim3((job->variant_cap - from) / 64, npad / 64), 256, 0, c->stream>>>(job->d_raw + static_cast<uint64_t>(from) * job->pitch, job->pitch, kstep_total, 0, job->d_raw_i + static_cast<uint64_t>(from / 32) * 1024);
+    c->launches++;
+    job->retiled_to = job->variant_cap;
   }
   // column group: up to 48 columns, padded to a multiple of 4 (the padding columns are zero digits and never written)
   auto group_scales = [&](const double* src, uint64_t rs, uint64_t cs, uint32_t rows, uint32_t valid, const double* mul1, const double* mul2) {
@@ -236,7 +211,7 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
   // 30 bits (pca_digits_kernel pass 1) - 60 bits below the column maximum, so the passes lose nothing against the
   // reference's fp64 dgemm (one 30-bit pass left the trailing, noise-level eigenvalues 2e-3 off)
   constexpr int kPasses = 2;
-  auto launch_xa_ts = [&](const double* g, uint32_t g_ld, double* hout, uint64_t h_ld, uint32_t hcol0, uint32_t cols_total) {
+  auto launch_xa = [&](const double* g, uint32_t g_ld, double* hout, uint64_t h_ld, uint32_t hcol0, uint32_t cols_total) {
     for (uint32_t cc = 0; cc < cols_total; cc += kPcaCgMax) {
       const uint32_t valid = std::min(kPcaCgMax, cols_total - cc), cg = kPcaCgMax;
       group_scales(g + cc, g_ld, 1, npad, valid, nullptr, nullptr);
@@ -248,7 +223,7 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
       }
     }
   };
-  auto launch_xtb_ts = [&](const double* hin, uint64_t h_ld, uint32_t hcol0, uint32_t cols_total, double* out, uint64_t out_rs, uint64_t out_cs) {
+  auto launch_xtb = [&](const double* hin, uint64_t h_ld, uint32_t hcol0, uint32_t cols_total, double* out, uint64_t out_rs, uint64_t out_cs) {
     for (uint32_t cc = 0; cc < cols_total; cc += kPcaCgMax) {
       const uint32_t valid = std::min(kPcaCgMax, cols_total - cc), cg = kPcaCgMax;
       const double* src = hin + static_cast<uint64_t>(hcol0 + cc) * h_ld;
@@ -261,28 +236,6 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
         c->launches += 3;
       }
     }
-  };
-  auto launch_xa_fp64 = [&](const double* g, uint32_t g_ld, double* hout, uint64_t h_ld, uint32_t hcol0, uint32_t cols_total) {
-    for (uint32_t cc = 0; cc < cols_total; cc += kPcaColsMax) {
-      const uint32_t cols = std::min(kPcaColsMax, cols_total - cc);
-      pca_xa_kernel<<<DivUpU32(m, 128), 32 * DivUpU32(cols, 4), (128 * cols + 4) * 8, c->stream>>>(job->d_raw, job->pitch, npad, m, job->d_ztab, g + cc, g_ld, 0, cols, hout + static_cast<uint64_t>(hcol0 + cc) * h_ld, h_ld, 0);
-      c->launches++;
-    }
-  };
-  auto launch_xtb_fp64 = [&](const double* hin, uint64_t h_ld, uint32_t hcol0, uint32_t cols_total, double* out, uint64_t out_rs, uint64_t out_cs) {
-    for (uint32_t cc = 0; cc < cols_total; cc += kPcaColsMax) {
-      const uint32_t cols = std::min(kPcaColsMax, cols_total - cc);
-      pca_xtb_kernel<<<DivUpU32(n, 128), 32 * DivUpU32(cols, 4), (128 * cols + 512) * 8, c->stream>>>(job->d_raw, job->pitch, n, m, job->d_ztab, hin + static_cast<uint64_t>(hcol0 + cc) * h_ld, h_ld, 0, 0, cols, out + static_cast<uint64_t>(cc) * out_cs, out_rs, out_cs);
-      c->launches++;
-    }
-  };
-  auto launch_xa = [&](const double* g, uint32_t g_ld, double* hout, uint64_t h_ld, uint32_t hcol0, uint32_t cols_total) {
-    if (tensor) launch_xa_ts(g, g_ld, hout, h_ld, hcol0, cols_total);
-    else launch_xa_fp64(g, g_ld, hout, h_ld, hcol0, cols_total);
-  };
-  auto launch_xtb = [&](const double* hin, uint64_t h_ld, uint32_t hcol0, uint32_t cols_total, double* out, uint64_t out_rs, uint64_t out_cs) {
-    if (tensor) launch_xtb_ts(hin, h_ld, hcol0, cols_total, out, out_rs, out_cs);
-    else launch_xtb_fp64(hin, h_ld, hcol0, cols_total, out, out_rs, out_cs);
   };
   // PL2_TIMING=1: phase times on stderr (stream-synchronising; development aid)
   const bool timing = getenv("PL2_TIMING") != nullptr;
@@ -326,137 +279,117 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
       break;
     }
     mark("power iterations (Y.G / Yt.H)");
-    // Orthonormal basis Q of the range of the Krylov matrix   :5860 (the reference takes the left singular vectors
-    // from dgesvd; only their span enters B = Y^T Q and everything after it).
-    //   Default: block classical Gram-Schmidt over the k + 1 Krylov blocks, three projection passes per block (the
-    //   blocks span 35 orders of magnitude - two passes are not enough), each followed by a Jacobi SVD of the M x 2k
-    //   residual whose unit left singular vectors replace the block.  O(M q^2) once instead of per Jacobi sweep.
-    //   PL2_PCA_BASIS=jacobi: one-sided Jacobi SVD of the whole M x q matrix (jacobi.cuh), the round-1 form.
-    //   Both give the structure PCs to 1e-13 of the LAPACK-based restatement and differ from it by 1e-4..1e-3 in the
-    //   noise-level eigenvalues (tests/harness/pca_basis_compare.py): the Krylov matrix is numerically rank deficient
-    //   and every method completes the basis differently there.
+    // Orthonormal basis Q of the range of the Krylov matrix, built in place in qq   :5860 (the reference takes the left
+    // singular vectors from dgesvd; only their span enters B = Y^T Q and everything after it).  Block classical
+    // Gram-Schmidt over the k + 1 Krylov blocks, three projection passes per block (the blocks span 35 orders of
+    // magnitude - two passes are not enough), each followed by a Jacobi SVD of the M x 2k residual whose unit left
+    // singular vectors replace the block: O(M q^2) in all, what a one-sided Jacobi SVD of the whole M x q matrix costs
+    // per sweep.  The structure PCs match the LAPACK-based restatement to 1e-13; the noise-level eigenvalues differ
+    // from it by 1e-4..1e-3, because the Krylov matrix is numerically rank deficient and every method completes the
+    // basis differently there.
     std::vector<double> s(q);
     const char* err = nullptr;
-    const char* basis_env = getenv("PL2_PCA_BASIS");
-    const bool bcgs = sharded || !(basis_env && !strcmp(basis_env, "jacobi"));
-    const double* d_basis = d_u;
-    if (!bcgs) {
-      if (JacobiSvd(c, d_qq, m, m, static_cast<uint32_t>(q), static_cast<uint32_t>(q), s.data(), d_u, m, nullptr, &err)) {
-        set_error("Failed to compute SVD of Krylov matrix (%s).", err ? err : "?");
-        break;
-      }
-    } else {
-      double *d_c = nullptr, *d_cpart = nullptr, *d_wg = nullptr, *d_wf = nullptr, *d_uf = nullptr, *d_sizes = nullptr;
-      uint64_t part_doubles = 1;
-      for (uint32_t t = 1; t <= k; ++t) part_doubles = std::max(part_doubles, DgemmTNPartialDoubles(c, t * c2, c2, m));
-      bool ok = cudaMalloc(&d_c, q * c2 * 8) == cudaSuccess && cudaMalloc(&d_cpart, part_doubles * 8) == cudaSuccess;
-      // sharded: every rank learns the shard sizes (one all-reduce of a world-length vector), blocks are exchanged
-      // in slots of the largest shard
-      uint64_t m_pad = m;
-      if (ok && sharded) {
-        std::vector<double> sizes(world, 0.0);
-        sizes[rank] = static_cast<double>(m);
-        ok = cudaMalloc(&d_sizes, 8ull * world) == cudaSuccess && cudaMemcpyAsync(d_sizes, sizes.data(), 8ull * world, cudaMemcpyHostToDevice, c->stream) == cudaSuccess &&
-             !CommAllReduceSumF64(c, d_sizes, world, c->stream) && cudaMemcpyAsync(sizes.data(), d_sizes, 8ull * world, cudaMemcpyDeviceToHost, c->stream) == cudaSuccess &&
-             cudaStreamSynchronize(c->stream) == cudaSuccess;
-        for (uint32_t r = 0; ok && r < world; ++r) m_pad = std::max<uint64_t>(m_pad, static_cast<uint64_t>(sizes[r]));
-        const uint64_t blk = m_pad * c2 * 8;
-        ok = ok && cudaMalloc(&d_wg, blk * world) == cudaSuccess && cudaMalloc(&d_wf, blk * world) == cudaSuccess && cudaMalloc(&d_uf, blk * world) == cudaSuccess;
-      }
-      const uint64_t m_full = m_pad * world;
-      for (uint32_t t = 0; ok && t <= k; ++t) {
-        double* w = d_qq + static_cast<uint64_t>(t) * c2 * m;
-        const uint32_t prev = t * c2;
-        for (int rep = 0; ok && rep < 3; ++rep) {
-          if (prev) {
-            ok = !DgemmTN(c, d_qq, m, prev, w, m, c2, m, d_cpart, d_c, prev) && !(sharded && CommAllReduceSumF64(c, d_c, static_cast<uint64_t>(prev) * c2, c->stream)) &&
-                 !DgemmNN(c, d_qq, m, m, prev, d_c, prev, c2, w, m, true, nullptr);
-            if (!ok) break;
+    double *d_c = nullptr, *d_cpart = nullptr, *d_wg = nullptr, *d_wf = nullptr, *d_uf = nullptr, *d_sizes = nullptr;
+    uint64_t part_doubles = 1;
+    for (uint32_t t = 1; t <= k; ++t) part_doubles = std::max(part_doubles, DgemmTNPartialDoubles(c, t * c2, c2, m));
+    bool ok = cudaMalloc(&d_c, q * c2 * 8) == cudaSuccess && cudaMalloc(&d_cpart, part_doubles * 8) == cudaSuccess;
+    // sharded: every rank learns the shard sizes (one all-reduce of a world-length vector), blocks are exchanged
+    // in slots of the largest shard
+    uint64_t m_pad = m;
+    if (ok && sharded) {
+      std::vector<double> sizes(world, 0.0);
+      sizes[rank] = static_cast<double>(m);
+      ok = cudaMalloc(&d_sizes, 8ull * world) == cudaSuccess && cudaMemcpyAsync(d_sizes, sizes.data(), 8ull * world, cudaMemcpyHostToDevice, c->stream) == cudaSuccess &&
+           !CommAllReduceSumF64(c, d_sizes, world, c->stream) && cudaMemcpyAsync(sizes.data(), d_sizes, 8ull * world, cudaMemcpyDeviceToHost, c->stream) == cudaSuccess &&
+           cudaStreamSynchronize(c->stream) == cudaSuccess;
+      for (uint32_t r = 0; ok && r < world; ++r) m_pad = std::max<uint64_t>(m_pad, static_cast<uint64_t>(sizes[r]));
+      const uint64_t blk = m_pad * c2 * 8;
+      ok = ok && cudaMalloc(&d_wg, blk * world) == cudaSuccess && cudaMalloc(&d_wf, blk * world) == cudaSuccess && cudaMalloc(&d_uf, blk * world) == cudaSuccess;
+    }
+    const uint64_t m_full = m_pad * world;
+    for (uint32_t t = 0; ok && t <= k; ++t) {
+      double* w = d_qq + static_cast<uint64_t>(t) * c2 * m;
+      const uint32_t prev = t * c2;
+      for (int rep = 0; ok && rep < 3; ++rep) {
+        if (prev) {
+          ok = !DgemmTN(c, d_qq, m, prev, w, m, c2, m, d_cpart, d_c, prev) && !(sharded && CommAllReduceSumF64(c, d_c, static_cast<uint64_t>(prev) * c2, c->stream)) &&
+               !DgemmNN(c, d_qq, m, m, prev, d_c, prev, c2, w, m, true, nullptr);
+          if (!ok) break;
+        }
+        if (!sharded) {
+          if (JacobiSvd(c, w, m, m, c2, c2, s.data(), d_u, m, nullptr, &err)) {
+            ok = false;
+            break;
           }
-          if (!sharded) {
-            if (JacobiSvd(c, w, m, m, c2, c2, s.data(), d_u, m, nullptr, &err)) {
-              ok = false;
-              break;
-            }
-            ok = cudaMemcpyAsync(w, d_u, static_cast<uint64_t>(m) * c2 * 8, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
-          } else {
-            // my rows into my slot (zero-padded to m_pad), all-gather, repack to one column-major (world m_pad) x 2k
-            // matrix, the same Jacobi SVD on every rank, my rows of the unit left singular vectors back into the block
-            double* slot = d_wg + static_cast<uint64_t>(rank) * m_pad * c2;
-            ok = cudaMemsetAsync(slot, 0, m_pad * c2 * 8, c->stream) == cudaSuccess &&
-                 cudaMemcpy2DAsync(slot, m_pad * 8, w, static_cast<uint64_t>(m) * 8, static_cast<uint64_t>(m) * 8, c2, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess &&
-                 !CommAllGatherInPlace(c, d_wg, m_pad * c2 * 8, c->stream);
-            for (uint32_t r = 0; ok && r < world; ++r)
-              ok = cudaMemcpy2DAsync(d_wf + static_cast<uint64_t>(r) * m_pad, m_full * 8, d_wg + static_cast<uint64_t>(r) * m_pad * c2, m_pad * 8, m_pad * 8, c2, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
-            if (!ok) break;
-            if (JacobiSvd(c, d_wf, m_full, static_cast<uint32_t>(m_full), c2, c2, s.data(), d_uf, m_full, nullptr, &err)) {
-              ok = false;
-              break;
-            }
-            ok = cudaMemcpy2DAsync(w, static_cast<uint64_t>(m) * 8, d_uf + static_cast<uint64_t>(rank) * m_pad, m_full * 8, static_cast<uint64_t>(m) * 8, c2, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
+          ok = cudaMemcpyAsync(w, d_u, static_cast<uint64_t>(m) * c2 * 8, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
+        } else {
+          // my rows into my slot (zero-padded to m_pad), all-gather, repack to one column-major (world m_pad) x 2k
+          // matrix, the same Jacobi SVD on every rank, my rows of the unit left singular vectors back into the block
+          double* slot = d_wg + static_cast<uint64_t>(rank) * m_pad * c2;
+          ok = cudaMemsetAsync(slot, 0, m_pad * c2 * 8, c->stream) == cudaSuccess &&
+               cudaMemcpy2DAsync(slot, m_pad * 8, w, static_cast<uint64_t>(m) * 8, static_cast<uint64_t>(m) * 8, c2, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess &&
+               !CommAllGatherInPlace(c, d_wg, m_pad * c2 * 8, c->stream);
+          for (uint32_t r = 0; ok && r < world; ++r)
+            ok = cudaMemcpy2DAsync(d_wf + static_cast<uint64_t>(r) * m_pad, m_full * 8, d_wg + static_cast<uint64_t>(r) * m_pad * c2, m_pad * 8, m_pad * 8, c2, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
+          if (!ok) break;
+          if (JacobiSvd(c, d_wf, m_full, static_cast<uint32_t>(m_full), c2, c2, s.data(), d_uf, m_full, nullptr, &err)) {
+            ok = false;
+            break;
           }
+          ok = cudaMemcpy2DAsync(w, static_cast<uint64_t>(m) * 8, d_uf + static_cast<uint64_t>(rank) * m_pad, m_full * 8, static_cast<uint64_t>(m) * 8, c2, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
         }
       }
-      cudaFree(d_c);
-      cudaFree(d_cpart);
-      cudaFree(d_wg);
-      cudaFree(d_wf);
-      cudaFree(d_uf);
-      cudaFree(d_sizes);
-      if (!ok) {
-        cudaGetLastError();
-        if (!err && *get_error()) break;  // a collective already recorded its message
-        set_error("Failed to orthonormalise the Krylov matrix (%s).", err ? err : "CUDA failure");
-        break;
-      }
-      d_basis = d_qq;
     }
-    mark(bcgs ? "orthonormal basis of the Krylov matrix (BCGS)" : "SVD of the M x q Krylov matrix");
+    cudaFree(d_c);
+    cudaFree(d_cpart);
+    cudaFree(d_wg);
+    cudaFree(d_wf);
+    cudaFree(d_uf);
+    cudaFree(d_sizes);
+    if (!ok) {
+      cudaGetLastError();
+      if (!err && *get_error()) break;  // a collective already recorded its message
+      set_error("Failed to orthonormalise the Krylov matrix (%s).", err ? err : "CUDA failure");
+      break;
+    }
+    mark("orthonormal basis of the Krylov matrix (BCGS)");
     // B = Y^T Q (N x q, column-major)   :5870-5916
     if (cudaMemsetAsync(d_b, 0, static_cast<uint64_t>(n) * q * 8, c->stream) != cudaSuccess) break;
-    launch_xtb(d_basis, m, 0, static_cast<uint32_t>(q), d_b, 1, n);
+    launch_xtb(d_qq, m, 0, static_cast<uint32_t>(q), d_b, 1, n);
     if (sharded && CommAllReduceSumF64(c, d_b, static_cast<uint64_t>(n) * q, c->stream)) break;
     mark("B = Yt.Q");
     // Top-k left singular pairs of B (:5920, dgesvd in the reference).  Only the leading k of q are wanted and they
     // are the well-conditioned ones, so they come from the q x q Gram matrix: G = B^T B (fp64, fixed-order split
     // sums), eigenpairs of G by one-sided Jacobi on its columns (G V = V Lambda for a symmetric PSD matrix), then
-    // U_k = B V_k Lambda_k^-1/2.  The relative error of sigma_i is eps (sigma_1 / sigma_i)^2 - 1e-14 here - and the
-    // N x q Jacobi sweep over B (1.2 s at N = 16,384, O(N q^2) per sweep) is gone.  PL2_PCA_FINAL=jacobi keeps it.
-    const char* final_env = getenv("PL2_PCA_FINAL");
-    if (final_env && !strcmp(final_env, "jacobi")) {
-      // Q (d_u) is dead once B is formed (stream order): reuse it for the left singular vectors of B
-      if (JacobiSvd(c, d_b, n, n, static_cast<uint32_t>(q), k, s.data(), d_u, n, nullptr, &err)) {
-        set_error("Failed to compute SVD of final matrix (%s).", err ? err : "?");
-        break;
-      }
-    } else {
-      const uint32_t q32 = static_cast<uint32_t>(q);
-      if (cudaMalloc(&d_gram, q * q * 8) != cudaSuccess || cudaMalloc(&d_gram_u, q * k * 8) != cudaSuccess || cudaMalloc(&d_gram_partial, DgemmTNPartialDoubles(c, q32, q32, n) * 8) != cudaSuccess ||
-          cudaMalloc(&d_colscale, 8ull * k) != cudaSuccess) {
-        cudaGetLastError();
-        set_error("pl2gpu_pca_run: insufficient device memory for the %llu x %llu Gram matrix", static_cast<unsigned long long>(q), static_cast<unsigned long long>(q));
-        break;
-      }
-      if (DgemmTN(c, d_b, n, q32, d_b, n, q32, n, d_gram_partial, d_gram, q)) break;
-      if (JacobiSvd(c, d_gram, q, q32, q32, k, s.data(), d_gram_u, q, nullptr, &err)) {
-        set_error("Failed to compute SVD of final matrix (%s).", err ? err : "?");
-        break;
-      }
-      std::vector<double> inv_sigma(k);
-      bool ok = true;
-      for (uint32_t p = 0; p < k; ++p) {
-        ok = ok && s[p] > 0.0;
-        s[p] = sqrt(s[p]);  // eigenvalue of B^T B -> singular value of B
-        inv_sigma[p] = ok ? 1.0 / s[p] : 0.0;
-      }
-      if (!ok) {
-        set_error("Failed to compute SVD of final matrix (rank below the requested number of PCs).");
-        break;
-      }
-      if (cudaMemcpyAsync(d_colscale, inv_sigma.data(), 8ull * k, cudaMemcpyHostToDevice, c->stream) != cudaSuccess) break;
-      // Q (d_u) is dead once B is formed (stream order): reuse it for U_k (N x k, column-major)
-      if (DgemmNN(c, d_b, n, n, q32, d_gram_u, q, k, d_u, n, false, d_colscale)) break;
+    // U_k = B V_k Lambda_k^-1/2.  The relative error of sigma_i is eps (sigma_1 / sigma_i)^2 - 1e-14 here - and no
+    // N x q Jacobi sweep over B is needed (1.2 s at N = 16,384, O(N q^2) per sweep).
+    const uint32_t q32 = static_cast<uint32_t>(q);
+    if (cudaMalloc(&d_gram, q * q * 8) != cudaSuccess || cudaMalloc(&d_gram_u, q * k * 8) != cudaSuccess || cudaMalloc(&d_gram_partial, DgemmTNPartialDoubles(c, q32, q32, n) * 8) != cudaSuccess ||
+        cudaMalloc(&d_colscale, 8ull * k) != cudaSuccess) {
+      cudaGetLastError();
+      set_error("pl2gpu_pca_run: insufficient device memory for the %llu x %llu Gram matrix", static_cast<unsigned long long>(q), static_cast<unsigned long long>(q));
+      break;
     }
+    if (DgemmTN(c, d_b, n, q32, d_b, n, q32, n, d_gram_partial, d_gram, q)) break;
+    if (JacobiSvd(c, d_gram, q, q32, q32, k, s.data(), d_gram_u, q, nullptr, &err)) {
+      set_error("Failed to compute SVD of final matrix (%s).", err ? err : "?");
+      break;
+    }
+    std::vector<double> inv_sigma(k);
+    ok = true;
+    for (uint32_t p = 0; p < k; ++p) {
+      ok = ok && s[p] > 0.0;
+      s[p] = sqrt(s[p]);  // eigenvalue of B^T B -> singular value of B
+      inv_sigma[p] = ok ? 1.0 / s[p] : 0.0;
+    }
+    if (!ok) {
+      set_error("Failed to compute SVD of final matrix (rank below the requested number of PCs).");
+      break;
+    }
+    if (cudaMemcpyAsync(d_colscale, inv_sigma.data(), 8ull * k, cudaMemcpyHostToDevice, c->stream) != cudaSuccess) break;
+    // d_u, the scratch of the basis construction, is free once B is formed (stream order): reuse it for U_k (N x k,
+    // column-major)
+    if (DgemmNN(c, d_b, n, n, q32, d_gram_u, q, k, d_u, n, false, d_colscale)) break;
     mark("top-k singular pairs of the N x q matrix B");
     // the context's stream is non-blocking: order the copy on it (a plain cudaMemcpy would not wait for the kernels)
     if (cudaMemcpyAsync(eigvecs_host, d_u, 8ull * k * n, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
@@ -513,8 +446,8 @@ static __global__ void __launch_bounds__(256) vscore_finish_kernel(const double*
 }
 
 int pl2gpu_pca_vscore(Pl2PcaJob* job, const double* weights_host, uint32_t cols, double* out_host) {
-  if (!job || !weights_host || !cols || !out_host || !job->tensor || !job->variant_ct) {
-    set_error("pl2gpu_pca_vscore: bad arguments (needs a non-empty tensor-path job)");
+  if (!job || !weights_host || !cols || !out_host || !job->variant_ct) {
+    set_error("pl2gpu_pca_vscore: bad arguments (needs a non-empty job)");
     return 1;
   }
   Ctx* c = &job->ctx->c;
@@ -589,7 +522,6 @@ int pl2gpu_pca_end(Pl2PcaJob* job) {
   cudaFree(job->d_slope);
   cudaFree(job->d_icpt);
   cudaFree(job->d_twof);
-  cudaFree(job->d_ztab);
   cudaFree(job->d_counts);
   cudaGetLastError();
   delete job;

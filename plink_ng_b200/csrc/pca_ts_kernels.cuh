@@ -314,4 +314,9 @@ static __global__ void __launch_bounds__(256) pca_xtb_reduce_kernel(const double
   out[static_cast<uint64_t>(s) * out_rs + static_cast<uint64_t>(c) * out_cs] += acc * scale;
 }
 
+static __global__ void scale_kernel(double* __restrict__ x, uint64_t n, double s) {
+  const uint64_t i = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
+  if (i < n) x[i] *= s;
+}
+
 }  // namespace pl2

@@ -39,12 +39,10 @@ def test_geno_counts(gpu_ctx):
     assert np.array_equal(got.astype(np.int64), want)
 
 
-@pytest.mark.parametrize("algo", ["tensor", "popcount"])
 @pytest.mark.parametrize("n,m,band", [(64, 200, 17), (333, 700, 49), (1000, 300, 130), (2100, 900, 500)])
-def test_ld_band_flags_match_oracle(gpu_ctx, n, m, band, algo, monkeypatch):
-    """Both pair kernels (default: int8 tensor contraction over the founders, ld_ts_kernel.cuh; cross-check: bit-plane
-    popcounts, ld_kernels.cuh) against the oracle's exact integer sums and fp64 test, pair by pair."""
-    monkeypatch.setenv("PL2_LD_ALGO", algo)
+def test_ld_band_flags_match_oracle(gpu_ctx, n, m, band):
+    """The pair kernel (int8 tensor contraction over the founders, ld_ts_kernel.cuh) against the oracle's exact
+    integer sums and fp64 test, pair by pair."""
     g = _ld_geno(m, n, seed=n + m)
     thr = 0.2 * (1 + orc.SMALL_EPSILON)
     got = ld_band_flags(gpu_ctx, pack_genotypes(g), n, band, thr)
