@@ -88,7 +88,7 @@ enum {
   kPl2KingAlgoAuto = 0,
   kPl2KingAlgoPopcount = 1, /* bit-plane AND/XOR + __popc over smem tiles */
   kPl2KingAlgoTensor = 2,   /* exact int8 wgmma contraction over {0,+-1} indicator planes, 128 x 96 tiles */
-  kPl2KingAlgoTensorTS = 3  /* same contraction, 128 x 80 tiles, double-buffered staging (the default) */
+  kPl2KingAlgoTensorTS = 3  /* same contraction, 128 x 64 tiles, double-buffered staging (the default) */
 };
 
 /* Rows [row_start, row_end) of the strict lower triangle over sample_ct samples (row = larger
@@ -260,7 +260,7 @@ int pl2gpu_score_get(Pl2ScoreJob* job, double* score_sums, uint64_t* named_dosag
 int pl2gpu_score_end(Pl2ScoreJob* job);
 
 /* ---- measured int8 tensor peak: two warpgroups per SM issue back-to-back int8 wgmma (M = 64, N = n_cols in
- * {80, 96}, K = 32; form 1 = A fragments in registers, B in shared memory, as the KING/GRM kernels use it) for at
+ * {64, 80, 96, 128}, K = 32; form 1 = A fragments in registers, B in shared memory, as the KING/GRM kernels use it) for at
  * least min_seconds; *tops_out = 2*64*n_cols*32 ops x wgmmas / elapsed (CUDA events), in TOP/s.
  * This is the roofline denominator bench.py reports against. ---- */
 int pl2gpu_int8_peak(Pl2GpuCtx* ctx, uint32_t n_cols, int form, double min_seconds, double* tops_out, double* seconds_out);

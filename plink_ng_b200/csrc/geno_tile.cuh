@@ -6,9 +6,12 @@
 
 namespace pl2 {
 
-// 128 x 80 pair tiles (the default KING tiling and the GRM tiling).
+// 128 x 80 pair tiles (the GRM tiling).
 constexpr uint32_t kTsCols = 80;
 constexpr uint32_t kTsSamplePad = 640;  // lcm(128, 80)
+// 128 x 64 pair tiles (the default KING tiling); its blocks keep the 640-sample padding.
+constexpr uint32_t kKingTsCols = 64;
+static_assert(kTsSamplePad % 128 == 0 && kTsSamplePad % kKingTsCols == 0, "padded samples: whole row and column tiles");
 
 // ---- operand re-tiling of the staged block raw[variant][pitch] (2-bit, variant-major) -------------
 // Row side:  raw_i[row tile rt][k-step ks][row 0..127][8 bytes]   8 bytes = 32 variants of one sample

@@ -21,7 +21,7 @@
 
 namespace pl2 {
 
-static_assert(kGrmTileCols == kTsCols && kGrmSamplePad == kTsSamplePad, "GRM shares the KING tiling");
+static_assert(kGrmTileCols == kTsCols && kGrmSamplePad == kTsSamplePad, "GRM uses the 80-column tiling of geno_tile.cuh");
 constexpr uint32_t kGwKs = 2;                                        // k32 steps per stage (64 variants)
 constexpr uint32_t kGwThreads = 256;
 constexpr uint32_t kGwSbo = 2 * kGwKs * kCoreBytes;                  // 512: next group of 8 B rows

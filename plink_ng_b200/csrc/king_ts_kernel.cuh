@@ -1,15 +1,18 @@
 // king_ts_kernel.cuh - KING pair counts on the int8 tensor pipe (wgmma, sm_90a).
 //
 //   D[r][c] += sum_v A_plane[r][v] * B_plane[c][v],  planes T (het), H (hom), S (+1 hom-REF / -1 hom-ALT),
-// exact int32 sums, the raw accumulator semantics of king_kernels.cuh.  One CTA = 64 rows (half of a 128-row
-// pair tile) x kCols columns, three warpgroups:
+// exact int32 sums, the raw accumulator semantics of king_kernels.cuh.  Two kernels:
+//   king_tile128_kernel   the default (`tensor_ts`): one CTA per 128 x 64 pair tile (described below it)
+//   king_wg_kernel<96>    the `tensor` algorithm, an independent cross-check: two CTAs per 128 x 96 pair tile
+//
+// king_wg_kernel: one CTA = 64 rows (half of a 128-row pair tile) x kCols columns, three warpgroups:
 //   warpgroup 0:  producer - stages the operands of the variant loop in a ring of shared-memory stages
 //   warpgroup 1:  T_I x T_J -> TT,  T_I x H_J -> TH,  S_I x S_J, columns [0, kS)
 //   warpgroup 2:  H_I x T_J -> HT,  H_I x H_J -> HH,  S_I x S_J, columns [kCols - kS, kCols)
 // so that each consumer thread keeps ~100-120 int32 accumulators in registers for the whole variant loop (the
 // 64 x 5 kCols accumulators of a half tile are 100-120 KB; a whole 128-row tile would not fit the register file).
-// Both consumers issue the same shapes (ptxas serialises a wgmma under a branch), so for 80 columns the S x S
-// halves overlap by 16 columns and warpgroup 2 stores only its last 32.
+// Both consumers issue the same shapes (ptxas serialises a wgmma under a branch), so where kCols / 2 is not a
+// multiple of 16 the S x S halves overlap and warpgroup 2 stores only the columns warpgroup 1 does not cover.
 //
 // Both operands come from the sample-major copy of the staged block written by geno_tile_rows_kernel
 // (raw_t[sample / 128][k-step][sample % 128][8 bytes = 32 variants]): K-major, which is what an 8-bit wgmma
@@ -29,8 +32,7 @@
 
 namespace pl2 {
 
-constexpr uint32_t kTsAccCols = 5 * kTsCols;   // 400
-constexpr uint32_t kTsTileAccWords = kTsAccCols * kTileRows;
+constexpr uint32_t kKingTsTileAccWords = 5 * kKingTsCols * kTileRows;
 
 constexpr uint32_t kKwProducerThreads = 128;  // warpgroup 0
 constexpr uint32_t kKwConsumerThreads = 256;  // warpgroups 1, 2
@@ -236,6 +238,171 @@ king_wg_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
   king_acc_add<kCols>(acc_tile + static_cast<uint64_t>((cw ? 3 : 1) * kCols) * kTileRows, acc_y, r, c);  // TH | HH
   // warpgroup 2 skips the columns warpgroup 1 already covers
   king_acc_add<S::kS>(acc_tile + static_cast<uint64_t>(4 * kCols + s_first) * kTileRows, acc_s, r, c, cw ? static_cast<int>((2 * S::kS - kCols) / 8) : 0);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// king_tile128_kernel: one CTA = one whole 128 x 64 pair tile, so each expansion of the column planes feeds 128 rows
+// (king_wg_kernel expands the same columns in both CTAs of a tile).  Three warpgroups:
+//   warpgroup 0:  producer.  One thread brings a stage's raw words into shared memory with bulk copies onto the
+//                 stage's `load` mbarrier (the row words: one contiguous 8 KB piece, [k-step][128 rows][8 B]; the
+//                 column words: 512 B per k-step), one stage ahead; all 128 threads then expand the column words
+//                 from shared memory into the T | H | S planes.  No global load passes through its registers, so
+//                 the proxy fence before the hand-off waits only for its own st.shared.
+//   warpgroups 1, 2:  consumer c owns rows 64 c .. 64 c + 63 and all five products.  The planes are stacked
+//                 T | H | S along N, so per k-step   T_I x [T_J | H_J] (n128) -> TT | TH,
+//                 H_I x [T_J | H_J] (n128) -> HT | HH,   S_I x S_J (n64) -> SS:  160 int32 accumulators per thread,
+//                 which fit once `setmaxnreg` moves registers from the producer (40) to the consumers (232):
+//                 232 * 256 + 40 * 128 = 168 * 384, the launch allocation.
+// The n128 fragments land on accumulator column blocks TT | TH and HT | HH of the raw layout as they are.
+// Hand-off as in king_wg_kernel: `full` (128 producer arrivals after the fence), `empty` (256 consumer arrivals
+// once `wgmma.wait_group 1` has retired the stage), one wgmma group in flight across stage boundaries.
+constexpr uint32_t kK128Ks = 8;      // k32 steps per stage: 256 variants, divides the variant padding
+constexpr uint32_t kK128Stages = 3;
+constexpr uint32_t kK128Sbo = 2 * kK128Ks * kKwChunkBytes;                // next group of 8 samples
+constexpr uint32_t kK128PlaneBytes = (kKingTsCols / 8) * kK128Sbo;        // one plane of the 64 column samples
+constexpr uint32_t kK128BBytes = 3 * kK128PlaneBytes;                     // T | H | S
+constexpr uint32_t kK128ABytes = kK128Ks * kTileRows * 8;                 // row words [k-step][128 rows][8 B]
+constexpr uint32_t kK128WBytes = kK128Ks * kKingTsCols * 8;               // column words [k-step][64 samples][8 B]
+constexpr uint32_t kK128StageBytes = kK128BBytes + kK128ABytes + kK128WBytes;
+constexpr uint32_t kK128SmemBytes = kK128Stages * kK128StageBytes + 128 + 3 * kK128Stages * 8;  // + alignment + mbarriers
+constexpr uint32_t kK128ItemsPerThread = kK128Ks * kKingTsCols / kKwProducerThreads;          // (sample, k-step) words
+static_assert(kKwProducerThreads % kKingTsCols == 0 && (kK128Ks * kKingTsCols) % kKwProducerThreads == 0, "producer item map");
+static_assert(kK128SmemBytes <= kKwSmemLimit, "exceeds the 227 KB shared-memory opt-in limit");
+
+// raw_t: sample-major copy of the whole padded block (sample 0 at row tile 0); grid: one CTA per tile.
+__global__ void __launch_bounds__(kKwThreads, 1)
+king_tile128_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* multiple of 256 */, const uint32_t* __restrict__ tile_order, const uint32_t* __restrict__ tile_rt, const uint32_t* __restrict__ tile_tc, int32_t* __restrict__ raw_acc) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  const uint32_t tid = threadIdx.x;
+  const uint32_t wg = tid >> 7;
+  const uint32_t tile = tile_order[blockIdx.x];
+  const uint32_t rt = tile_rt[tile];
+  const uint32_t ct = tile_tc[tile];
+  const uint32_t kstep_ct = variant_ct_padded / 32;
+  const uint32_t stage_ct = kstep_ct / kK128Ks;
+  const uint32_t smem_base = (static_cast<uint32_t>(__cvta_generic_to_shared(smem)) + 127u) & ~127u;
+  const uint32_t bar_full = smem_base + kK128Stages * kK128StageBytes;  // full[s] = bar_full + 8 s
+  const uint32_t bar_empty = bar_full + kK128Stages * 8;
+  const uint32_t bar_load = bar_empty + kK128Stages * 8;
+  if (tid == 0) {
+    for (uint32_t s = 0; s < kK128Stages; ++s) {
+      mbar_init(bar_full + 8 * s, kKwProducerThreads);
+      mbar_init(bar_empty + 8 * s, kKwConsumerThreads);
+      mbar_init(bar_load + 8 * s, 1);
+    }
+    mbar_init_fence();
+  }
+  __syncthreads();
+
+  const uint32_t thread_zero = tid * (variant_ct_padded >> 31);  // 0; keeps the plane tables in vector registers
+  const uint32_t tab_t = table_reg(kTabHet, thread_zero), tab_h = table_reg(kTabHom, thread_zero), tab_s = table_reg(kTabSgn, thread_zero);
+
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    // ---- producer
+    const uint8_t* a_src = raw_t + static_cast<uint64_t>(rt) * kstep_ct * 1024;
+    // column samples 64 ct .. 64 ct + 63: half (ct & 1) of 128-sample block ct >> 1
+    const uint8_t* w_src = raw_t + static_cast<uint64_t>(ct >> 1) * kstep_ct * 1024 + (ct & 1) * 512;
+    auto issue_loads = [&](uint32_t st, uint32_t slot) {
+      const uint32_t base = smem_base + slot * kK128StageBytes;
+      const uint32_t bar = bar_load + 8 * slot;
+      const uint64_t off = static_cast<uint64_t>(st) * kK128Ks * 1024;
+      mbar_arrive_expect_tx(bar, kK128ABytes + kK128WBytes);
+      bulk_copy_g2s(base + kK128BBytes, a_src + off, kK128ABytes, bar);
+#pragma unroll
+      for (uint32_t ks = 0; ks < kK128Ks; ++ks) bulk_copy_g2s(base + kK128BBytes + kK128ABytes + ks * 512, w_src + off + ks * 1024, 512, bar);
+    };
+    // item q of this thread: column sample n = tid % 64, k-step ks = tid / 64 + 2 q (reads and stores are
+    // contiguous across each quarter warp)
+    const uint32_t n = tid & (kKingTsCols - 1), ks0 = tid / kKingTsCols;
+    constexpr uint32_t kKsStride = kKwProducerThreads / kKingTsCols;
+    const uint32_t w_off = kK128BBytes + kK128ABytes + ks0 * 512 + n * 8;
+    const uint32_t b_off = (n >> 3) * kK128Sbo + 2 * ks0 * kKwChunkBytes + (n & 7) * 16;
+
+    if (tid == 0) issue_loads(0, 0);
+    uint32_t slot = 0, phase = 0;
+    for (uint32_t st = 0; st < stage_ct; ++st) {
+      // the next stage's words go into its slot once the consumers have retired the stage that used it last;
+      // the first pass over the ring finds every slot free (parity 1 = the phase before a fresh barrier's first)
+      const uint32_t nslot = slot + 1 == kK128Stages ? 0 : slot + 1;
+      const uint32_t nphase = nslot ? phase : phase ^ 1;
+      if (st + 1 < stage_ct) {
+        mbar_wait(bar_empty + 8 * nslot, nphase ^ 1);
+        if (tid == 0) issue_loads(st + 1, nslot);
+      }
+      const uint32_t base = smem_base + slot * kK128StageBytes;
+      mbar_wait(bar_load + 8 * slot, phase);
+#pragma unroll
+      for (uint32_t q = 0; q < kK128ItemsPerThread; ++q) {
+        uint2 w;
+        asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w.x), "=r"(w.y) : "r"(base + w_off + q * kKsStride * 512) : "memory");
+        const uint32_t addr = base + b_off + q * kKsStride * 2 * kKwChunkBytes;
+#pragma unroll
+        for (uint32_t h = 0; h < 2; ++h) {
+          const Sel4 sel = make_selectors(h ? w.y : w.x);
+          const uint4 vt = expand16(tab_t, sel), vh = expand16(tab_h, sel), vs = expand16(tab_s, sel);
+          asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + h * kKwChunkBytes), "r"(vt.x), "r"(vt.y), "r"(vt.z), "r"(vt.w) : "memory");
+          asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + kK128PlaneBytes + h * kKwChunkBytes), "r"(vh.x), "r"(vh.y), "r"(vh.z), "r"(vh.w) : "memory");
+          asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + 2 * kK128PlaneBytes + h * kKwChunkBytes), "r"(vs.x), "r"(vs.y), "r"(vs.z), "r"(vs.w) : "memory");
+        }
+      }
+      fence_proxy_async_smem();  // this thread's st.shared -> visible to the consumers' wgmma operand fetch
+      mbar_arrive(bar_full + 8 * slot);
+      slot = nslot;
+      phase = nphase;
+    }
+    return;
+  }
+
+  // ---- consumers
+  setmaxnreg_inc<232>();
+  const uint32_t cw = wg - 1;
+  const uint32_t warp4 = (tid >> 5) & 3;
+  const uint32_t lane = tid & 31;
+  const uint32_t g = lane >> 2, c = lane & 3;
+  int32_t acc_t[kKingTsCols], acc_h[kKingTsCols], acc_s[kKingTsCols / 2];  // TT | TH, HT | HH, SS (n128, n128, n64)
+#pragma unroll
+  for (uint32_t i = 0; i < kKingTsCols; ++i) acc_t[i] = acc_h[i] = 0;
+#pragma unroll
+  for (uint32_t i = 0; i < kKingTsCols / 2; ++i) acc_s[i] = 0;
+  const uint32_t r_lo = 64 * cw + 16 * warp4 + g;  // this thread's fragment rows r_lo, r_lo + 8 of the tile
+
+  uint32_t slot = 0, phase = 0, prev_slot = 0;
+  for (uint32_t st = 0; st < stage_ct; ++st) {
+    mbar_wait(bar_full + 8 * slot, phase);
+    const uint32_t base = smem_base + slot * kK128StageBytes;
+    const uint64_t desc_t = make_wg_desc(base, kKwChunkBytes, kK128Sbo);
+#pragma unroll
+    for (uint32_t ks = 0; ks < kK128Ks; ++ks) {
+      const uint32_t a_row = base + kK128BBytes + ks * kTileRows * 8;
+      uint2 w_lo, w_hi;
+      asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w_lo.x), "=r"(w_lo.y) : "r"(a_row + r_lo * 8) : "memory");
+      asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w_hi.x), "=r"(w_hi.y) : "r"(a_row + (r_lo + 8) * 8) : "memory");
+      const ASel sel = make_asel(w_lo, w_hi, c);
+      uint32_t ft[4], fh[4], fs[4];
+      afrag(tab_t, sel, ft);
+      afrag(tab_h, sel, fh);
+      afrag(tab_s, sel, fs);
+      const uint64_t dk = desc_t + ((ks * 2 * kKwChunkBytes) >> 4);
+      wgmma_fence();
+      wgmma_s8_rs<2 * kKingTsCols>(acc_t, ft, dk);                          // x [T_J | H_J]
+      wgmma_s8_rs<2 * kKingTsCols>(acc_h, fh, dk);                          // x [T_J | H_J]
+      wgmma_s8_rs<kKingTsCols>(acc_s, fs, dk + ((2 * kK128PlaneBytes) >> 4));  // x S_J
+      wgmma_commit();
+      wgmma_wait<1>();
+      // every group but the one just issued has retired, the previous stage's last one included: hand that slot back
+      if (ks == 0 && st > 0) mbar_arrive(bar_empty + 8 * prev_slot);
+    }
+    prev_slot = slot;
+    if (++slot == kK128Stages) slot = 0, phase ^= 1;
+  }
+  wgmma_wait<0>();
+
+  // ---- epilogue: registers -> raw accumulators (+=); rows are in natural sample order
+  int32_t* acc_tile = raw_acc + static_cast<uint64_t>(tile) * kKingTsTileAccWords;
+  king_acc_add<2 * kKingTsCols>(acc_tile, acc_t, r_lo, c);                                                   // TT | TH
+  king_acc_add<2 * kKingTsCols>(acc_tile + static_cast<uint64_t>(2 * kKingTsCols) * kTileRows, acc_h, r_lo, c);  // HT | HH
+  king_acc_add<kKingTsCols>(acc_tile + static_cast<uint64_t>(4 * kKingTsCols) * kTileRows, acc_s, r_lo, c);      // SS
 }
 
 }  // namespace pl2

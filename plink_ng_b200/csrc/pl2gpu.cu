@@ -283,7 +283,7 @@ int pl2gpu_ctx_create(int device_idx, Pl2GpuCtx** ctx_ptr) {
     PL2_CUDA_OK(cudaStreamCreateWithPriority(&ctx->c.copy_stream, cudaStreamNonBlocking, prio_hi));
   }
   PL2_CUDA_OK(cudaFuncSetAttribute(king_wg_kernel<kTileCols>, cudaFuncAttributeMaxDynamicSharedMemorySize, KingWgShape<kTileCols>::kSmemBytes));
-  PL2_CUDA_OK(cudaFuncSetAttribute(king_wg_kernel<kTsCols>, cudaFuncAttributeMaxDynamicSharedMemorySize, KingWgShape<kTsCols>::kSmemBytes));
+  PL2_CUDA_OK(cudaFuncSetAttribute(king_tile128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kK128SmemBytes));
   *ctx_ptr = ctx;
   return 0;
 }
@@ -431,10 +431,10 @@ uint64_t pl2gpu_king_mem_required(uint32_t sample_ct, uint32_t row_start, uint32
   const uint64_t tiles = CountTiles(row_start, row_end, false);
   const uint64_t npad = RoundUpU32(sample_ct, kSamplePad);
   const uint64_t need_ss = tiles * kKingTileAccWords * 4 + cap * (npad / 4) + 3ull * (cap / 32) * npad * 4 + tiles * 16;
-  // 128 x 80 tiles (the default): two raw blocks + two sample-major copies
-  const uint64_t tiles_ts = CountTiles(row_start, row_end, false, kTsCols);
+  // 128 x 64 tiles (the default): two raw blocks + two sample-major copies
+  const uint64_t tiles_ts = CountTiles(row_start, row_end, false, kKingTsCols);
   const uint64_t npad_ts = RoundUpU32(sample_ct, kTsSamplePad);
-  const uint64_t need_ts = tiles_ts * kTsTileAccWords * 4 + 4 * cap * (npad_ts / 4) + tiles_ts * 16;
+  const uint64_t need_ts = tiles_ts * kKingTsTileAccWords * 4 + 4 * cap * (npad_ts / 4) + tiles_ts * 16;
   return (need_ss > need_ts ? need_ss : need_ts) + kKingOutStageBytes + slack;
 }
 
@@ -478,7 +478,7 @@ int pl2gpu_king_begin_ex(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start,
     set_error("pl2gpu_king_begin: cudaEventCreate failed");
     return fail();
   }
-  job->tile_cols = ts ? kTsCols : kTileCols;
+  job->tile_cols = ts ? kKingTsCols : kTileCols;
   if (BuildTileList(row_start, row_end, false, &job->tiles, job->tile_cols)) return fail();
   for (int b = 0; b < (ts ? 2 : 1); ++b) {
     if (StageAlloc(sample_ct, cap, &job->stage[b], ts ? kTsSamplePad : kSamplePad)) return fail();
@@ -543,7 +543,7 @@ static int KingTsPrepAndLaunch(Pl2KingJob* job, uint32_t b, uint32_t cur, bool p
   PL2_CUDA_OK(cudaEventRecord(job->ev_prep_done[b], prep));
   PL2_CUDA_OK(cudaStreamWaitEvent(c->stream, job->ev_prep_done[b], 0));
   PL2_CUDA_OK(cudaEventRecord(job->ev_kernel_start[b], c->stream));
-  king_wg_kernel<kTsCols><<<2 * job->tiles.tile_ct, kKwThreads, KingWgShape<kTsCols>::kSmemBytes, c->stream>>>(job->d_raw_t[b], padded, job->tiles.d_tile_order, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->d_raw_acc);
+  king_tile128_kernel<<<job->tiles.tile_ct, kKwThreads, kK128SmemBytes, c->stream>>>(job->d_raw_t[b], padded, job->tiles.d_tile_order, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->d_raw_acc);
   c->launches++;
   PL2_CUDA_OK(cudaGetLastError());
   PL2_CUDA_OK(cudaEventRecord(job->ev_kernel_done[b], c->stream));
@@ -702,9 +702,9 @@ static int KingGet(Pl2KingJob* job, uint32_t r0, uint32_t r1, void* dst, int dst
         const int32_t* acc0 = job->d_raw_acc + static_cast<uint64_t>(tile_a) * (5ull * job->tile_cols * kTileRows);
         const uint32_t* trt = job->tiles.d_tile_rt + tile_a;
         const uint32_t* ttc = job->tiles.d_tile_tc + tile_a;
-        if (job->tile_cols == kTsCols) {
-          if (kinship) king_finalize_kernel<true, kTsCols><<<grid, 256, 0, c->stream>>>(acc0, trt, ttc, job->sample_ct, cur0, cur1, nullptr, static_cast<double*>(d_dst));
-          else king_finalize_kernel<false, kTsCols><<<grid, 256, 0, c->stream>>>(acc0, trt, ttc, job->sample_ct, cur0, cur1, static_cast<uint32_t*>(d_dst), nullptr);
+        if (job->tile_cols == kKingTsCols) {
+          if (kinship) king_finalize_kernel<true, kKingTsCols><<<grid, 256, 0, c->stream>>>(acc0, trt, ttc, job->sample_ct, cur0, cur1, nullptr, static_cast<double*>(d_dst));
+          else king_finalize_kernel<false, kKingTsCols><<<grid, 256, 0, c->stream>>>(acc0, trt, ttc, job->sample_ct, cur0, cur1, static_cast<uint32_t*>(d_dst), nullptr);
         } else {
           if (kinship) king_finalize_kernel<true, kTileCols><<<grid, 256, 0, c->stream>>>(acc0, trt, ttc, job->sample_ct, cur0, cur1, nullptr, static_cast<double*>(d_dst));
           else king_finalize_kernel<false, kTileCols><<<grid, 256, 0, c->stream>>>(acc0, trt, ttc, job->sample_ct, cur0, cur1, static_cast<uint32_t*>(d_dst), nullptr);
@@ -759,8 +759,8 @@ int pl2gpu_king_get_filtered(Pl2KingJob* job, uint32_t r0, uint32_t r1, double m
       break;
     }
     if (cudaMemsetAsync(d_found, 0, 8, c->stream) != cudaSuccess) break;
-    if (job->tile_cols == kTsCols) {
-      king_filter_kernel<kTsCols><<<job->tiles.tile_ct, kTileRows, 0, c->stream>>>(job->d_raw_acc, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->sample_ct, r0, r1, min_kinship, max_out, d_found, d_pairs, d_counts, d_kin);
+    if (job->tile_cols == kKingTsCols) {
+      king_filter_kernel<kKingTsCols><<<job->tiles.tile_ct, kTileRows, 0, c->stream>>>(job->d_raw_acc, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->sample_ct, r0, r1, min_kinship, max_out, d_found, d_pairs, d_counts, d_kin);
     } else {
       king_filter_kernel<kTileCols><<<job->tiles.tile_ct, kTileRows, 0, c->stream>>>(job->d_raw_acc, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->sample_ct, r0, r1, min_kinship, max_out, d_found, d_pairs, d_counts, d_kin);
     }
@@ -951,8 +951,8 @@ int pl2gpu_king_pairs_end(Pl2KingPairJob* job) {
 // ------------------------------------------------------------------------------------------ probe
 
 int pl2gpu_int8_peak(Pl2GpuCtx* ctx, uint32_t n_cols, int form, double min_seconds, double* tops_out, double* seconds_out) {
-  if (!ctx || !tops_out || (n_cols != 80 && n_cols != 96) || form != 1) {
-    set_error("pl2gpu_int8_peak: bad arguments (n_cols must be 80 or 96, form 1 = A in registers)");
+  if (!ctx || !tops_out || (n_cols != 64 && n_cols != 80 && n_cols != 96 && n_cols != 128) || form != 1) {
+    set_error("pl2gpu_int8_peak: bad arguments (n_cols must be 64, 80, 96 or 128, form 1 = A in registers)");
     return 1;
   }
   Ctx* c = &ctx->c;
@@ -965,8 +965,10 @@ int pl2gpu_int8_peak(Pl2GpuCtx* ctx, uint32_t n_cols, int form, double min_secon
   const uint32_t blocks = 4096;  // x 32 wgmmas x 2 warpgroups per SM
   const double ops_per_launch = 2.0 * 64 * n_cols * 32 * 32.0 * 2 * blocks * c->sm_count;
   auto launch = [&]() {
-    if (n_cols == 80) wgmma_peak_kernel<80><<<c->sm_count, 256, 0, c->stream>>>(blocks, d_sink);
-    else wgmma_peak_kernel<96><<<c->sm_count, 256, 0, c->stream>>>(blocks, d_sink);
+    if (n_cols == 64) wgmma_peak_kernel<64><<<c->sm_count, 256, 0, c->stream>>>(blocks, d_sink);
+    else if (n_cols == 80) wgmma_peak_kernel<80><<<c->sm_count, 256, 0, c->stream>>>(blocks, d_sink);
+    else if (n_cols == 96) wgmma_peak_kernel<96><<<c->sm_count, 256, 0, c->stream>>>(blocks, d_sink);
+    else wgmma_peak_kernel<128><<<c->sm_count, 256, 0, c->stream>>>(blocks, d_sink);
     c->launches++;
   };
   launch();  // warm-up

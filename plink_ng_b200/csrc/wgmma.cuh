@@ -52,6 +52,25 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {
   }
 }
+// initialised mbarriers -> visible to the async proxy (the complete_tx of a bulk copy)
+__device__ __forceinline__ void mbar_init_fence() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+// arrive and add `bytes` to the transaction count the phase waits for
+__device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t bytes) {
+  asm volatile("{\n\t.reg .b64 state;\n\tmbarrier.arrive.expect_tx.shared::cta.b64 state, [%0], %1;\n\t}" ::"r"(bar), "r"(bytes) : "memory");
+}
+// 1-D bulk copy global -> shared (async proxy); its bytes complete on `bar`.  Addresses and size: multiples of 16.
+__device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+}
+// move registers between the warpgroups of a warp-specialised kernel (values: multiples of 8 in [24, 256])
+template <uint32_t kRegs>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs));
+}
+template <uint32_t kRegs>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs));
+}
 
 // A fragment of one k32 step (m64nNk32, 8-bit): thread (warp w of the warpgroup, lane = 4 g + c) holds rows
 // 16 w + g and 16 w + g + 8, K bytes 4 c .. 4 c + 3 (regs 0, 1) and 16 + 4 c .. 16 + 4 c + 3 (regs 2, 3).
