@@ -259,14 +259,16 @@ int pl2gpu_score_get(Pl2ScoreJob* job, double* score_sums, uint64_t* named_dosag
 /* Idempotent; accepts NULL. */
 int pl2gpu_score_end(Pl2ScoreJob* job);
 
-/* ---- measured int8 tensor peak: two warpgroups per SM issue back-to-back int8 wgmma (M = 64, N = n_cols in
- * {64, 80, 96, 128}, K = 32; form 1 = A fragments in registers, B in shared memory, as the KING/GRM kernels use it) for at
- * least min_seconds; *tops_out = 2*64*n_cols*32 ops x wgmmas / elapsed (CUDA events), in TOP/s.
- * This is the roofline denominator bench.py reports against. ---- */
+/* ---- measured tensor peak: two warpgroups per SM issue back-to-back wgmmas with A fragments in registers and B in
+ * shared memory, as the KING/GRM kernels use them, for at least min_seconds.  form 1: int8 (M = 64, N = n_cols in
+ * {64, 80, 96, 128}, K = 32), *tops_out = 2*64*n_cols*32 ops x wgmmas / elapsed (CUDA events), in TOP/s; this is the
+ * roofline denominator bench.py reports against.  form 2: binary AND-POPC (M = 64, N = n_cols in {64, 128}, K = 256
+ * bits), *tops_out = 2*64*n_cols*256 bit ops x wgmmas / elapsed. ---- */
 int pl2gpu_int8_peak(Pl2GpuCtx* ctx, uint32_t n_cols, int form, double min_seconds, double* tops_out, double* seconds_out);
 
 /* ---- self-test of the tensor operand path (fragment / descriptor layout probe); returns 0 iff int8 wgmmas
- * with A fragments in registers and B in the library's shared-memory layout reproduce a scalar host reference. ---- */
+ * with A fragments in registers and B in the library's shared-memory layout reproduce a scalar host reference, and
+ * binary AND-POPC wgmmas in the same layout reproduce a host popcount. ---- */
 int pl2gpu_selftest_umma(Pl2GpuCtx* ctx, int verbose);
 
 #ifdef __cplusplus

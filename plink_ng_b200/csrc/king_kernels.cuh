@@ -189,8 +189,8 @@ king_popc_kernel(const uint32_t* __restrict__ planes, uint32_t sample_ct_padded,
 }
 
 // ---------------------------------------------------------------------------------------------
-// Tensor path: the same five counts as an exact int8 contraction on the tensor pipe,
-// king_tile128_kernel (128 x 64 tiles, the default) and king_wg_kernel<kTileCols> (king_ts_kernel.cuh).
+// Tensor path: the same five counts as exact contractions on the tensor pipe (binary AND-POPC or int8),
+// king_b1_kernel (128 x 64 tiles, the default) and king_wg_kernel<kTileCols> (king_ts_kernel.cuh).
 // ---------------------------------------------------------------------------------------------
 
 // ---------------------------------------------------------------------------------------------

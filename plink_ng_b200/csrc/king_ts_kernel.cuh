@@ -1,9 +1,10 @@
-// king_ts_kernel.cuh - KING pair counts on the int8 tensor pipe (wgmma, sm_90a).
+// king_ts_kernel.cuh - KING pair counts on the tensor pipe (wgmma, sm_90a).
 //
 //   D[r][c] += sum_v A_plane[r][v] * B_plane[c][v],  planes T (het), H (hom), S (+1 hom-REF / -1 hom-ALT),
 // exact int32 sums, the raw accumulator semantics of king_kernels.cuh.  Two kernels:
-//   king_tile128_kernel   the default (`tensor_ts`): one CTA per 128 x 64 pair tile (described below it)
-//   king_wg_kernel<96>    the `tensor` algorithm, an independent cross-check: two CTAs per 128 x 96 pair tile
+//   king_b1_kernel        the default (`tensor_ts`): binary AND-POPC wgmma on bit planes, one CTA per 128 x 64 pair
+//                         tile (described below it)
+//   king_wg_kernel<96>    the `tensor` algorithm, an independent int8 cross-check: two CTAs per 128 x 96 pair tile
 //
 // king_wg_kernel: one CTA = 64 rows (half of a 128-row pair tile) x kCols columns, three warpgroups:
 //   warpgroup 0:  producer - stages the operands of the variant loop in a ring of shared-memory stages
@@ -241,37 +242,59 @@ king_wg_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// king_tile128_kernel: one CTA = one whole 128 x 64 pair tile, so each expansion of the column planes feeds 128 rows
-// (king_wg_kernel expands the same columns in both CTAs of a tile).  Three warpgroups:
+// king_b1_kernel: the KING counts as AND-popcounts of bit planes on the binary tensor pipe (wgmma .b1 AND.POPC,
+// m64nNk256).  From the low and high bits (lo, hi) of each 2-bit code:
+//   T = lo & ~hi (het),  H = ~lo (hom),  R = ~lo & ~hi (hom-REF),  A = ~lo & hi (hom-ALT);
+// missing data and padding (code 3) are zero in every plane.  One CTA = one whole 128 x 64 pair tile, three warpgroups:
 //   warpgroup 0:  producer.  One thread brings a stage's raw words into shared memory with bulk copies onto the
-//                 stage's `load` mbarrier (the row words: one contiguous 8 KB piece, [k-step][128 rows][8 B]; the
-//                 column words: 512 B per k-step), one stage ahead; all 128 threads then expand the column words
-//                 from shared memory into the T | H | S planes.  No global load passes through its registers, so
-//                 the proxy fence before the hand-off waits only for its own st.shared.
-//   warpgroups 1, 2:  consumer c owns rows 64 c .. 64 c + 63 and all five products.  The planes are stacked
-//                 T | H | S along N, so per k-step   T_I x [T_J | H_J] (n128) -> TT | TH,
-//                 H_I x [T_J | H_J] (n128) -> HT | HH,   S_I x S_J (n64) -> SS:  160 int32 accumulators per thread,
-//                 which fit once `setmaxnreg` moves registers from the producer (40) to the consumers (232):
-//                 232 * 256 + 40 * 128 = 168 * 384, the launch allocation.
-// The n128 fragments land on accumulator column blocks TT | TH and HT | HH of the raw layout as they are.
-// Hand-off as in king_wg_kernel: `full` (128 producer arrivals after the fence), `empty` (256 consumer arrivals
-// once `wgmma.wait_group 1` has retired the stage), one wgmma group in flight across stage boundaries.
-constexpr uint32_t kK128Ks = 8;      // k32 steps per stage: 256 variants, divides the variant padding
-constexpr uint32_t kK128Stages = 3;
-constexpr uint32_t kK128Sbo = 2 * kK128Ks * kKwChunkBytes;                // next group of 8 samples
-constexpr uint32_t kK128PlaneBytes = (kKingTsCols / 8) * kK128Sbo;        // one plane of the 64 column samples
-constexpr uint32_t kK128BBytes = 3 * kK128PlaneBytes;                     // T | H | S
-constexpr uint32_t kK128ABytes = kK128Ks * kTileRows * 8;                 // row words [k-step][128 rows][8 B]
-constexpr uint32_t kK128WBytes = kK128Ks * kKingTsCols * 8;               // column words [k-step][64 samples][8 B]
-constexpr uint32_t kK128StageBytes = kK128BBytes + kK128ABytes + kK128WBytes;
-constexpr uint32_t kK128SmemBytes = kK128Stages * kK128StageBytes + 128 + 3 * kK128Stages * 8;  // + alignment + mbarriers
-constexpr uint32_t kK128ItemsPerThread = kK128Ks * kKingTsCols / kKwProducerThreads;          // (sample, k-step) words
-static_assert(kKwProducerThreads % kKingTsCols == 0 && (kK128Ks * kKingTsCols) % kKwProducerThreads == 0, "producer item map");
-static_assert(kK128SmemBytes <= kKwSmemLimit, "exceeds the 227 KB shared-memory opt-in limit");
+//                 stage's `load` mbarrier (the row words: one contiguous piece, [k32 step][128 rows][8 B]; the column
+//                 words: 512 B per k32 step), one stage ahead; all 128 threads then split the column words into the
+//                 four planes T | H | R | A (K-major, no swizzle; one core matrix = 8 samples x 128 variants).
+//   warpgroups 1, 2:  consumer c owns rows 64 c .. 64 c + 63.  Per k256 step it splits its own row words straight
+//                 into fragment registers and issues   T_I x [T_J | H_J] (n128) -> TT | TH,
+//                 H_I x [T_J | H_J] (n128) -> HT | HH,   R_I x A_J + A_I x R_J (n64, one accumulator) -> IBS0:
+//                 160 int32 accumulators per thread, which fit once `setmaxnreg` moves registers from the producer
+//                 (40) to the consumers (232).
+// The epilogue writes SS = HH - 2 IBS0 (= the int8 form's S_I x S_J with S = R - A), so the raw accumulator layout
+// {TT, TH, HT, HH, SS} is that of king_wg_kernel.  Hand-off as in king_wg_kernel: `full` (128 producer arrivals
+// after the fence), `empty` (256 consumer arrivals once `wgmma.wait_group 1` has retired the stage), one wgmma group
+// in flight across stage boundaries.  A stage holds kKb1Ks k256 steps; the last one may be short (the block is padded
+// to 256 variants only): its missing steps are neither copied nor split, and run on zero planes.
+constexpr uint32_t kKb1Ks = 2;       // k256 steps per stage
+constexpr uint32_t kKb1Stages = 4;
+constexpr uint32_t kKb1Sbo = 2 * kKb1Ks * kKwChunkBytes;                 // next group of 8 samples
+constexpr uint32_t kKb1PlaneBytes = (kKingTsCols / 8) * kKb1Sbo;         // one plane of the 64 column samples
+constexpr uint32_t kKb1BBytes = 4 * kKb1PlaneBytes;                      // T | H | R | A
+constexpr uint32_t kKb1AStepBytes = 8 * kTileRows * 8;                   // row words of one k256 step
+constexpr uint32_t kKb1WStepBytes = 8 * kKingTsCols * 8;                 // column words of one k256 step
+constexpr uint32_t kKb1ABytes = kKb1Ks * kKb1AStepBytes;                 // [k32 step][128 rows][8 B]
+constexpr uint32_t kKb1WBytes = kKb1Ks * kKb1WStepBytes;                 // [k32 step][64 samples][8 B]
+constexpr uint32_t kKb1StageBytes = kKb1BBytes + kKb1ABytes + kKb1WBytes;
+constexpr uint32_t kKb1SmemBytes = kKb1Stages * kKb1StageBytes + 128 + 3 * kKb1Stages * 8;  // + alignment + mbarriers
+static_assert(kKwProducerThreads == 2 * kKingTsCols, "producer item map: (column sample, half of a k256 step)");
+static_assert(kKb1SmemBytes <= kKwSmemLimit, "exceeds the 227 KB shared-memory opt-in limit");
+
+// The 64-bit raw word of one sample (32 variants, code of variant v at bits 2 v, 2 v + 1) -> its low and high code
+// bits, variant v at bit v of each.
+__device__ __forceinline__ void split_codes(uint2 w, uint32_t& lo, uint32_t& hi) {
+  uint32_t x[2] = {w.x, w.y};
+#pragma unroll
+  for (int i = 0; i < 2; ++i) {
+    // within each 16 bits: even bits -> byte 0, odd bits -> byte 1
+    uint32_t t = (x[i] ^ (x[i] >> 1)) & 0x22222222u;
+    x[i] ^= t ^ (t << 1);
+    t = (x[i] ^ (x[i] >> 2)) & 0x0C0C0C0Cu;
+    x[i] ^= t ^ (t << 2);
+    t = (x[i] ^ (x[i] >> 4)) & 0x00F000F0u;
+    x[i] ^= t ^ (t << 4);
+  }
+  lo = __byte_perm(x[0], x[1], 0x6420);
+  hi = __byte_perm(x[0], x[1], 0x7531);
+}
 
 // raw_t: sample-major copy of the whole padded block (sample 0 at row tile 0); grid: one CTA per tile.
 __global__ void __launch_bounds__(kKwThreads, 1)
-king_tile128_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* multiple of 256 */, const uint32_t* __restrict__ tile_order, const uint32_t* __restrict__ tile_rt, const uint32_t* __restrict__ tile_tc, int32_t* __restrict__ raw_acc) {
+king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* multiple of 256 */, const uint32_t* __restrict__ tile_order, const uint32_t* __restrict__ tile_rt, const uint32_t* __restrict__ tile_tc, int32_t* __restrict__ raw_acc) {
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t tid = threadIdx.x;
   const uint32_t wg = tid >> 7;
@@ -279,13 +302,14 @@ king_tile128_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padde
   const uint32_t rt = tile_rt[tile];
   const uint32_t ct = tile_tc[tile];
   const uint32_t kstep_ct = variant_ct_padded / 32;
-  const uint32_t stage_ct = kstep_ct / kK128Ks;
+  const uint32_t k256_ct = variant_ct_padded / 256;
+  const uint32_t stage_ct = (k256_ct + kKb1Ks - 1) / kKb1Ks;
   const uint32_t smem_base = (static_cast<uint32_t>(__cvta_generic_to_shared(smem)) + 127u) & ~127u;
-  const uint32_t bar_full = smem_base + kK128Stages * kK128StageBytes;  // full[s] = bar_full + 8 s
-  const uint32_t bar_empty = bar_full + kK128Stages * 8;
-  const uint32_t bar_load = bar_empty + kK128Stages * 8;
+  const uint32_t bar_full = smem_base + kKb1Stages * kKb1StageBytes;  // full[s] = bar_full + 8 s
+  const uint32_t bar_empty = bar_full + kKb1Stages * 8;
+  const uint32_t bar_load = bar_empty + kKb1Stages * 8;
   if (tid == 0) {
-    for (uint32_t s = 0; s < kK128Stages; ++s) {
+    for (uint32_t s = 0; s < kKb1Stages; ++s) {
       mbar_init(bar_full + 8 * s, kKwProducerThreads);
       mbar_init(bar_empty + 8 * s, kKwConsumerThreads);
       mbar_init(bar_load + 8 * s, 1);
@@ -294,57 +318,57 @@ king_tile128_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padde
   }
   __syncthreads();
 
-  const uint32_t thread_zero = tid * (variant_ct_padded >> 31);  // 0; keeps the plane tables in vector registers
-  const uint32_t tab_t = table_reg(kTabHet, thread_zero), tab_h = table_reg(kTabHom, thread_zero), tab_s = table_reg(kTabSgn, thread_zero);
-
   if (wg == 0) {
     setmaxnreg_dec<40>();
     // ---- producer
     const uint8_t* a_src = raw_t + static_cast<uint64_t>(rt) * kstep_ct * 1024;
     // column samples 64 ct .. 64 ct + 63: half (ct & 1) of 128-sample block ct >> 1
     const uint8_t* w_src = raw_t + static_cast<uint64_t>(ct >> 1) * kstep_ct * 1024 + (ct & 1) * 512;
-    auto issue_loads = [&](uint32_t st, uint32_t slot) {
-      const uint32_t base = smem_base + slot * kK128StageBytes;
+    auto issue_loads = [&](uint32_t st, uint32_t slot, uint32_t steps) {
+      const uint32_t base = smem_base + slot * kKb1StageBytes;
       const uint32_t bar = bar_load + 8 * slot;
-      const uint64_t off = static_cast<uint64_t>(st) * kK128Ks * 1024;
-      mbar_arrive_expect_tx(bar, kK128ABytes + kK128WBytes);
-      bulk_copy_g2s(base + kK128BBytes, a_src + off, kK128ABytes, bar);
-#pragma unroll
-      for (uint32_t ks = 0; ks < kK128Ks; ++ks) bulk_copy_g2s(base + kK128BBytes + kK128ABytes + ks * 512, w_src + off + ks * 1024, 512, bar);
+      const uint64_t off = static_cast<uint64_t>(st) * kKb1Ks * 8 * 1024;
+      mbar_arrive_expect_tx(bar, steps * (kKb1AStepBytes + kKb1WStepBytes));
+      bulk_copy_g2s(base + kKb1BBytes, a_src + off, steps * kKb1AStepBytes, bar);
+      for (uint32_t k = 0; k < 8 * steps; ++k) bulk_copy_g2s(base + kKb1BBytes + kKb1ABytes + k * 512, w_src + off + k * 1024, 512, bar);
     };
-    // item q of this thread: column sample n = tid % 64, k-step ks = tid / 64 + 2 q (reads and stores are
-    // contiguous across each quarter warp)
-    const uint32_t n = tid & (kKingTsCols - 1), ks0 = tid / kKingTsCols;
-    constexpr uint32_t kKsStride = kKwProducerThreads / kKingTsCols;
-    const uint32_t w_off = kK128BBytes + kK128ABytes + ks0 * 512 + n * 8;
-    const uint32_t b_off = (n >> 3) * kK128Sbo + 2 * ks0 * kKwChunkBytes + (n & 7) * 16;
+    // item of this thread in each k256 step j: column sample n = tid % 64, k32 steps 8 j + 4 h .. 8 j + 4 h + 3
+    // (h = tid / 64), i.e. the 16-byte half h of row n of each plane's core matrices for step j
+    const uint32_t n = tid & (kKingTsCols - 1), h = tid / kKingTsCols;
+    const uint32_t w_off = kKb1BBytes + kKb1ABytes + 4 * h * 512 + n * 8;
+    const uint32_t b_off = (n >> 3) * kKb1Sbo + h * kKwChunkBytes + (n & 7) * 16;
+    auto steps_of = [&](uint32_t st) { return min(kKb1Ks, k256_ct - st * kKb1Ks); };
 
-    if (tid == 0) issue_loads(0, 0);
+    if (tid == 0) issue_loads(0, 0, steps_of(0));
     uint32_t slot = 0, phase = 0;
     for (uint32_t st = 0; st < stage_ct; ++st) {
       // the next stage's words go into its slot once the consumers have retired the stage that used it last;
       // the first pass over the ring finds every slot free (parity 1 = the phase before a fresh barrier's first)
-      const uint32_t nslot = slot + 1 == kK128Stages ? 0 : slot + 1;
+      const uint32_t nslot = slot + 1 == kKb1Stages ? 0 : slot + 1;
       const uint32_t nphase = nslot ? phase : phase ^ 1;
       if (st + 1 < stage_ct) {
         mbar_wait(bar_empty + 8 * nslot, nphase ^ 1);
-        if (tid == 0) issue_loads(st + 1, nslot);
+        if (tid == 0) issue_loads(st + 1, nslot, steps_of(st + 1));
       }
-      const uint32_t base = smem_base + slot * kK128StageBytes;
+      const uint32_t base = smem_base + slot * kKb1StageBytes;
+      const uint32_t steps = steps_of(st);
       mbar_wait(bar_load + 8 * slot, phase);
 #pragma unroll
-      for (uint32_t q = 0; q < kK128ItemsPerThread; ++q) {
-        uint2 w;
-        asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w.x), "=r"(w.y) : "r"(base + w_off + q * kKsStride * 512) : "memory");
-        const uint32_t addr = base + b_off + q * kKsStride * 2 * kKwChunkBytes;
+      for (uint32_t j = 0; j < kKb1Ks; ++j) {
+        uint32_t lo[4] = {~0u, ~0u, ~0u, ~0u}, hi[4] = {~0u, ~0u, ~0u, ~0u};  // missing step: code 3, zero planes
+        if (j < steps) {
 #pragma unroll
-        for (uint32_t h = 0; h < 2; ++h) {
-          const Sel4 sel = make_selectors(h ? w.y : w.x);
-          const uint4 vt = expand16(tab_t, sel), vh = expand16(tab_h, sel), vs = expand16(tab_s, sel);
-          asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + h * kKwChunkBytes), "r"(vt.x), "r"(vt.y), "r"(vt.z), "r"(vt.w) : "memory");
-          asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + kK128PlaneBytes + h * kKwChunkBytes), "r"(vh.x), "r"(vh.y), "r"(vh.z), "r"(vh.w) : "memory");
-          asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + 2 * kK128PlaneBytes + h * kKwChunkBytes), "r"(vs.x), "r"(vs.y), "r"(vs.z), "r"(vs.w) : "memory");
+          for (uint32_t q = 0; q < 4; ++q) {
+            uint2 w;
+            asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w.x), "=r"(w.y) : "r"(base + w_off + (8 * j + q) * 512) : "memory");
+            split_codes(w, lo[q], hi[q]);
+          }
         }
+        const uint32_t addr = base + b_off + 2 * j * kKwChunkBytes;
+        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(lo[0] & ~hi[0]), "r"(lo[1] & ~hi[1]), "r"(lo[2] & ~hi[2]), "r"(lo[3] & ~hi[3]) : "memory");
+        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + kKb1PlaneBytes), "r"(~lo[0]), "r"(~lo[1]), "r"(~lo[2]), "r"(~lo[3]) : "memory");
+        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + 2 * kKb1PlaneBytes), "r"(~(lo[0] | hi[0])), "r"(~(lo[1] | hi[1])), "r"(~(lo[2] | hi[2])), "r"(~(lo[3] | hi[3])) : "memory");
+        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + 3 * kKb1PlaneBytes), "r"(~lo[0] & hi[0]), "r"(~lo[1] & hi[1]), "r"(~lo[2] & hi[2]), "r"(~lo[3] & hi[3]) : "memory");
       }
       fence_proxy_async_smem();  // this thread's st.shared -> visible to the consumers' wgmma operand fetch
       mbar_arrive(bar_full + 8 * slot);
@@ -360,49 +384,67 @@ king_tile128_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padde
   const uint32_t warp4 = (tid >> 5) & 3;
   const uint32_t lane = tid & 31;
   const uint32_t g = lane >> 2, c = lane & 3;
-  int32_t acc_t[kKingTsCols], acc_h[kKingTsCols], acc_s[kKingTsCols / 2];  // TT | TH, HT | HH, SS (n128, n128, n64)
+  int32_t acc_t[kKingTsCols], acc_h[kKingTsCols], acc_i[kKingTsCols / 2];  // TT | TH, HT | HH, IBS0 (n128, n128, n64)
 #pragma unroll
   for (uint32_t i = 0; i < kKingTsCols; ++i) acc_t[i] = acc_h[i] = 0;
 #pragma unroll
-  for (uint32_t i = 0; i < kKingTsCols / 2; ++i) acc_s[i] = 0;
+  for (uint32_t i = 0; i < kKingTsCols / 2; ++i) acc_i[i] = 0;
   const uint32_t r_lo = 64 * cw + 16 * warp4 + g;  // this thread's fragment rows r_lo, r_lo + 8 of the tile
 
   uint32_t slot = 0, phase = 0, prev_slot = 0;
   for (uint32_t st = 0; st < stage_ct; ++st) {
     mbar_wait(bar_full + 8 * slot, phase);
-    const uint32_t base = smem_base + slot * kK128StageBytes;
-    const uint64_t desc_t = make_wg_desc(base, kKwChunkBytes, kK128Sbo);
+    const uint32_t base = smem_base + slot * kKb1StageBytes;
+    const uint32_t steps = min(kKb1Ks, k256_ct - st * kKb1Ks);
+    const uint64_t desc = make_wg_desc(base, kKwChunkBytes, kKb1Sbo);
 #pragma unroll
-    for (uint32_t ks = 0; ks < kK128Ks; ++ks) {
-      const uint32_t a_row = base + kK128BBytes + ks * kTileRows * 8;
-      uint2 w_lo, w_hi;
-      asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w_lo.x), "=r"(w_lo.y) : "r"(a_row + r_lo * 8) : "memory");
-      asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w_hi.x), "=r"(w_hi.y) : "r"(a_row + (r_lo + 8) * 8) : "memory");
-      const ASel sel = make_asel(w_lo, w_hi, c);
-      uint32_t ft[4], fh[4], fs[4];
-      afrag(tab_t, sel, ft);
-      afrag(tab_h, sel, fh);
-      afrag(tab_s, sel, fs);
-      const uint64_t dk = desc_t + ((ks * 2 * kKwChunkBytes) >> 4);
+    for (uint32_t j = 0; j < kKb1Ks; ++j) {
+      // fragment register q: row r_lo + 8 (q & 1), K bits 32 (c + 4 (q >> 1)) .. of the step = k32 step c + 4 (q >> 1)
+      uint32_t lo[4] = {~0u, ~0u, ~0u, ~0u}, hi[4] = {~0u, ~0u, ~0u, ~0u};  // missing step: code 3, zero planes
+      if (j < steps) {
+#pragma unroll
+        for (uint32_t q = 0; q < 4; ++q) {
+          uint2 w;
+          const uint32_t a = base + kKb1BBytes + (8 * j + c + 4 * (q >> 1)) * (kTileRows * 8) + (r_lo + 8 * (q & 1)) * 8;
+          asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w.x), "=r"(w.y) : "r"(a) : "memory");
+          split_codes(w, lo[q], hi[q]);
+        }
+      }
+      uint32_t ft[4], fh[4], fr[4], fa[4];
+#pragma unroll
+      for (uint32_t q = 0; q < 4; ++q) {
+        ft[q] = lo[q] & ~hi[q];
+        fh[q] = ~lo[q];
+        fr[q] = ~(lo[q] | hi[q]);
+        fa[q] = ~lo[q] & hi[q];
+      }
+      const uint64_t dk = desc + ((j * 2 * kKwChunkBytes) >> 4);
       wgmma_fence();
-      wgmma_s8_rs<2 * kKingTsCols>(acc_t, ft, dk);                          // x [T_J | H_J]
-      wgmma_s8_rs<2 * kKingTsCols>(acc_h, fh, dk);                          // x [T_J | H_J]
-      wgmma_s8_rs<kKingTsCols>(acc_s, fs, dk + ((2 * kK128PlaneBytes) >> 4));  // x S_J
+      wgmma_b1_rs<2 * kKingTsCols>(acc_t, ft, dk);                               // x [T_J | H_J]
+      wgmma_b1_rs<2 * kKingTsCols>(acc_h, fh, dk);                               // x [T_J | H_J]
+      wgmma_b1_rs<kKingTsCols>(acc_i, fr, dk + ((3 * kKb1PlaneBytes) >> 4));     // R_I x A_J
+      wgmma_b1_rs<kKingTsCols>(acc_i, fa, dk + ((2 * kKb1PlaneBytes) >> 4));     // + A_I x R_J
       wgmma_commit();
       wgmma_wait<1>();
       // every group but the one just issued has retired, the previous stage's last one included: hand that slot back
-      if (ks == 0 && st > 0) mbar_arrive(bar_empty + 8 * prev_slot);
+      if (j == 0 && st > 0) mbar_arrive(bar_empty + 8 * prev_slot);
     }
     prev_slot = slot;
-    if (++slot == kK128Stages) slot = 0, phase ^= 1;
+    if (++slot == kKb1Stages) slot = 0, phase ^= 1;
   }
   wgmma_wait<0>();
+  wgmma_fence_operand(acc_t);
+  wgmma_fence_operand(acc_h);
+  wgmma_fence_operand(acc_i);
 
-  // ---- epilogue: registers -> raw accumulators (+=); rows are in natural sample order
+  // ---- epilogue: registers -> raw accumulators (+=); rows are in natural sample order.  HH column 8 j + .. sits
+  // in acc_h[32 + 4 j + i], the IBS0 of the same pair in acc_i[4 j + i]: SS = HH - 2 IBS0 in place.
+#pragma unroll
+  for (uint32_t i = 0; i < kKingTsCols / 2; ++i) acc_i[i] = acc_h[kKingTsCols / 2 + i] - 2 * acc_i[i];
   int32_t* acc_tile = raw_acc + static_cast<uint64_t>(tile) * kKingTsTileAccWords;
   king_acc_add<2 * kKingTsCols>(acc_tile, acc_t, r_lo, c);                                                   // TT | TH
   king_acc_add<2 * kKingTsCols>(acc_tile + static_cast<uint64_t>(2 * kKingTsCols) * kTileRows, acc_h, r_lo, c);  // HT | HH
-  king_acc_add<kKingTsCols>(acc_tile + static_cast<uint64_t>(4 * kKingTsCols) * kTileRows, acc_s, r_lo, c);      // SS
+  king_acc_add<kKingTsCols>(acc_tile + static_cast<uint64_t>(4 * kKingTsCols) * kTileRows, acc_i, r_lo, c);      // SS
 }
 
 }  // namespace pl2

@@ -283,7 +283,7 @@ int pl2gpu_ctx_create(int device_idx, Pl2GpuCtx** ctx_ptr) {
     PL2_CUDA_OK(cudaStreamCreateWithPriority(&ctx->c.copy_stream, cudaStreamNonBlocking, prio_hi));
   }
   PL2_CUDA_OK(cudaFuncSetAttribute(king_wg_kernel<kTileCols>, cudaFuncAttributeMaxDynamicSharedMemorySize, KingWgShape<kTileCols>::kSmemBytes));
-  PL2_CUDA_OK(cudaFuncSetAttribute(king_tile128_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kK128SmemBytes));
+  PL2_CUDA_OK(cudaFuncSetAttribute(king_b1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kKb1SmemBytes));
   *ctx_ptr = ctx;
   return 0;
 }
@@ -543,7 +543,7 @@ static int KingTsPrepAndLaunch(Pl2KingJob* job, uint32_t b, uint32_t cur, bool p
   PL2_CUDA_OK(cudaEventRecord(job->ev_prep_done[b], prep));
   PL2_CUDA_OK(cudaStreamWaitEvent(c->stream, job->ev_prep_done[b], 0));
   PL2_CUDA_OK(cudaEventRecord(job->ev_kernel_start[b], c->stream));
-  king_tile128_kernel<<<job->tiles.tile_ct, kKwThreads, kK128SmemBytes, c->stream>>>(job->d_raw_t[b], padded, job->tiles.d_tile_order, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->d_raw_acc);
+  king_b1_kernel<<<job->tiles.tile_ct, kKwThreads, kKb1SmemBytes, c->stream>>>(job->d_raw_t[b], padded, job->tiles.d_tile_order, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->d_raw_acc);
   c->launches++;
   PL2_CUDA_OK(cudaGetLastError());
   PL2_CUDA_OK(cudaEventRecord(job->ev_kernel_done[b], c->stream));
@@ -951,8 +951,8 @@ int pl2gpu_king_pairs_end(Pl2KingPairJob* job) {
 // ------------------------------------------------------------------------------------------ probe
 
 int pl2gpu_int8_peak(Pl2GpuCtx* ctx, uint32_t n_cols, int form, double min_seconds, double* tops_out, double* seconds_out) {
-  if (!ctx || !tops_out || (n_cols != 64 && n_cols != 80 && n_cols != 96 && n_cols != 128) || form != 1) {
-    set_error("pl2gpu_int8_peak: bad arguments (n_cols must be 64, 80, 96 or 128, form 1 = A in registers)");
+  if (!ctx || !tops_out || (form != 1 && form != 2) || (n_cols != 64 && n_cols != 128 && (form == 2 || (n_cols != 80 && n_cols != 96)))) {
+    set_error("pl2gpu_int8_peak: bad arguments (form 1 = int8, n_cols 64, 80, 96 or 128; form 2 = b1 AND-POPC, n_cols 64 or 128)");
     return 1;
   }
   Ctx* c = &ctx->c;
@@ -963,9 +963,12 @@ int pl2gpu_int8_peak(Pl2GpuCtx* ctx, uint32_t n_cols, int form, double min_secon
   PL2_CUDA_OK(cudaEventCreate(&e0));
   PL2_CUDA_OK(cudaEventCreate(&e1));
   const uint32_t blocks = 4096;  // x 32 wgmmas x 2 warpgroups per SM
-  const double ops_per_launch = 2.0 * 64 * n_cols * 32 * 32.0 * 2 * blocks * c->sm_count;
+  const double k_per_wgmma = form == 2 ? 256 : 32;
+  const double ops_per_launch = 2.0 * 64 * n_cols * k_per_wgmma * 32.0 * 2 * blocks * c->sm_count;
   auto launch = [&]() {
-    if (n_cols == 64) wgmma_peak_kernel<64><<<c->sm_count, 256, 0, c->stream>>>(blocks, d_sink);
+    if (form == 2 && n_cols == 64) wgmma_b1_peak_kernel<64><<<c->sm_count, 256, 0, c->stream>>>(blocks, d_sink);
+    else if (form == 2) wgmma_b1_peak_kernel<128><<<c->sm_count, 256, 0, c->stream>>>(blocks, d_sink);
+    else if (n_cols == 64) wgmma_peak_kernel<64><<<c->sm_count, 256, 0, c->stream>>>(blocks, d_sink);
     else if (n_cols == 80) wgmma_peak_kernel<80><<<c->sm_count, 256, 0, c->stream>>>(blocks, d_sink);
     else if (n_cols == 96) wgmma_peak_kernel<96><<<c->sm_count, 256, 0, c->stream>>>(blocks, d_sink);
     else wgmma_peak_kernel<128><<<c->sm_count, 256, 0, c->stream>>>(blocks, d_sink);
@@ -997,7 +1000,9 @@ int pl2gpu_int8_peak(Pl2GpuCtx* ctx, uint32_t n_cols, int form, double min_secon
 }
 
 // The int8 wgmma form of every tensor kernel (A fragments in registers, B K-major in shared memory) against a
-// scalar product on the host: M = 64, N = 80, K = 64 (two k-steps).
+// scalar product on the host: M = 64, N = 80, K = 64 (two k-steps); then the binary AND-POPC form against a host
+// popcount: M = 64, N = 64, K = 512 bits (two k256 steps), which fixes how the 32 K-bits of an A fragment register
+// line up with the bits of a B row in shared memory.
 int pl2gpu_selftest_umma(Pl2GpuCtx* ctx, int verbose) {
   if (!ctx) {
     set_error("pl2gpu_selftest_umma: null context");
@@ -1042,6 +1047,39 @@ int pl2gpu_selftest_umma(Pl2GpuCtx* ctx, int verbose) {
     }
   if (bad) {
     set_error("pl2gpu_selftest_umma: %u of %u accumulator entries differ from the scalar reference", bad, M * N);
+    return 1;
+  }
+
+  constexpr uint32_t kB1Words = kProbeB1K / 32, kB1N = kProbeB1N;
+  std::vector<uint32_t> ab(M * kB1Words), bb(kB1N * kB1Words);
+  for (auto& v : ab) v = (seed = seed * 1664525u + 1013904223u);
+  for (auto& v : bb) v = (seed = seed * 1664525u + 1013904223u) ^ (seed >> 13);
+  std::vector<int32_t> db(M * kB1N);
+  uint32_t *d_ab = nullptr, *d_bb = nullptr;
+  PL2_CUDA_OK(cudaMalloc(&d_ab, 4ull * ab.size()));
+  PL2_CUDA_OK(cudaMalloc(&d_bb, 4ull * bb.size()));
+  PL2_CUDA_OK(cudaMalloc(&d_d, 4ull * db.size()));
+  PL2_CUDA_OK(cudaMemcpyAsync(d_ab, ab.data(), 4ull * ab.size(), cudaMemcpyHostToDevice, c->stream));
+  PL2_CUDA_OK(cudaMemcpyAsync(d_bb, bb.data(), 4ull * bb.size(), cudaMemcpyHostToDevice, c->stream));
+  wgmma_b1_probe_kernel<<<1, 128, 0, c->stream>>>(d_ab, d_bb, d_d);
+  c->launches++;
+  PL2_CUDA_OK(cudaGetLastError());
+  PL2_CUDA_OK(cudaMemcpyAsync(db.data(), d_d, 4ull * db.size(), cudaMemcpyDeviceToHost, c->stream));
+  PL2_CUDA_OK(cudaStreamSynchronize(c->stream));
+  cudaFree(d_ab);
+  cudaFree(d_bb);
+  cudaFree(d_d);
+  for (uint32_t m = 0; m < M; ++m)
+    for (uint32_t n = 0; n < kB1N; ++n) {
+      int32_t ref = 0;
+      for (uint32_t w = 0; w < kB1Words; ++w) ref += __builtin_popcount(ab[m * kB1Words + w] & bb[n * kB1Words + w]);
+      if (ref != db[m * kB1N + n]) {
+        if (verbose && bad < 8) fprintf(stderr, "selftest_umma b1 mismatch m=%u n=%u got=%d want=%d\n", m, n, db[m * kB1N + n], ref);
+        ++bad;
+      }
+    }
+  if (bad) {
+    set_error("pl2gpu_selftest_umma: %u of %u binary AND-POPC accumulator entries differ from the host popcount", bad, M * kB1N);
     return 1;
   }
   return 0;

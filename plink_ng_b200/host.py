@@ -83,7 +83,7 @@ class GpuContext:
         return int(lib.pl2gpu_ctx_stream(self._h) or 0)
 
     def int8_peak(self, n_cols: int = 96, form: int = 1, min_seconds: float = 2.0):
-        """Measured chip-wide int8 wgmma rate (TOP/s, seconds): the roofline denominator."""
+        """Measured chip-wide wgmma rate (TOP/s, seconds): form 1 int8 (the roofline denominator), form 2 binary AND-POPC."""
         tops, secs = C.c_double(), C.c_double()
         check(lib.pl2gpu_int8_peak(self._h, n_cols, form, min_seconds, C.byref(tops), C.byref(secs)), "pl2gpu_int8_peak")
         return float(tops.value), float(secs.value)
