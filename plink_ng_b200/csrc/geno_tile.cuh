@@ -18,6 +18,12 @@ static_assert(kTsSamplePad % 128 == 0 && kTsSamplePad % kKingTsCols == 0, "padde
 // One CTA = 64 variants x 64 samples through a shared-memory byte tile.
 // Only samples [s_base, s_base + 64 * gridDim.y) are written (a job re-tiles its own row tiles only);
 // row tile s_base / 128 is stored at index 0.
+// The 8 bytes of a word hold, by kSplitBits:
+//   false  the 2-bit codes, variant 32 k + v at bits 2 v, 2 v + 1 (the staged block's own form; GRM, PCA and
+//          king_wg_kernel read this)
+//   true   {lo32, hi32}: bit v of lo32 is the low code bit of variant 32 k + v, bit v of hi32 its high bit (the
+//          default KING path, king_b1_kernel: its bit planes are single LOP3s of these halves)
+template <bool kSplitBits = false>
 static __global__ void __launch_bounds__(256) geno_tile_rows_kernel(const uint8_t* __restrict__ raw, uint32_t pitch, uint32_t kstep_ct, uint32_t s_base, uint8_t* __restrict__ raw_i) {
   __shared__ uint8_t tile[64][68];
   const uint32_t v0 = blockIdx.x * 64, s0 = s_base + blockIdx.y * 64;
@@ -32,8 +38,22 @@ static __global__ void __launch_bounds__(256) geno_tile_rows_kernel(const uint8_
   {
     const uint32_t sl = t >> 2, vw = t & 3;
     uint32_t w = 0;
+    if constexpr (kSplitBits) {
+      uint32_t lo = 0, hi = 0;
 #pragma unroll
-    for (uint32_t j = 0; j < 16; ++j) w |= static_cast<uint32_t>(tile[16 * vw + j][sl]) << (2 * j);
+      for (uint32_t j = 0; j < 16; ++j) {
+        const uint32_t code = tile[16 * vw + j][sl];
+        lo |= (code & 1u) << j;
+        hi |= (code >> 1) << j;
+      }
+      // lanes t, t ^ 1 hold the two 16-variant halves of one word: the even lane writes lo32, the odd one hi32
+      const uint32_t odd = vw & 1;
+      const uint32_t other = __shfl_xor_sync(0xFFFFFFFFu, odd ? lo : hi, 1);
+      w = odd ? other | (hi << 16) : lo | (other << 16);
+    } else {
+#pragma unroll
+      for (uint32_t j = 0; j < 16; ++j) w |= static_cast<uint32_t>(tile[16 * vw + j][sl]) << (2 * j);
+    }
     const uint32_t s = s0 + sl, v = v0 + 16 * vw;
     *reinterpret_cast<uint32_t*>(raw_i + (static_cast<uint64_t>((s - s_base) >> 7) * kstep_ct + (v >> 5)) * 1024 + (s & 127) * 8 + 4 * ((v >> 4) & 1)) = w;
   }

@@ -243,14 +243,15 @@ king_wg_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
 
 // ---------------------------------------------------------------------------------------------------------------
 // king_b1_kernel: the KING counts as AND-popcounts of bit planes on the binary tensor pipe (wgmma .b1 AND.POPC,
-// m64nNk256).  From the low and high bits (lo, hi) of each 2-bit code:
+// m64nNk256).  From the low and high bits (lo, hi) of each 2-bit code, which the split form of the sample-major copy
+// (geno_tile_rows_kernel<true>) already holds as two 32-variant halves of each word:
 //   T = lo & ~hi (het),  H = ~lo (hom),  R = ~lo & ~hi (hom-REF),  A = ~lo & hi (hom-ALT);
 // missing data and padding (code 3) are zero in every plane.  One CTA = one whole 128 x 64 pair tile, three warpgroups:
 //   warpgroup 0:  producer.  One thread brings a stage's raw words into shared memory with bulk copies onto the
 //                 stage's `load` mbarrier (the row words: one contiguous piece, [k32 step][128 rows][8 B]; the column
-//                 words: 512 B per k32 step), one stage ahead; all 128 threads then split the column words into the
+//                 words: 512 B per k32 step), one stage ahead; all 128 threads then turn the column words into the
 //                 four planes T | H | R | A (K-major, no swizzle; one core matrix = 8 samples x 128 variants).
-//   warpgroups 1, 2:  consumer c owns rows 64 c .. 64 c + 63.  Per k256 step it splits its own row words straight
+//   warpgroups 1, 2:  consumer c owns rows 64 c .. 64 c + 63.  Per k256 step it turns its own row words straight
 //                 into fragment registers and issues   T_I x [T_J | H_J] (n128) -> TT | TH,
 //                 H_I x [T_J | H_J] (n128) -> HT | HH,   R_I x A_J + A_I x R_J (n64, one accumulator) -> IBS0:
 //                 160 int32 accumulators per thread, which fit once `setmaxnreg` moves registers from the producer
@@ -274,25 +275,8 @@ constexpr uint32_t kKb1SmemBytes = kKb1Stages * kKb1StageBytes + 128 + 3 * kKb1S
 static_assert(kKwProducerThreads == 2 * kKingTsCols, "producer item map: (column sample, half of a k256 step)");
 static_assert(kKb1SmemBytes <= kKwSmemLimit, "exceeds the 227 KB shared-memory opt-in limit");
 
-// The 64-bit raw word of one sample (32 variants, code of variant v at bits 2 v, 2 v + 1) -> its low and high code
-// bits, variant v at bit v of each.
-__device__ __forceinline__ void split_codes(uint2 w, uint32_t& lo, uint32_t& hi) {
-  uint32_t x[2] = {w.x, w.y};
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    // within each 16 bits: even bits -> byte 0, odd bits -> byte 1
-    uint32_t t = (x[i] ^ (x[i] >> 1)) & 0x22222222u;
-    x[i] ^= t ^ (t << 1);
-    t = (x[i] ^ (x[i] >> 2)) & 0x0C0C0C0Cu;
-    x[i] ^= t ^ (t << 2);
-    t = (x[i] ^ (x[i] >> 4)) & 0x00F000F0u;
-    x[i] ^= t ^ (t << 4);
-  }
-  lo = __byte_perm(x[0], x[1], 0x6420);
-  hi = __byte_perm(x[0], x[1], 0x7531);
-}
-
-// raw_t: sample-major copy of the whole padded block (sample 0 at row tile 0); grid: one CTA per tile.
+// raw_t: sample-major copy of the whole padded block (sample 0 at row tile 0) in the split form of
+// geno_tile_rows_kernel<true>: each 8-byte word is {lo32, hi32} of 32 variants; grid: one CTA per tile.
 __global__ void __launch_bounds__(kKwThreads, 1)
 king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* multiple of 256 */, const uint32_t* __restrict__ tile_order, const uint32_t* __restrict__ tile_rt, const uint32_t* __restrict__ tile_tc, int32_t* __restrict__ raw_acc) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -358,11 +342,8 @@ king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
         uint32_t lo[4] = {~0u, ~0u, ~0u, ~0u}, hi[4] = {~0u, ~0u, ~0u, ~0u};  // missing step: code 3, zero planes
         if (j < steps) {
 #pragma unroll
-          for (uint32_t q = 0; q < 4; ++q) {
-            uint2 w;
-            asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w.x), "=r"(w.y) : "r"(base + w_off + (8 * j + q) * 512) : "memory");
-            split_codes(w, lo[q], hi[q]);
-          }
+          for (uint32_t q = 0; q < 4; ++q)
+            asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(lo[q]), "=r"(hi[q]) : "r"(base + w_off + (8 * j + q) * 512) : "memory");
         }
         const uint32_t addr = base + b_off + 2 * j * kKwChunkBytes;
         asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(lo[0] & ~hi[0]), "r"(lo[1] & ~hi[1]), "r"(lo[2] & ~hi[2]), "r"(lo[3] & ~hi[3]) : "memory");
@@ -404,10 +385,8 @@ king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
       if (j < steps) {
 #pragma unroll
         for (uint32_t q = 0; q < 4; ++q) {
-          uint2 w;
           const uint32_t a = base + kKb1BBytes + (8 * j + c + 4 * (q >> 1)) * (kTileRows * 8) + (r_lo + 8 * (q & 1)) * 8;
-          asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(w.x), "=r"(w.y) : "r"(a) : "memory");
-          split_codes(w, lo[q], hi[q]);
+          asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(lo[q]), "=r"(hi[q]) : "r"(a) : "memory");
         }
       }
       uint32_t ft[4], fh[4], fr[4], fa[4];

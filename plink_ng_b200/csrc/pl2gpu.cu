@@ -224,7 +224,7 @@ struct Pl2KingJob {
   // row re-tiling of batch k+1 (prep stream) overlap the tensor kernel of batch k (compute stream).
   // The other algorithms use buffer 0 on the compute stream only.
   GenoStage stage[2];
-  uint8_t* d_raw_t[2] = {nullptr, nullptr};  // tensor paths: sample-major copy of the staged block (geno_tile.cuh)
+  uint8_t* d_raw_t[2] = {nullptr, nullptr};  // tensor paths: sample-major copy of the staged block (geno_tile.cuh; split form on the TS path)
   cudaEvent_t ev_prep_done[2] = {nullptr, nullptr};
   cudaEvent_t ev_kernel_start[2] = {nullptr, nullptr};  // timing-enabled pair around the tensor kernel (pl2gpu_king_last_kernel_ms)
   cudaEvent_t ev_kernel_done[2] = {nullptr, nullptr};
@@ -537,7 +537,7 @@ static int KingTsPrepAndLaunch(Pl2KingJob* job, uint32_t b, uint32_t cur, bool p
     job->kernel_pending[b] = true;
     return 0;
   }
-  geno_tile_rows_kernel<<<dim3(padded / 64, st.sample_ct_padded / 64), 256, 0, prep>>>(st.d_raw, st.pitch, padded / 32, 0, job->d_raw_t[b]);
+  geno_tile_rows_kernel<true><<<dim3(padded / 64, st.sample_ct_padded / 64), 256, 0, prep>>>(st.d_raw, st.pitch, padded / 32, 0, job->d_raw_t[b]);
   c->launches++;
   PL2_CUDA_OK(cudaGetLastError());
   PL2_CUDA_OK(cudaEventRecord(job->ev_prep_done[b], prep));
