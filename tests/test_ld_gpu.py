@@ -39,10 +39,14 @@ def test_geno_counts(gpu_ctx):
     assert np.array_equal(got.astype(np.int64), want)
 
 
-@pytest.mark.parametrize("n,m,band", [(64, 200, 17), (333, 700, 49), (1000, 300, 130), (2100, 900, 500)])
+_FOUNDER_EDGES = [(n, 300, 70) for n in (1, 2, 31, 32, 33, 63, 65, 127, 129)]  # 64-founder stages
+_BAND_EDGES = [(150, 700, band) for band in (1, 2, 63, 64, 65, 127, 128, 129)] + [(150, 120, 200)]  # column tiles of 64; band > m
+
+
+@pytest.mark.parametrize("n,m,band", [(64, 200, 17), (333, 700, 49), (1000, 300, 130), (2100, 900, 500)] + _FOUNDER_EDGES + _BAND_EDGES)
 def test_ld_band_flags_match_oracle(gpu_ctx, n, m, band):
     """The pair kernel (int8 tensor contraction over the founders, ld_ts_kernel.cuh) against the oracle's exact
-    integer sums and fp64 test, pair by pair."""
+    integer sums and fp64 test, pair by pair (only pairs with b >= 0: the other entries of a row are never written)."""
     g = _ld_geno(m, n, seed=n + m)
     thr = 0.2 * (1 + orc.SMALL_EPSILON)
     got = ld_band_flags(gpu_ctx, pack_genotypes(g), n, band, thr)
