@@ -266,6 +266,12 @@ int pl2gpu_score_end(Pl2ScoreJob* job);
  * bits), *tops_out = 2*64*n_cols*256 bit ops x wgmmas / elapsed. ---- */
 int pl2gpu_int8_peak(Pl2GpuCtx* ctx, uint32_t n_cols, int form, double min_seconds, double* tops_out, double* seconds_out);
 
+/* ---- measured operand-feed rate: every SM keeps inflight_bytes (a multiple of 4096) of 4 KB bulk copies global ->
+ * shared in flight, the copy instruction the KING kernel feeds itself with, reading a working set of
+ * working_set_bytes (small enough for L2, or much larger: HBM), for at least min_seconds.  *tbps_out = bytes copied /
+ * elapsed (CUDA events), in TB/s. ---- */
+int pl2gpu_bulk_read_rate(Pl2GpuCtx* ctx, uint64_t working_set_bytes, uint32_t inflight_bytes, double min_seconds, double* tbps_out, double* seconds_out);
+
 /* ---- self-test of the tensor operand path (fragment / descriptor layout probe); returns 0 iff int8 wgmmas
  * with A fragments in registers and B in the library's shared-memory layout reproduce a scalar host reference, and
  * binary AND-POPC wgmmas in the same layout reproduce a host popcount. ---- */

@@ -247,9 +247,8 @@ king_wg_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
 // (geno_tile_rows_kernel<true>) already holds as two 32-variant halves of each word:
 //   T = lo & ~hi (het),  H = ~lo (hom),  R = ~lo & ~hi (hom-REF),  A = ~lo & hi (hom-ALT);
 // missing data and padding (code 3) are zero in every plane.  One CTA = one whole 128 x 64 pair tile, three warpgroups:
-//   warpgroup 0:  producer.  One thread brings a stage's raw words into shared memory with bulk copies onto the
-//                 stage's `load` mbarrier (the row words: one contiguous piece, [k32 step][128 rows][8 B]; the column
-//                 words: 512 B per k32 step), one stage ahead; all 128 threads then turn the column words into the
+//   warpgroup 0:  producer.  Warp 0 brings a stage's raw words into a slot of the ring with bulk copies onto the
+//                 slot's `load` mbarrier as soon as the slot is free; warps 2 and 3 turn the column words into the
 //                 four planes T | H | R | A (K-major, no swizzle; one core matrix = 8 samples x 128 variants).
 //   warpgroups 1, 2:  consumer c owns rows 64 c .. 64 c + 63.  Per k256 step it turns its own row words straight
 //                 into fragment registers and issues   T_I x [T_J | H_J] (n128) -> TT | TH,
@@ -257,12 +256,12 @@ king_wg_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
 //                 160 int32 accumulators per thread, which fit once `setmaxnreg` moves registers from the producer
 //                 (40) to the consumers (232).
 // The epilogue writes SS = HH - 2 IBS0 (= the int8 form's S_I x S_J with S = R - A), so the raw accumulator layout
-// {TT, TH, HT, HH, SS} is that of king_wg_kernel.  Hand-off as in king_wg_kernel: `full` (128 producer arrivals
+// {TT, TH, HT, HH, SS} is that of king_wg_kernel.  Hand-off as in king_wg_kernel: `full` (64 producer arrivals
 // after the fence), `empty` (256 consumer arrivals once `wgmma.wait_group 1` has retired the stage), one wgmma group
 // in flight across stage boundaries.  A stage holds kKb1Ks k256 steps; the last one may be short (the block is padded
 // to 256 variants only): its missing steps are neither copied nor split, and run on zero planes.
 constexpr uint32_t kKb1Ks = 2;       // k256 steps per stage
-constexpr uint32_t kKb1Stages = 4;
+constexpr uint32_t kKb1Stages = 5;
 constexpr uint32_t kKb1Sbo = 2 * kKb1Ks * kKwChunkBytes;                 // next group of 8 samples
 constexpr uint32_t kKb1PlaneBytes = (kKingTsCols / 8) * kKb1Sbo;         // one plane of the 64 column samples
 constexpr uint32_t kKb1BBytes = 4 * kKb1PlaneBytes;                      // T | H | R | A
@@ -272,7 +271,8 @@ constexpr uint32_t kKb1ABytes = kKb1Ks * kKb1AStepBytes;                 // [k32
 constexpr uint32_t kKb1WBytes = kKb1Ks * kKb1WStepBytes;                 // [k32 step][64 samples][8 B]
 constexpr uint32_t kKb1StageBytes = kKb1BBytes + kKb1ABytes + kKb1WBytes;
 constexpr uint32_t kKb1SmemBytes = kKb1Stages * kKb1StageBytes + 128 + 3 * kKb1Stages * 8;  // + alignment + mbarriers
-static_assert(kKwProducerThreads == 2 * kKingTsCols, "producer item map: (column sample, half of a k256 step)");
+constexpr uint32_t kKb1SplitThreads = kKingTsCols;  // producer warps 2, 3: one column sample each
+static_assert(kKwProducerThreads == 2 * kKingTsCols, "producer warps: copier, idle, two split warps");
 static_assert(kKb1SmemBytes <= kKwSmemLimit, "exceeds the 227 KB shared-memory opt-in limit");
 
 // raw_t: sample-major copy of the whole padded block (sample 0 at row tile 0) in the split form of
@@ -294,7 +294,7 @@ king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
   const uint32_t bar_load = bar_empty + kKb1Stages * 8;
   if (tid == 0) {
     for (uint32_t s = 0; s < kKb1Stages; ++s) {
-      mbar_init(bar_full + 8 * s, kKwProducerThreads);
+      mbar_init(bar_full + 8 * s, kKb1SplitThreads);
       mbar_init(bar_empty + 8 * s, kKwConsumerThreads);
       mbar_init(bar_load + 8 * s, 1);
     }
@@ -305,56 +305,61 @@ king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
   if (wg == 0) {
     setmaxnreg_dec<40>();
     // ---- producer
-    const uint8_t* a_src = raw_t + static_cast<uint64_t>(rt) * kstep_ct * 1024;
-    // column samples 64 ct .. 64 ct + 63: half (ct & 1) of 128-sample block ct >> 1
-    const uint8_t* w_src = raw_t + static_cast<uint64_t>(ct >> 1) * kstep_ct * 1024 + (ct & 1) * 512;
-    auto issue_loads = [&](uint32_t st, uint32_t slot, uint32_t steps) {
-      const uint32_t base = smem_base + slot * kKb1StageBytes;
-      const uint32_t bar = bar_load + 8 * slot;
-      const uint64_t off = static_cast<uint64_t>(st) * kKb1Ks * 8 * 1024;
-      mbar_arrive_expect_tx(bar, steps * (kKb1AStepBytes + kKb1WStepBytes));
-      bulk_copy_g2s(base + kKb1BBytes, a_src + off, steps * kKb1AStepBytes, bar);
-      for (uint32_t k = 0; k < 8 * steps; ++k) bulk_copy_g2s(base + kKb1BBytes + kKb1ABytes + k * 512, w_src + off + k * 1024, 512, bar);
-    };
-    // item of this thread in each k256 step j: column sample n = tid % 64, k32 steps 8 j + 4 h .. 8 j + 4 h + 3
-    // (h = tid / 64), i.e. the 16-byte half h of row n of each plane's core matrices for step j
-    const uint32_t n = tid & (kKingTsCols - 1), h = tid / kKingTsCols;
-    const uint32_t w_off = kKb1BBytes + kKb1ABytes + 4 * h * 512 + n * 8;
-    const uint32_t b_off = (n >> 3) * kKb1Sbo + h * kKwChunkBytes + (n & 7) * 16;
-    auto steps_of = [&](uint32_t st) { return min(kKb1Ks, k256_ct - st * kKb1Ks); };
-
-    if (tid == 0) issue_loads(0, 0, steps_of(0));
-    uint32_t slot = 0, phase = 0;
-    for (uint32_t st = 0; st < stage_ct; ++st) {
-      // the next stage's words go into its slot once the consumers have retired the stage that used it last;
-      // the first pass over the ring finds every slot free (parity 1 = the phase before a fresh barrier's first)
-      const uint32_t nslot = slot + 1 == kKb1Stages ? 0 : slot + 1;
-      const uint32_t nphase = nslot ? phase : phase ^ 1;
-      if (st + 1 < stage_ct) {
-        mbar_wait(bar_empty + 8 * nslot, nphase ^ 1);
-        if (tid == 0) issue_loads(st + 1, nslot, steps_of(st + 1));
+    const uint32_t pw = tid >> 5;
+    if (pw == 0) {
+      // copier warp: the row words (one contiguous piece, [k32 step][128 rows][8 B]) and the column words of this
+      // tile (512 B per k32 step) of a stage, one bulk copy per lane onto the slot's `load` mbarrier.  It refills a
+      // slot as soon as the consumers have handed it back, so every slot but the one being read has its copies in
+      // flight.  These threads never split planes: the proxy fence after the split waits for every memory access
+      // of the thread still in flight, bulk copies included, which would hold the split up by a whole copy latency.
+      const uint8_t* a_src = raw_t + static_cast<uint64_t>(rt) * kstep_ct * 1024;
+      // column samples 64 ct .. 64 ct + 63: half (ct & 1) of 128-sample block ct >> 1
+      const uint8_t* w_src = raw_t + static_cast<uint64_t>(ct >> 1) * kstep_ct * 1024 + (ct & 1) * 512;
+      const uint32_t lane = tid & 31;
+      for (uint32_t st = 0; st < stage_ct; ++st) {
+        const uint32_t slot = st % kKb1Stages;
+        // the first pass over the ring finds every slot free (parity 1 = the phase before a fresh barrier's first)
+        mbar_wait(bar_empty + 8 * slot, ((st / kKb1Stages) & 1) ^ 1);
+        const uint32_t base = smem_base + slot * kKb1StageBytes;
+        const uint32_t bar = bar_load + 8 * slot;
+        const uint32_t steps = min(kKb1Ks, k256_ct - st * kKb1Ks);
+        const uint64_t off = static_cast<uint64_t>(st) * kKb1Ks * 8 * 1024;
+        if (lane == 0) mbar_arrive_expect_tx(bar, steps * (kKb1AStepBytes + kKb1WStepBytes));
+        if (lane < 8 * steps) bulk_copy_g2s(base + kKb1BBytes + kKb1ABytes + lane * 512, w_src + off + lane * 1024, 512, bar);
+        if (lane == 31) bulk_copy_g2s(base + kKb1BBytes, a_src + off, steps * kKb1AStepBytes, bar);
+        __syncwarp();
       }
-      const uint32_t base = smem_base + slot * kKb1StageBytes;
-      const uint32_t steps = steps_of(st);
-      mbar_wait(bar_load + 8 * slot, phase);
+    } else if (pw >= 2) {
+      // split warps 2, 3: column sample n = tid % 64; for each k256 step j and half h, k32 steps 8 j + 4 h ..
+      // 8 j + 4 h + 3, i.e. the 16-byte half h of row n of each plane's core matrices for step j
+      const uint32_t n = tid & (kKingTsCols - 1);
+      for (uint32_t st = 0; st < stage_ct; ++st) {
+        const uint32_t slot = st % kKb1Stages, phase = (st / kKb1Stages) & 1;
+        const uint32_t base = smem_base + slot * kKb1StageBytes;
+        const uint32_t steps = min(kKb1Ks, k256_ct - st * kKb1Ks);
+        // the copies into this slot were issued once it was free; the planes go in after the same wait
+        if (st >= kKb1Stages) mbar_wait(bar_empty + 8 * slot, phase ^ 1);
+        mbar_wait(bar_load + 8 * slot, phase);
 #pragma unroll
-      for (uint32_t j = 0; j < kKb1Ks; ++j) {
-        uint32_t lo[4] = {~0u, ~0u, ~0u, ~0u}, hi[4] = {~0u, ~0u, ~0u, ~0u};  // missing step: code 3, zero planes
-        if (j < steps) {
+        for (uint32_t j = 0; j < kKb1Ks; ++j) {
 #pragma unroll
-          for (uint32_t q = 0; q < 4; ++q)
-            asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(lo[q]), "=r"(hi[q]) : "r"(base + w_off + (8 * j + q) * 512) : "memory");
+          for (uint32_t h = 0; h < 2; ++h) {
+            uint32_t lo[4] = {~0u, ~0u, ~0u, ~0u}, hi[4] = {~0u, ~0u, ~0u, ~0u};  // missing step: code 3, zero planes
+            if (j < steps) {
+#pragma unroll
+              for (uint32_t q = 0; q < 4; ++q)
+                asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(lo[q]), "=r"(hi[q]) : "r"(base + kKb1BBytes + kKb1ABytes + (8 * j + 4 * h + q) * 512 + n * 8) : "memory");
+            }
+            const uint32_t addr = base + (n >> 3) * kKb1Sbo + (2 * j + h) * kKwChunkBytes + (n & 7) * 16;
+            asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(lo[0] & ~hi[0]), "r"(lo[1] & ~hi[1]), "r"(lo[2] & ~hi[2]), "r"(lo[3] & ~hi[3]) : "memory");
+            asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + kKb1PlaneBytes), "r"(~lo[0]), "r"(~lo[1]), "r"(~lo[2]), "r"(~lo[3]) : "memory");
+            asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + 2 * kKb1PlaneBytes), "r"(~(lo[0] | hi[0])), "r"(~(lo[1] | hi[1])), "r"(~(lo[2] | hi[2])), "r"(~(lo[3] | hi[3])) : "memory");
+            asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + 3 * kKb1PlaneBytes), "r"(~lo[0] & hi[0]), "r"(~lo[1] & hi[1]), "r"(~lo[2] & hi[2]), "r"(~lo[3] & hi[3]) : "memory");
+          }
         }
-        const uint32_t addr = base + b_off + 2 * j * kKwChunkBytes;
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(lo[0] & ~hi[0]), "r"(lo[1] & ~hi[1]), "r"(lo[2] & ~hi[2]), "r"(lo[3] & ~hi[3]) : "memory");
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + kKb1PlaneBytes), "r"(~lo[0]), "r"(~lo[1]), "r"(~lo[2]), "r"(~lo[3]) : "memory");
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + 2 * kKb1PlaneBytes), "r"(~(lo[0] | hi[0])), "r"(~(lo[1] | hi[1])), "r"(~(lo[2] | hi[2])), "r"(~(lo[3] | hi[3])) : "memory");
-        asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + 3 * kKb1PlaneBytes), "r"(~lo[0] & hi[0]), "r"(~lo[1] & hi[1]), "r"(~lo[2] & hi[2]), "r"(~lo[3] & hi[3]) : "memory");
+        fence_proxy_async_smem();  // this thread's st.shared -> visible to the consumers' wgmma operand fetch
+        mbar_arrive(bar_full + 8 * slot);
       }
-      fence_proxy_async_smem();  // this thread's st.shared -> visible to the consumers' wgmma operand fetch
-      mbar_arrive(bar_full + 8 * slot);
-      slot = nslot;
-      phase = nphase;
     }
     return;
   }

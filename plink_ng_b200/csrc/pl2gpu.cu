@@ -70,8 +70,8 @@ int BuildTileList(uint32_t row_start, uint32_t row_end, bool include_diag, TileL
   }
   PL2_CUDA_OK(cudaMemcpy(tl->d_rowtile_offset, off_v.data(), off_v.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
   tl->h_rowtile_offset = off_v;
-  // launch order: blocks of kBand x kBand tiles (~ one wave of 148 CTAs) so that the CTAs resident at
-  // the same time stream the same few row/column sample ranges and hit in L2
+  // launch order: blocks of kBand x kBand tiles (144, about one wave on the 132 SMs of an H100 SXM) so that the
+  // CTAs resident at the same time stream the same few row/column sample ranges and hit in L2
   constexpr uint32_t kBand = 12;
   std::vector<uint32_t> order;
   order.reserve(rt_v.size());
@@ -995,6 +995,62 @@ int pl2gpu_int8_peak(Pl2GpuCtx* ctx, uint32_t n_cols, int form, double min_secon
   cudaEventDestroy(e1);
   cudaFree(d_sink);
   *tops_out = total_ops / total_s / 1e12;
+  if (seconds_out) *seconds_out = total_s;
+  return 0;
+}
+
+int pl2gpu_bulk_read_rate(Pl2GpuCtx* ctx, uint64_t working_set_bytes, uint32_t inflight_bytes, double min_seconds, double* tbps_out, double* seconds_out) {
+  const uint64_t max_inflight = (kKwSmemLimit - 128) / (kFeedChunk + 8) * kFeedChunk;
+  if (!ctx || !tbps_out || inflight_bytes == 0 || inflight_bytes % kFeedChunk || inflight_bytes > max_inflight || working_set_bytes < kFeedChunk || working_set_bytes / kFeedChunk > 0xFFFFFFFFull) {
+    set_error("pl2gpu_bulk_read_rate: bad arguments (inflight_bytes: a multiple of %u up to %llu; working_set_bytes: at least %u)", kFeedChunk, static_cast<unsigned long long>(max_inflight), kFeedChunk);
+    return 1;
+  }
+  Ctx* c = &ctx->c;
+  PL2_CUDA_OK(cudaSetDevice(c->device));
+  const uint32_t ws_chunks = static_cast<uint32_t>(working_set_bytes / kFeedChunk);
+  const uint32_t chunks = inflight_bytes / kFeedChunk;
+  const uint32_t smem = chunks * (kFeedChunk + 8) + 128;
+  // about 64 MB per SM and launch
+  const uint32_t rounds = std::max<uint32_t>(2, (64u << 20) / inflight_bytes);
+  const double bytes_per_launch = static_cast<double>(kFeedChunk) * chunks * rounds * c->sm_count;
+  uint8_t* d_src = nullptr;
+  PL2_CUDA_OK(cudaMalloc(&d_src, static_cast<uint64_t>(ws_chunks) * kFeedChunk));
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  auto release = [&]() {
+    cudaFree(d_src);
+    if (e0) cudaEventDestroy(e0);
+    if (e1) cudaEventDestroy(e1);
+  };
+  auto fail = [&]() {
+    release();
+    return 1;
+  };
+  if (cudaMemsetAsync(d_src, 0x5A, static_cast<uint64_t>(ws_chunks) * kFeedChunk, c->stream) != cudaSuccess || cudaEventCreate(&e0) != cudaSuccess || cudaEventCreate(&e1) != cudaSuccess ||
+      cudaFuncSetAttribute(bulk_read_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
+    set_error("pl2gpu_bulk_read_rate: set-up failed: %s", cudaGetErrorString(cudaGetLastError()));
+    return fail();
+  }
+  auto launch = [&]() {
+    bulk_read_probe_kernel<<<c->sm_count, 32, smem, c->stream>>>(d_src, ws_chunks, chunks, rounds);
+    c->launches++;
+  };
+  launch();  // warm-up: also brings an L2-sized working set into L2
+  double total_s = 0, total_bytes = 0;
+  const uint32_t per_batch = 4;
+  while (true) {
+    if (cudaEventRecord(e0, c->stream) != cudaSuccess) return fail();
+    for (uint32_t k = 0; k < per_batch; ++k) launch();
+    float ms = 0;
+    if (cudaEventRecord(e1, c->stream) != cudaSuccess || cudaEventSynchronize(e1) != cudaSuccess || cudaGetLastError() != cudaSuccess || cudaEventElapsedTime(&ms, e0, e1) != cudaSuccess) {
+      set_error("pl2gpu_bulk_read_rate: probe run failed: %s", cudaGetErrorString(cudaGetLastError()));
+      return fail();
+    }
+    total_s += ms * 1e-3;
+    total_bytes += bytes_per_launch * per_batch;
+    if (total_s >= min_seconds) break;
+  }
+  release();
+  *tbps_out = total_bytes / total_s / 1e12;
   if (seconds_out) *seconds_out = total_s;
   return 0;
 }

@@ -132,4 +132,32 @@ static __global__ void __launch_bounds__(256, 1) wgmma_b1_peak_kernel(uint32_t b
   if (s == 0x7FFFFFFF) sink[threadIdx.x] = s;  // keeps the loop alive
 }
 
+// Read-rate probe of the operand feed: one thread per CTA (one CTA per SM) keeps `chunks` bulk copies of kFeedChunk
+// bytes (global -> shared, each onto its own mbarrier, the instruction king_b1_kernel feeds itself with) in flight and
+// discards what arrives.  CTA b reads chunks b, b + gridDim.x, ... of a working set of ws_chunks chunks, wrapping
+// around, `rounds` x `chunks` copies in all.
+constexpr uint32_t kFeedChunk = 4096;
+static __global__ void __launch_bounds__(32, 1) bulk_read_probe_kernel(const uint8_t* __restrict__ src, uint32_t ws_chunks, uint32_t chunks, uint32_t rounds) {
+  extern __shared__ __align__(128) uint8_t smem[];
+  if (threadIdx.x != 0) return;
+  const uint32_t base = (static_cast<uint32_t>(__cvta_generic_to_shared(smem)) + 127u) & ~127u;
+  const uint32_t bar = base + chunks * kFeedChunk;
+  for (uint32_t i = 0; i < chunks; ++i) mbar_init(bar + 8 * i, 1);
+  mbar_init_fence();
+  uint32_t next = blockIdx.x % ws_chunks;
+  auto issue = [&](uint32_t i) {
+    mbar_arrive_expect_tx(bar + 8 * i, kFeedChunk);
+    bulk_copy_g2s(base + i * kFeedChunk, src + static_cast<uint64_t>(next) * kFeedChunk, kFeedChunk, bar + 8 * i);
+    next += gridDim.x;
+    if (next >= ws_chunks) next %= ws_chunks;
+  };
+  for (uint32_t i = 0; i < chunks; ++i) issue(i);
+  for (uint32_t r = 1; r < rounds; ++r)
+    for (uint32_t i = 0; i < chunks; ++i) {
+      mbar_wait(bar + 8 * i, (r - 1) & 1);
+      issue(i);
+    }
+  for (uint32_t i = 0; i < chunks; ++i) mbar_wait(bar + 8 * i, (rounds - 1) & 1);
+}
+
 }  // namespace pl2

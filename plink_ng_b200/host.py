@@ -88,6 +88,12 @@ class GpuContext:
         check(lib.pl2gpu_int8_peak(self._h, n_cols, form, min_seconds, C.byref(tops), C.byref(secs)), "pl2gpu_int8_peak")
         return float(tops.value), float(secs.value)
 
+    def bulk_read_rate(self, working_set_bytes: int, inflight_bytes: int, min_seconds: float = 0.5):
+        """Measured bulk-copy read rate (TB/s, seconds) with inflight_bytes of copies in flight per SM."""
+        tbps, secs = C.c_double(), C.c_double()
+        check(lib.pl2gpu_bulk_read_rate(self._h, working_set_bytes, inflight_bytes, min_seconds, C.byref(tbps), C.byref(secs)), "pl2gpu_bulk_read_rate")
+        return float(tbps.value), float(secs.value)
+
     def comm_init(self, rank: int, world: int, unique_id: bytes):
         """Attach an NCCL communicator (collective over all ranks; rank 0 makes the id with comm_unique_id())."""
         buf = (C.c_uint8 * 128).from_buffer_copy(unique_id)
