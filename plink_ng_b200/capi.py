@@ -71,6 +71,7 @@ SIGNATURES = {
     "pl2gpu_pca_vscore": (C.c_int, [vp, vp, C.c_uint32, vp]),
     "pl2gpu_pca_begin_shard": (C.c_int, [vp, C.c_uint32, C.c_uint32, C.c_uint32, vp]),
     "pl2gpu_pca_run_sharded": (C.c_int, [vp, vp, C.c_uint64, vp, vp]),
+    "pl2gpu_pca_products": (C.c_int, [vp, vp, C.c_uint32, vp, vp, C.c_uint32, vp]),
     "pl2gpu_pca_end": (C.c_int, [vp]),
     "pl2gpu_geno_counts": (C.c_int, [vp, vp, C.c_uint64, C.c_uint32, C.c_uint32, C.c_int, vp]),
     "pl2gpu_ld_band_flags": (C.c_int, [vp, vp, C.c_uint64, C.c_uint32, C.c_uint32, C.c_int, C.c_uint32, C.c_double, vp]),

@@ -3015,7 +3015,7 @@ int RunVscore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   for (uint32_t p0 = 0; p0 < m; p0 += piece) {
     const uint32_t p1 = std::min(m, p0 + piece);
     Pl2PcaJob* job = nullptr;
-    if (pl2gpu_pca_begin_shard(ctx, n, p1 - p0, 1, &job)) return GpuFail("pl2gpu_pca_begin_shard");
+    if (pl2gpu_pca_begin_shard(ctx, n, p1 - p0, 0, &job)) return GpuFail("pl2gpu_pca_begin_shard");  // pc_ct 0: a --variant-score job
     struct Guard {
       Pl2PcaJob* j;
       ~Guard() { pl2gpu_pca_end(j); }

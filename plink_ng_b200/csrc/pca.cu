@@ -34,6 +34,7 @@ struct Pl2PcaJob {
   double* d_twof = nullptr;     // per variant: 2 alt_freq (the mean-imputation value of --variant-score)
   std::vector<double> h_slope, h_icpt, h_twof;
   uint32_t retiled_to = 0;      // variants [0, retiled_to) are in d_raw_i (multiple of 64)
+  bool vscore_only = false;     // begun with pc_ct = 0: a --variant-score job (no approx-PCA requirements, see the header)
 };
 
 extern "C" {
@@ -42,16 +43,18 @@ int pl2gpu_pca_end(Pl2PcaJob* job);
 
 static int PcaBeginImpl(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t variant_ct_total, uint32_t pc_ct, bool shard, Pl2PcaJob** job_ptr) {
   *job_ptr = nullptr;
-  if (!ctx || !sample_ct || !variant_ct_total || !pc_ct) {
+  if (!ctx || !sample_ct || !variant_ct_total || (!pc_ct && !shard)) {
     set_error("pl2gpu_pca_begin: bad arguments");
     return 1;
   }
+  // the approx-PCA size requirements; a shard is judged at run time (PcaRunImpl), which leaves a --variant-score job
+  // (pc_ct = 0) without any: VscoreReport scores any number of samples
   const uint64_t q = 2ull * pc_ct * (pc_ct + 1);
-  if (q > variant_ct_total && !shard) {  // :5716-5719 (a shard is judged on the total, at run time)
+  if (q > variant_ct_total && !shard) {  // :5716-5719
     set_error("Too few variants to compute %u PCs with \"--pca approx\" (%llu required).", pc_ct, static_cast<unsigned long long>(q));
     return 2;
   }
-  if (q > sample_ct) {
+  if (q > sample_ct && !shard) {
     set_error("pl2gpu_pca_begin: \"--pca approx\" with %u PCs needs at least %llu samples in this implementation (tall thin SVD)", pc_ct, static_cast<unsigned long long>(q));
     return 1;
   }
@@ -63,6 +66,7 @@ static int PcaBeginImpl(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t variant_ct_
   job->pitch = job->sample_ct_padded / 4;
   job->variant_cap = RoundUpU32(variant_ct_total, 128);
   job->pc_ct = pc_ct;
+  job->vscore_only = pc_ct == 0;
   if (cudaMalloc(&job->d_raw, static_cast<uint64_t>(job->variant_cap) * job->pitch) != cudaSuccess || cudaMalloc(&job->d_counts, 16ull * 65536) != cudaSuccess ||
       cudaMalloc(&job->d_raw_i, static_cast<uint64_t>(job->sample_ct_padded) * (job->variant_cap / 4)) != cudaSuccess || cudaMalloc(&job->d_slope, 8ull * job->variant_cap) != cudaSuccess ||
       cudaMalloc(&job->d_icpt, 8ull * job->variant_cap) != cudaSuccess || cudaMalloc(&job->d_twof, 8ull * job->variant_cap) != cudaSuccess) {
@@ -123,7 +127,7 @@ int pl2gpu_pca_add_variants(Pl2PcaJob* job, const void* genovecs, uint64_t varia
         if (variance != variance) bad = bad || n0 || n2;
         else if (ref_freq > 0.5) bad = bad || n2;
         else bad = bad || n0;
-        if (bad) {
+        if (bad && !job->vscore_only) {  // CalcPca's consistency check (VscoreReport has none)
           set_error("pl2gpu_pca_add_variants: variant %u has zero-variance allele frequency %g but non-monomorphic genotypes (kPglRetDegenerateData)", job->variant_ct + v, ref_freq);
           return 2;
         }
@@ -145,15 +149,133 @@ int pl2gpu_pca_add_variants(Pl2PcaJob* job, const void* genovecs, uint64_t varia
 
 }  // extern "C"
 
-// The run itself.  sharded: the job holds ONE variant shard of a world-size team (contexts joined by pl2gpu_comm_init;
+// ---- the two products on the int8 tensor pipe (pca_ts_kernels.cuh), shared by the run, --variant-score and
+// pl2gpu_pca_products ----
+// every dense operand goes through the tensor pipe twice: 30-bit fixed point, then the exact residual at another
+// 30 bits (pca_digits_kernel pass 1) - 60 bits below the column maximum, so the passes lose nothing against the
+// reference's fp64 dgemm (one 30-bit pass left the trailing, noise-level eigenvalues 2e-3 off)
+constexpr int kPcaPasses = 2;
+// The int32 digit accumulators of pca_xtb_wg_kernel gain at most 2 * 128 + 128 = 384 per variant (a dosage <= 2 and
+// an indicator <= 1, each times a digit in [-128, 127]), 32 variants per k-step: a split of at most this many k-steps
+// cannot overflow them.  An 80 GB card never holds a shard long enough for the cap to bind.
+constexpr uint32_t kPcaXtbMaxKsteps = (0x7FFFFFFFu / (384u * 32u)) / 4 * 4;  // 174,760
+
+// scratch of one job's products: digit planes, per-column scales, split-K partial sums of Y^T H
+struct PcaTs {
+  uint8_t *gdig = nullptr, *hs = nullptr, *hi = nullptr;
+  double *scale = nullptr, *inv_scale = nullptr, *partial = nullptr;
+  unsigned long long* colmax = nullptr;
+  uint32_t splits = 0, ksteps_per_split = 0;
+};
+
+static void PcaTsFree(PcaTs* ts) {
+  cudaFree(ts->gdig);
+  cudaFree(ts->hs);
+  cudaFree(ts->hi);
+  cudaFree(ts->scale);
+  cudaFree(ts->inv_scale);
+  cudaFree(ts->colmax);
+  cudaFree(ts->partial);
+  *ts = PcaTs();
+}
+
+// xtb: also the slope.H / icpt.H digit planes and the split-K partial sums.  Split plan of Y^T H: about two CTAs per
+// SM over the 128-sample row tiles, at least 64 k-steps (2,048 variants) per split, a whole number of 4-k-step stages
+// per split, the last split short.
+static int PcaTsAlloc(const Pl2PcaJob* job, bool xtb, PcaTs* ts) {
+  const Ctx* c = &job->ctx->c;
+  const uint32_t npad = job->sample_ct_padded, kstep_total = job->variant_cap / 32, tiles2 = npad / 128;
+  uint32_t splits = std::max(1u, std::min(DivUpU32(2 * static_cast<uint32_t>(c->sm_count), tiles2), kstep_total / 64));
+  ts->ksteps_per_split = std::min(kPcaXtbMaxKsteps, RoundUpU32(DivUpU32(kstep_total, splits), 4));
+  ts->splits = DivUpU32(kstep_total, ts->ksteps_per_split);
+  if (cudaMalloc(&ts->gdig, static_cast<uint64_t>(npad) * kPcaNMax) != cudaSuccess || cudaMalloc(&ts->scale, 8 * kPcaCgMax) != cudaSuccess || cudaMalloc(&ts->inv_scale, 8 * kPcaCgMax) != cudaSuccess ||
+      cudaMalloc(&ts->colmax, 8 * kPcaCgMax) != cudaSuccess ||
+      (xtb && (cudaMalloc(&ts->hs, static_cast<uint64_t>(job->variant_cap) * kPcaNMax) != cudaSuccess || cudaMalloc(&ts->hi, static_cast<uint64_t>(job->variant_cap) * kPcaNMax) != cudaSuccess ||
+               cudaMalloc(&ts->partial, static_cast<uint64_t>(ts->splits) * npad * kPcaCgMax * 8) != cudaSuccess))) {
+    cudaGetLastError();
+    set_error("pl2gpu_pca: insufficient device memory for the digit planes");
+    PcaTsFree(ts);
+    return 1;
+  }
+  return 0;
+}
+
+// rows [variant_ct, variant_cap) must decode to "missing" in both layouts; sample_major: finish the sample-major copy
+// (what Y^T H reads)
+static int PcaFinishLayouts(Pl2PcaJob* job, bool sample_major) {
+  Ctx* c = &job->ctx->c;
+  const uint32_t m = job->variant_ct;
+  if (job->variant_cap > m) PL2_TRY(LaunchPadGenotypes(c, job->d_raw + static_cast<uint64_t>(m) * job->pitch, job->pitch, job->sample_ct, 0, job->variant_cap - m));
+  if (sample_major && job->retiled_to < job->variant_cap) {
+    const uint32_t from = job->retiled_to;
+    geno_tile_rows_kernel<<<dim3((job->variant_cap - from) / 64, job->sample_ct_padded / 64), 256, 0, c->stream>>>(job->d_raw + static_cast<uint64_t>(from) * job->pitch, job->pitch, job->variant_cap / 32, 0,
+                                                                                                                 job->d_raw_i + static_cast<uint64_t>(from / 32) * 1024);
+    c->launches++;
+    job->retiled_to = job->variant_cap;
+  }
+  return 0;
+}
+
+// column group: up to kPcaCgMax columns (the columns past the valid ones are zero digits and never written)
+static int PcaGroupScales(Ctx* c, PcaTs* ts, const double* src, uint64_t rs, uint64_t cs, uint32_t rows, uint32_t valid, const double* mul1, const double* mul2) {
+  const int rc = cudaMemsetAsync(ts->colmax, 0, 8 * kPcaCgMax, c->stream) != cudaSuccess;
+  pca_colmax_kernel<<<dim3(valid, std::min<uint32_t>(64, DivUpU32(rows, 256))), 256, 0, c->stream>>>(src, rs, cs, rows, mul1, mul2, ts->colmax);
+  pca_scales_kernel<<<1, 64, 0, c->stream>>>(ts->colmax, kPcaCgMax, ts->scale, ts->inv_scale);
+  c->launches += 2;
+  return rc;
+}
+
+// H = Y G with y_vs = slope_v g_vs + icpt_v m_vs (the job's own per-variant arrays, or --variant-score's centring): G
+// row-major (element (s, c) at g[s g_ld + c], sample_ct_padded rows, zero past sample_ct), H column-major (ld h_ld);
+// cols columns
+static int PcaLaunchXa(Pl2PcaJob* job, PcaTs* ts, const double* slope, const double* icpt, const double* g, uint32_t g_ld, double* h, uint64_t h_ld, uint32_t cols) {
+  Ctx* c = &job->ctx->c;
+  const uint32_t npad = job->sample_ct_padded;
+  int rc = 0;
+  for (uint32_t cc = 0; cc < cols; cc += kPcaCgMax) {
+    const uint32_t valid = std::min(kPcaCgMax, cols - cc), cg = kPcaCgMax;
+    rc |= PcaGroupScales(c, ts, g + cc, g_ld, 1, npad, valid, nullptr, nullptr);
+    for (int pass = 0; pass < kPcaPasses; ++pass) {
+      pca_digits_kernel<<<npad / 64, 256, 0, c->stream>>>(g + cc, g_ld, 1, npad, cg, valid, nullptr, nullptr, ts->scale, ts->gdig, nullptr, pass);
+      pca_xa_wg_kernel<<<job->variant_cap / 128, kPcaThreads, kPxaSmemBytes, c->stream>>>(job->d_raw, job->pitch, npad, job->variant_ct, ts->gdig, valid, slope, icpt, ts->inv_scale, h + static_cast<uint64_t>(cc) * h_ld, h_ld,
+                                                                                        pass ? 1.0 / kPcaPass1Scale : 1.0, pass);
+      c->launches += 2;
+    }
+  }
+  return rc;
+}
+
+// O += Y^T H: H column-major (ld h_ld, variant_ct rows), O element (s, c) at out[s out_rs + c out_cs]; cols columns.
+// Needs the sample-major copy (PcaFinishLayouts) and the xtb scratch.
+static int PcaLaunchXtb(Pl2PcaJob* job, PcaTs* ts, const double* h, uint64_t h_ld, uint32_t cols, double* out, uint64_t out_rs, uint64_t out_cs) {
+  Ctx* c = &job->ctx->c;
+  const uint32_t n = job->sample_ct, npad = job->sample_ct_padded, m = job->variant_ct;
+  int rc = 0;
+  for (uint32_t cc = 0; cc < cols; cc += kPcaCgMax) {
+    const uint32_t valid = std::min(kPcaCgMax, cols - cc), cg = kPcaCgMax;
+    const double* src = h + static_cast<uint64_t>(cc) * h_ld;
+    rc |= PcaGroupScales(c, ts, src, 1, h_ld, m, valid, job->d_slope, job->d_icpt);
+    for (int pass = 0; pass < kPcaPasses; ++pass) {
+      pca_digits_kernel<<<job->variant_cap / 64, 256, 0, c->stream>>>(src, 1, h_ld, m, cg, valid, job->d_slope, job->d_icpt, ts->scale, ts->hs, ts->hi, pass);
+      if (cudaMemsetAsync(ts->partial, 0, static_cast<uint64_t>(ts->splits) * npad * cg * 8, c->stream) != cudaSuccess) rc = 1;
+      pca_xtb_wg_kernel<<<dim3(npad / 128, ts->splits), kPcaThreads, kPxtSmemBytes, c->stream>>>(job->d_raw_i, job->variant_cap / 32, ts->ksteps_per_split, n, ts->hs, ts->hi, ts->inv_scale, ts->partial, npad);
+      pca_xtb_reduce_kernel<<<static_cast<uint32_t>(DivUpU64(static_cast<uint64_t>(n) * cg, 256)), 256, 0, c->stream>>>(ts->partial, ts->splits, n, npad, cg, valid, pass ? 1.0 / kPcaPass1Scale : 1.0,
+                                                                                                                      out + static_cast<uint64_t>(cc) * out_cs, out_rs, out_cs);
+      c->launches += 3;
+    }
+  }
+  return rc;
+}
+
+// The run itself.  sharded:the job holds ONE variant shard of a world-size team (contexts joined by pl2gpu_comm_init;
 // collective call).  Everything that contracts over variants is a partial sum on each rank and is completed by an
 // in-place fp64 all-reduce (NCCL returns the same bits on every rank, so the replicated small steps stay in lockstep):
 // G' = Y^T H per pass (N x 2k - the exchange SURVEY 8e names), the block Gram-Schmidt coefficients, B = Y^T Q.  The
 // M x 2k block of each orthonormalisation pass is all-gathered (320 bytes per variant) and every rank runs the same
 // Jacobi SVD on it, keeping its own rows.
 static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_variant_ct, bool sharded, double* eigvals_host, double* eigvecs_host) {
-  if (!job || !g1_host) {
-    set_error("pl2gpu_pca_run: bad arguments");
+  if (!job || !g1_host || !job->pc_ct) {
+    set_error("pl2gpu_pca_run: bad arguments (needs g1 and a job begun with pc_ct > 0)");
     return 1;
   }
   Ctx* c = &job->ctx->c;
@@ -174,69 +296,10 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
   double *d_qq = nullptr, *d_u = nullptr, *d_g1 = nullptr, *d_g2 = nullptr, *d_b = nullptr, *d_gram = nullptr, *d_gram_u = nullptr, *d_gram_partial = nullptr, *d_colscale = nullptr;
   int rc = 1;
   const double m_recip = 1.0 / static_cast<double>(total_variant_ct);
-  // ---- tensor pass scratch (pca_ts_kernels.cuh): digit planes, per-column scales, split-K partial sums ----
-  uint8_t *d_gdig = nullptr, *d_hs = nullptr, *d_hi = nullptr;
-  double *d_scale = nullptr, *d_inv_scale = nullptr, *d_partial = nullptr;
-  unsigned long long* d_colmax = nullptr;
-  const uint32_t kstep_total = job->variant_cap / 32;
-  const uint32_t tiles2 = npad / 128;
-  uint32_t splits = std::max(1u, std::min(DivUpU32(2 * static_cast<uint32_t>(c->sm_count), tiles2), kstep_total / 64));
-  const uint32_t ksteps_per_split = RoundUpU32(DivUpU32(kstep_total, splits), 4);
-  splits = DivUpU32(kstep_total, ksteps_per_split);
+  PL2_TRY(PcaFinishLayouts(job, true));
+  PcaTs ts;
+  PL2_TRY(PcaTsAlloc(job, true, &ts));
   int ts_rc = 0;
-  if (cudaMalloc(&d_gdig, static_cast<uint64_t>(npad) * kPcaNMax) != cudaSuccess || cudaMalloc(&d_hs, static_cast<uint64_t>(job->variant_cap) * kPcaNMax) != cudaSuccess ||
-      cudaMalloc(&d_hi, static_cast<uint64_t>(job->variant_cap) * kPcaNMax) != cudaSuccess || cudaMalloc(&d_scale, 8 * kPcaCgMax) != cudaSuccess || cudaMalloc(&d_inv_scale, 8 * kPcaCgMax) != cudaSuccess ||
-      cudaMalloc(&d_colmax, 8 * kPcaCgMax) != cudaSuccess || cudaMalloc(&d_partial, static_cast<uint64_t>(splits) * npad * kPcaCgMax * 8) != cudaSuccess) {
-    cudaGetLastError();
-    set_error("pl2gpu_pca_run: insufficient device memory for the digit planes");
-    cudaFree(d_gdig); cudaFree(d_hs); cudaFree(d_hi); cudaFree(d_scale); cudaFree(d_inv_scale); cudaFree(d_colmax); cudaFree(d_partial);
-    return 1;
-  }
-  // rows [variant_ct, variant_cap) must decode to "missing" in both layouts; finish the sample-major copy
-  if (job->variant_cap > m) PL2_TRY(LaunchPadGenotypes(c, job->d_raw + static_cast<uint64_t>(m) * job->pitch, job->pitch, job->sample_ct, 0, job->variant_cap - m));
-  if (job->retiled_to < job->variant_cap) {
-    const uint32_t from = job->retiled_to;
-    geno_tile_rows_kernel<<<dim3((job->variant_cap - from) / 64, npad / 64), 256, 0, c->stream>>>(job->d_raw + static_cast<uint64_t>(from) * job->pitch, job->pitch, kstep_total, 0, job->d_raw_i + static_cast<uint64_t>(from / 32) * 1024);
-    c->launches++;
-    job->retiled_to = job->variant_cap;
-  }
-  // column group: up to 48 columns, padded to a multiple of 4 (the padding columns are zero digits and never written)
-  auto group_scales = [&](const double* src, uint64_t rs, uint64_t cs, uint32_t rows, uint32_t valid, const double* mul1, const double* mul2) {
-    if (cudaMemsetAsync(d_colmax, 0, 8 * kPcaCgMax, c->stream) != cudaSuccess) ts_rc = 1;
-    pca_colmax_kernel<<<dim3(valid, std::min<uint32_t>(64, DivUpU32(rows, 256))), 256, 0, c->stream>>>(src, rs, cs, rows, mul1, mul2, d_colmax);
-    pca_scales_kernel<<<1, 64, 0, c->stream>>>(d_colmax, kPcaCgMax, d_scale, d_inv_scale);
-    c->launches += 2;
-  };
-  // every dense operand goes through the tensor pipe twice: 30-bit fixed point, then the exact residual at another
-  // 30 bits (pca_digits_kernel pass 1) - 60 bits below the column maximum, so the passes lose nothing against the
-  // reference's fp64 dgemm (one 30-bit pass left the trailing, noise-level eigenvalues 2e-3 off)
-  constexpr int kPasses = 2;
-  auto launch_xa = [&](const double* g, uint32_t g_ld, double* hout, uint64_t h_ld, uint32_t hcol0, uint32_t cols_total) {
-    for (uint32_t cc = 0; cc < cols_total; cc += kPcaCgMax) {
-      const uint32_t valid = std::min(kPcaCgMax, cols_total - cc), cg = kPcaCgMax;
-      group_scales(g + cc, g_ld, 1, npad, valid, nullptr, nullptr);
-      for (int pass = 0; pass < kPasses; ++pass) {
-        pca_digits_kernel<<<npad / 64, 256, 0, c->stream>>>(g + cc, g_ld, 1, npad, cg, valid, nullptr, nullptr, d_scale, d_gdig, nullptr, pass);
-        pca_xa_wg_kernel<<<job->variant_cap / 128, kPcaThreads, kPxaSmemBytes, c->stream>>>(job->d_raw, job->pitch, npad, m, d_gdig, valid, job->d_slope, job->d_icpt, d_inv_scale, hout + static_cast<uint64_t>(hcol0 + cc) * h_ld, h_ld,
-                                                                                          pass ? 1.0 / kPcaPass1Scale : 1.0, pass);
-        c->launches += 2;
-      }
-    }
-  };
-  auto launch_xtb = [&](const double* hin, uint64_t h_ld, uint32_t hcol0, uint32_t cols_total, double* out, uint64_t out_rs, uint64_t out_cs) {
-    for (uint32_t cc = 0; cc < cols_total; cc += kPcaCgMax) {
-      const uint32_t valid = std::min(kPcaCgMax, cols_total - cc), cg = kPcaCgMax;
-      const double* src = hin + static_cast<uint64_t>(hcol0 + cc) * h_ld;
-      group_scales(src, 1, h_ld, m, valid, job->d_slope, job->d_icpt);
-      for (int pass = 0; pass < kPasses; ++pass) {
-        pca_digits_kernel<<<job->variant_cap / 64, 256, 0, c->stream>>>(src, 1, h_ld, m, cg, valid, job->d_slope, job->d_icpt, d_scale, d_hs, d_hi, pass);
-        if (cudaMemsetAsync(d_partial, 0, static_cast<uint64_t>(splits) * npad * cg * 8, c->stream) != cudaSuccess) ts_rc = 1;
-        pca_xtb_wg_kernel<<<dim3(tiles2, splits), kPcaThreads, kPxtSmemBytes, c->stream>>>(job->d_raw_i, kstep_total, ksteps_per_split, n, d_hs, d_hi, d_inv_scale, d_partial, npad);
-        pca_xtb_reduce_kernel<<<static_cast<uint32_t>(DivUpU64(static_cast<uint64_t>(n) * cg, 256)), 256, 0, c->stream>>>(d_partial, splits, n, npad, cg, valid, pass ? 1.0 / kPcaPass1Scale : 1.0, out + static_cast<uint64_t>(cc) * out_cs, out_rs, out_cs);
-        c->launches += 3;
-      }
-    }
-  };
   // PL2_TIMING=1: phase times on stderr (stream-synchronising; development aid)
   const bool timing = getenv("PL2_TIMING") != nullptr;
   cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;
@@ -264,10 +327,11 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
     if (cudaMemsetAsync(d_g1, 0, static_cast<uint64_t>(npad) * c2 * 8, c->stream) != cudaSuccess || cudaMemcpyAsync(d_g1, g1_host, static_cast<uint64_t>(n) * c2 * 8, cudaMemcpyHostToDevice, c->stream) != cudaSuccess) break;
     // k+1 projections; every H_t = Y G_t is kept side by side in qq (column-major M x q)   :5783-5855
     for (uint32_t iter = 0; iter <= k; ++iter) {
-      launch_xa(d_g1, c2, d_qq, m, iter * c2, c2);
+      double* h_t = d_qq + static_cast<uint64_t>(iter * c2) * m;
+      ts_rc |= PcaLaunchXa(job, &ts, job->d_slope, job->d_icpt, d_g1, c2, h_t, m, c2);
       if (iter < k) {
         if (cudaMemsetAsync(d_g2, 0, static_cast<uint64_t>(npad) * c2 * 8, c->stream) != cudaSuccess) break;
-        launch_xtb(d_qq, m, iter * c2, c2, d_g2, c2, 1);
+        ts_rc |= PcaLaunchXtb(job, &ts, h_t, m, c2, d_g2, c2, 1);
         if (sharded && CommAllReduceSumF64(c, d_g2, static_cast<uint64_t>(npad) * c2, c->stream)) break;
         scale_kernel<<<static_cast<uint32_t>(DivUpU64(static_cast<uint64_t>(npad) * c2, 256)), 256, 0, c->stream>>>(d_g2, static_cast<uint64_t>(npad) * c2, m_recip);
         c->launches++;
@@ -355,7 +419,7 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
     mark("orthonormal basis of the Krylov matrix (BCGS)");
     // B = Y^T Q (N x q, column-major)   :5870-5916
     if (cudaMemsetAsync(d_b, 0, static_cast<uint64_t>(n) * q * 8, c->stream) != cudaSuccess) break;
-    launch_xtb(d_qq, m, 0, static_cast<uint32_t>(q), d_b, 1, n);
+    ts_rc |= PcaLaunchXtb(job, &ts, d_qq, m, static_cast<uint32_t>(q), d_b, 1, n);
     if (sharded && CommAllReduceSumF64(c, d_b, static_cast<uint64_t>(n) * q, c->stream)) break;
     mark("B = Yt.Q");
     // Top-k left singular pairs of B (:5920, dgesvd in the reference).  Only the leading k of q are wanted and they
@@ -405,13 +469,7 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
     set_error("pl2gpu_pca_run: a tensor-path launch failed");
     rc = 1;
   }
-  cudaFree(d_gdig);
-  cudaFree(d_hs);
-  cudaFree(d_hi);
-  cudaFree(d_scale);
-  cudaFree(d_inv_scale);
-  cudaFree(d_colmax);
-  cudaFree(d_partial);
+  PcaTsFree(&ts);
   cudaFree(d_gram);
   cudaFree(d_gram_u);
   cudaFree(d_gram_partial);
@@ -432,17 +490,77 @@ int pl2gpu_pca_run_sharded(Pl2PcaJob* job, const double* g1_host, uint64_t total
   return PcaRunImpl(job, g1_host, total_variant_ct, true, eigvals_host, eigvecs_host);
 }
 
+int pl2gpu_pca_products(Pl2PcaJob* job, const double* g_host, uint32_t g_cols, double* yg_host, const double* h_host, uint32_t h_cols, double* yth_host) {
+  if (!job || !job->variant_ct || (g_cols && (!g_host || !yg_host)) || (h_cols && (!h_host || !yth_host))) {
+    set_error("pl2gpu_pca_products: bad arguments (needs a non-empty job)");
+    return 1;
+  }
+  Ctx* c = &job->ctx->c;
+  PL2_CUDA_OK(cudaSetDevice(c->device));
+  const uint32_t n = job->sample_ct, npad = job->sample_ct_padded, m = job->variant_ct;
+  PL2_TRY(PcaFinishLayouts(job, h_cols != 0));
+  PcaTs ts;
+  PL2_TRY(PcaTsAlloc(job, h_cols != 0, &ts));
+  double *d_g = nullptr, *d_yg = nullptr, *d_h = nullptr, *d_yth = nullptr;
+  int rc = 1;
+  do {
+    if (g_cols) {
+      if (cudaMalloc(&d_g, static_cast<uint64_t>(npad) * g_cols * 8) != cudaSuccess || cudaMalloc(&d_yg, static_cast<uint64_t>(m) * g_cols * 8) != cudaSuccess) {
+        cudaGetLastError();
+        set_error("pl2gpu_pca_products: insufficient device memory for %u columns of Y G", g_cols);
+        break;
+      }
+      if (cudaMemsetAsync(d_g, 0, static_cast<uint64_t>(npad) * g_cols * 8, c->stream) != cudaSuccess ||
+          cudaMemcpyAsync(d_g, g_host, static_cast<uint64_t>(n) * g_cols * 8, cudaMemcpyHostToDevice, c->stream) != cudaSuccess || PcaLaunchXa(job, &ts, job->d_slope, job->d_icpt, d_g, g_cols, d_yg, m, g_cols) ||
+          cudaMemcpyAsync(yg_host, d_yg, static_cast<uint64_t>(m) * g_cols * 8, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess) {
+        set_error("pl2gpu_pca_products: Y G: %s", cudaGetErrorString(cudaGetLastError()));
+        break;
+      }
+    }
+    if (h_cols) {
+      if (cudaMalloc(&d_h, static_cast<uint64_t>(m) * h_cols * 8) != cudaSuccess || cudaMalloc(&d_yth, static_cast<uint64_t>(n) * h_cols * 8) != cudaSuccess) {
+        cudaGetLastError();
+        set_error("pl2gpu_pca_products: insufficient device memory for %u columns of Y^T H", h_cols);
+        break;
+      }
+      if (cudaMemcpyAsync(d_h, h_host, static_cast<uint64_t>(m) * h_cols * 8, cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
+          cudaMemsetAsync(d_yth, 0, static_cast<uint64_t>(n) * h_cols * 8, c->stream) != cudaSuccess || PcaLaunchXtb(job, &ts, d_h, m, h_cols, d_yth, h_cols, 1) ||
+          cudaMemcpyAsync(yth_host, d_yth, static_cast<uint64_t>(n) * h_cols * 8, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess) {
+        set_error("pl2gpu_pca_products: Y^T H: %s", cudaGetErrorString(cudaGetLastError()));
+        break;
+      }
+    }
+    if (cudaStreamSynchronize(c->stream) != cudaSuccess || cudaGetLastError() != cudaSuccess) {
+      set_error("pl2gpu_pca_products: %s", cudaGetErrorString(cudaGetLastError()));
+      break;
+    }
+    rc = 0;
+  } while (0);
+  PcaTsFree(&ts);
+  cudaFree(d_g);
+  cudaFree(d_yg);
+  cudaFree(d_h);
+  cudaFree(d_yth);
+  return rc;
+}
+
 // `--variant-score` (VscoreReport, 2.0/plink2_matrix_calc.cc:9274): per variant the dot product of sample weights with
 // the ALT dosages, a missing call replaced by 2 x ALT frequency.  One H = Y W pass of the approx-PCA tile path does it:
-// with Y the standardised matrix (y = (g - 2 f) / sd for a called genotype, 0 for a missing one)
-//   sum_s w_s dosage_vs  =  (Y W)_v sd_v + 2 f_v sum_s w_s ,
-// so the int8 tensor kernel runs unchanged and a small epilogue un-standardises (variants without variance: 2 f W).
-static __global__ void __launch_bounds__(256) vscore_finish_kernel(const double* __restrict__ h, uint64_t h_ld, uint32_t variant_ct, uint32_t cols, const double* __restrict__ slope, const double* __restrict__ twof, const double* __restrict__ wtot, double* __restrict__ out) {
+// with Y the centred dosage (y = g - 2 f for a called genotype, 0 for a missing one: slope 1, intercept -2 f, whatever
+// the variance - not the job's standardised matrix)
+//   sum_s w_s dosage_vs  =  (Y W)_v + 2 f_v sum_s w_s .
+static __global__ void __launch_bounds__(256) vscore_centre_kernel(const double* __restrict__ twof, uint32_t variant_ct, double* __restrict__ slope, double* __restrict__ icpt) {
+  const uint32_t v = blockIdx.x * blockDim.x + threadIdx.x;
+  if (v >= variant_ct) return;
+  slope[v] = 1.0;
+  icpt[v] = -twof[v];
+}
+
+static __global__ void __launch_bounds__(256) vscore_finish_kernel(const double* __restrict__ h, uint64_t h_ld, uint32_t variant_ct, uint32_t cols, const double* __restrict__ twof, const double* __restrict__ wtot, double* __restrict__ out) {
   const uint64_t idx = static_cast<uint64_t>(blockIdx.x) * blockDim.x + threadIdx.x;
   if (idx >= static_cast<uint64_t>(variant_ct) * cols) return;
   const uint32_t v = static_cast<uint32_t>(idx / cols), c = static_cast<uint32_t>(idx % cols);
-  const double sl = slope[v];
-  out[idx] = (sl != 0.0 ? h[static_cast<uint64_t>(c) * h_ld + v] / sl : 0.0) + twof[v] * wtot[c];
+  out[idx] = h[static_cast<uint64_t>(c) * h_ld + v] + twof[v] * wtot[c];
 }
 
 int pl2gpu_pca_vscore(Pl2PcaJob* job, const double* weights_host, uint32_t cols, double* out_host) {
@@ -453,14 +571,15 @@ int pl2gpu_pca_vscore(Pl2PcaJob* job, const double* weights_host, uint32_t cols,
   Ctx* c = &job->ctx->c;
   PL2_CUDA_OK(cudaSetDevice(c->device));
   const uint32_t n = job->sample_ct, npad = job->sample_ct_padded, m = job->variant_ct;
-  uint8_t* d_gdig = nullptr;
-  double *d_scale = nullptr, *d_inv_scale = nullptr, *d_w = nullptr, *d_h = nullptr, *d_wtot = nullptr, *d_out = nullptr;
-  unsigned long long* d_colmax = nullptr;
+  PL2_TRY(PcaFinishLayouts(job, false));
+  PcaTs ts;
+  PL2_TRY(PcaTsAlloc(job, false, &ts));
+  double *d_w = nullptr, *d_h = nullptr, *d_wtot = nullptr, *d_out = nullptr, *d_slope = nullptr, *d_icpt = nullptr;
   int rc = 1;
   do {
-    if (cudaMalloc(&d_gdig, static_cast<uint64_t>(npad) * kPcaNMax) != cudaSuccess || cudaMalloc(&d_scale, 8 * kPcaCgMax) != cudaSuccess || cudaMalloc(&d_inv_scale, 8 * kPcaCgMax) != cudaSuccess ||
-        cudaMalloc(&d_colmax, 8 * kPcaCgMax) != cudaSuccess || cudaMalloc(&d_w, static_cast<uint64_t>(npad) * cols * 8) != cudaSuccess || cudaMalloc(&d_h, static_cast<uint64_t>(m) * cols * 8) != cudaSuccess ||
-        cudaMalloc(&d_wtot, 8ull * cols) != cudaSuccess || cudaMalloc(&d_out, static_cast<uint64_t>(m) * cols * 8) != cudaSuccess) {
+    if (cudaMalloc(&d_w, static_cast<uint64_t>(npad) * cols * 8) != cudaSuccess || cudaMalloc(&d_h, static_cast<uint64_t>(m) * cols * 8) != cudaSuccess ||
+        cudaMalloc(&d_wtot, 8ull * cols) != cudaSuccess || cudaMalloc(&d_out, static_cast<uint64_t>(m) * cols * 8) != cudaSuccess || cudaMalloc(&d_slope, 8ull * m) != cudaSuccess ||
+        cudaMalloc(&d_icpt, 8ull * m) != cudaSuccess) {
       cudaGetLastError();
       set_error("pl2gpu_pca_vscore: insufficient device memory for %u score columns", cols);
       break;
@@ -471,28 +590,13 @@ int pl2gpu_pca_vscore(Pl2PcaJob* job, const double* weights_host, uint32_t cols,
     if (cudaMemsetAsync(d_w, 0, static_cast<uint64_t>(npad) * cols * 8, c->stream) != cudaSuccess || cudaMemcpyAsync(d_w, weights_host, static_cast<uint64_t>(n) * cols * 8, cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
         cudaMemcpyAsync(d_wtot, wtot.data(), 8ull * cols, cudaMemcpyHostToDevice, c->stream) != cudaSuccess)
       break;
-    // rows [variant_ct, variant_cap) must decode to "missing"
-    if (job->variant_cap > m && LaunchPadGenotypes(c, job->d_raw + static_cast<uint64_t>(m) * job->pitch, job->pitch, job->sample_ct, 0, job->variant_cap - m)) break;
-    bool ok = true;
-    for (uint32_t cc = 0; ok && cc < cols; cc += kPcaCgMax) {
-      const uint32_t valid = std::min(kPcaCgMax, cols - cc), cg = kPcaCgMax;
-      ok = cudaMemsetAsync(d_colmax, 0, 8 * kPcaCgMax, c->stream) == cudaSuccess;
-      pca_colmax_kernel<<<dim3(valid, std::min<uint32_t>(64, DivUpU32(npad, 256))), 256, 0, c->stream>>>(d_w + cc, cols, 1, npad, nullptr, nullptr, d_colmax);
-      pca_scales_kernel<<<1, 64, 0, c->stream>>>(d_colmax, kPcaCgMax, d_scale, d_inv_scale);
-      c->launches += 2;
-      for (int pass = 0; pass < 2; ++pass) {
-        pca_digits_kernel<<<npad / 64, 256, 0, c->stream>>>(d_w + cc, cols, 1, npad, cg, valid, nullptr, nullptr, d_scale, d_gdig, nullptr, pass);
-        pca_xa_wg_kernel<<<job->variant_cap / 128, kPcaThreads, kPxaSmemBytes, c->stream>>>(job->d_raw, job->pitch, npad, m, d_gdig, valid, job->d_slope, job->d_icpt, d_inv_scale, d_h + static_cast<uint64_t>(cc) * m, m,
-                                                                                          pass ? 1.0 / kPcaPass1Scale : 1.0, pass);
-        c->launches += 2;
-      }
-      ok = ok && cudaGetLastError() == cudaSuccess;
-    }
-    if (!ok) {
+    vscore_centre_kernel<<<DivUpU32(m, 256), 256, 0, c->stream>>>(job->d_twof, m, d_slope, d_icpt);
+    c->launches++;
+    if (PcaLaunchXa(job, &ts, d_slope, d_icpt, d_w, cols, d_h, m, cols) || cudaGetLastError() != cudaSuccess) {
       set_error("pl2gpu_pca_vscore: kernel launch failed");
       break;
     }
-    vscore_finish_kernel<<<static_cast<uint32_t>(DivUpU64(static_cast<uint64_t>(m) * cols, 256)), 256, 0, c->stream>>>(d_h, m, m, cols, job->d_slope, job->d_twof, d_wtot, d_out);
+    vscore_finish_kernel<<<static_cast<uint32_t>(DivUpU64(static_cast<uint64_t>(m) * cols, 256)), 256, 0, c->stream>>>(d_h, m, m, cols, job->d_twof, d_wtot, d_out);
     c->launches++;
     if (cudaMemcpyAsync(out_host, d_out, static_cast<uint64_t>(m) * cols * 8, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
       set_error("pl2gpu_pca_vscore: %s", cudaGetErrorString(cudaGetLastError()));
@@ -500,14 +604,13 @@ int pl2gpu_pca_vscore(Pl2PcaJob* job, const double* weights_host, uint32_t cols,
     }
     rc = 0;
   } while (0);
-  cudaFree(d_gdig);
-  cudaFree(d_scale);
-  cudaFree(d_inv_scale);
-  cudaFree(d_colmax);
+  PcaTsFree(&ts);
   cudaFree(d_w);
   cudaFree(d_h);
   cudaFree(d_wtot);
   cudaFree(d_out);
+  cudaFree(d_slope);
+  cudaFree(d_icpt);
   return rc;
 }
 

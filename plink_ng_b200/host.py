@@ -348,6 +348,36 @@ def pca_approx(ctx: GpuContext, genovecs: np.ndarray, sample_ct: int, pc_ct: int
         lib.pl2gpu_pca_end(h)
 
 
+def pca_products(ctx: GpuContext, genovecs: np.ndarray, sample_ct: int, g=None, h=None, ref_freqs=None, calls=None):
+    """The two products of `--pca approx` (pl2gpu_pca_products) on the standardised matrix Y [variants, samples] of an
+    in-memory block: g [sample_ct, cx] -> Y g [variants, cx]; h [variants, ct] -> Y^T h [sample_ct, ct].  calls: the
+    variant counts of successive add_variants calls (default: one call).  Returns (Y g or None, Y^T h or None)."""
+    gv = np.ascontiguousarray(genovecs)
+    m = gv.shape[0]
+    calls = [m] if calls is None else list(calls)
+    assert sum(calls) == m
+    rf = None if ref_freqs is None else np.ascontiguousarray(ref_freqs, dtype=np.float64)
+    ga = None if g is None else np.ascontiguousarray(g, dtype=np.float64)
+    ha = None if h is None else np.asfortranarray(h, dtype=np.float64)  # column-major [ct][variant]
+    assert ga is None or ga.shape[0] == sample_ct
+    assert ha is None or ha.shape[0] == m
+    yg = None if ga is None else np.empty((ga.shape[1], m), dtype=np.float64)
+    yth = None if ha is None else np.empty((sample_ct, ha.shape[1]), dtype=np.float64)
+    job = C.c_void_p()
+    check(lib.pl2gpu_pca_begin_shard(ctx.handle, sample_ct, m, 1, C.byref(job)), "pl2gpu_pca_begin_shard")
+    try:
+        s = 0
+        for ct in calls:
+            part = None if rf is None else rf[s : s + ct]
+            check(lib.pl2gpu_pca_add_variants(job, gv[s:].ctypes.data, gv.strides[0], ct, 0, part.ctypes.data if part is not None else None), "pl2gpu_pca_add_variants")
+            s += ct
+        check(lib.pl2gpu_pca_products(job, ga.ctypes.data if ga is not None else None, 0 if ga is None else ga.shape[1], yg.ctypes.data if yg is not None else None,
+                                      ha.ctypes.data if ha is not None else None, 0 if ha is None else ha.shape[1], yth.ctypes.data if yth is not None else None), "pl2gpu_pca_products")
+        return (None if yg is None else yg.T), yth
+    finally:
+        lib.pl2gpu_pca_end(job)
+
+
 def score_sums(ctx: GpuContext, genovecs: np.ndarray, sample_ct: int, weights4: np.ndarray, named_dosages: np.ndarray):
     """`--score` accumulation (pl2gpu_score_*) over an in-memory block of scored entries: genovecs [entries, words]
     PgrGet rows, weights4 [entries, 4] fp64 contributions of genotype codes 0..3, named_dosages [entries] uint8
@@ -376,7 +406,7 @@ def variant_scores(ctx: GpuContext, genovecs: np.ndarray, sample_ct: int, weight
     assert w.shape[0] == sample_ct
     rf = None if ref_freqs is None else np.ascontiguousarray(ref_freqs, dtype=np.float64)
     h = C.c_void_p()
-    check(lib.pl2gpu_pca_begin_shard(ctx.handle, sample_ct, g.shape[0], 1, C.byref(h)), "pl2gpu_pca_begin_shard")
+    check(lib.pl2gpu_pca_begin_shard(ctx.handle, sample_ct, g.shape[0], 0, C.byref(h)), "pl2gpu_pca_begin_shard")  # pc_ct 0: a --variant-score job
     try:
         check(lib.pl2gpu_pca_add_variants(h, g.ctypes.data, g.strides[0], g.shape[0], 0, rf.ctypes.data if rf is not None else None), "pl2gpu_pca_add_variants")
         out = np.empty((g.shape[0], w.shape[1]), dtype=np.float64)

@@ -94,7 +94,7 @@ def test_approx_pca_matches_oracle_same_gaussian_start(gpu_ctx):
     from the same Gaussian start matrix."""
     from plink_ng_b200.host import pca_approx
 
-    n, m, k = 400, 6000, 5  # 2k = 10 columns: a column group padded to 12; q = 60 -> groups of 48 + 12
+    n, m, k = 400, 6000, 5  # 2k = 10 columns: one partial column group of 32; q = 60 -> groups of 32 + 28
     geno = _structured_geno(m, n, seed=9, pops=6, fst=0.1)
     g1 = np.random.default_rng(1).standard_normal((n, 2 * k))
     want_vals, want_vecs = orc.pca_approx(geno, k, g1)
@@ -110,8 +110,8 @@ def test_approx_pca_matches_oracle_same_gaussian_start(gpu_ctx):
 
 
 def test_approx_pca_k20_tensor_path_matches_oracle(gpu_ctx):
-    """BASELINE's --pca 20 shape at a size numpy finishes in seconds: 40-column passes (one column group of N = 160),
-    840-column final projection (17 groups of 48 + one of 24), several 128-variant / 256-sample tiles and split-K."""
+    """BASELINE's --pca 20 shape at a size numpy finishes in seconds: 40-column passes (column groups of 32 + 8),
+    840-column final projection (26 groups of 32 + one of 8), several 128-variant / 128-sample tiles and split-K."""
     from plink_ng_b200.host import pca_approx
 
     n, m, k = 1100, 9000, 20

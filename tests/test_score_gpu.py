@@ -89,8 +89,8 @@ def test_score_header_read_names_the_column(golden_dir, tmp_path):
 
 @pytest.mark.parametrize("n,m,cols", [(300, 1000, 3), (2000, 5000, 50)])
 def test_variant_scores_match_oracle(gpu_ctx, n, m, cols):
-    """--variant-score on the approx-PCA tile path: several 128-variant CTAs, a second column group (50 > 48 columns),
-    monomorphic variants (no variance -> the 2 f W term alone), samples with weight 0."""
+    """--variant-score on the approx-PCA tile path: several 128-variant CTAs, a second column group (50 > 32 columns),
+    monomorphic variants (centred dosage 0 -> the 2 f W term alone), samples with weight 0."""
     from plink_ng_b200.host import variant_scores
 
     rng = np.random.default_rng(n + cols)
