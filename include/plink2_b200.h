@@ -103,6 +103,19 @@ int pl2gpu_king_begin_ex(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start,
 /* Bytes of device memory pl2gpu_king_begin_ex would need for that row range and chunk size (for pass planning,
  * the analogue of CountTrianglePasses, 2.0/plink2_matrix_calc.cc:216-255). */
 uint64_t pl2gpu_king_mem_required(uint32_t sample_ct, uint32_t row_start, uint32_t row_end, uint32_t max_variants_per_add);
+/* Mapped job (single device, default algorithm): the same counts over a caller-chosen device sample order, cut at a column
+ * bound.  order[p] = the sample index (column of the PgrGet rows) placed at device position p, a permutation of
+ * [0, sample_ct); NULL = identity.  The job holds the pairs of positions (j, i), row_start <= j < row_end, i < min(j, col_end)
+ * (1 <= col_end <= sample_ct); column tiles entirely at or past col_end are never computed.  add_variants still takes rows
+ * in sample-index order: the permutation is applied on the device, overlapped with the previous batch's tensor kernel.
+ * get_counts / get_kinship / get_filtered take and return POSITIONS ("1" = the smaller position) and skip every pair whose
+ * column is at or past col_end, so row j of get_counts holds min(j, col_end) pairs.  With order == NULL and
+ * col_end == sample_ct this is pl2gpu_king_begin_ex with the default algorithm.  The sharded entry points refuse a mapped
+ * job.  Use: samples that a table must pair with everyone (`--king-table-require`) placed last, so that their pairs are
+ * the row slab [n0, sample_ct), or that slab cut at column n0 (`--king-table-require-xor`). */
+int pl2gpu_king_begin_mapped(Pl2GpuCtx* ctx, uint32_t sample_ct, const uint32_t* order, uint32_t row_start, uint32_t row_end, uint32_t col_end, uint32_t max_variants_per_add, Pl2KingJob** job_ptr);
+/* Bytes of device memory pl2gpu_king_begin_mapped would need (pass planning). */
+uint64_t pl2gpu_king_mapped_mem_required(uint32_t sample_ct, uint32_t row_start, uint32_t row_end, uint32_t col_end, uint32_t max_variants_per_add);
 /* Accumulate `variant_ct` more variants.  `genovecs` is host memory unless src_is_device != 0;
  * consecutive variants are `variant_stride_bytes` apart (>= 8*ceil(sample_ct/32), multiple of 8).
  * src_is_device: 0 = host memory (the call returns once the buffer has been consumed; the kernels keep

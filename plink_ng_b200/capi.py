@@ -47,6 +47,8 @@ SIGNATURES = {
     "pl2gpu_king_begin_ex": (C.c_int, [vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, C.c_uint32, C.POINTER(vp)]),
     "pl2gpu_king_add_variants_sharded": (C.c_int, [vp, vp, C.c_uint64, C.c_uint32, C.c_int]),
     "pl2gpu_king_mem_required": (C.c_uint64, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]),
+    "pl2gpu_king_begin_mapped": (C.c_int, [vp, C.c_uint32, vp, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.POINTER(vp)]),
+    "pl2gpu_king_mapped_mem_required": (C.c_uint64, [C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32, C.c_uint32]),
     "pl2gpu_king_add_variants": (C.c_int, [vp, vp, C.c_uint64, C.c_uint32, C.c_int]),
     "pl2gpu_king_get_counts": (C.c_int, [vp, C.c_uint32, C.c_uint32, vp, C.c_int]),
     "pl2gpu_king_get_kinship": (C.c_int, [vp, C.c_uint32, C.c_uint32, vp, C.c_int]),

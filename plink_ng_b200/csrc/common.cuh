@@ -77,8 +77,9 @@ struct TileList {
   std::vector<uint32_t> h_rowtile_offset;  // host copy of the same
 };
 
-uint64_t CountTiles(uint32_t row_start, uint32_t row_end, bool include_diag, uint32_t tile_cols = kTileCols);
-int BuildTileList(uint32_t row_start, uint32_t row_end, bool include_diag, TileList* tl, uint32_t tile_cols = kTileCols);
+// col_end: tiles that lie entirely at or past this column are left out (a KING job cut at a column bound)
+uint64_t CountTiles(uint32_t row_start, uint32_t row_end, bool include_diag, uint32_t tile_cols = kTileCols, uint32_t col_end = 0xFFFFFFFFu);
+int BuildTileList(uint32_t row_start, uint32_t row_end, bool include_diag, TileList* tl, uint32_t tile_cols = kTileCols, uint32_t col_end = 0xFFFFFFFFu);
 void FreeTileList(TileList* tl);
 
 // ---- staged genotype block on the device (implemented in pl2gpu.cu) ----

@@ -129,6 +129,20 @@ int MarkFamilyFile(const std::string& path, const SampleInfo& S, const std::unor
 
 }  // namespace
 
+int MarkSampleIds(const std::vector<std::string>& files, const char* flag, const SampleInfo& S, std::vector<uint8_t>* marked, uint64_t* dup_ct, std::string* err) {
+  const uint32_t n = S.size();
+  std::unordered_multimap<std::string, uint32_t> index;
+  index.reserve(static_cast<size_t>(n) * 2);
+  for (uint32_t k = n; k--;) index.emplace(S.fid[k] + "\t" + S.iid[k], k);
+  marked->assign(n, 0);
+  *dup_ct = 0;
+  for (const std::string& path : files) {
+    const int rc = MarkSampleFile(path, flag, S, index, marked, dup_ct, err);
+    if (rc) return rc;
+  }
+  return 0;
+}
+
 bool ParseChrList(const std::vector<std::string>& args, const char* flag, std::vector<uint8_t>* mask, std::string* err) {
   mask->assign(27, 0);
   std::string joined;

@@ -54,6 +54,11 @@ int CountGenotypes(Dataset* ds, uint32_t thread_ct, VariantGenoCounts* vc, std::
 // REF allele "ddosage" pair of a variant from those counts (the numbers behind --freq; see RunFreq)
 void FounderAlleleDd(const VariantGenoCounts& vc, uint32_t v, uint32_t chr_code, uint32_t founder_ct, uint32_t founder_male_ct, uint64_t* alt_dd, uint64_t* tot_dd);
 
+// Marks the samples named in one or more ID files read like --keep files (LoadSampleIds with kfLoadSampleIdsMultifile,
+// plink2_common.cc:1707: the lists are merged): (*marked)[k] = 1.  `flag` names the option in messages.  Returns 0, or 3
+// (open failure) / 6 (malformed file) with *err set.  *dup_ct counts IDs named more than once.
+int MarkSampleIds(const std::vector<std::string>& files, const char* flag, const SampleInfo& S, std::vector<uint8_t>* marked, uint64_t* dup_ct, std::string* err);
+
 // keep[k] != 0: sample / variant k (current numbering) stays.  Compacts the tables and updates the reader view.
 void KeepSamples(Dataset* ds, const std::vector<uint8_t>& keep);
 void KeepVariants(Dataset* ds, const std::vector<uint8_t>& keep);

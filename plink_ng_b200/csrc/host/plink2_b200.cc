@@ -119,6 +119,9 @@ struct Cmd {
   double king_cutoff_prefix_thresh = -1;
   std::string king_table_subset;          // --king-table-subset <file> [kinship threshold]
   double king_table_subset_thresh = -DBL_MAX;
+  std::vector<std::string> king_table_require;  // --king-table-require[-xor] <file...>: only pairs with >= 1 (-xor: exactly 1) listed sample
+  bool king_table_require_xor = false;
+  uint32_t king_table_require_flags = 0;        // how many of the two flags were given
   bool make_grm_sparse = false;            // --make-grm-sparse <cutoff>
   double grm_sparse_cutoff = -DBL_MAX;
   bool make_grm_bin = false, make_grm_list = false, make_rel = false, grm_cov = false, grm_meanimpute = false, grm_id_header = false;
@@ -283,6 +286,11 @@ int ParseArgs(int argc, char** argv, Cmd* c) {
       if (!need(1, 2)) return Usage("--king-table-subset requires a filename and an optional kinship threshold.");
       c->king_table_subset = prm[0];
       if (nparam == 2 && !ParseDouble(prm[1], &c->king_table_subset_thresh)) return Usage("Invalid --king-table-subset threshold.");
+    } else if (flag == "--king-table-require" || flag == "--king-table-require-xor") {
+      if (nparam < 1) return Usage((flag + " requires at least one filename.").c_str());
+      c->king_table_require.assign(prm, prm + nparam);
+      c->king_table_require_xor = flag == "--king-table-require-xor";
+      ++c->king_table_require_flags;
     } else if (flag == "--king-cutoff") {
       if (nparam == 2) {
         // plink2.cc:7671-7700: <prefix> <threshold> prunes from a matrix written earlier by --make-king bin[4] triangle
@@ -665,6 +673,13 @@ int ParseArgs(int argc, char** argv, Cmd* c) {
   }
   if (c->pgen.empty() || c->pvar.empty() || c->psam.empty()) return Usage("No input dataset (--bfile / --pfile / --bed+--bim+--fam / --pgen+--pvar+--psam).");
   if (!c->indep_preferred.empty() && !c->indep_pairwise) return Usage("--indep-preferred must be used with --indep-pairwise.");
+  if (c->king_table_require_flags) {
+    // the reference's checks (plink2.cc:7732-7750, :8467, :8571), in the order it meets them
+    if (c->king_cutoff >= 0 || !c->king_cutoff_prefix.empty()) return Usage("--king-table-require[-xor] cannot be used with --king-cutoff.");
+    if (c->king_table_require_flags > 1) return Usage("--king-table-require cannot be used with --king-table-require-xor.");
+    if (c->make_king) return Usage("--make-king cannot be used with --king-table-subset or\n--king-table-require[-xor].");
+    if (c->make_king_table && !c->col_id) return Usage("--king-table-require[-xor] requires --make-king-table cols= to include\nthe 'id' column set.");
+  }
   if (c->pca) {
     // 2.0/plink2.cc:10207-10232
     if (c->pca_approx) {
@@ -1135,7 +1150,8 @@ int NaturalCompare(const std::string& a, const std::string& b) {
 // "--make-king-table rel-check" (GetRelCheckOrKTRequirePairs, 2.0/plink2_matrix_calc.cc:2975-3043): the samples in
 // natural order of FID<tab>IID[<tab>SID]; inside every block of equal FID (equal up to capitalisation, see below) each
 // sample is paired with all earlier ones, the later sample listed first.
-void RelCheckPairs(const SampleInfo& S, std::vector<uint32_t>* pairs) {
+// The sample indices in natural order of FID<tab>IID[<tab>SID] (the reference's nsorted_xidbox); *key_out gets the keys.
+std::vector<uint32_t> NaturalSampleOrder(const SampleInfo& S, std::vector<std::string>* key_out = nullptr) {
   const uint32_t n = S.size();
   std::vector<std::string> key(n);
   for (uint32_t k = 0; k < n; ++k) {
@@ -1145,6 +1161,14 @@ void RelCheckPairs(const SampleInfo& S, std::vector<uint32_t>* pairs) {
   std::vector<uint32_t> ord(n);
   for (uint32_t k = 0; k < n; ++k) ord[k] = k;
   std::stable_sort(ord.begin(), ord.end(), [&](uint32_t x, uint32_t y) { return NaturalCompare(key[x], key[y]) < 0; });
+  if (key_out) *key_out = std::move(key);
+  return ord;
+}
+
+void RelCheckPairs(const SampleInfo& S, std::vector<uint32_t>* pairs) {
+  const uint32_t n = S.size();
+  std::vector<std::string> key;
+  const std::vector<uint32_t> ord = NaturalSampleOrder(S, &key);
   for (uint32_t b0 = 0; b0 < n;) {
     // block end as the reference finds it (:3030-3042): the first sorted key not below "<FID of the block's first
     // entry> " in natural order - which also takes in FIDs that differ from it only in capitalisation
@@ -1160,11 +1184,48 @@ void RelCheckPairs(const SampleInfo& S, std::vector<uint32_t>* pairs) {
   }
 }
 
-int RunKingSubset(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
+// --king-table-require[-xor] sample set (CalcKingTableSubset, 2.0/plink2_matrix_calc.cc:3248-3267): IDs read like --keep
+// files, the lists of all files merged.
+int LoadKingRequire(const Cmd& c, const SampleInfo& S, std::vector<uint8_t>* req) {
+  std::string err;
+  uint64_t dup_ct = 0;
+  const int rc = MarkSampleIds(c.king_table_require, c.king_table_require_xor ? "king-table-require-xor" : "king-table-require", S, req, &dup_ct, &err);
+  if (rc) {
+    logprintf("Error: %s\n", err.c_str());
+    return rc == 3 ? kRetOpenFail : kRetMalformedInput;
+  }
+  uint32_t ct = 0;
+  for (uint8_t f : *req) ct += f;
+  if (!ct) {
+    logprintf("Error: No sample ID(s) in --king-table-require[-xor] file(s) are in the current\ndataset.\n");
+    return kRetInconsistentInput;
+  }
+  if (c.king_table_require_xor && ct == S.size()) {
+    logprintf("Error: All sample ID(s) in --king-table-require-xor file(s) are in the current\ndataset.\n");
+    return kRetInconsistentInput;
+  }
+  logprintf("--king-table-require%s: %u sample ID%s loaded.\n", c.king_table_require_xor ? "-xor" : "", ct, ct == 1 ? "" : "s");
+  return 0;
+}
+
+// A listed or rel-check pair is kept when it includes at least one required sample (-xor: exactly one), :2777-2779.
+inline bool KingRequireKeeps(const Cmd& c, const std::vector<uint8_t>& req, uint32_t a, uint32_t b) {
+  return c.king_table_require_xor ? req[a] != req[b] : (req[a] || req[b]);
+}
+
+int RunKingRequireDense(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, const std::vector<uint32_t>& vidx, const std::vector<uint8_t>& req);
+
+// rel_check: pairs of same-FID samples when there is no subset file.  Without a subset file or rel-check, the
+// --king-table-require[-xor] pairs go to RunKingRequireDense instead of a pair list.
+int RunKingSubset(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, bool rel_check) {
   const SampleInfo& S = ds->samples;
   const uint32_t n = S.size();
   if (c.parallel_tot != 1) {
-    logprintf("Error: --king-table-subset with --parallel is not supported by plink2_b200 yet.\n");
+    logprintf("Error: %s with --parallel is not supported by plink2_b200 yet.\n", c.king_table_subset.empty() && !rel_check ? "--king-table-require[-xor]" : "--king-table-subset");
+    return kRetNotYetSupported;
+  }
+  if (!c.king_table_require.empty() && c.gpus > 1) {
+    logprintf("Error: --king-table-require[-xor] runs on one GPU; --gpus %u is not supported with it.\n", c.gpus);
     return kRetNotYetSupported;
   }
   if (n < 2) {
@@ -1182,9 +1243,25 @@ int RunKingSubset(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
     logprintf("Error: No variants remaining for KING-robust calculation.\n");
     return kRetDegenerateData;
   }
+  std::vector<uint8_t> req;
+  if (!c.king_table_require.empty()) {
+    const int rrc = LoadKingRequire(c, S, &req);
+    if (rrc) return rrc;
+    if (c.king_table_subset.empty() && !rel_check) return RunKingRequireDense(c, ds, ctx, vidx, req);
+  }
   std::vector<uint32_t> pairs;
   if (c.king_table_subset.empty()) {
     RelCheckPairs(S, &pairs);  // rel-check without a subset file
+    if (!req.empty()) {
+      // the same pairs in the same order as GetRelCheckOrKTRequirePairs' require branch (:3045-3160)
+      size_t w = 0;
+      for (size_t p = 0; p < pairs.size(); p += 2) {
+        if (!KingRequireKeeps(c, req, pairs[p], pairs[p + 1])) continue;
+        pairs[w++] = pairs[p];
+        pairs[w++] = pairs[p + 1];
+      }
+      pairs.resize(w);
+    }
   } else {
   // ---- header (:3391-3452): [#FID1|FID] (ID1|IID1) [SID1] [FID2] (ID2|IID2) [SID2] ... [KINSHIP|Kinship]
   std::vector<std::string> lines;
@@ -1268,6 +1345,7 @@ int RunKingSubset(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
       logprintf("Error: Identical sample IDs on line %zu of --king-table-subset file.\n", li + 1);
       return kRetInconsistentInput;
     }
+    if (!req.empty() && !KingRequireKeeps(c, req, i1->second, i2->second)) continue;
     if (thresh != -DBL_MAX) {
       if (f.size() <= kinship_col) {
         logprintf("Error: Line %zu of --king-table-subset file has fewer tokens than expected.\n", li + 1);
@@ -1350,6 +1428,169 @@ int RunKingSubset(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   logprintf("Results written to %s .\n", tab_name.c_str());
   if (c.king_table_filter != -DBL_MAX) {
     logprintf("--king-table-filter: %llu relationship%s reported (%llu filtered out).\n", static_cast<unsigned long long>(pair_ct - filter_ct), (pair_ct - filter_ct == 1) ? "" : "s", static_cast<unsigned long long>(filter_ct));
+  }
+  return 0;
+}
+
+// --king-table-require[-xor] without a pair list (GetRelCheckOrKTRequirePairs' require branch, :3045-3160): in natural
+// sample order, row idx1 ascending, then idx2 < idx1 ascending, the pair (idx1, idx2) is written when it includes a
+// required sample (-xor: exactly one).  Instead of listing those pairs, the device holds the samples in the order
+// "non-required, then required" (each in index order): with n0 non-required samples the wanted pairs are exactly rows
+// [n0, N) of the strict lower triangle over positions, cut at column n0 for -xor, so one mapped KING job computes them
+// on the tensor tile path with work in proportion to r x N.  The results come back in positions, are oriented to the
+// reference's row ("1" = the sample listed first) and sorted into its order on the host.  Without --king-table-filter
+// every pair is held in host memory (28 bytes each) until the sort; with it only the qualifying pairs leave the device.
+// NSNP is the dense count: CalcKingTableSubset has no rare-variant pre-scan.
+int RunKingRequireDense(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, const std::vector<uint32_t>& vidx, const std::vector<uint8_t>& req) {
+  const SampleInfo& S = ds->samples;
+  const uint32_t n = S.size();
+  std::vector<uint32_t> order;
+  order.reserve(n);
+  for (uint32_t k = 0; k < n; ++k)
+    if (!req[k]) order.push_back(k);
+  const uint32_t n0 = static_cast<uint32_t>(order.size());
+  for (uint32_t k = 0; k < n; ++k)
+    if (req[k]) order.push_back(k);
+  const uint32_t col_end = c.king_table_require_xor ? n0 : n;
+  auto pairs_below = [col_end](uint64_t r) { return r <= col_end ? (r ? r * (r - 1) / 2 : 0) : (col_end ? static_cast<uint64_t>(col_end) * (col_end - 1) / 2 : 0) + (r - col_end) * col_end; };
+  const uint64_t pair_ct = pairs_below(n) - pairs_below(n0);
+  const bool filter = c.king_table_filter != -DBL_MAX;
+  logprintf("--king-table-require%s: %llu pair%s on the device (rows %u-%u of the sample order with the required samples last).\n", c.king_table_require_xor ? "-xor" : "", static_cast<unsigned long long>(pair_ct), pair_ct == 1 ? "" : "s", n0, n - 1);
+  if (!filter) logprintf("--king-table-require%s: the unfiltered table is sorted in host memory (%.1f MB) before it is written.\n", c.king_table_require_xor ? "-xor" : "", pair_ct * 28.0 / 1e6);
+  std::vector<uint32_t> rank(n);
+  {
+    const std::vector<uint32_t> nat = NaturalSampleOrder(S);
+    for (uint32_t r = 0; r < n; ++r) rank[nat[r]] = r;
+  }
+  // pass planning against free device memory (or --gpu-memory), as RunKing does; each pass re-streams the variants
+  uint64_t free_b = 0, total_b = 0;
+  if (pl2gpu_ctx_mem_info(ctx, &free_b, &total_b)) return GpuFail("pl2gpu_ctx_mem_info");
+  uint64_t budget = free_b - free_b / 10;
+  if (c.gpu_memory_mib && (c.gpu_memory_mib << 20) < budget) budget = c.gpu_memory_mib << 20;
+  uint32_t batch = 65536;
+  while (batch > 2048 && 5ull * batch * ((n + 639) / 640 * 160) > budget / 4) batch /= 2;
+  auto fits = [&](uint32_t a, uint32_t b) { return pl2gpu_king_mapped_mem_required(n, a, b, col_end, batch) <= budget; };
+  std::vector<uint32_t> bounds{n0};
+  while (bounds.back() < n) {
+    const uint32_t r = bounds.back();
+    if (!fits(r, r + 1)) {
+      logprintf("Error: Insufficient GPU memory for --make-king-table on %u samples.\n", n);
+      return kRetNomem;
+    }
+    uint32_t lo = r + 1, hi = n;
+    while (lo < hi) {
+      const uint32_t mid = lo + (hi - lo + 1) / 2;
+      if (fits(r, mid)) lo = mid;
+      else hi = mid - 1;
+    }
+    bounds.push_back(lo);
+  }
+  const uint32_t pass_ct = static_cast<uint32_t>(bounds.size() - 1);
+  if (pass_ct > 1) logprintf("--make-king-table: %u passes over the variants (device accumulators planned against %llu MiB).\n", pass_ct, static_cast<unsigned long long>(budget >> 20));
+  struct Row {
+    uint32_t r1, r2;  // natural-order ranks of the sample listed first (the larger) and second
+    uint32_t cc[5];
+  };
+  std::vector<Row> rows;
+  rows.reserve(filter ? 0 : pair_ct);
+  // device pair (position pj, position pi < pj), counts with "1" = pi: listed first is the sample of larger rank
+  auto add_row = [&](uint32_t pj, uint32_t pi, const uint32_t* cc) {
+    const uint32_t sj = order[pj], si = order[pi];
+    Row row;
+    memcpy(row.cc, cc, 20);
+    if (rank[sj] > rank[si]) {
+      row.r1 = rank[sj];
+      row.r2 = rank[si];
+      std::swap(row.cc[2], row.cc[3]);  // "1" becomes the sample at the larger position
+    } else {
+      row.r1 = rank[si];
+      row.r2 = rank[sj];
+    }
+    rows.push_back(row);
+  };
+  BlockStreamer bs(ds, &vidx, n, batch);
+  if (!bs.Init()) return GpuFail("pl2gpu_host_alloc");
+  for (uint32_t pass = 1; pass <= pass_ct; ++pass) {
+    const uint32_t p0 = bounds[pass - 1], p1 = bounds[pass];
+    Pl2KingJob* job = nullptr;
+    if (pl2gpu_king_begin_mapped(ctx, n, order.data(), p0, p1, col_end, batch, &job)) return GpuFail("pl2gpu_king_begin_mapped");
+    bs.Rewind();
+    std::string err;
+    uint32_t done = 0;
+    for (;;) {
+      const int got = bs.Next(&err);
+      if (got < 0) {
+        logprintf("\nError: %s\n", err.c_str());
+        pl2gpu_king_end(job);
+        return kRetMalformedInput;
+      }
+      if (!got) break;
+      if (pl2gpu_king_add_variants(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0)) {
+        pl2gpu_king_end(job);
+        return GpuFail("pl2gpu_king_add_variants");
+      }
+      done += static_cast<uint32_t>(got);
+      printf("\r--make-king-table pass %u/%u: %u variants complete.", pass, pass_ct, done);
+      fflush(stdout);
+    }
+    if (filter) {
+      std::vector<uint32_t> fp, fc;
+      std::vector<double> fk;
+      uint64_t cap = 1ull << 22, found = 0;
+      for (;;) {
+        fp.resize(cap * 2);
+        fc.resize(cap * 5);
+        fk.resize(cap);
+        if (pl2gpu_king_get_filtered(job, p0, p1, c.king_table_filter, cap, fp.data(), fc.data(), fk.data(), &found)) {
+          pl2gpu_king_end(job);
+          return GpuFail("pl2gpu_king_get_filtered");
+        }
+        if (found <= cap) break;
+        cap = found;
+      }
+      for (uint64_t q = 0; q < found; ++q) add_row(fp[2 * q], fp[2 * q + 1], &fc[5 * q]);
+    } else {
+      const uint64_t max_pairs = (512ull << 20) / 20;
+      std::vector<uint32_t> counts;
+      for (uint32_t c0 = p0; c0 < p1;) {
+        uint32_t c1 = c0 + 1;
+        while (c1 < p1 && pairs_below(c1 + 1) - pairs_below(c0) <= max_pairs) ++c1;
+        counts.resize((pairs_below(c1) - pairs_below(c0)) * 5);
+        if (!counts.empty() && pl2gpu_king_get_counts(job, c0, c1, counts.data(), 0)) {
+          pl2gpu_king_end(job);
+          return GpuFail("pl2gpu_king_get_counts");
+        }
+        const uint32_t* cc = counts.data();
+        for (uint32_t pj = c0; pj < c1; ++pj)
+          for (uint32_t pi = 0; pi < std::min(pj, col_end); ++pi, cc += 5) add_row(pj, pi, cc);
+        c0 = c1;
+      }
+    }
+    pl2gpu_king_end(job);
+  }
+  printf("\r--make-king-table: Writing...                   ");
+  fflush(stdout);
+  std::sort(rows.begin(), rows.end(), [](const Row& a, const Row& b) { return a.r1 != b.r1 ? a.r1 < b.r1 : a.r2 < b.r2; });
+  const IdFmt idf = KingIdFmt(c, S);
+  const std::string tab_name = c.out + (c.king_table_zs ? ".kin0.zst" : ".kin0");
+  OutFile ftab;
+  if (!ftab.Open(tab_name, c.king_table_zs)) {
+    logprintf("Error: Failed to open %s for writing.\n", tab_name.c_str());
+    return kRetOpenFail;
+  }
+  ftab.Puts(KingTableHeader(c, idf).c_str());
+  {
+    std::vector<uint32_t> by_rank(n);
+    for (uint32_t k = 0; k < n; ++k) by_rank[rank[k]] = k;
+    for (const Row& row : rows) WriteKingTableRow(c, FmtId(S, by_rank[row.r1], idf), FmtId(S, by_rank[row.r2], idf), row.cc, KinshipFromCounts(row.cc), &ftab);
+  }
+  if (!ftab.Close()) return kRetWriteFail;
+  printf("\r");
+  logprintf("--make-king-table: %u variant%s processed.\n", static_cast<uint32_t>(vidx.size()), vidx.size() == 1 ? "" : "s");
+  logprintf("Results written to %s .\n", tab_name.c_str());
+  if (filter) {
+    const uint64_t kept = rows.size();
+    logprintf("--king-table-filter: %llu relationship%s reported (%llu filtered out).\n", static_cast<unsigned long long>(kept), kept == 1 ? "" : "s", static_cast<unsigned long long>(pair_ct - kept));
   }
   return 0;
 }
@@ -4210,12 +4451,12 @@ int main(int argc, char** argv) {
     for (uint32_t k = 1; k < ds.samples.size() && !rel_check_pairs; ++k) rel_check_pairs = ds.samples.fid[k] != ds.samples.fid[0];
     if (!rel_check_pairs) logprintf("Warning: --make-king-table 'rel-check' modifier has no effect since only one FID is present.\n");
   }
-  if (!c.king_table_subset.empty() || rel_check_pairs) {
+  if (!c.king_table_subset.empty() || rel_check_pairs || (!c.king_table_require.empty() && c.make_king_table)) {
     if (!c.make_king_table || c.make_king || c.king_cutoff >= 0) {
       logprintf("Error: --king-table-subset must be used with --make-king-table (and without --make-king / --king-cutoff).\n");
       return kRetInvalidCmdline;
     }
-    rc = RunKingSubset(c, &ds, ctx);
+    rc = RunKingSubset(c, &ds, ctx, rel_check_pairs);
     if (rc) return rc;
   } else if (c.make_king || c.make_king_table || c.king_cutoff >= 0) {
     rc = RunKing(c, &ds, ctx, &cutoff_removed);

@@ -197,12 +197,18 @@ king_popc_kernel(const uint32_t* __restrict__ planes, uint32_t sample_ct_padded,
 // Finalisation: raw tiles -> the reference's in-memory results for rows [out_row_start, out_row_end).
 //   counts : uint32 [pair][5] = {IBS0, HETHET, HET2HOM1, HET1HOM2, HOMHOM} (plink2_matrix_calc.cc:864-868)
 //   kinship: fp64 per pair (ComputeKinship, :1566-1573)
-// pair order: for j in rows: for i in [0, j)  (:1545-1547).
+// pair order: for j in rows: for i in [0, min(j, col_end))  (:1545-1547; col_end = sample_ct for a full triangle).
 // One CTA per (tile, 16-row sub-block): coalesced tile reads -> smem -> row-contiguous writes.
 // ---------------------------------------------------------------------------------------------
+// Pairs (j, i) with j < r and i < min(j, col_end): the strict lower triangle cut at column col_end.
+__host__ __device__ inline uint64_t KingPairsBelow(uint64_t r, uint64_t col_end) {
+  if (r <= col_end) return r ? r * (r - 1) / 2 : 0;
+  return (col_end ? col_end * (col_end - 1) / 2 : 0) + (r - col_end) * col_end;
+}
+
 template <bool kKinship, uint32_t kCols>
 __global__ void __launch_bounds__(256)
-king_finalize_kernel(const int32_t* __restrict__ raw_acc, const uint32_t* __restrict__ tile_rt, const uint32_t* __restrict__ tile_tc, uint32_t sample_ct, uint32_t out_row_start, uint32_t out_row_end, uint32_t* __restrict__ out_counts, double* __restrict__ out_kinship) {
+king_finalize_kernel(const int32_t* __restrict__ raw_acc, const uint32_t* __restrict__ tile_rt, const uint32_t* __restrict__ tile_tc, uint32_t sample_ct, uint32_t col_end, uint32_t out_row_start, uint32_t out_row_end, uint32_t* __restrict__ out_counts, double* __restrict__ out_kinship) {
   __shared__ int32_t s_acc[16][(5 * kCols) + 1];
   const uint32_t tile = blockIdx.x >> 3;
   const uint32_t sub = blockIdx.x & 7;
@@ -218,15 +224,15 @@ king_finalize_kernel(const int32_t* __restrict__ raw_acc, const uint32_t* __rest
     s_acc[r][cidx] = acc_tile[static_cast<uint64_t>(cidx) * kTileRows + r];
   }
   __syncthreads();
-  const uint64_t tri_base = static_cast<uint64_t>(out_row_start) * (out_row_start - (out_row_start ? 1 : 0)) / 2;
+  const uint64_t tri_base = KingPairsBelow(out_row_start, col_end);
   for (uint32_t rr = 0; rr < 16; ++rr) {
     const uint32_t j = row_base + rr;
     if (j < out_row_start || j >= out_row_end || j >= sample_ct) continue;
-    const uint64_t pair_row = static_cast<uint64_t>(j) * (j - 1) / 2 - tri_base;  // j >= 1 whenever any i < j exists
+    const uint64_t pair_row = KingPairsBelow(j, col_end) - tri_base;
     if (kKinship) {
       for (uint32_t cl = threadIdx.x; cl < kCols; cl += 256) {
         const uint32_t i = col_base + cl;
-        if (i >= j) continue;
+        if (i >= j || i >= col_end) continue;
         const int32_t tt = s_acc[rr][cl];
         const int32_t th = s_acc[rr][kCols + cl];
         const int32_t ht = s_acc[rr][2 * kCols + cl];
@@ -241,7 +247,7 @@ king_finalize_kernel(const int32_t* __restrict__ raw_acc, const uint32_t* __rest
       for (uint32_t idx = threadIdx.x; idx < kCols * 5; idx += 256) {
         const uint32_t cl = idx / 5, q = idx % 5;
         const uint32_t i = col_base + cl;
-        if (i >= j) continue;
+        if (i >= j || i >= col_end) continue;
         uint32_t val;
         if (q == 0) {
           val = static_cast<uint32_t>((s_acc[rr][3 * kCols + cl] - s_acc[rr][4 * kCols + cl]) >> 1);  // IBS0
@@ -261,15 +267,15 @@ king_finalize_kernel(const int32_t* __restrict__ raw_acc, const uint32_t* __rest
 }
 
 // ---------------------------------------------------------------------------------------------
-// `--king-table-filter` on the device: append only the pairs of rows [row_start, row_end) whose
-// kinship is not below `min_kinship` (NaN is kept, as the reference's `kinship < filter` test does,
+// `--king-table-filter` on the device: append only the pairs of rows [row_start, row_end) and columns
+// below col_end whose kinship is not below `min_kinship` (NaN is kept, as the reference's `kinship < filter` test does,
 // 2.0/plink2_matrix_calc.cc:2296-2300).  At 100k samples the unfiltered table is 5e9 pairs = 100 GB of
 // counts; relationship screening keeps a few thousand of them.  One CTA per tile, thread = tile row.
 // Slots are handed out with an atomic counter, so the output order is arbitrary (the host sorts).
 // ---------------------------------------------------------------------------------------------
 template <uint32_t kCols>
 __global__ void __launch_bounds__(kTileRows)
-king_filter_kernel(const int32_t* __restrict__ raw_acc, const uint32_t* __restrict__ tile_rt, const uint32_t* __restrict__ tile_tc, uint32_t sample_ct, uint32_t row_start, uint32_t row_end, double min_kinship, unsigned long long max_out,
+king_filter_kernel(const int32_t* __restrict__ raw_acc, const uint32_t* __restrict__ tile_rt, const uint32_t* __restrict__ tile_tc, uint32_t sample_ct, uint32_t col_end, uint32_t row_start, uint32_t row_end, double min_kinship, unsigned long long max_out,
                    unsigned long long* __restrict__ found, uint32_t* __restrict__ out_pairs, uint32_t* __restrict__ out_counts, double* __restrict__ out_kinship) {
   const uint32_t tile = blockIdx.x;
   const uint32_t j = tile_rt[tile] * kTileRows + threadIdx.x;
@@ -278,7 +284,7 @@ king_filter_kernel(const int32_t* __restrict__ raw_acc, const uint32_t* __restri
   const int32_t* acc = raw_acc + static_cast<uint64_t>(tile) * (5 * kCols * kTileRows) + threadIdx.x;
   for (uint32_t cl = 0; cl < kCols; ++cl) {
     const uint32_t i = col_base + cl;
-    if (i >= j) break;
+    if (i >= j || i >= col_end) break;
     const int32_t tt = acc[static_cast<uint64_t>(cl) * kTileRows];
     const int32_t th = acc[static_cast<uint64_t>(kCols + cl) * kTileRows];
     const int32_t ht = acc[static_cast<uint64_t>(2 * kCols + cl) * kTileRows];

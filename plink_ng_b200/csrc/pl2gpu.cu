@@ -13,6 +13,7 @@
 #include "king_kernels.cuh"
 #include "king_ts_kernel.cuh"
 #include "king_pairs_kernel.cuh"
+#include "ld_kernels.cuh"
 #include "wgmma_probe.cuh"
 
 namespace pl2 {
@@ -28,30 +29,31 @@ void set_error(const char* fmt, ...) {
 const char* get_error() { return g_err; }
 
 // ---- tile list over the strict lower triangle restricted to rows [row_start,row_end) ----
-static uint32_t ColTilesForRowTile(uint32_t rt, uint32_t row_end, bool include_diag, uint32_t tile_cols) {
+static uint32_t ColTilesForRowTile(uint32_t rt, uint32_t row_end, bool include_diag, uint32_t tile_cols, uint32_t col_end) {
   uint32_t tile_row_end = (rt + 1) * kTileRows;
   if (tile_row_end > row_end) tile_row_end = row_end;
-  // columns 0 .. tile_row_end-2 are needed (.. tile_row_end-1 with the diagonal)
-  const uint32_t cols = include_diag ? tile_row_end : (tile_row_end ? tile_row_end - 1 : 0);
+  // columns 0 .. tile_row_end-2 are needed (.. tile_row_end-1 with the diagonal), none at or past col_end
+  uint32_t cols = include_diag ? tile_row_end : (tile_row_end ? tile_row_end - 1 : 0);
+  if (cols > col_end) cols = col_end;
   if (!cols) return 0;
   return DivUpU32(cols, tile_cols);
 }
 
-uint64_t CountTiles(uint32_t row_start, uint32_t row_end, bool include_diag, uint32_t tile_cols) {
+uint64_t CountTiles(uint32_t row_start, uint32_t row_end, bool include_diag, uint32_t tile_cols, uint32_t col_end) {
   if (row_end <= row_start) return 0;
   uint64_t n = 0;
-  for (uint32_t rt = row_start / kTileRows; rt * kTileRows < row_end; ++rt) n += ColTilesForRowTile(rt, row_end, include_diag, tile_cols);
+  for (uint32_t rt = row_start / kTileRows; rt * kTileRows < row_end; ++rt) n += ColTilesForRowTile(rt, row_end, include_diag, tile_cols, col_end);
   return n;
 }
 
-int BuildTileList(uint32_t row_start, uint32_t row_end, bool include_diag, TileList* tl, uint32_t tile_cols) {
+int BuildTileList(uint32_t row_start, uint32_t row_end, bool include_diag, TileList* tl, uint32_t tile_cols, uint32_t col_end) {
   std::vector<uint32_t> rt_v, tc_v, off_v;
   tl->row_tile_first = row_start / kTileRows;
   uint32_t rt = tl->row_tile_first;
   // an empty row range (a rank of a multi-GPU team that owns no rows) has no tiles at all
   for (; row_end > row_start && rt * kTileRows < row_end; ++rt) {
     off_v.push_back(static_cast<uint32_t>(rt_v.size()));
-    const uint32_t nct = ColTilesForRowTile(rt, row_end, include_diag, tile_cols);
+    const uint32_t nct = ColTilesForRowTile(rt, row_end, include_diag, tile_cols, col_end);
     for (uint32_t tc = 0; tc < nct; ++tc) {
       rt_v.push_back(rt);
       tc_v.push_back(tc);
@@ -218,6 +220,9 @@ using namespace pl2;
 struct Pl2KingJob {
   Pl2GpuCtx* ctx = nullptr;
   uint32_t sample_ct = 0, row_start = 0, row_end = 0;
+  uint32_t col_end = 0;              // pairs with a column at or past this are never returned (sample_ct: none cut)
+  uint32_t* d_order = nullptr;       // mapped job: device position -> sample index; null = identity
+  uint8_t* d_unmapped = nullptr;     // mapped job: the block as the caller gave it, before the gather into position order
   int algo = kPl2KingAlgoTensor;
   TileList tiles;
   // TS path: two staged blocks + two row-side re-tiled copies, so that the copy / all-gather, padding and
@@ -442,7 +447,16 @@ int pl2gpu_king_begin(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start, ui
   return pl2gpu_king_begin_ex(ctx, sample_ct, row_start, row_end, algo, 0, job_ptr);
 }
 
-int pl2gpu_king_begin_ex(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start, uint32_t row_end, int algo, uint32_t max_variants_per_add, Pl2KingJob** job_ptr) {
+uint64_t pl2gpu_king_mapped_mem_required(uint32_t sample_ct, uint32_t row_start, uint32_t row_end, uint32_t col_end, uint32_t max_variants_per_add) {
+  // what pl2gpu_king_begin_mapped allocates: the TS accumulators of the cut tile list, two raw blocks + two sample-major
+  // copies, the unmapped block, the position map, the output staging buffer, plus slack for allocator granularity
+  const uint64_t cap = ClampStageCap(max_variants_per_add);
+  const uint64_t tiles_ts = CountTiles(row_start, row_end, false, kKingTsCols, col_end);
+  const uint64_t npad_ts = RoundUpU32(sample_ct, kTsSamplePad);
+  return tiles_ts * kKingTsTileAccWords * 4 + 5 * cap * (npad_ts / 4) + tiles_ts * 16 + 4ull * sample_ct + kKingOutStageBytes + (128ull << 20);
+}
+
+static int KingBegin(Pl2GpuCtx* ctx, uint32_t sample_ct, const uint32_t* order, uint32_t row_start, uint32_t row_end, uint32_t col_end, int algo, uint32_t max_variants_per_add, Pl2KingJob** job_ptr) {
   *job_ptr = nullptr;
   if (!ctx) {
     set_error("pl2gpu_king_begin: null context");
@@ -450,6 +464,10 @@ int pl2gpu_king_begin_ex(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start,
   }
   if (sample_ct < 2 || row_end > sample_ct || row_start > row_end) {  // row_start == row_end: a rank that only takes part in the all-gathers
     set_error("pl2gpu_king_begin: bad row range [%u,%u) for %u samples", row_start, row_end, sample_ct);
+    return 1;
+  }
+  if (!col_end || col_end > sample_ct) {
+    set_error("pl2gpu_king_begin: bad column bound %u for %u samples", col_end, sample_ct);
     return 1;
   }
   if (algo == kPl2KingAlgoAuto) algo = kPl2KingAlgoTensorTS;
@@ -463,6 +481,7 @@ int pl2gpu_king_begin_ex(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start,
   job->sample_ct = sample_ct;
   job->row_start = row_start;
   job->row_end = row_end;
+  job->col_end = col_end;
   job->algo = algo;
   auto fail = [&]() {
     pl2gpu_king_end(job);
@@ -479,9 +498,18 @@ int pl2gpu_king_begin_ex(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start,
     return fail();
   }
   job->tile_cols = ts ? kKingTsCols : kTileCols;
-  if (BuildTileList(row_start, row_end, false, &job->tiles, job->tile_cols)) return fail();
+  if (BuildTileList(row_start, row_end, false, &job->tiles, job->tile_cols, col_end)) return fail();
+  if (order && (cudaMalloc(&job->d_order, 4ull * sample_ct) != cudaSuccess || cudaMemcpy(job->d_order, order, 4ull * sample_ct, cudaMemcpyHostToDevice) != cudaSuccess)) {
+    set_error("pl2gpu_king_begin_mapped: position map upload failed: %s", cudaGetErrorString(cudaGetLastError()));
+    return fail();
+  }
   for (int b = 0; b < (ts ? 2 : 1); ++b) {
     if (StageAlloc(sample_ct, cap, &job->stage[b], ts ? kTsSamplePad : kSamplePad)) return fail();
+    if (order && b == 0 && cudaMalloc(&job->d_unmapped, static_cast<uint64_t>(job->stage[0].variant_cap) * job->stage[0].pitch) != cudaSuccess) {
+      cudaGetLastError();
+      set_error("pl2gpu_king_begin_mapped: insufficient device memory for the unmapped genotype block");
+      return fail();
+    }
     if (algo != kPl2KingAlgoPopcount) {
       const uint64_t raw_t_bytes = static_cast<uint64_t>(job->stage[b].sample_ct_padded) * (job->stage[b].variant_cap / 4);
       if (cudaMalloc(&job->d_raw_t[b], raw_t_bytes) != cudaSuccess) {
@@ -517,6 +545,25 @@ int pl2gpu_king_begin_ex(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start,
   }
   *job_ptr = job;
   return 0;
+}
+
+int pl2gpu_king_begin_ex(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start, uint32_t row_end, int algo, uint32_t max_variants_per_add, Pl2KingJob** job_ptr) {
+  return KingBegin(ctx, sample_ct, nullptr, row_start, row_end, sample_ct, algo, max_variants_per_add, job_ptr);
+}
+
+int pl2gpu_king_begin_mapped(Pl2GpuCtx* ctx, uint32_t sample_ct, const uint32_t* order, uint32_t row_start, uint32_t row_end, uint32_t col_end, uint32_t max_variants_per_add, Pl2KingJob** job_ptr) {
+  if (order) {
+    // a permutation of the samples: every index once
+    std::vector<uint8_t> seen(sample_ct, 0);
+    for (uint32_t p = 0; p < sample_ct; ++p) {
+      if (order[p] >= sample_ct || seen[order[p]]++) {
+        *job_ptr = nullptr;
+        set_error("pl2gpu_king_begin_mapped: order[] is not a permutation of the %u samples (position %u)", sample_ct, p);
+        return 1;
+      }
+    }
+  }
+  return KingBegin(ctx, sample_ct, order, row_start, row_end, col_end, kPl2KingAlgoTensorTS, max_variants_per_add, job_ptr);
 }
 
 // TS path: the staged block stage[b] holds `cur` variants (rows [0, cur)); pad it, write its sample-major copy
@@ -584,8 +631,17 @@ int pl2gpu_king_add_variants(Pl2KingJob* job, const void* genovecs, uint64_t var
         PL2_CUDA_OK(cudaEventRecord(job->ev_src_ready, c->stream));
         PL2_CUDA_OK(cudaStreamWaitEvent(prep, job->ev_src_ready, 0));
       }
-      PL2_CUDA_OK(cudaMemcpy2DAsync(st.d_raw, st.pitch, src_cur, variant_stride_bytes, DivUpU32(st.sample_ct, 4), cur, src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, prep));
+      // a mapped job lands the caller's rows in d_unmapped and gathers them into position order (the prep stream runs
+      // copy and gather in turn, so one unmapped block serves both staged buffers)
+      uint8_t* const land = job->d_order ? job->d_unmapped : st.d_raw;
+      PL2_CUDA_OK(cudaMemcpy2DAsync(land, st.pitch, src_cur, variant_stride_bytes, DivUpU32(st.sample_ct, 4), cur, src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, prep));
       PL2_CUDA_OK(cudaEventRecord(job->ev_copied, prep));
+      for (uint32_t v0 = 0; job->d_order && v0 < cur; v0 += 32768) {  // grid.y is at most 65,535 rows
+        const uint32_t rows = std::min(cur - v0, 32768u);
+        geno_gather_kernel<<<dim3(DivUpU32(st.pitch, 256), rows), 256, 0, prep>>>(land + static_cast<uint64_t>(v0) * st.pitch, st.pitch, st.d_raw + static_cast<uint64_t>(v0) * st.pitch, st.pitch, job->d_order, st.sample_ct);
+        c->launches++;
+        PL2_CUDA_OK(cudaGetLastError());
+      }
       PL2_TRY(KingTsPrepAndLaunch(job, b, cur, true));
       if (!src_is_device) PL2_CUDA_OK(cudaEventSynchronize(job->ev_copied));  // the caller may reuse its buffer; the kernels keep running
     } else {
@@ -626,6 +682,10 @@ int pl2gpu_king_add_variants_sharded(Pl2KingJob* job, const void* slice, uint64_
   PL2_CUDA_OK(cudaSetDevice(c->device));
   if (job->algo != kPl2KingAlgoTensorTS) {
     set_error("pl2gpu_king_add_variants_sharded: only the default (TS tensor) algorithm is sharded");
+    return 1;
+  }
+  if (job->d_order || job->col_end != job->sample_ct) {
+    set_error("pl2gpu_king_add_variants_sharded: a mapped job (pl2gpu_king_begin_mapped) runs on one device");
     return 1;
   }
   const uint64_t total64 = static_cast<uint64_t>(slice_variant_ct) * c->comm_world;
@@ -672,7 +732,8 @@ static int KingGet(Pl2KingJob* job, uint32_t r0, uint32_t r1, void* dst, int dst
   Ctx* c = &job->ctx->c;
   PL2_CUDA_OK(cudaSetDevice(c->device));
   const uint64_t bytes_per_pair = kinship ? 8 : 20;
-  auto tri = [](uint64_t r) { return r ? r * (r - 1) / 2 : 0ull; };
+  const uint32_t col_end = job->col_end;
+  auto tri = [col_end](uint64_t r) { return KingPairsBelow(r, col_end); };
   uint8_t* out = static_cast<uint8_t*>(dst);
   uint32_t cur0 = r0;
   while (cur0 < r1) {
@@ -703,11 +764,11 @@ static int KingGet(Pl2KingJob* job, uint32_t r0, uint32_t r1, void* dst, int dst
         const uint32_t* trt = job->tiles.d_tile_rt + tile_a;
         const uint32_t* ttc = job->tiles.d_tile_tc + tile_a;
         if (job->tile_cols == kKingTsCols) {
-          if (kinship) king_finalize_kernel<true, kKingTsCols><<<grid, 256, 0, c->stream>>>(acc0, trt, ttc, job->sample_ct, cur0, cur1, nullptr, static_cast<double*>(d_dst));
-          else king_finalize_kernel<false, kKingTsCols><<<grid, 256, 0, c->stream>>>(acc0, trt, ttc, job->sample_ct, cur0, cur1, static_cast<uint32_t*>(d_dst), nullptr);
+          if (kinship) king_finalize_kernel<true, kKingTsCols><<<grid, 256, 0, c->stream>>>(acc0, trt, ttc, job->sample_ct, col_end, cur0, cur1, nullptr, static_cast<double*>(d_dst));
+          else king_finalize_kernel<false, kKingTsCols><<<grid, 256, 0, c->stream>>>(acc0, trt, ttc, job->sample_ct, col_end, cur0, cur1, static_cast<uint32_t*>(d_dst), nullptr);
         } else {
-          if (kinship) king_finalize_kernel<true, kTileCols><<<grid, 256, 0, c->stream>>>(acc0, trt, ttc, job->sample_ct, cur0, cur1, nullptr, static_cast<double*>(d_dst));
-          else king_finalize_kernel<false, kTileCols><<<grid, 256, 0, c->stream>>>(acc0, trt, ttc, job->sample_ct, cur0, cur1, static_cast<uint32_t*>(d_dst), nullptr);
+          if (kinship) king_finalize_kernel<true, kTileCols><<<grid, 256, 0, c->stream>>>(acc0, trt, ttc, job->sample_ct, col_end, cur0, cur1, nullptr, static_cast<double*>(d_dst));
+          else king_finalize_kernel<false, kTileCols><<<grid, 256, 0, c->stream>>>(acc0, trt, ttc, job->sample_ct, col_end, cur0, cur1, static_cast<uint32_t*>(d_dst), nullptr);
         }
         c->launches++;
         PL2_CUDA_OK(cudaGetLastError());
@@ -760,9 +821,9 @@ int pl2gpu_king_get_filtered(Pl2KingJob* job, uint32_t r0, uint32_t r1, double m
     }
     if (cudaMemsetAsync(d_found, 0, 8, c->stream) != cudaSuccess) break;
     if (job->tile_cols == kKingTsCols) {
-      king_filter_kernel<kKingTsCols><<<job->tiles.tile_ct, kTileRows, 0, c->stream>>>(job->d_raw_acc, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->sample_ct, r0, r1, min_kinship, max_out, d_found, d_pairs, d_counts, d_kin);
+      king_filter_kernel<kKingTsCols><<<job->tiles.tile_ct, kTileRows, 0, c->stream>>>(job->d_raw_acc, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->sample_ct, job->col_end, r0, r1, min_kinship, max_out, d_found, d_pairs, d_counts, d_kin);
     } else {
-      king_filter_kernel<kTileCols><<<job->tiles.tile_ct, kTileRows, 0, c->stream>>>(job->d_raw_acc, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->sample_ct, r0, r1, min_kinship, max_out, d_found, d_pairs, d_counts, d_kin);
+      king_filter_kernel<kTileCols><<<job->tiles.tile_ct, kTileRows, 0, c->stream>>>(job->d_raw_acc, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->sample_ct, job->col_end, r0, r1, min_kinship, max_out, d_found, d_pairs, d_counts, d_kin);
     }
     c->launches++;
     unsigned long long found = 0;
@@ -829,6 +890,8 @@ int pl2gpu_king_end(Pl2KingJob* job) {
     StageFree(&job->stage[b]);
     cudaFree(job->d_raw_t[b]);
   }
+  cudaFree(job->d_order);
+  cudaFree(job->d_unmapped);
   cudaFree(job->d_planes);
   cudaFree(job->d_raw_acc);
   cudaFree(job->d_out_stage);

@@ -124,8 +124,14 @@ def comm_unique_id() -> bytes:
     return bytes(buf)
 
 
-def _pairs(r0: int, r1: int) -> int:
-    tri = lambda r: r * (r - 1) // 2 if r else 0  # noqa: E731
+def _pairs(r0: int, r1: int, col_end: int = None) -> int:
+    """Pairs (j, i) of rows [r0, r1) with i < j, and i < col_end when a column bound is given."""
+
+    def tri(r):
+        if col_end is None or r <= col_end:
+            return r * (r - 1) // 2 if r else 0
+        return col_end * (col_end - 1) // 2 + (r - col_end) * col_end
+
     return tri(r1) - tri(r0)
 
 
@@ -137,6 +143,7 @@ class KingJob:
         self.sample_ct = sample_ct
         self.row_start = row_start
         self.row_end = sample_ct if row_end is None else row_end
+        self.col_end = sample_ct
         self._h = C.c_void_p()
         check(lib.pl2gpu_king_begin_ex(ctx.handle, sample_ct, self.row_start, self.row_end, algo, max_variants_per_add, C.byref(self._h)), "pl2gpu_king_begin_ex")
 
@@ -162,14 +169,14 @@ class KingJob:
     def counts(self, row_start: int = None, row_end: int = None) -> np.ndarray:
         r0 = self.row_start if row_start is None else row_start
         r1 = self.row_end if row_end is None else row_end
-        out = np.empty((_pairs(r0, r1), 5), dtype=np.uint32)
+        out = np.empty((_pairs(r0, r1, self.col_end), 5), dtype=np.uint32)
         check(lib.pl2gpu_king_get_counts(self._h, r0, r1, out.ctypes.data, 0), "pl2gpu_king_get_counts")
         return out
 
     def kinship(self, row_start: int = None, row_end: int = None) -> np.ndarray:
         r0 = self.row_start if row_start is None else row_start
         r1 = self.row_end if row_end is None else row_end
-        out = np.empty(_pairs(r0, r1), dtype=np.float64)
+        out = np.empty(_pairs(r0, r1, self.col_end), dtype=np.float64)
         check(lib.pl2gpu_king_get_kinship(self._h, r0, r1, out.ctypes.data, 0), "pl2gpu_king_get_kinship")
         return out
 
@@ -205,6 +212,23 @@ class KingJob:
 
     def __exit__(self, *exc):
         self.close()
+
+
+class MappedKingJob(KingJob):
+    """pl2gpu_king_begin_mapped: KingJob over device positions, order[p] = sample index at position p (None = identity),
+    rows [row_start, row_end), columns below col_end.  add_variants takes rows in sample-index order; every result is in
+    positions ("1" = the smaller position)."""
+
+    def __init__(self, ctx: GpuContext, sample_ct: int, order=None, row_start: int = 0, row_end: int = None, col_end: int = None, max_variants_per_add: int = 0):
+        self.ctx = ctx
+        self.sample_ct = sample_ct
+        self.row_start = row_start
+        self.row_end = sample_ct if row_end is None else row_end
+        self.col_end = sample_ct if col_end is None else col_end
+        self._h = C.c_void_p()
+        self._order = None if order is None else np.ascontiguousarray(order, dtype=np.uint32)
+        optr = None if self._order is None else self._order.ctypes.data
+        check(lib.pl2gpu_king_begin_mapped(ctx.handle, sample_ct, optr, self.row_start, self.row_end, self.col_end, max_variants_per_add, C.byref(self._h)), "pl2gpu_king_begin_mapped")
 
 
 class KingPairJob:
