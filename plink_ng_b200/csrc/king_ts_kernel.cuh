@@ -254,21 +254,26 @@ king_wg_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
 //                 into fragment registers and issues   T_I x [T_J | H_J] (n128) -> TT | TH,
 //                 H_I x [T_J | H_J] (n128) -> HT | HH,   R_I x A_J + A_I x R_J (n64, one accumulator) -> IBS0:
 //                 160 int32 accumulators per thread, which fit once `setmaxnreg` moves registers from the producer
-//                 (40) to the consumers (232).
+//                 (40) to the consumers (232).  The row words of the next k256 step are loaded while this step's
+//                 group is being issued, so only LOP3s stand between a retired group and the next one.
 // The epilogue writes SS = HH - 2 IBS0 (= the int8 form's S_I x S_J with S = R - A), so the raw accumulator layout
 // {TT, TH, HT, HH, SS} is that of king_wg_kernel.  Hand-off as in king_wg_kernel: `full` (64 producer arrivals
 // after the fence), `empty` (256 consumer arrivals once `wgmma.wait_group 1` has retired the stage), one wgmma group
 // in flight across stage boundaries.  A stage holds kKb1Ks k256 steps; the last one may be short (the block is padded
 // to 256 variants only): its missing steps are neither copied nor split, and run on zero planes.
+// The sample-major copy keeps each sample's 256 variants of a k256 step as one 64-byte piece, 16-byte chunk c = k32
+// words c and c + 4 (geno_tile.cuh), so the row words of a k256 step are one contiguous 8 KB and the 64 column
+// samples one contiguous 4 KB (half of a 128-sample block).
 constexpr uint32_t kKb1Ks = 2;       // k256 steps per stage
 constexpr uint32_t kKb1Stages = 5;
 constexpr uint32_t kKb1Sbo = 2 * kKb1Ks * kKwChunkBytes;                 // next group of 8 samples
 constexpr uint32_t kKb1PlaneBytes = (kKingTsCols / 8) * kKb1Sbo;         // one plane of the 64 column samples
 constexpr uint32_t kKb1BBytes = 4 * kKb1PlaneBytes;                      // T | H | R | A
-constexpr uint32_t kKb1AStepBytes = 8 * kTileRows * 8;                   // row words of one k256 step
-constexpr uint32_t kKb1WStepBytes = 8 * kKingTsCols * 8;                 // column words of one k256 step
-constexpr uint32_t kKb1ABytes = kKb1Ks * kKb1AStepBytes;                 // [k32 step][128 rows][8 B]
-constexpr uint32_t kKb1WBytes = kKb1Ks * kKb1WStepBytes;                 // [k32 step][64 samples][8 B]
+constexpr uint32_t kKb1SampleBytes = 64;                                 // one sample's words of one k256 step
+constexpr uint32_t kKb1AStepBytes = kTileRows * kKb1SampleBytes;         // row words of one k256 step
+constexpr uint32_t kKb1WStepBytes = kKingTsCols * kKb1SampleBytes;       // column words of one k256 step
+constexpr uint32_t kKb1ABytes = kKb1Ks * kKb1AStepBytes;                 // [k256 step][128 rows][64 B]
+constexpr uint32_t kKb1WBytes = kKb1Ks * kKb1WStepBytes;                 // [k256 step][64 samples][64 B]
 constexpr uint32_t kKb1StageBytes = kKb1BBytes + kKb1ABytes + kKb1WBytes;
 constexpr uint32_t kKb1SmemBytes = kKb1Stages * kKb1StageBytes + 128 + 3 * kKb1Stages * 8;  // + alignment + mbarriers
 constexpr uint32_t kKb1SplitThreads = kKingTsCols;  // producer warps 2, 3: one column sample each
@@ -276,7 +281,8 @@ static_assert(kKwProducerThreads == 2 * kKingTsCols, "producer warps: copier, id
 static_assert(kKb1SmemBytes <= kKwSmemLimit, "exceeds the 227 KB shared-memory opt-in limit");
 
 // raw_t: sample-major copy of the whole padded block (sample 0 at row tile 0) in the split form of
-// geno_tile_rows_kernel<true>: each 8-byte word is {lo32, hi32} of 32 variants; grid: one CTA per tile.
+// geno_tile_rows_kernel<true>: [sample / 128][k256 step][sample % 128][64 B], each 8-byte word {lo32, hi32} of 32
+// variants; grid: one CTA per tile.
 __global__ void __launch_bounds__(kKwThreads, 1)
 king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* multiple of 256 */, const uint32_t* __restrict__ tile_order, const uint32_t* __restrict__ tile_rt, const uint32_t* __restrict__ tile_tc, int32_t* __restrict__ raw_acc) {
   extern __shared__ __align__(128) uint8_t smem[];
@@ -285,7 +291,6 @@ king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
   const uint32_t tile = tile_order[blockIdx.x];
   const uint32_t rt = tile_rt[tile];
   const uint32_t ct = tile_tc[tile];
-  const uint32_t kstep_ct = variant_ct_padded / 32;
   const uint32_t k256_ct = variant_ct_padded / 256;
   const uint32_t stage_ct = (k256_ct + kKb1Ks - 1) / kKb1Ks;
   const uint32_t smem_base = (static_cast<uint32_t>(__cvta_generic_to_shared(smem)) + 127u) & ~127u;
@@ -307,14 +312,14 @@ king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
     // ---- producer
     const uint32_t pw = tid >> 5;
     if (pw == 0) {
-      // copier warp: the row words (one contiguous piece, [k32 step][128 rows][8 B]) and the column words of this
-      // tile (512 B per k32 step) of a stage, one bulk copy per lane onto the slot's `load` mbarrier.  It refills a
-      // slot as soon as the consumers have handed it back, so every slot but the one being read has its copies in
+      // copier warp: the row words of a stage (one contiguous piece, [k256 step][128 rows][64 B]) and the column
+      // words of this tile (4 KB per k256 step), one bulk copy per lane onto the slot's `load` mbarrier.  It refills
+      // a slot as soon as the consumers have handed it back, so every slot but the one being read has its copies in
       // flight.  These threads never split planes: the proxy fence after the split waits for every memory access
       // of the thread still in flight, bulk copies included, which would hold the split up by a whole copy latency.
-      const uint8_t* a_src = raw_t + static_cast<uint64_t>(rt) * kstep_ct * 1024;
+      const uint8_t* a_src = raw_t + static_cast<uint64_t>(rt) * k256_ct * kKb1AStepBytes;
       // column samples 64 ct .. 64 ct + 63: half (ct & 1) of 128-sample block ct >> 1
-      const uint8_t* w_src = raw_t + static_cast<uint64_t>(ct >> 1) * kstep_ct * 1024 + (ct & 1) * 512;
+      const uint8_t* w_src = raw_t + static_cast<uint64_t>(ct >> 1) * k256_ct * kKb1AStepBytes + (ct & 1) * kKb1WStepBytes;
       const uint32_t lane = tid & 31;
       for (uint32_t st = 0; st < stage_ct; ++st) {
         const uint32_t slot = st % kKb1Stages;
@@ -323,16 +328,22 @@ king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
         const uint32_t base = smem_base + slot * kKb1StageBytes;
         const uint32_t bar = bar_load + 8 * slot;
         const uint32_t steps = min(kKb1Ks, k256_ct - st * kKb1Ks);
-        const uint64_t off = static_cast<uint64_t>(st) * kKb1Ks * 8 * 1024;
+        const uint64_t off = static_cast<uint64_t>(st) * kKb1Ks * kKb1AStepBytes;
         if (lane == 0) mbar_arrive_expect_tx(bar, steps * (kKb1AStepBytes + kKb1WStepBytes));
-        if (lane < 8 * steps) bulk_copy_g2s(base + kKb1BBytes + kKb1ABytes + lane * 512, w_src + off + lane * 1024, 512, bar);
+        if (lane < steps) bulk_copy_g2s(base + kKb1BBytes + kKb1ABytes + lane * kKb1WStepBytes, w_src + off + lane * kKb1AStepBytes, kKb1WStepBytes, bar);
         if (lane == 31) bulk_copy_g2s(base + kKb1BBytes, a_src + off, steps * kKb1AStepBytes, bar);
         __syncwarp();
       }
     } else if (pw >= 2) {
       // split warps 2, 3: column sample n = tid % 64; for each k256 step j and half h, k32 steps 8 j + 4 h ..
-      // 8 j + 4 h + 3, i.e. the 16-byte half h of row n of each plane's core matrices for step j
+      // 8 j + 4 h + 3, i.e. the 16-byte half h of row n of each plane's core matrices for step j.
+      // Sample n's 64 bytes of step j sit at n * 64, chunk m (k32 words m, m + 4) at + 16 m: banks 16 (n & 1) + 4 m
+      // .. + 3.  An LDS.128 serves 8 threads per wavefront; if the 8 threads n = 8 a .. 8 a + 7 all read the same
+      // chunk m, the four even (and the four odd) ones land on the same four banks: 4 wavefronts instead of 1.  So
+      // load i reads chunk (i + (n >> 1)) & 3: the four even threads then take four different chunks, the 8 threads
+      // cover the 32 banks once, and the chunks are rotated back into order in registers.
       const uint32_t n = tid & (kKingTsCols - 1);
+      const uint32_t rot = (n >> 1) & 3;
       for (uint32_t st = 0; st < stage_ct; ++st) {
         const uint32_t slot = st % kKb1Stages, phase = (st / kKb1Stages) & 1;
         const uint32_t base = smem_base + slot * kKb1StageBytes;
@@ -342,14 +353,33 @@ king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
         mbar_wait(bar_load + 8 * slot, phase);
 #pragma unroll
         for (uint32_t j = 0; j < kKb1Ks; ++j) {
+          uint32_t w[4][4];  // w[m] = chunk m = {lo, hi of k32 word m, lo, hi of word m + 4}
+#pragma unroll
+          for (uint32_t m = 0; m < 4; ++m) w[m][0] = w[m][1] = w[m][2] = w[m][3] = ~0u;  // missing step: code 3, zero planes
+          if (j < steps) {
+#pragma unroll
+            for (uint32_t i = 0; i < 4; ++i)
+              asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(w[i][0]), "=r"(w[i][1]), "=r"(w[i][2]), "=r"(w[i][3]) : "r"(base + kKb1BBytes + kKb1ABytes + j * kKb1WStepBytes + n * kKb1SampleBytes + 16 * ((i + rot) & 3)) : "memory");
+          }
+          // w[i] holds chunk (i + rot) & 3: rotate by rot & 1, then by rot & 2
+#pragma unroll
+          for (uint32_t r = 1; r <= 2; r <<= 1) {
+            const bool on = rot & r;
+            uint32_t t[4][4];
+#pragma unroll
+            for (uint32_t m = 0; m < 4; ++m)
+#pragma unroll
+              for (uint32_t e = 0; e < 4; ++e) t[m][e] = on ? w[(m - r) & 3][e] : w[m][e];
+#pragma unroll
+            for (uint32_t m = 0; m < 4; ++m)
+#pragma unroll
+              for (uint32_t e = 0; e < 4; ++e) w[m][e] = t[m][e];
+          }
 #pragma unroll
           for (uint32_t h = 0; h < 2; ++h) {
-            uint32_t lo[4] = {~0u, ~0u, ~0u, ~0u}, hi[4] = {~0u, ~0u, ~0u, ~0u};  // missing step: code 3, zero planes
-            if (j < steps) {
+            uint32_t lo[4], hi[4];  // k32 words 4 h + q
 #pragma unroll
-              for (uint32_t q = 0; q < 4; ++q)
-                asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(lo[q]), "=r"(hi[q]) : "r"(base + kKb1BBytes + kKb1ABytes + (8 * j + 4 * h + q) * 512 + n * 8) : "memory");
-            }
+            for (uint32_t q = 0; q < 4; ++q) lo[q] = w[q][2 * h], hi[q] = w[q][2 * h + 1];
             const uint32_t addr = base + (n >> 3) * kKb1Sbo + (2 * j + h) * kKwChunkBytes + (n & 7) * 16;
             asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(lo[0] & ~hi[0]), "r"(lo[1] & ~hi[1]), "r"(lo[2] & ~hi[2]), "r"(lo[3] & ~hi[3]) : "memory");
             asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + kKb1PlaneBytes), "r"(~lo[0]), "r"(~lo[1]), "r"(~lo[2]), "r"(~lo[3]) : "memory");
@@ -377,23 +407,31 @@ king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
   for (uint32_t i = 0; i < kKingTsCols / 2; ++i) acc_i[i] = 0;
   const uint32_t r_lo = 64 * cw + 16 * warp4 + g;  // this thread's fragment rows r_lo, r_lo + 8 of the tile
 
+  // Fragment register q: row r_lo + 8 (q & 1), K bits 32 (c + 4 (q >> 1)) .. of the step = k32 step c + 4 (q >> 1).
+  // Chunk c of a row's 64 bytes holds exactly k32 words c and c + 4, so a thread's words of a k256 step are two
+  // LDS.128, one per row; a warp's 8 rows x 64 B are 512 contiguous bytes, 4 wavefronts without a conflict.
+  // w[0] = {lo, hi of k32 word c, lo, hi of word c + 4} of row r_lo, w[1] the same of row r_lo + 8.
+  uint4 w[2];
+  auto load_words = [&](uint32_t base, uint32_t j) {
+    const uint32_t a = base + kKb1BBytes + j * kKb1AStepBytes + r_lo * kKb1SampleBytes + 16 * c;
+    asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(w[0].x), "=r"(w[0].y), "=r"(w[0].z), "=r"(w[0].w) : "r"(a) : "memory");
+    asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(w[1].x), "=r"(w[1].y), "=r"(w[1].z), "=r"(w[1].w) : "r"(a + 8 * kKb1SampleBytes) : "memory");
+  };
+  // The words of step j + 1 are loaded right after step j's group is issued and before the wait that retires step
+  // j - 1's group; the first step of the next stage only after that stage's `full` wait.  Every word load from a
+  // slot has been consumed by the LOP3s of its step before the slot is handed back.
   uint32_t slot = 0, phase = 0, prev_slot = 0;
+  mbar_wait(bar_full, 0);
+  load_words(smem_base, 0);
   for (uint32_t st = 0; st < stage_ct; ++st) {
-    mbar_wait(bar_full + 8 * slot, phase);
     const uint32_t base = smem_base + slot * kKb1StageBytes;
     const uint32_t steps = min(kKb1Ks, k256_ct - st * kKb1Ks);
+    const uint32_t next_slot = slot + 1 == kKb1Stages ? 0 : slot + 1;
+    const uint32_t next_phase = slot + 1 == kKb1Stages ? phase ^ 1 : phase;
     const uint64_t desc = make_wg_desc(base, kKwChunkBytes, kKb1Sbo);
 #pragma unroll
     for (uint32_t j = 0; j < kKb1Ks; ++j) {
-      // fragment register q: row r_lo + 8 (q & 1), K bits 32 (c + 4 (q >> 1)) .. of the step = k32 step c + 4 (q >> 1)
-      uint32_t lo[4] = {~0u, ~0u, ~0u, ~0u}, hi[4] = {~0u, ~0u, ~0u, ~0u};  // missing step: code 3, zero planes
-      if (j < steps) {
-#pragma unroll
-        for (uint32_t q = 0; q < 4; ++q) {
-          const uint32_t a = base + kKb1BBytes + (8 * j + c + 4 * (q >> 1)) * (kTileRows * 8) + (r_lo + 8 * (q & 1)) * 8;
-          asm volatile("ld.shared.v2.b32 {%0,%1}, [%2];" : "=r"(lo[q]), "=r"(hi[q]) : "r"(a) : "memory");
-        }
-      }
+      const uint32_t lo[4] = {w[0].x, w[1].x, w[0].z, w[1].z}, hi[4] = {w[0].y, w[1].y, w[0].w, w[1].w};
       uint32_t ft[4], fh[4], fr[4], fa[4];
 #pragma unroll
       for (uint32_t q = 0; q < 4; ++q) {
@@ -409,12 +447,22 @@ king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
       wgmma_b1_rs<kKingTsCols>(acc_i, fr, dk + ((3 * kKb1PlaneBytes) >> 4));     // R_I x A_J
       wgmma_b1_rs<kKingTsCols>(acc_i, fa, dk + ((2 * kKb1PlaneBytes) >> 4));     // + A_I x R_J
       wgmma_commit();
+      if (j + 1 < kKb1Ks) {
+        if (j + 1 < steps) {
+          load_words(base, j + 1);
+        } else {
+          w[0] = w[1] = make_uint4(~0u, ~0u, ~0u, ~0u);  // missing step: code 3, zero planes
+        }
+      } else if (st + 1 < stage_ct) {
+        mbar_wait(bar_full + 8 * next_slot, next_phase);
+        load_words(smem_base + next_slot * kKb1StageBytes, 0);
+      }
       wgmma_wait<1>();
       // every group but the one just issued has retired, the previous stage's last one included: hand that slot back
       if (j == 0 && st > 0) mbar_arrive(bar_empty + 8 * prev_slot);
     }
     prev_slot = slot;
-    if (++slot == kKb1Stages) slot = 0, phase ^= 1;
+    slot = next_slot, phase = next_phase;
   }
   wgmma_wait<0>();
   wgmma_fence_operand(acc_t);

@@ -584,7 +584,7 @@ static int KingTsPrepAndLaunch(Pl2KingJob* job, uint32_t b, uint32_t cur, bool p
     job->kernel_pending[b] = true;
     return 0;
   }
-  geno_tile_rows_kernel<true><<<dim3(padded / 64, st.sample_ct_padded / 64), 256, 0, prep>>>(st.d_raw, st.pitch, padded / 32, 0, job->d_raw_t[b]);
+  geno_tile_rows_kernel<true><<<dim3(padded / 256, st.sample_ct_padded / 64), 256, 0, prep>>>(st.d_raw, st.pitch, padded / 32, 0, job->d_raw_t[b]);
   c->launches++;
   PL2_CUDA_OK(cudaGetLastError());
   PL2_CUDA_OK(cudaEventRecord(job->ev_prep_done[b], prep));
