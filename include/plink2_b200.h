@@ -273,9 +273,16 @@ int pl2_ld_prune_walk(uint32_t variant_ct, const uint32_t* chr_codes, const uint
  * bits each (bits 0-1, 2-3, 4-5): 0x24 when the ALT allele is named, 0x06 when REF is ('dominant': 0x14 / 0x05,
  * 'recessive': 0x10 / 0x01).  pl2gpu_score_get returns per sample the weighted sum, the named-allele dosage
  * sum over nonmissing calls (NAMED_ALLELE_DOSAGE_SUM) and the number of missing calls (ALLELE_CT = 2 x (entries -
- * missing), :8581).  Partial sums are combined in a fixed order: results are bit-reproducible. ---- */
+ * missing), :8581).  Partial sums are combined in a fixed order: results are bit-reproducible.
+ * A job begun with pl2gpu_score_begin scores one coefficient column.  One begun with pl2gpu_score_begin_cols scores
+ * score_ct >= 1 columns (--score-col-nums) in one pass over the genotypes: pl2gpu_score_add_variants then takes
+ * weights4 as [entry][score_ct][4] and pl2gpu_score_get returns score_sums row-major [sample][score_ct]; the dosage
+ * sums and missing counts do not depend on the column and keep their form.  Column j of such a job is bit-identical
+ * to a one-column job fed only column j (same adds in the same order), unless the weights of a full staging batch
+ * (16,384 entries x score_ct x 32 bytes) did not fit in device memory and batches were shortened. ---- */
 typedef struct Pl2ScoreJob Pl2ScoreJob;
 int pl2gpu_score_begin(Pl2GpuCtx* ctx, uint32_t sample_ct, Pl2ScoreJob** job_ptr);
+int pl2gpu_score_begin_cols(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t score_ct, Pl2ScoreJob** job_ptr);
 int pl2gpu_score_add_variants(Pl2ScoreJob* job, const void* genovecs, uint64_t variant_stride_bytes, uint32_t variant_ct, int src_is_device, const double* weights4, const uint8_t* named_dosages);
 int pl2gpu_score_get(Pl2ScoreJob* job, double* score_sums, uint64_t* named_dosage_sums, uint32_t* missing_cts);
 /* Idempotent; accepts NULL. */

@@ -80,6 +80,7 @@ SIGNATURES = {
     "pl2_indep_pairwise": (C.c_int, [vp, vp, C.c_uint64, C.c_uint32, C.c_uint32, vp, vp, C.c_uint32, C.c_uint32, C.c_double, C.c_int, vp, vp, C.c_int, vp]),
     "pl2_indep_pairwise_ex": (C.c_int, [vp, vp, C.c_uint64, C.c_uint32, C.c_uint32, vp, vp, C.c_uint32, C.c_uint32, C.c_double, C.c_int, vp, vp, C.c_int, vp, C.c_uint32, vp]),
     "pl2gpu_score_begin": (C.c_int, [vp, C.c_uint32, vp]),
+    "pl2gpu_score_begin_cols": (C.c_int, [vp, C.c_uint32, C.c_uint32, vp]),
     "pl2gpu_score_add_variants": (C.c_int, [vp, vp, C.c_uint64, C.c_uint32, C.c_int, vp, vp]),
     "pl2gpu_score_get": (C.c_int, [vp, vp, vp, vp]),
     "pl2gpu_score_end": (C.c_int, [vp]),

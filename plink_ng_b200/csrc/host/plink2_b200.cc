@@ -94,7 +94,9 @@ struct Cmd {
   std::string read_freq;                  // --read-freq <PLINK 2 --freq report>
   // --score <file> [i] [j] [k] [header | header-read] [no-mean-imputation] [zs] [cols=]
   std::string score_file;
-  uint32_t score_id_col = 1, score_allele_col = 2, score_coef_col = 3;
+  uint32_t score_id_col = 1, score_allele_col = 2, score_coef_col = 3, score_numeric_params = 0;
+  std::vector<uint32_t> score_col_nums;   // --score-col-nums: 1-based coefficient columns, increasing, no duplicates
+  std::vector<uint32_t> vscore_col_nums;  // --vscore-col-nums: 1-based weight columns, increasing, no duplicates
   bool score_header = false, score_header_read = false, score_no_meanimpute = false, score_zs = false, score_center = false, score_varstd = false, score_dominant = false, score_recessive = false, score_list_variants = false;
   bool sc_fid_maybe = true, sc_fid = false, sc_sid_maybe = true, sc_sid = false, sc_pheno1 = false, sc_phenos = true, sc_nallele = true, sc_denom = false, sc_dosagesum = true, sc_avgs = true, sc_sums = false;
   std::string vscore_file;                // --variant-score <file> ['zs'] ['cols=' chrom,pos,ref,alt,maybeprovref,provref,altfreq]
@@ -150,6 +152,68 @@ bool ParseDouble(const char* s, double* out) {
 int Usage(const char* msg) {
   logprintf("Error: %s\n", msg);
   return kRetInvalidCmdline;
+}
+
+// --score-col-nums / --vscore-col-nums (ParseNameRanges with positive integers, 2.0/plink2_cmdline.cc:2185-2330):
+// comma-separated column numbers and a-b ranges (b > a) over one or more parameters.  The columns come back in
+// increasing order, each once, whatever order they were given in and however the ranges overlap.
+int ParseColNums(const std::string& flag, char** prm, int nparam, std::vector<uint32_t>* out) {
+  std::vector<std::pair<std::string, std::string>> items;  // (start, end or "" for a single column)
+  for (int k = 0; k < nparam; ++k) {
+    const std::string a = prm[k];
+    size_t pos = 0;
+    while (pos < a.size()) {
+      if (a[pos] == ',') {
+        ++pos;
+        continue;
+      }
+      size_t e = a.find(',', pos);
+      if (e == std::string::npos) e = a.size();
+      const std::string tok = a.substr(pos, e - pos);
+      pos = e;
+      const size_t dash = tok.find('-');
+      if (dash == std::string::npos) {
+        items.emplace_back(tok, "");
+        continue;
+      }
+      if (dash == 0 || dash + 1 == tok.size() || tok.find('-', dash + 1) != std::string::npos) return Usage(("Invalid " + flag + " argument '" + a + "'.").c_str());
+      items.emplace_back(tok.substr(0, dash), tok.substr(dash + 1));
+    }
+  }
+  if (items.empty()) return Usage((flag + " requires at least one value.").c_str());
+  // the same token twice is an error, before any is read as a number; overlapping ranges are not
+  std::vector<std::string> seen;
+  for (const auto& it : items) {
+    for (const std::string* t : {&it.first, &it.second}) {
+      if (t->empty()) continue;
+      if (std::find(seen.begin(), seen.end(), *t) != seen.end()) return Usage(("Duplicate " + flag + " argument '" + *t + "'.").c_str());
+      seen.push_back(*t);
+    }
+  }
+  auto posint = [&](const std::string& t, uint32_t* v) {
+    if (t.empty() || t.find_first_not_of("0123456789") != std::string::npos || t.size() > 10) return false;
+    const uint64_t x = std::stoull(t);
+    if (!x || x > 0x7ffffffe) return false;
+    *v = static_cast<uint32_t>(x);
+    return true;
+  };
+  std::vector<uint32_t> cols;
+  for (const auto& it : items) {
+    uint32_t a, b;
+    if (!posint(it.first, &a)) return Usage(("Invalid " + flag + " argument '" + it.first + "'.").c_str());
+    if (it.second.empty()) {
+      cols.push_back(a);
+      continue;
+    }
+    if (!posint(it.second, &b)) return Usage(("Invalid " + flag + " argument '" + it.second + "'.").c_str());
+    if (b <= a) return Usage(("Invalid " + flag + " range '" + it.first + "-" + it.second + "'.").c_str());
+    if (b - a > (1u << 24)) return Usage((flag + " range '" + it.first + "-" + it.second + "' names more columns than a line can hold.").c_str());
+    for (uint32_t v = a; v <= b; ++v) cols.push_back(v);
+  }
+  std::sort(cols.begin(), cols.end());
+  cols.erase(std::unique(cols.begin(), cols.end()), cols.end());
+  *out = std::move(cols);
+  return 0;
 }
 
 // --make-king-table cols= (default maybefid,id,maybesid,nsnp,hethet,ibs0,kinship; plink2_matrix_calc.h:60)
@@ -363,7 +427,7 @@ int ParseArgs(int argc, char** argv, Cmd* c) {
       if (nnum >= 1) c->score_id_col = nums[0];
       c->score_allele_col = nnum >= 2 ? nums[1] : c->score_id_col + 1;
       c->score_coef_col = nnum >= 3 ? nums[2] : c->score_allele_col + 1;
-      if (c->score_id_col == c->score_allele_col || c->score_id_col == c->score_coef_col || c->score_allele_col == c->score_coef_col) return Usage("--score variant ID, allele and coefficient column numbers must be distinct.");
+      c->score_numeric_params = nnum;
       for (; k < nparam; ++k) {
         const std::string m = prm[k];
         if (m == "header") c->score_header = true;
@@ -414,6 +478,9 @@ int ParseArgs(int argc, char** argv, Cmd* c) {
       }
       if (c->score_header && c->score_header_read) return Usage("--score 'header' and 'header-read' modifiers cannot be used together.");
       if ((c->score_dominant || c->score_recessive) && (c->score_center || (c->score_dominant && c->score_recessive))) return Usage("--score 'dominant' / 'recessive' cannot be combined with each other or with 'center' / 'variance-standardize'.");
+    } else if (flag == "--score-col-nums" || flag == "--vscore-col-nums") {
+      const bool vs = flag == "--vscore-col-nums";
+      if (int rc = ParseColNums(flag, prm, nparam, vs ? &c->vscore_col_nums : &c->score_col_nums)) return rc;
     } else if (flag == "--variant-score" || flag == "--vscore") {
       if (nparam < 1) return Usage("--variant-score requires a filename.");
       c->vscore_file = prm[0];
@@ -673,6 +740,17 @@ int ParseArgs(int argc, char** argv, Cmd* c) {
   }
   if (c->pgen.empty() || c->pvar.empty() || c->psam.empty()) return Usage("No input dataset (--bfile / --pfile / --bed+--bim+--fam / --pgen+--pvar+--psam).");
   if (!c->indep_preferred.empty() && !c->indep_pairwise) return Usage("--indep-preferred must be used with --indep-pairwise.");
+  // --score / --score-col-nums / --vscore-col-nums, in the reference's order (plink2.cc:11573-11582, :12566-12574,
+  // :12955; column overlaps 2.0/plink2_matrix_calc.cc:7186-7234)
+  if (!c->vscore_col_nums.empty() && c->vscore_file.empty()) return Usage("--vscore-col-nums must be used with --variant-score.");
+  if (!c->score_col_nums.empty()) {
+    if (c->score_file.empty()) return Usage("--score-col-nums must be used with --score[-list].");
+    if (c->score_numeric_params == 3) return Usage("--score-col-nums cannot be used when three numeric arguments are\nprovided to --score.");
+    if (std::binary_search(c->score_col_nums.begin(), c->score_col_nums.end(), c->score_id_col)) return Usage("--score variant ID column index matches a coefficient column index.");
+    if (std::binary_search(c->score_col_nums.begin(), c->score_col_nums.end(), c->score_allele_col)) return Usage("--score allele column index matches a coefficient column index.");
+  } else if (!c->score_file.empty() && (c->score_id_col == c->score_allele_col || c->score_id_col == c->score_coef_col || c->score_allele_col == c->score_coef_col)) {
+    return Usage("--score variant ID, allele and coefficient column numbers must be distinct.");
+  }
   if (c->king_table_require_flags) {
     // the reference's checks (plink2.cc:7732-7750, :8467, :8571), in the order it meets them
     if (c->king_cutoff >= 0 || !c->king_cutoff_prefix.empty()) return Usage("--king-table-require[-xor] cannot be used with --king-cutoff.");
@@ -2889,8 +2967,9 @@ bool TypePheno(const std::string& name, const std::vector<std::string>& tok, Phe
 }
 
 // `--score` (ScoreReport, 2.0/plink2_matrix_calc.cc:6892-9270) for diploid hard calls: default report columns plus
-// denom / scoresums, 'header' / 'header-read', 'no-mean-imputation'.  The per-sample sums come from the device
-// (pl2gpu_score_*); the file parsing, allele matching, mean-imputation weights and the report are here.
+// denom / scoresums, 'header' / 'header-read', 'no-mean-imputation', and any number of coefficient columns
+// (--score-col-nums).  The per-sample sums of every column come from one device pass (pl2gpu_score_*); the file
+// parsing, allele matching, mean-imputation weights and the report are here.
 int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   const SampleInfo& S = ds->samples;
   const VariantInfo& V = ds->variants;
@@ -2909,13 +2988,19 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   struct Entry {
     uint32_t v;
     uint8_t aidx;  // 0 = REF named, 1 = ALT named
-    double coef;
+    size_t coef_row;  // coefficients at coefs[coef_row * score_ct ...]
   };
   std::vector<Entry> entries;
+  std::vector<double> coefs;
   std::vector<uint8_t> seen(2ull * V.size(), 0);
   uint64_t missing_id = 0, missing_allele = 0;
-  const uint32_t need_cols = std::max(c.score_id_col, std::max(c.score_allele_col, c.score_coef_col));
-  std::string score_name = "SCORE1";
+  // coefficient columns in file order (1-based); without --score-col-nums the one column --score names
+  const std::vector<uint32_t> score_cols = c.score_col_nums.empty() ? std::vector<uint32_t>{c.score_coef_col} : c.score_col_nums;
+  const uint32_t score_ct = static_cast<uint32_t>(score_cols.size());
+  const uint32_t need_cols = std::max({c.score_id_col, c.score_allele_col, score_cols.back()});
+  // names: the header tokens with 'header-read', else SCORE1 .. by position in the column list (:7620-7672)
+  std::vector<std::string> score_names(score_ct);
+  for (uint32_t j = 0; j < score_ct; ++j) score_names[j] = "SCORE" + std::to_string(j + 1);
   size_t li = 0;
   if ((c.score_header || c.score_header_read) && !lines.empty()) {
     if (c.score_header_read) {
@@ -2924,7 +3009,13 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
         logprintf("Error: Line 1 of --score file has fewer tokens than expected.\n");
         return kRetMalformedInput;
       }
-      score_name = h[c.score_coef_col - 1];
+      for (uint32_t j = 0; j < score_ct; ++j) score_names[j] = h[score_cols[j] - 1];
+      std::vector<std::string> sorted_names(score_names);
+      std::sort(sorted_names.begin(), sorted_names.end());
+      if (std::adjacent_find(sorted_names.begin(), sorted_names.end()) != sorted_names.end()) {
+        logprintf("Error: --score: Score IDs are not unique.\n");
+        return kRetMalformedInput;
+      }
     }
     li = 1;
   }
@@ -2932,7 +3023,8 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
     if (lines[li].empty()) continue;
     const std::vector<std::string> t = SplitWs(lines[li]);
     if (t.empty()) continue;
-    if (t.size() < need_cols) {
+    // the ID and allele tokens are needed first; the coefficients only on lines that are scored (:7712-7790)
+    if (t.size() < std::max(c.score_id_col, c.score_allele_col)) {
       logprintf("Error: Line %zu of --score file has fewer tokens than expected.\n", li + 1);
       return kRetMalformedInput;
     }
@@ -2960,16 +3052,23 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
       return kRetMalformedInput;
     }
     seen[2ull * v + aidx] = 1;
-    double coef;
-    if (!ParseDouble(t[c.score_coef_col - 1].c_str(), &coef)) {
-      logprintf("Error: Line %zu of --score file has an invalid coefficient.\n", li + 1);
+    if (t.size() < need_cols) {
+      logprintf("Error: Line %zu of --score file has fewer tokens than expected.\n", li + 1);
       return kRetMalformedInput;
+    }
+    for (const uint32_t col : score_cols) {
+      double coef;
+      if (!ParseDouble(t[col - 1].c_str(), &coef)) {
+        logprintf("Error: Line %zu of --score file has an invalid coefficient.\n", li + 1);
+        return kRetMalformedInput;
+      }
+      coefs.push_back(coef);
     }
     if (V.chr_code[v] == 23 || V.chr_code[v] == 24 || V.chr_code[v] == 26) {
       logprintf("Error: --score on chrX / chrY / chrMT variants (sex-dependent ploidy) is not supported by plink2_b200 yet ('%s').\n", id.c_str());
       return kRetNotYetSupported;
     }
-    entries.push_back({v, aidx, coef});
+    entries.push_back({v, aidx, entries.size()});
   }
   if (missing_id || missing_allele) {
     logprintf("Warning: --score: %llu entr%s in %s %s skipped due to missing variant IDs, and %llu %s skipped due to mismatching allele codes.\n", static_cast<unsigned long long>(missing_id), missing_id == 1 ? "y" : "ies",
@@ -3003,7 +3102,11 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
     ApplyReadFreq(*ds, vidx, &ref_freqs, have);
   }
   Pl2ScoreJob* job = nullptr;
-  if (pl2gpu_score_begin(ctx, n, &job)) return GpuFail("pl2gpu_score_begin");
+  if (score_ct == 1) {  // the one-column job (same device work as pl2gpu_score_begin_cols with one column)
+    if (pl2gpu_score_begin(ctx, n, &job)) return GpuFail("pl2gpu_score_begin");
+  } else if (pl2gpu_score_begin_cols(ctx, n, score_ct, &job)) {
+    return GpuFail("pl2gpu_score_begin_cols");
+  }
   struct JobGuard {
     Pl2ScoreJob* j;
     ~JobGuard() { pl2gpu_score_end(j); }
@@ -3012,6 +3115,7 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   if (!bs.Init()) return GpuFail("pl2gpu_host_alloc");
   std::vector<double> w4;
   std::vector<uint8_t> d4;
+  std::vector<int64_t> repeat_miss(n, 0);
   size_t base = 0;
   for (;;) {
     const int got = bs.Next(&err);
@@ -3020,12 +3124,13 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
       return kRetMalformedInput;
     }
     if (!got) break;
-    w4.resize(4ull * got);
+    w4.resize(4ull * score_ct * got);
     d4.resize(got);
     for (int k = 0; k < got; ++k) {
       const Entry& e = entries[base + k];
       const double f_named = e.aidx ? (1.0 - ref_freqs[base + k]) : ref_freqs[base + k];
-      // genotype code = ALT allele count; named-allele dosage of codes 0, 1, 2.  'center' / 'variance-standardize'
+      // genotype code = ALT allele count; named-allele dosage of codes 0, 1, 2.  The tables below do not depend on
+      // the column; each column scales them by its coefficient.  'center' / 'variance-standardize'
       // (:8003-8033): dosage x slope + intercept with intercept = -2 f slope and slope = 1 / sqrt(2 f (1 - f)) (0 when
       // the variance is not above 2^-44).  A missing call contributes 2 f slope WITHOUT the intercept in the reference
       // (missing_effect, :6756-6762) - kept, since the outputs are compared with its files.
@@ -3052,19 +3157,36 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
         e0 = d0 ? 1 : 0, e1 = 0, e2 = d2 ? 1 : 0;
         miss_dosage = f_named;
       }
-      w4[4ull * k + 0] = e.coef * (static_cast<double>(e0) * slope + icpt);
-      w4[4ull * k + 1] = e.coef * (static_cast<double>(e1) * slope + icpt);
-      w4[4ull * k + 2] = e.coef * (static_cast<double>(e2) * slope + icpt);
-      w4[4ull * k + 3] = c.score_no_meanimpute ? 0.0 : e.coef * (miss_dosage * slope);
+      const double t0 = static_cast<double>(e0) * slope + icpt, t1 = static_cast<double>(e1) * slope + icpt, t2 = static_cast<double>(e2) * slope + icpt, t3 = miss_dosage * slope;
+      for (uint32_t j = 0; j < score_ct; ++j) {
+        const double coef = coefs[e.coef_row * score_ct + j];
+        double* w = &w4[4ull * (static_cast<uint64_t>(k) * score_ct + j)];
+        w[0] = coef * t0;
+        w[1] = coef * t1;
+        w[2] = coef * t2;
+        w[3] = c.score_no_meanimpute ? 0.0 : coef * t3;
+      }
       d4[k] = static_cast<uint8_t>(e0 | (e1 << 2) | (e2 << 4));
+      // a file that names both alleles of a variant (PC projection with allele weights): the device counts the missing
+      // calls of both entries, the reference counts them once per variant (:7788), so the second entry's are taken
+      // back out here
+      if (base + k > 0 && entries[base + k - 1].v == e.v) {
+        const uint64_t* row = bs.buf + static_cast<uint64_t>(k) * bs.words;
+        for (uint32_t w = 0; w < bs.words; ++w) {
+          uint64_t ms = row[w] & (row[w] >> 1) & 0x5555555555555555ull;
+          if (32ull * (w + 1) > n) ms &= (1ull << (2 * (n - 32 * w))) - 1;
+          for (; ms; ms &= ms - 1) --repeat_miss[32 * w + __builtin_ctzll(ms) / 2];
+        }
+      }
     }
     if (pl2gpu_score_add_variants(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0, w4.data(), d4.data())) return GpuFail("pl2gpu_score_add_variants");
     base += static_cast<size_t>(got);
   }
-  std::vector<double> sums(n);
+  std::vector<double> sums(static_cast<uint64_t>(n) * score_ct);  // [sample][score_ct]
   std::vector<uint64_t> dos(n);
   std::vector<uint32_t> miss(n);
   if (pl2gpu_score_get(job, sums.data(), dos.data(), miss.data())) return GpuFail("pl2gpu_score_get");
+  for (uint32_t k = 0; k < n; ++k) miss[k] = static_cast<uint32_t>(miss[k] + repeat_miss[k]);
   logprintf("--score: %zu variant%s processed.\n", entries.size(), entries.size() == 1 ? "" : "s");
   if (c.score_list_variants) {
     OutFile fv;
@@ -3098,11 +3220,16 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   if (c.sc_nallele) hdr += "\tALLELE_CT";
   if (c.sc_denom) hdr += "\tDENOM";
   if (c.sc_dosagesum) hdr += "\tNAMED_ALLELE_DOSAGE_SUM";
-  if (c.sc_avgs) hdr += "\t" + score_name + "_AVG";
-  if (c.sc_sums) hdr += "\t" + score_name + "_SUM";
+  // every _AVG column, then every _SUM column (:8520-8539)
+  if (c.sc_avgs)
+    for (const std::string& nm : score_names) hdr += "\t" + nm + "_AVG";
+  if (c.sc_sums)
+    for (const std::string& nm : score_names) hdr += "\t" + nm + "_SUM";
   hdr += "\n";
   f.Puts(hdr.c_str());
-  const uint32_t denom_full = 2 * static_cast<uint32_t>(entries.size());
+  uint32_t scored_variants = 0;
+  for (size_t k = 0; k < entries.size(); ++k) scored_variants += !k || entries[k - 1].v != entries[k].v;
+  const uint32_t denom_full = 2 * scored_variants;
   char num[64];
   for (uint32_t k = 0; k < n; ++k) {
     std::string row = FmtId(S, k, idf);
@@ -3118,13 +3245,18 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
       row += std::string("\t") + num;
     }
     if (c.sc_dosagesum) row += "\t" + std::to_string(dos[k]);
+    const double* ks = &sums[static_cast<uint64_t>(k) * score_ct];
     if (c.sc_avgs) {
-      *dtoa_g(sums[k] * (1.0 / static_cast<double>(denom)), num) = '\0';
-      row += std::string("\t") + num;
+      for (uint32_t j = 0; j < score_ct; ++j) {
+        *dtoa_g(ks[j] * (1.0 / static_cast<double>(denom)), num) = '\0';
+        row += std::string("\t") + num;
+      }
     }
     if (c.sc_sums) {
-      *dtoa_g(sums[k], num) = '\0';
-      row += std::string("\t") + num;
+      for (uint32_t j = 0; j < score_ct; ++j) {
+        *dtoa_g(ks[j], num) = '\0';
+        row += std::string("\t") + num;
+      }
     }
     row += "\n";
     f.Write(row.data(), row.size());
@@ -3156,6 +3288,7 @@ int RunVscore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   bool fid_col = true, sid_col = false;
   std::vector<std::string> names;
   size_t id_tokens = 2;
+  const size_t first_line = li;
   if (lines[li][0] == '#') {
     const std::vector<std::string> h = SplitWs(lines[li].substr(1));
     size_t t = 0;
@@ -3177,11 +3310,33 @@ int RunVscore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
     const size_t tok_ct = SplitWs(lines[li]).size();
     for (size_t k = 2; k < tok_ct; ++k) names.push_back("VSCORE" + std::to_string(k - 1));
   }
-  const uint32_t cols = static_cast<uint32_t>(names.size());
-  if (!cols) {
+  if (names.empty()) {
     logprintf("Error: No score columns in --variant-score file.\n");
     return kRetMalformedInput;
   }
+  // weight columns as token indices: all after the IDs, or those --vscore-col-nums selects (1-based over the whole
+  // line; 2.0/plink2_matrix_calc.cc:9343-9384); a headerless file names them VSCORE1 .. by position in the selection
+  std::vector<uint32_t> wcols;
+  if (c.vscore_col_nums.empty()) {
+    for (size_t k = 0; k < names.size(); ++k) wcols.push_back(static_cast<uint32_t>(id_tokens + k));
+  } else {
+    if (c.vscore_col_nums.back() > id_tokens + names.size()) {
+      logprintf("Error: Line %zu of --variant-score file has fewer tokens than expected.\n", first_line + 1);
+      return kRetInconsistentInput;
+    }
+    if (c.vscore_col_nums.front() <= id_tokens) {
+      logprintf("Error: --vscore-col-nums argument overlaps with ID columns.\n");
+      return kRetInconsistentInput;
+    }
+    std::vector<std::string> picked;
+    for (const uint32_t col : c.vscore_col_nums) {
+      wcols.push_back(col - 1);
+      picked.push_back(li > first_line ? names[col - 1 - id_tokens] : "VSCORE" + std::to_string(picked.size() + 1));
+    }
+    names = std::move(picked);
+  }
+  const uint32_t cols = static_cast<uint32_t>(names.size());
+  const size_t need_tokens = wcols.back() + 1;
   auto key = [&](const std::string& fid, const std::string& iid, const std::string& sid) {
     std::string k = (fid_col ? fid : std::string("0")) + "\t" + iid;  // no FID column: FID 0 (XidRead, plink2_common.cc:1280)
     if (sid_col && S.sid_present) k += "\t" + sid;
@@ -3200,7 +3355,7 @@ int RunVscore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   for (; li < lines.size(); ++li) {
     if (lines[li].empty()) continue;
     const std::vector<std::string> t = SplitWs(lines[li]);
-    if (t.size() < id_tokens + cols) {
+    if (t.size() < need_tokens) {
       logprintf("Error: Line %zu of --variant-score file has fewer tokens than expected.\n", li + 1);
       return kRetMalformedInput;
     }
@@ -3222,7 +3377,7 @@ int RunVscore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
     ++loaded;
     for (uint32_t cc = 0; cc < cols; ++cc) {
       double d;
-      if (!ParseDouble(t[id_tokens + cc].c_str(), &d) || d != d) {
+      if (!ParseDouble(t[wcols[cc]].c_str(), &d) || d != d) {
         logprintf("Error: Invalid coefficient on line %zu of --variant-score file.\n", li + 1);
         return kRetMalformedInput;
       }

@@ -4,7 +4,9 @@
 // and the number of missing calls.  The caller supplies, per entry, the four weights of the genotype codes
 // (coefficient x named-allele dosage for codes 0/1/2, coefficient x 2 x allele frequency for a missing call - or 0
 // with 'no-mean-imputation', :6605-6607) and the integer named-allele dosages, so centring / dominant / recessive
-// variants are a matter of the table the caller builds.
+// variants are a matter of the table the caller builds.  A job carries score_ct coefficient columns
+// (--score-col-nums): the weight table is [entry][score_ct][4], the columns are scored in groups of kScoreGroup per
+// launch over the batch already staged, and every column's adds are those of a one-column job in the same order.
 //
 // Streaming: every 32-bit word of a variant row (16 samples) is read once.  A CTA covers 128 words x a chunk of
 // variants and writes per-chunk partial sums; a second kernel adds the partials in chunk order, so results do not
@@ -22,31 +24,39 @@ namespace {
 constexpr uint32_t kScoreThreads = 128;
 constexpr uint32_t kScoreTile = 64;  // variants whose tables are staged in shared memory at a time (even)
 
-// One thread owns one 32-bit word column (16 samples) of a chunk of variants.
-//  * fp64 sums: variants are taken in PAIRS; s_t2[pair][ca + 4 cb] = w_a[ca] + w_b[cb] (16 doubles = 128 bytes, one
-//    bank group: conflict-free for any index pattern), and the two words are merged into per-sample nibbles
-//    (x: even samples, y: odd samples), so a sample costs one bit-field extract, one LDS.64 and one DADD per TWO variants.
-//  * integer sums: the named-allele dosage (0..2) and the missing flag are added bit-parallel for all 16 samples at
-//    once in 4-bit fields (8 samples per register), spilled to 8-bit fields every 7 variants and to the 32-bit
-//    per-sample counters every 127 variants.  A REF-named entry flips hom-REF <-> hom-ALT first
-//    (w ^= (~w & 0x5555...) << 1), after which the dosage is the code itself with "missing" cleared.
-// raw: [variant][pitch] bytes (pitch multiple of 4, padding samples coded missing); w4: [variant][4] weights;
-// d4: [variant] packed named-allele dosages of codes 0..2 (2 bits each): 0x24 = ALT named, 0x06 = REF named; the
-// 'dominant' / 'recessive' forms 0x14 / 0x05 and 0x10 / 0x01 count min(copies, 1) / max(copies - 1, 0).
-__global__ void __launch_bounds__(kScoreThreads) score_kernel(const uint8_t* __restrict__ raw, uint32_t pitch, uint32_t words, uint32_t variant_ct, uint32_t chunk_variants, const double* __restrict__ w4, const uint8_t* __restrict__ d4,
-                                                           double* __restrict__ part_sum, uint32_t* __restrict__ part_dos, uint32_t* __restrict__ part_miss, uint32_t samples_padded) {
-  __shared__ double s_t2[(kScoreTile / 2) * 16];
+// One thread owns one 32-bit word column (16 samples) of a chunk of variants, for NC score columns of the entries.
+//  * fp64 sums: variants are taken in PAIRS; s_t2[c][pair][ca + 4 cb] = w_a[c][ca] + w_b[c][cb] (16 doubles = 128
+//    bytes, one bank group: conflict-free for any index pattern), and the two words are merged into per-sample nibbles
+//    (x: even samples, y: odd samples), so a sample costs one bit-field extract, one LDS.64 and one DADD per TWO
+//    variants and column.  Each column's adds are the same, in the same order, whatever NC is: column j of a
+//    several-column job is bit-identical to a one-column job of column j.
+//  * integer sums (kInts; they do not depend on the column, so one launch per batch computes them): the named-allele
+//    dosage (0..2) and the missing flag are added bit-parallel for all 16 samples at once in 4-bit fields (8 samples
+//    per register), spilled to 8-bit fields every 7 variants and to the 32-bit per-sample counters every 127 variants.
+//    A REF-named entry flips hom-REF <-> hom-ALT first (w ^= (~w & 0x5555...) << 1), after which the dosage is the code
+//    itself with "missing" cleared.
+// raw: [variant][pitch] bytes (pitch multiple of 4, padding samples coded missing); w4: [variant][score_ct][4] weights,
+// of which columns col0 .. col0 + NC - 1 are scored here; d4: [variant] packed named-allele dosages of codes 0..2 (2 bits
+// each): 0x24 = ALT named, 0x06 = REF named; the 'dominant' / 'recessive' forms 0x14 / 0x05 and 0x10 / 0x01 count
+// min(copies, 1) / max(copies - 1, 0).  part_sum: [chunk][NC][samples_padded].
+template <int NC, bool kInts>
+__global__ void __launch_bounds__(kScoreThreads, NC == 1 ? 8 : 3) score_kernel(const uint8_t* __restrict__ raw, uint32_t pitch, uint32_t words, uint32_t variant_ct, uint32_t chunk_variants, const double* __restrict__ w4, uint32_t score_ct,
+                                                           uint32_t col0, const uint8_t* __restrict__ d4, double* __restrict__ part_sum, uint32_t* __restrict__ part_dos, uint32_t* __restrict__ part_miss,
+                                                           uint32_t samples_padded) {
+  __shared__ double s_t2[NC][(kScoreTile / 2) * 16];
   __shared__ uint32_t s_flip[kScoreTile];
   __shared__ uint8_t s_mode[kScoreTile];  // 0 additive, 1 dominant (dosage min(count, 1)), 2 recessive (max(count - 1, 0))
   const uint32_t widx = blockIdx.x * kScoreThreads + threadIdx.x;
   const uint32_t v_begin = blockIdx.y * chunk_variants, v_end = min(variant_ct, v_begin + chunk_variants);
-  double sum[16];
+  double sum[NC][16];
 #pragma unroll
-  for (int s = 0; s < 16; ++s) sum[s] = 0.0;
+  for (int c = 0; c < NC; ++c)
+#pragma unroll
+    for (int s = 0; s < 16; ++s) sum[c][s] = 0.0;
   // the integer partial sums live in this thread's own 16 slots of the per-chunk partial arrays (zeroed here, added to
   // at every 8-bit spill): 32 registers fewer than keeping them in the thread
   const uint64_t base = static_cast<uint64_t>(blockIdx.y) * samples_padded + 16ull * widx;
-  if (widx < words) {
+  if (kInts && widx < words) {
 #pragma unroll
     for (int s = 0; s < 16; ++s) {
       part_dos[base + s] = 0;
@@ -90,12 +100,17 @@ __global__ void __launch_bounds__(kScoreThreads) score_kernel(const uint8_t* __r
     for (uint32_t e = threadIdx.x; e < pairs * 16; e += kScoreThreads) {
       const uint32_t pr = e >> 4, ca = e & 3, cb = (e >> 2) & 3;
       const uint32_t va = v0 + 2 * pr, vb = va + 1;
-      s_t2[e] = w4[4ull * va + ca] + ((vb < v_end) ? w4[4ull * vb + cb] : 0.0);
+      const double* wa = w4 + 4ull * (static_cast<uint64_t>(va) * score_ct + col0) + ca;
+      const double* wb = w4 + 4ull * (static_cast<uint64_t>(vb) * score_ct + col0) + cb;
+#pragma unroll
+      for (int c = 0; c < NC; ++c) s_t2[c][e] = wa[4 * c] + ((vb < v_end) ? wb[4 * c] : 0.0);
     }
-    for (uint32_t e = threadIdx.x; e < tile; e += kScoreThreads) {
-      const uint32_t dd = d4[v0 + e], da = dd & 3, db = (dd >> 2) & 3, dc = (dd >> 4) & 3;
-      s_flip[e] = da ? 0xFFFFFFFFu : 0u;  // dosage of code 0 nonzero: REF named
-      s_mode[e] = (da == 2 || dc == 2) ? 0 : (db ? 1 : 2);
+    if (kInts) {
+      for (uint32_t e = threadIdx.x; e < tile; e += kScoreThreads) {
+        const uint32_t dd = d4[v0 + e], da = dd & 3, db = (dd >> 2) & 3, dc = (dd >> 4) & 3;
+        s_flip[e] = da ? 0xFFFFFFFFu : 0u;  // dosage of code 0 nonzero: REF named
+        s_mode[e] = (da == 2 || dc == 2) ? 0 : (db ? 1 : 2);
+      }
     }
     __syncthreads();
     if (widx >= words) continue;
@@ -107,66 +122,115 @@ __global__ void __launch_bounds__(kScoreThreads) score_kernel(const uint8_t* __r
       // fp64: combined nibbles (code_a | code_b << 2); a missing second word indexes cb = 0, whose table part is 0
       const uint32_t x = (wa & 0x33333333u) | ((wb & 0x33333333u) << 2);
       const uint32_t y = ((wa >> 2) & 0x33333333u) | (wb & 0xCCCCCCCCu);
-      const double* t2 = &s_t2[16 * pr];
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        sum[2 * j] += t2[(x >> (4 * j)) & 15u];
-        sum[2 * j + 1] += t2[(y >> (4 * j)) & 15u];
+      for (int c = 0; c < NC; ++c) {
+        const double* t2 = &s_t2[c][16 * pr];
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          sum[c][2 * j] += t2[(x >> (4 * j)) & 15u];
+          sum[c][2 * j + 1] += t2[(y >> (4 * j)) & 15u];
+        }
       }
-      // integers, bit-parallel
+      if constexpr (kInts) {  // integers, bit-parallel
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        if (h && !has_b) break;
-        uint32_t w = h ? wb : wa;
-        const uint32_t ms = w & (w >> 1) & 0x55555555u;  // missing flag at the even bit of each 2-bit field
-        w ^= ((~w & 0x55555555u) << 1) & s_flip[2 * pr + h];  // REF named: 0 <-> 2 (1 and 3 keep their value)
-        uint32_t d = w ^ (ms * 3u);                         // missing -> 0
-        const uint32_t mode = s_mode[2 * pr + h];
-        if (mode == 1) d = (d | (d >> 1)) & 0x55555555u;    // dominant: 1 for one or two copies
-        else if (mode == 2) d = (d >> 1) & 0x55555555u;     // recessive: 1 for two copies
-        d4e += d & 0x33333333u;
-        d4o += (d >> 2) & 0x33333333u;
-        m4e += ms & 0x11111111u;
-        m4o += (ms >> 2) & 0x11111111u;
-        if (++n4 == 7) {
-          spill4();
-          if (++n8 == 18) spill8();  // 18 x 7 x 2 = 252 <= 255
+        for (int h = 0; h < 2; ++h) {
+          if (h && !has_b) break;
+          uint32_t w = h ? wb : wa;
+          const uint32_t ms = w & (w >> 1) & 0x55555555u;  // missing flag at the even bit of each 2-bit field
+          w ^= ((~w & 0x55555555u) << 1) & s_flip[2 * pr + h];  // REF named: 0 <-> 2 (1 and 3 keep their value)
+          uint32_t d = w ^ (ms * 3u);                         // missing -> 0
+          const uint32_t mode = s_mode[2 * pr + h];
+          if (mode == 1) d = (d | (d >> 1)) & 0x55555555u;    // dominant: 1 for one or two copies
+          else if (mode == 2) d = (d >> 1) & 0x55555555u;     // recessive: 1 for two copies
+          d4e += d & 0x33333333u;
+          d4o += (d >> 2) & 0x33333333u;
+          m4e += ms & 0x11111111u;
+          m4o += (ms >> 2) & 0x11111111u;
+          if (++n4 == 7) {
+            spill4();
+            if (++n8 == 18) spill8();  // 18 x 7 x 2 = 252 <= 255
+          }
         }
       }
     }
   }
   if (widx >= words) return;
-  spill4();
-  spill8();
+  if constexpr (kInts) {
+    spill4();
+    spill8();
+  }
 #pragma unroll
-  for (int s = 0; s < 16; ++s) part_sum[base + s] = sum[s];
+  for (int c = 0; c < NC; ++c)
+#pragma unroll
+    for (int s = 0; s < 16; ++s) part_sum[(static_cast<uint64_t>(blockIdx.y) * NC + c) * samples_padded + 16ull * widx + s] = sum[c][s];
 }
 
-__global__ void __launch_bounds__(256) score_reduce_kernel(const double* __restrict__ part_sum, const uint32_t* __restrict__ part_dos, const uint32_t* __restrict__ part_miss, uint32_t chunks, uint32_t samples_padded, uint32_t sample_ct,
-                                                          double* __restrict__ acc_sum, unsigned long long* __restrict__ acc_dos, uint32_t* __restrict__ acc_miss) {
+// acc_sum: [sample][score_ct]; columns col0 .. col0 + NC - 1 get the partials of this launch, added in chunk order.
+template <int NC, bool kInts>
+__global__ void __launch_bounds__(256, 1) score_reduce_kernel(const double* __restrict__ part_sum, const uint32_t* __restrict__ part_dos, const uint32_t* __restrict__ part_miss, uint32_t chunks, uint32_t samples_padded, uint32_t sample_ct,
+                                                          uint32_t score_ct, uint32_t col0, double* __restrict__ acc_sum, unsigned long long* __restrict__ acc_dos, uint32_t* __restrict__ acc_miss) {
   const uint32_t s = blockIdx.x * blockDim.x + threadIdx.x;
   if (s >= sample_ct) return;
-  double a = acc_sum[s];
+#pragma unroll
+  for (int c = 0; c < NC; ++c) {
+    double* acc = acc_sum + static_cast<uint64_t>(s) * score_ct + col0 + c;
+    double a = *acc;
+    for (uint32_t k = 0; k < chunks; ++k) a += part_sum[(static_cast<uint64_t>(k) * NC + c) * samples_padded + s];
+    *acc = a;
+  }
+  if (!kInts) return;
   unsigned long long d = acc_dos[s];
   uint32_t m = acc_miss[s];
   for (uint32_t k = 0; k < chunks; ++k) {
-    a += part_sum[static_cast<uint64_t>(k) * samples_padded + s];
     d += part_dos[static_cast<uint64_t>(k) * samples_padded + s];
     m += part_miss[static_cast<uint64_t>(k) * samples_padded + s];
   }
-  acc_sum[s] = a;
   acc_dos[s] = d;
   acc_miss[s] = m;
 }
 
 constexpr uint32_t kScoreStageVariants = 16384;
 constexpr uint32_t kScoreMaxChunks = 64;
+// Score columns per launch: 16 fp64 sums per column and thread live in registers, so 4 columns (128 of them) is the most
+// that compiles without spills (ptxas -v: 168 registers, three CTAs per SM) with the integer sums alongside.  The
+// one-column kernel keeps the 64 registers (eight CTAs per SM) of the one-column-only kernel it replaced.
+constexpr uint32_t kScoreGroup = 4;
+
+struct ScoreLaunch {
+  const uint8_t* raw;
+  uint32_t pitch, words, variant_ct, chunk_variants, chunks, col_ctas, score_ct, col0, samples_padded, sample_ct;
+  const double* w4;
+  const uint8_t* d4;
+  double* part_sum;
+  uint32_t *part_dos, *part_miss;
+  double* acc_sum;
+  unsigned long long* acc_dos;
+  uint32_t* acc_miss;
+};
+
+template <int NC, bool kInts>
+void LaunchScoreGroup(const ScoreLaunch& a, cudaStream_t st) {
+  score_kernel<NC, kInts><<<dim3(a.col_ctas, a.chunks), kScoreThreads, 0, st>>>(a.raw, a.pitch, a.words, a.variant_ct, a.chunk_variants, a.w4, a.score_ct, a.col0, a.d4, a.part_sum, a.part_dos, a.part_miss, a.samples_padded);
+  score_reduce_kernel<NC, kInts><<<DivUpU32(a.sample_ct, 256), 256, 0, st>>>(a.part_sum, a.part_dos, a.part_miss, a.chunks, a.samples_padded, a.sample_ct, a.score_ct, a.col0, a.acc_sum, a.acc_dos, a.acc_miss);
+}
+
+template <bool kInts>
+void LaunchScoreGroup(uint32_t nc, const ScoreLaunch& a, cudaStream_t st) {
+  static_assert(kScoreGroup == 4, "one case per group width");
+  switch (nc) {
+    case 1: LaunchScoreGroup<1, kInts>(a, st); break;
+    case 2: LaunchScoreGroup<2, kInts>(a, st); break;
+    case 3: LaunchScoreGroup<3, kInts>(a, st); break;
+    default: LaunchScoreGroup<4, kInts>(a, st); break;
+  }
+}
 
 }  // namespace
 
 struct Pl2ScoreJob {
   Pl2GpuCtx* ctx = nullptr;
-  uint32_t sample_ct = 0;
+  uint32_t sample_ct = 0, score_ct = 1;
+  uint32_t stage_variants = kScoreStageVariants;  // entries per staged batch
   GenoStage stage;
   double *d_w4 = nullptr, *d_part_sum = nullptr, *d_acc_sum = nullptr;
   uint8_t* d_d4 = nullptr;
@@ -197,36 +261,52 @@ int pl2gpu_score_end(Pl2ScoreJob* job) {
   return 0;
 }
 
-int pl2gpu_score_begin(Pl2GpuCtx* ctx, uint32_t sample_ct, Pl2ScoreJob** job_ptr) {
+int pl2gpu_score_begin_cols(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t score_ct, Pl2ScoreJob** job_ptr) {
   if (job_ptr) *job_ptr = nullptr;
-  if (!ctx || !job_ptr || !sample_ct) {
-    set_error("pl2gpu_score_begin: bad arguments");
+  if (!ctx || !job_ptr || !sample_ct || !score_ct) {
+    set_error("pl2gpu_score_begin_cols: bad arguments");
     return 1;
   }
   PL2_CUDA_OK(cudaSetDevice(ctx->c.device));
   Pl2ScoreJob* job = new Pl2ScoreJob();
   job->ctx = ctx;
   job->sample_ct = sample_ct;
+  job->score_ct = score_ct;
   auto fail = [&]() {
     pl2gpu_score_end(job);
     return 1;
   };
   if (StageAlloc(sample_ct, kScoreStageVariants, &job->stage, 64)) return fail();
   const uint64_t np = job->stage.sample_ct_padded;
-  if (cudaMalloc(&job->d_w4, 32ull * kScoreStageVariants) != cudaSuccess || cudaMalloc(&job->d_d4, kScoreStageVariants) != cudaSuccess || cudaMalloc(&job->d_part_sum, 8 * np * kScoreMaxChunks) != cudaSuccess ||
-      cudaMalloc(&job->d_part_dos, 4 * np * kScoreMaxChunks) != cudaSuccess || cudaMalloc(&job->d_part_miss, 4 * np * kScoreMaxChunks) != cudaSuccess || cudaMalloc(&job->d_acc_sum, 8 * np) != cudaSuccess ||
-      cudaMalloc(&job->d_acc_dos, 8 * np) != cudaSuccess || cudaMalloc(&job->d_acc_miss, 4 * np) != cudaSuccess) {
+  const uint64_t group = std::min(score_ct, kScoreGroup);
+  if (cudaMalloc(&job->d_d4, kScoreStageVariants) != cudaSuccess || cudaMalloc(&job->d_part_sum, 8 * np * kScoreMaxChunks * group) != cudaSuccess || cudaMalloc(&job->d_part_dos, 4 * np * kScoreMaxChunks) != cudaSuccess ||
+      cudaMalloc(&job->d_part_miss, 4 * np * kScoreMaxChunks) != cudaSuccess || cudaMalloc(&job->d_acc_sum, 8 * np * score_ct) != cudaSuccess || cudaMalloc(&job->d_acc_dos, 8 * np) != cudaSuccess ||
+      cudaMalloc(&job->d_acc_miss, 4 * np) != cudaSuccess) {
     cudaGetLastError();
-    set_error("pl2gpu_score_begin: insufficient device memory for %u samples", sample_ct);
+    set_error("pl2gpu_score_begin_cols: insufficient device memory for %u samples x %u score columns", sample_ct, score_ct);
     return fail();
   }
-  if (cudaMemsetAsync(job->d_acc_sum, 0, 8 * np, ctx->c.stream) != cudaSuccess || cudaMemsetAsync(job->d_acc_dos, 0, 8 * np, ctx->c.stream) != cudaSuccess || cudaMemsetAsync(job->d_acc_miss, 0, 4 * np, ctx->c.stream) != cudaSuccess) {
-    set_error("pl2gpu_score_begin: %s", cudaGetErrorString(cudaGetLastError()));
+  // the staged weights ([entry][score_ct][4]) are the one buffer that grows with the column count and the batch: when
+  // they do not fit, batches get fewer entries (then the chunk plan, and so the last bits of a sum, can differ from a
+  // job with fewer columns)
+  while (cudaMalloc(&job->d_w4, 32ull * score_ct * job->stage_variants) != cudaSuccess) {
+    cudaGetLastError();
+    if (job->stage_variants <= kScoreTile) {
+      set_error("pl2gpu_score_begin_cols: insufficient device memory for the weights of %u score columns", score_ct);
+      return fail();
+    }
+    job->stage_variants /= 2;
+  }
+  if (cudaMemsetAsync(job->d_acc_sum, 0, 8 * np * score_ct, ctx->c.stream) != cudaSuccess || cudaMemsetAsync(job->d_acc_dos, 0, 8 * np, ctx->c.stream) != cudaSuccess ||
+      cudaMemsetAsync(job->d_acc_miss, 0, 4 * np, ctx->c.stream) != cudaSuccess) {
+    set_error("pl2gpu_score_begin_cols: %s", cudaGetErrorString(cudaGetLastError()));
     return fail();
   }
   *job_ptr = job;
   return 0;
 }
+
+int pl2gpu_score_begin(Pl2GpuCtx* ctx, uint32_t sample_ct, Pl2ScoreJob** job_ptr) { return pl2gpu_score_begin_cols(ctx, sample_ct, 1, job_ptr); }
 
 int pl2gpu_score_add_variants(Pl2ScoreJob* job, const void* genovecs, uint64_t variant_stride_bytes, uint32_t variant_ct, int src_is_device, const double* weights4, const uint8_t* named_dosages) {
   if (!job || (variant_ct && (!genovecs || !weights4 || !named_dosages))) {
@@ -244,20 +324,29 @@ int pl2gpu_score_add_variants(Pl2ScoreJob* job, const void* genovecs, uint64_t v
   PL2_CUDA_OK(cudaSetDevice(c->device));
   const uint8_t* src = static_cast<const uint8_t*>(genovecs);
   const uint32_t np = job->stage.sample_ct_padded, words = np / 16;
+  const uint64_t w_row = 4ull * job->score_ct;  // doubles of weights per entry
   for (uint32_t done = 0; done < variant_ct;) {
-    const uint32_t cur = std::min(kScoreStageVariants, variant_ct - done);
+    const uint32_t cur = std::min(job->stage_variants, variant_ct - done);
     uint32_t padded = 0;
     PL2_TRY(StageUpload(c, &job->stage, src + static_cast<uint64_t>(done) * variant_stride_bytes, variant_stride_bytes, cur, src_is_device, &padded));
-    PL2_CUDA_OK(cudaMemcpyAsync(job->d_w4, weights4 + 4ull * done, 32ull * cur, cudaMemcpyHostToDevice, c->stream));
+    PL2_CUDA_OK(cudaMemcpyAsync(job->d_w4, weights4 + w_row * done, 8 * w_row * cur, cudaMemcpyHostToDevice, c->stream));
     PL2_CUDA_OK(cudaMemcpyAsync(job->d_d4, named_dosages + done, cur, cudaMemcpyHostToDevice, c->stream));
-    // enough chunks to fill the GPU, each a multiple of the shared-memory tile
+    // enough chunks to fill the GPU, each a multiple of the shared-memory tile; the plan does not depend on the column
+    // count, so every column is added in the order of a one-column job
     const uint32_t col_ctas = DivUpU32(words, kScoreThreads);
     uint32_t chunks = std::max(1u, std::min({kScoreMaxChunks, DivUpU32(7 * static_cast<uint32_t>(c->sm_count), col_ctas), DivUpU32(cur, kScoreTile)}));
     const uint32_t chunk_variants = RoundUpU32(DivUpU32(cur, chunks), kScoreTile);
     chunks = DivUpU32(cur, chunk_variants);
-    score_kernel<<<dim3(col_ctas, chunks), kScoreThreads, 0, c->stream>>>(job->stage.d_raw, job->stage.pitch, words, cur, chunk_variants, job->d_w4, job->d_d4, job->d_part_sum, job->d_part_dos, job->d_part_miss, np);
-    score_reduce_kernel<<<DivUpU32(job->sample_ct, 256), 256, 0, c->stream>>>(job->d_part_sum, job->d_part_dos, job->d_part_miss, chunks, np, job->sample_ct, job->d_acc_sum, job->d_acc_dos, job->d_acc_miss);
-    c->launches += 2;
+    ScoreLaunch a{job->stage.d_raw, job->stage.pitch, words, cur, chunk_variants, chunks, col_ctas, job->score_ct, 0, np, job->sample_ct, job->d_w4, job->d_d4, job->d_part_sum, job->d_part_dos, job->d_part_miss,
+                  job->d_acc_sum, job->d_acc_dos, job->d_acc_miss};
+    // column groups over the resident batch; the first also adds the integer sums
+    for (uint32_t col0 = 0; col0 < job->score_ct; col0 += kScoreGroup) {
+      a.col0 = col0;
+      const uint32_t nc = std::min(kScoreGroup, job->score_ct - col0);
+      if (col0 == 0) LaunchScoreGroup<true>(nc, a, c->stream);
+      else LaunchScoreGroup<false>(nc, a, c->stream);
+      c->launches += 2;
+    }
     PL2_CUDA_OK(cudaGetLastError());
     PL2_CUDA_OK(cudaStreamSynchronize(c->stream));  // host tables and a host source may be reused by the caller
     job->entries += cur;
@@ -273,7 +362,7 @@ int pl2gpu_score_get(Pl2ScoreJob* job, double* score_sums, uint64_t* named_dosag
   }
   Ctx* c = &job->ctx->c;
   PL2_CUDA_OK(cudaSetDevice(c->device));
-  PL2_CUDA_OK(cudaMemcpyAsync(score_sums, job->d_acc_sum, 8ull * job->sample_ct, cudaMemcpyDeviceToHost, c->stream));
+  PL2_CUDA_OK(cudaMemcpyAsync(score_sums, job->d_acc_sum, 8ull * job->sample_ct * job->score_ct, cudaMemcpyDeviceToHost, c->stream));
   if (named_dosage_sums) PL2_CUDA_OK(cudaMemcpyAsync(named_dosage_sums, job->d_acc_dos, 8ull * job->sample_ct, cudaMemcpyDeviceToHost, c->stream));
   if (missing_cts) PL2_CUDA_OK(cudaMemcpyAsync(missing_cts, job->d_acc_miss, 4ull * job->sample_ct, cudaMemcpyDeviceToHost, c->stream));
   PL2_CUDA_OK(cudaStreamSynchronize(c->stream));

@@ -423,6 +423,27 @@ def score_sums(ctx: GpuContext, genovecs: np.ndarray, sample_ct: int, weights4: 
         lib.pl2gpu_score_end(h)
 
 
+def score_sums_cols(ctx: GpuContext, genovecs: np.ndarray, sample_ct: int, weights4: np.ndarray, named_dosages: np.ndarray):
+    """Several `--score` coefficient columns in one pass (pl2gpu_score_begin_cols): weights4 [entries, score_ct, 4] ->
+    (score sums [sample_ct, score_ct], named-allele dosage sums, missing counts); otherwise as score_sums."""
+    g = np.ascontiguousarray(genovecs)
+    w = np.ascontiguousarray(weights4, dtype=np.float64)
+    d = np.ascontiguousarray(named_dosages, dtype=np.uint8)
+    assert w.ndim == 3 and w.shape[0] == g.shape[0] and w.shape[2] == 4 and d.shape == (g.shape[0],)
+    score_ct = w.shape[1]
+    h = C.c_void_p()
+    check(lib.pl2gpu_score_begin_cols(ctx.handle, sample_ct, score_ct, C.byref(h)), "pl2gpu_score_begin_cols")
+    try:
+        check(lib.pl2gpu_score_add_variants(h, g.ctypes.data, g.strides[0], g.shape[0], 0, w.ctypes.data, d.ctypes.data), "pl2gpu_score_add_variants")
+        sums = np.empty((sample_ct, score_ct), dtype=np.float64)
+        dos = np.empty(sample_ct, dtype=np.uint64)
+        miss = np.empty(sample_ct, dtype=np.uint32)
+        check(lib.pl2gpu_score_get(h, sums.ctypes.data, dos.ctypes.data, miss.ctypes.data), "pl2gpu_score_get")
+        return sums, dos, miss
+    finally:
+        lib.pl2gpu_score_end(h)
+
+
 def variant_scores(ctx: GpuContext, genovecs: np.ndarray, sample_ct: int, weights: np.ndarray, ref_freqs=None) -> np.ndarray:
     """`--variant-score` sums (pl2gpu_pca_vscore) for an in-memory block: weights [sample_ct, cols] -> [variants, cols]."""
     g = np.ascontiguousarray(genovecs)
