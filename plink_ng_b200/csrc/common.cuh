@@ -101,6 +101,37 @@ void StageFree(GenoStage* gs);
 // samples / rows [dst_row + variant_ct, dst_row + padded) to "missing".
 int StageUpload(Ctx* ctx, GenoStage* gs, const void* src, uint64_t src_stride, uint32_t variant_ct, int src_is_device, uint32_t* padded_ct_ptr, uint32_t dst_row = 0, uint32_t pad_to = kVariantPad);
 
+// Two staged blocks used in turn (implemented in pl2gpu.cu): the copy / all-gather and padding of batch k+1 on the
+// prep stream (Ctx::copy_stream) overlap the kernel of batch k on the compute stream.  That is correct because the
+// prep stream waits for a slot's last reader before overwriting it (mark_busy, acquire) and for the compute stream
+// when a source is written there (acquire, src_is_device == 1), the compute stream waits for the prep work (fence),
+// and a host source goes back to the caller only once its copy has finished (release_host_source).
+struct StageRing {
+  Ctx* ctx = nullptr;
+  GenoStage stage[2];
+  cudaEvent_t ev_prep_done[2] = {nullptr, nullptr};
+  cudaEvent_t ev_free[2] = {nullptr, nullptr};  // the slot's last reader has finished; timing-enabled for pl2gpu_king_last_kernel_ms
+  bool free_pending[2] = {false, false};
+  uint32_t next = 0;                   // the slot the next acquire returns
+  cudaEvent_t ev_src_ready = nullptr;  // the compute stream has reached the copy of a src_is_device == 1 source
+  cudaEvent_t ev_copied = nullptr;     // the caller's rows have been copied (prep stream)
+
+  int alloc(Ctx* c, uint32_t sample_ct, uint32_t variant_cap, uint32_t sample_pad);
+  void free();
+  int acquire(int src_is_device, uint32_t* slot);
+  // `rows` rows into the slot, or into dst (same pitch) when dst is not null
+  int land(uint32_t slot, uint8_t* dst, const void* src, uint64_t src_stride, uint32_t rows, int src_is_device);
+  // sharded form: this rank's slice lands at rows [rank * slice_rows, (rank + 1) * slice_rows), is padded there, and one
+  // in-place all-gather makes the block complete on every rank
+  int land_slice(uint32_t slot, const void* src, uint64_t src_stride, uint32_t slice_rows, int src_is_device);
+  // rows [cur, *padded) become "missing", *padded = cur rounded up to pad_to; so do the padding samples of rows [0, cur)
+  // when pad_valid_rows (land_slice has already padded them otherwise)
+  int pad(uint32_t slot, uint32_t cur, bool pad_valid_rows, uint32_t pad_to, uint32_t* padded);
+  int fence(uint32_t slot);
+  int mark_busy(uint32_t slot, cudaStream_t stream);
+  int release_host_source(int src_is_device);
+};
+
 static inline uint32_t DivUpU32(uint32_t a, uint32_t b) { return (a + b - 1) / b; }
 static inline uint64_t DivUpU64(uint64_t a, uint64_t b) { return (a + b - 1) / b; }
 static inline uint32_t RoundUpU32(uint32_t a, uint32_t b) { return DivUpU32(a, b) * b; }

@@ -24,20 +24,13 @@ struct Pl2GrmJob {
   uint32_t sample_ct = 0, row_start = 0, row_end = 0;
   int flags = 0;
   TileList tiles;
-  // Double-buffered like the KING job (pl2gpu.cu): copy / all-gather, padding, genotype counts, digit tables and
-  // row re-tiling of batch k+1 run on the prep stream while the tensor kernel of batch k runs.
-  GenoStage stage[2];
+  StageRing ring;  // genotype counts, digit tables and row re-tiling of each slot also run on the prep stream
   uint8_t* d_raw_i[2] = {nullptr, nullptr};  // sample-major copy of the staged block (geno_tile.cuh)
   uint8_t* d_tab[2] = {nullptr, nullptr};    // digit tables (grm_tables_kernel)
   double* d_lvals[2] = {nullptr, nullptr};
   uint32_t* d_counts[2] = {nullptr, nullptr};
   double* h_lvals[2] = {nullptr, nullptr};     // pinned
   uint32_t* h_counts[2] = {nullptr, nullptr};  // pinned
-  cudaEvent_t ev_prep_done[2] = {nullptr, nullptr};
-  cudaEvent_t ev_kernel_done[2] = {nullptr, nullptr};
-  cudaEvent_t ev_src_ready = nullptr;
-  bool kernel_pending[2] = {false, false};
-  uint32_t buf_idx = 0;
   double* d_acc_g = nullptr;
   int32_t* d_acc_obs = nullptr;
   void* d_out_stage = nullptr;
@@ -71,16 +64,15 @@ int pl2gpu_grm_begin(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start, uin
   if (BuildTileList(row_start, row_end, true, &job->tiles, kGrmTileCols)) return fail();
   const uint64_t words = static_cast<uint64_t>(job->tiles.tile_ct) * kGrmTileWords;
   job->out_stage_bytes = 256ull << 20;
-  bool ok = cudaEventCreateWithFlags(&job->ev_src_ready, cudaEventDisableTiming) == cudaSuccess;
+  if (job->ring.alloc(&ctx->c, sample_ct, kMaxStageVariants, kGrmSamplePad)) return fail();
+  const uint64_t cap = job->ring.stage[0].variant_cap;
+  const uint64_t raw_i_bytes = static_cast<uint64_t>(job->ring.stage[0].sample_ct_padded) * (cap / 4);
+  bool ok = true;
   for (int b = 0; b < 2 && ok; ++b) {
-    if (StageAlloc(sample_ct, kMaxStageVariants, &job->stage[b], kGrmSamplePad)) return fail();
-    const uint64_t cap = job->stage[b].variant_cap;
-    const uint64_t raw_i_bytes = static_cast<uint64_t>(job->stage[b].sample_ct_padded) * (cap / 4);
     ok = cudaMalloc(&job->d_raw_i[b], raw_i_bytes ? raw_i_bytes : 16) == cudaSuccess && cudaMalloc(&job->d_tab[b], cap / 16 * kGrmTabChunkBytes) == cudaSuccess &&
          cudaMalloc(&job->d_lvals[b], cap * 6 * 8) == cudaSuccess && cudaMalloc(&job->d_counts[b], cap * 16) == cudaSuccess &&
          cudaHostAlloc(reinterpret_cast<void**>(&job->h_lvals[b]), cap * 6 * 8, cudaHostAllocDefault) == cudaSuccess &&
-         cudaHostAlloc(reinterpret_cast<void**>(&job->h_counts[b]), cap * 16, cudaHostAllocDefault) == cudaSuccess &&
-         cudaEventCreateWithFlags(&job->ev_prep_done[b], cudaEventDisableTiming) == cudaSuccess && cudaEventCreateWithFlags(&job->ev_kernel_done[b], cudaEventDisableTiming) == cudaSuccess;
+         cudaHostAlloc(reinterpret_cast<void**>(&job->h_counts[b]), cap * 16, cudaHostAllocDefault) == cudaSuccess;
   }
   if (!ok || cudaMalloc(&job->d_acc_g, words * 8 + 8) != cudaSuccess || cudaMalloc(&job->d_acc_obs, words * 4 + 4) != cudaSuccess || cudaMalloc(&job->d_out_stage, job->out_stage_bytes) != cudaSuccess) {
     cudaGetLastError();
@@ -95,20 +87,16 @@ int pl2gpu_grm_begin(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start, uin
   return 0;
 }
 
-// One staged batch: stage[b] rows [0, cur) hold the (already sample-padded when !pad_valid_rows) genotypes.
+// One staged batch: ring slot b rows [0, cur) hold the (already sample-padded when !pad_valid_rows) genotypes.
 // Counts -> per-variant lookup values (host, a few microseconds per thousand variants) -> fixed-point digit
 // tables, row re-tiling, tensor kernel.  ref_freqs: this batch's REF frequencies or nullptr.
 static int GrmPrepAndLaunch(Pl2GrmJob* job, uint32_t b, uint32_t cur, bool pad_valid_rows, const double* ref_freqs) {
   Ctx* c = &job->ctx->c;
   cudaStream_t prep = c->copy_stream;
-  GenoStage& st = job->stage[b];
+  const GenoStage& st = job->ring.stage[b];
   const bool cov = (job->flags & kPl2GrmCov) != 0;
-  const uint32_t padded = RoundUpU32(cur, kVariantPad);
-  if (pad_valid_rows) {
-    PL2_TRY(LaunchPadGenotypes(c, st.d_raw, st.pitch, st.sample_ct, cur, padded, prep));
-  } else if (padded > cur) {
-    PL2_TRY(LaunchPadGenotypes(c, st.d_raw + static_cast<uint64_t>(cur) * st.pitch, st.pitch, st.sample_ct, 0, padded - cur, prep));
-  }
+  uint32_t padded;
+  PL2_TRY(job->ring.pad(b, cur, pad_valid_rows, kVariantPad, &padded));
   // genotype counts of the batch: missingness presence, the zero-variance consistency check
   // (ExpandCenteredVarmaj :3844-3868) and, when the caller passes no frequencies, ComputeAlleleFreqs.
   geno_counts_kernel<<<DivUpU32(cur, 8), 256, 0, prep>>>(st.d_raw, st.pitch, st.sample_ct, st.sample_ct_padded, cur, job->d_counts[b]);
@@ -179,28 +167,12 @@ static int GrmPrepAndLaunch(Pl2GrmJob* job, uint32_t b, uint32_t cur, bool pad_v
     geno_tile_rows_kernel<<<dim3(padded / 64, st.sample_ct_padded / 64), 256, 0, prep>>>(st.d_raw, st.pitch, padded / 32, 0, job->d_raw_i[b]);
     c->launches++;
     PL2_CUDA_OK(cudaGetLastError());
-    PL2_CUDA_OK(cudaEventRecord(job->ev_prep_done[b], prep));
-    PL2_CUDA_OK(cudaStreamWaitEvent(c->stream, job->ev_prep_done[b], 0));
+    PL2_TRY(job->ring.fence(b));
     grm_wg_kernel<<<2 * job->tiles.tile_ct, kGwThreads, kGwSmemBytes, c->stream>>>(job->d_raw_i[b], padded, job->d_tab[b], inv_scale, job->tiles.d_tile_order, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->d_acc_g, job->d_acc_obs);
     c->launches++;
     PL2_CUDA_OK(cudaGetLastError());
-    PL2_CUDA_OK(cudaEventRecord(job->ev_kernel_done[b], c->stream));
-    job->kernel_pending[b] = true;
   }
-  return 0;
-}
-
-static int GrmAcquireBuffer(Pl2GrmJob* job, int src_is_device, uint32_t* b_out) {
-  Ctx* c = &job->ctx->c;
-  const uint32_t b = job->buf_idx;
-  job->buf_idx ^= 1;
-  if (job->kernel_pending[b]) PL2_CUDA_OK(cudaStreamWaitEvent(c->copy_stream, job->ev_kernel_done[b], 0));
-  if (src_is_device == 1) {
-    PL2_CUDA_OK(cudaEventRecord(job->ev_src_ready, c->stream));
-    PL2_CUDA_OK(cudaStreamWaitEvent(c->copy_stream, job->ev_src_ready, 0));
-  }
-  *b_out = b;
-  return 0;
+  return job->ring.mark_busy(b, job->tiles.tile_ct ? c->stream : prep);
 }
 
 int pl2gpu_grm_add_variants(Pl2GrmJob* job, const void* genovecs, uint64_t variant_stride_bytes, uint32_t variant_ct, int src_is_device, const double* ref_freqs) {
@@ -216,11 +188,10 @@ int pl2gpu_grm_add_variants(Pl2GrmJob* job, const void* genovecs, uint64_t varia
   }
   const uint8_t* src = static_cast<const uint8_t*>(genovecs);
   for (uint32_t done = 0; done < variant_ct;) {
-    const uint32_t cur = std::min(job->stage[0].variant_cap, variant_ct - done);
+    const uint32_t cur = std::min(job->ring.stage[0].variant_cap, variant_ct - done);
     uint32_t b;
-    PL2_TRY(GrmAcquireBuffer(job, src_is_device, &b));
-    GenoStage& st = job->stage[b];
-    PL2_CUDA_OK(cudaMemcpy2DAsync(st.d_raw, st.pitch, src + static_cast<uint64_t>(done) * variant_stride_bytes, variant_stride_bytes, DivUpU32(st.sample_ct, 4), cur, src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, c->copy_stream));
+    PL2_TRY(job->ring.acquire(src_is_device, &b));
+    PL2_TRY(job->ring.land(b, nullptr, src + static_cast<uint64_t>(done) * variant_stride_bytes, variant_stride_bytes, cur, src_is_device));
     // GrmPrepAndLaunch synchronises the prep stream (it needs the counts on the host), so a host source has been
     // consumed when it returns; the tensor kernel keeps running
     const int rc = GrmPrepAndLaunch(job, b, cur, true, ref_freqs ? ref_freqs + done : nullptr);
@@ -239,8 +210,8 @@ int pl2gpu_grm_add_variants_sharded(Pl2GrmJob* job, const void* slice, uint64_t 
   Ctx* c = &job->ctx->c;
   PL2_CUDA_OK(cudaSetDevice(c->device));
   const uint64_t total64 = static_cast<uint64_t>(slice_variant_ct) * c->comm_world;
-  if (!slice_variant_ct || total64 > job->stage[0].variant_cap || !batch_variant_ct || batch_variant_ct > total64) {
-    set_error("pl2gpu_grm_add_variants_sharded: bad slice (%u variants x %d ranks, batch %u, stage capacity %u)", slice_variant_ct, c->comm_world, batch_variant_ct, job->stage[0].variant_cap);
+  if (!slice_variant_ct || total64 > job->ring.stage[0].variant_cap || !batch_variant_ct || batch_variant_ct > total64) {
+    set_error("pl2gpu_grm_add_variants_sharded: bad slice (%u variants x %d ranks, batch %u, stage capacity %u)", slice_variant_ct, c->comm_world, batch_variant_ct, job->ring.stage[0].variant_cap);
     return 1;
   }
   if (variant_stride_bytes < DivUpU32(job->sample_ct, 4)) {
@@ -248,13 +219,8 @@ int pl2gpu_grm_add_variants_sharded(Pl2GrmJob* job, const void* slice, uint64_t 
     return 1;
   }
   uint32_t b;
-  PL2_TRY(GrmAcquireBuffer(job, src_is_device, &b));
-  GenoStage& st = job->stage[b];
-  cudaStream_t prep = c->copy_stream;
-  uint8_t* mine = st.d_raw + static_cast<uint64_t>(c->comm_rank) * slice_variant_ct * st.pitch;
-  PL2_CUDA_OK(cudaMemcpy2DAsync(mine, st.pitch, slice, variant_stride_bytes, DivUpU32(st.sample_ct, 4), slice_variant_ct, src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, prep));
-  PL2_TRY(LaunchPadGenotypes(c, mine, st.pitch, st.sample_ct, slice_variant_ct, slice_variant_ct, prep));
-  PL2_TRY(CommAllGatherInPlace(c, st.d_raw, static_cast<uint64_t>(slice_variant_ct) * st.pitch, prep));
+  PL2_TRY(job->ring.acquire(src_is_device, &b));
+  PL2_TRY(job->ring.land_slice(b, slice, variant_stride_bytes, slice_variant_ct, src_is_device));
   // only the first batch_variant_ct rows of the gathered tile are real variants (the last slice of a file is
   // topped up with filler rows); the rest is overwritten with "missing" by the tail padding
   const int rc = GrmPrepAndLaunch(job, b, batch_variant_ct, false, ref_freqs);
@@ -454,18 +420,15 @@ int pl2gpu_grm_end(Pl2GrmJob* job) {
     cudaStreamSynchronize(job->ctx->c.copy_stream);
   }
   FreeTileList(&job->tiles);
+  job->ring.free();
   for (int b = 0; b < 2; ++b) {
-    StageFree(&job->stage[b]);
     cudaFree(job->d_raw_i[b]);
     cudaFree(job->d_tab[b]);
     cudaFree(job->d_lvals[b]);
     cudaFree(job->d_counts[b]);
     if (job->h_lvals[b]) cudaFreeHost(job->h_lvals[b]);
     if (job->h_counts[b]) cudaFreeHost(job->h_counts[b]);
-    if (job->ev_prep_done[b]) cudaEventDestroy(job->ev_prep_done[b]);
-    if (job->ev_kernel_done[b]) cudaEventDestroy(job->ev_kernel_done[b]);
   }
-  if (job->ev_src_ready) cudaEventDestroy(job->ev_src_ready);
   cudaFree(job->d_acc_g);
   cudaFree(job->d_acc_obs);
   cudaFree(job->d_out_stage);

@@ -80,19 +80,12 @@ int pl2gpu_ld_band_flags(Pl2GpuCtx* ctx, const void* genovecs, uint64_t variant_
   PL2_CUDA_OK(cudaSetDevice(c->device));
   const uint32_t band_r = RoundUpU32(band, 64);
   const uint32_t rows_cap = kLdChunkVariants + band_r;
-  // two staged chunks: the copy of chunk k+1 (prep stream) overlaps the pair kernel of chunk k; flags come back
-  // through two pinned-size device buffers in the same rhythm
-  GenoStage st[2];
+  // the copy of chunk k+1 (prep stream) overlaps the pair kernel of chunk k; flags come back through two device
+  // buffers in the same rhythm
+  StageRing ring;
   DevBuf d_flags[2];
-  cudaEvent_t ev_copied[2] = {nullptr, nullptr};
-  int rc = 0;
-  for (int b = 0; b < 2 && !rc; ++b) {
-    rc = StageAlloc(founder_ct, rows_cap, &st[b], 64) || d_flags[b].alloc(static_cast<uint64_t>(kLdChunkVariants) * band);
-    if (!rc && cudaEventCreateWithFlags(&ev_copied[b], cudaEventDisableTiming) != cudaSuccess) {
-      set_error("pl2gpu_ld_band_flags: cudaEventCreate failed");
-      rc = 1;
-    }
-  }
+  int rc = ring.alloc(c, founder_ct, rows_cap, 64);
+  for (int b = 0; b < 2 && !rc; ++b) rc = d_flags[b].alloc(static_cast<uint64_t>(kLdChunkVariants) * band);
   if (!rc && cudaFuncSetAttribute(ld_ts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kLdtSmemBytes) != cudaSuccess) {
     set_error("pl2gpu_ld_band_flags: %s", cudaGetErrorString(cudaGetLastError()));
     rc = 1;
@@ -112,24 +105,16 @@ int pl2gpu_ld_band_flags(Pl2GpuCtx* ctx, const void* genovecs, uint64_t variant_
     }
     return 0;
   };
-  uint32_t chunk_idx = 0;
-  for (uint32_t a0 = 0; a0 < variant_ct && !rc; a0 += kLdChunkVariants, ++chunk_idx) {
-    const int b = chunk_idx & 1;
+  for (uint32_t a0 = 0; a0 < variant_ct && !rc; a0 += kLdChunkVariants) {
     const uint32_t a1 = std::min(variant_ct, a0 + kLdChunkVariants);
     const uint32_t lo = (a0 > band_r) ? (a0 - band_r) : 0;
-    rc = drain(b);  // buffer b is free again (its kernel has finished, its flags are on the host)
+    uint32_t b, padded;
+    // drain(b): slot b is free again (its kernel has finished, its flags are on the host)
+    rc = ring.acquire(src_is_device, &b) || drain(b) || ring.land(b, nullptr, src + static_cast<uint64_t>(lo) * variant_stride_bytes, variant_stride_bytes, a1 - lo, src_is_device) ||
+         ring.pad(b, a1 - lo, true, 64, &padded) || ring.fence(b);
     if (rc) break;
-    const uint32_t rows = a1 - lo, padded = RoundUpU32(rows, 64);
-    if (cudaMemcpy2DAsync(st[b].d_raw, st[b].pitch, src + static_cast<uint64_t>(lo) * variant_stride_bytes, variant_stride_bytes, DivUpU32(founder_ct, 4), rows, src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, c->copy_stream) != cudaSuccess) {
-      set_error("pl2gpu_ld_band_flags: %s", cudaGetErrorString(cudaGetLastError()));
-      rc = 1;
-      break;
-    }
-    rc = LaunchPadGenotypes(c, st[b].d_raw, st[b].pitch, st[b].sample_ct, rows, padded, c->copy_stream);
-    if (rc) break;
-    cudaEventRecord(ev_copied[b], c->copy_stream);
-    cudaStreamWaitEvent(c->stream, ev_copied[b], 0);
-    ld_ts_kernel<<<dim3(DivUpU32(a1 - a0, kLdtRows), (kLdtRows - kLdtCols + band_r) / kLdtCols + 1), kLdtThreads, kLdtSmemBytes, c->stream>>>(st[b].d_raw, st[b].pitch, st[b].sample_ct_padded, lo, a0, a1, band, prune_ld_thresh, static_cast<uint8_t*>(d_flags[b].p));
+    const GenoStage& st = ring.stage[b];
+    ld_ts_kernel<<<dim3(DivUpU32(a1 - a0, kLdtRows), (kLdtRows - kLdtCols + band_r) / kLdtCols + 1), kLdtThreads, kLdtSmemBytes, c->stream>>>(st.d_raw, st.pitch, st.sample_ct_padded, lo, a0, a1, band, prune_ld_thresh, static_cast<uint8_t*>(d_flags[b].p));
     c->launches++;
     if (cudaGetLastError() != cudaSuccess) {
       set_error("pl2gpu_ld_band_flags: %s", cudaGetErrorString(cudaGetLastError()));
@@ -140,21 +125,14 @@ int pl2gpu_ld_band_flags(Pl2GpuCtx* ctx, const void* genovecs, uint64_t variant_
     pend[b].a1 = a1;
     pend[b].live = true;
     // a host source may be reused by the caller only after the copy; chunks overlap by band_r rows, so wait here
-    if (!src_is_device && cudaEventSynchronize(ev_copied[b]) != cudaSuccess) {
-      set_error("pl2gpu_ld_band_flags: %s", cudaGetErrorString(cudaGetLastError()));
-      rc = 1;
-    }
+    rc = ring.release_host_source(src_is_device);
   }
-  for (int b = 0; b < 2; ++b) {
-    const int other = (chunk_idx + b) & 1;  // oldest pending first
-    if (!rc) rc = drain(other);
+  for (uint32_t b = 0; b < 2; ++b) {
+    if (!rc) rc = drain((ring.next + b) & 1);  // oldest pending first
   }
   cudaStreamSynchronize(c->stream);
   cudaStreamSynchronize(c->copy_stream);
-  for (int b = 0; b < 2; ++b) {
-    StageFree(&st[b]);
-    if (ev_copied[b]) cudaEventDestroy(ev_copied[b]);
-  }
+  ring.free();
   return rc;
 }
 

@@ -213,6 +213,80 @@ int StageUpload(Ctx* ctx, GenoStage* gs, const void* src, uint64_t src_stride, u
   return 0;
 }
 
+int StageRing::alloc(Ctx* c, uint32_t sample_ct, uint32_t variant_cap, uint32_t sample_pad) {
+  ctx = c;
+  for (int s = 0; s < 2; ++s) {
+    PL2_TRY(StageAlloc(sample_ct, variant_cap, &stage[s], sample_pad));
+    PL2_CUDA_OK(cudaEventCreateWithFlags(&ev_prep_done[s], cudaEventDisableTiming));
+    PL2_CUDA_OK(cudaEventCreate(&ev_free[s]));
+  }
+  PL2_CUDA_OK(cudaEventCreateWithFlags(&ev_src_ready, cudaEventDisableTiming));
+  PL2_CUDA_OK(cudaEventCreateWithFlags(&ev_copied, cudaEventDisableTiming));
+  return 0;
+}
+
+void StageRing::free() {
+  for (int s = 0; s < 2; ++s) {
+    StageFree(&stage[s]);
+    if (ev_prep_done[s]) cudaEventDestroy(ev_prep_done[s]);
+    if (ev_free[s]) cudaEventDestroy(ev_free[s]);
+  }
+  if (ev_src_ready) cudaEventDestroy(ev_src_ready);
+  if (ev_copied) cudaEventDestroy(ev_copied);
+}
+
+int StageRing::acquire(int src_is_device, uint32_t* slot) {
+  const uint32_t s = next;
+  next ^= 1;
+  if (free_pending[s]) PL2_CUDA_OK(cudaStreamWaitEvent(ctx->copy_stream, ev_free[s], 0));
+  if (src_is_device == 1) {
+    PL2_CUDA_OK(cudaEventRecord(ev_src_ready, ctx->stream));
+    PL2_CUDA_OK(cudaStreamWaitEvent(ctx->copy_stream, ev_src_ready, 0));
+  }
+  *slot = s;
+  return 0;
+}
+
+int StageRing::land(uint32_t slot, uint8_t* dst, const void* src, uint64_t src_stride, uint32_t rows, int src_is_device) {
+  const GenoStage& st = stage[slot];
+  PL2_CUDA_OK(cudaMemcpy2DAsync(dst ? dst : st.d_raw, st.pitch, src, src_stride, DivUpU32(st.sample_ct, 4), rows, src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->copy_stream));
+  PL2_CUDA_OK(cudaEventRecord(ev_copied, ctx->copy_stream));
+  return 0;
+}
+
+int StageRing::land_slice(uint32_t slot, const void* src, uint64_t src_stride, uint32_t slice_rows, int src_is_device) {
+  const GenoStage& st = stage[slot];
+  uint8_t* mine = st.d_raw + static_cast<uint64_t>(ctx->comm_rank) * slice_rows * st.pitch;
+  PL2_TRY(land(slot, mine, src, src_stride, slice_rows, src_is_device));
+  PL2_TRY(LaunchPadGenotypes(ctx, mine, st.pitch, st.sample_ct, slice_rows, slice_rows, ctx->copy_stream));
+  return CommAllGatherInPlace(ctx, st.d_raw, static_cast<uint64_t>(slice_rows) * st.pitch, ctx->copy_stream);
+}
+
+int StageRing::pad(uint32_t slot, uint32_t cur, bool pad_valid_rows, uint32_t pad_to, uint32_t* padded) {
+  const GenoStage& st = stage[slot];
+  *padded = RoundUpU32(cur, pad_to);
+  if (pad_valid_rows) return LaunchPadGenotypes(ctx, st.d_raw, st.pitch, st.sample_ct, cur, *padded, ctx->copy_stream);
+  if (*padded > cur) return LaunchPadGenotypes(ctx, st.d_raw + static_cast<uint64_t>(cur) * st.pitch, st.pitch, st.sample_ct, 0, *padded - cur, ctx->copy_stream);
+  return 0;
+}
+
+int StageRing::fence(uint32_t slot) {
+  PL2_CUDA_OK(cudaEventRecord(ev_prep_done[slot], ctx->copy_stream));
+  PL2_CUDA_OK(cudaStreamWaitEvent(ctx->stream, ev_prep_done[slot], 0));
+  return 0;
+}
+
+int StageRing::mark_busy(uint32_t slot, cudaStream_t stream) {
+  PL2_CUDA_OK(cudaEventRecord(ev_free[slot], stream));
+  free_pending[slot] = true;
+  return 0;
+}
+
+int StageRing::release_host_source(int src_is_device) {
+  if (!src_is_device) PL2_CUDA_OK(cudaEventSynchronize(ev_copied));  // the kernels keep running
+  return 0;
+}
+
 }  // namespace pl2
 
 using namespace pl2;
@@ -225,25 +299,17 @@ struct Pl2KingJob {
   uint8_t* d_unmapped = nullptr;     // mapped job: the block as the caller gave it, before the gather into position order
   int algo = kPl2KingAlgoTensor;
   TileList tiles;
-  // TS path: two staged blocks + two row-side re-tiled copies, so that the copy / all-gather, padding and
-  // row re-tiling of batch k+1 (prep stream) overlap the tensor kernel of batch k (compute stream).
-  // The other algorithms use buffer 0 on the compute stream only.
-  GenoStage stage[2];
+  StageRing ring;   // TS path: the row re-tiling of each slot also runs on the prep stream
+  GenoStage stage;  // the other algorithms: one block on the compute stream
   uint8_t* d_raw_t[2] = {nullptr, nullptr};  // tensor paths: sample-major copy of the staged block (geno_tile.cuh; split form on the TS path)
-  cudaEvent_t ev_prep_done[2] = {nullptr, nullptr};
-  cudaEvent_t ev_kernel_start[2] = {nullptr, nullptr};  // timing-enabled pair around the tensor kernel (pl2gpu_king_last_kernel_ms)
-  cudaEvent_t ev_kernel_done[2] = {nullptr, nullptr};
+  cudaEvent_t ev_kernel_start[2] = {nullptr, nullptr};  // with the ring's ev_free, the timed pair around the tensor kernel (pl2gpu_king_last_kernel_ms)
   int last_buf = -1;
-  bool kernel_pending[2] = {false, false};
-  uint32_t buf_idx = 0;
   uint32_t* d_planes = nullptr;  // popcount path only
   uint32_t tile_cols = kTileCols;
   int32_t* d_raw_acc = nullptr;
   void* d_out_stage = nullptr;   // bounded staging for host downloads
   uint64_t out_stage_bytes = 0;
   uint64_t variants_added = 0;
-  cudaEvent_t ev_copied = nullptr;     // the caller's buffer has been consumed (prep stream)
-  cudaEvent_t ev_src_ready = nullptr;  // device sources ordered on the compute stream
 };
 
 extern "C" {
@@ -489,11 +555,7 @@ static int KingBegin(Pl2GpuCtx* ctx, uint32_t sample_ct, const uint32_t* order, 
   };
   const bool ts = algo == kPl2KingAlgoTensorTS;
   const uint32_t cap = ClampStageCap(max_variants_per_add);
-  bool ev_ok = cudaEventCreateWithFlags(&job->ev_copied, cudaEventDisableTiming) == cudaSuccess && cudaEventCreateWithFlags(&job->ev_src_ready, cudaEventDisableTiming) == cudaSuccess;
-  for (int b = 0; b < 2 && ev_ok; ++b) {
-    ev_ok = cudaEventCreateWithFlags(&job->ev_prep_done[b], cudaEventDisableTiming) == cudaSuccess && cudaEventCreate(&job->ev_kernel_start[b]) == cudaSuccess && cudaEventCreate(&job->ev_kernel_done[b]) == cudaSuccess;
-  }
-  if (!ev_ok) {
+  if (cudaEventCreate(&job->ev_kernel_start[0]) != cudaSuccess || cudaEventCreate(&job->ev_kernel_start[1]) != cudaSuccess) {
     set_error("pl2gpu_king_begin: cudaEventCreate failed");
     return fail();
   }
@@ -503,20 +565,18 @@ static int KingBegin(Pl2GpuCtx* ctx, uint32_t sample_ct, const uint32_t* order, 
     set_error("pl2gpu_king_begin_mapped: position map upload failed: %s", cudaGetErrorString(cudaGetLastError()));
     return fail();
   }
-  for (int b = 0; b < (ts ? 2 : 1); ++b) {
-    if (StageAlloc(sample_ct, cap, &job->stage[b], ts ? kTsSamplePad : kSamplePad)) return fail();
-    if (order && b == 0 && cudaMalloc(&job->d_unmapped, static_cast<uint64_t>(job->stage[0].variant_cap) * job->stage[0].pitch) != cudaSuccess) {
+  if (ts ? job->ring.alloc(&ctx->c, sample_ct, cap, kTsSamplePad) : StageAlloc(sample_ct, cap, &job->stage, kSamplePad)) return fail();
+  const GenoStage& st0 = ts ? job->ring.stage[0] : job->stage;
+  if (order && cudaMalloc(&job->d_unmapped, static_cast<uint64_t>(st0.variant_cap) * st0.pitch) != cudaSuccess) {
+    cudaGetLastError();
+    set_error("pl2gpu_king_begin_mapped: insufficient device memory for the unmapped genotype block");
+    return fail();
+  }
+  for (int b = 0; b < (ts ? 2 : 1) && algo != kPl2KingAlgoPopcount; ++b) {
+    if (cudaMalloc(&job->d_raw_t[b], static_cast<uint64_t>(st0.sample_ct_padded) * (st0.variant_cap / 4)) != cudaSuccess) {
       cudaGetLastError();
-      set_error("pl2gpu_king_begin_mapped: insufficient device memory for the unmapped genotype block");
+      set_error("pl2gpu_king_begin: insufficient device memory for the sample-major genotype copy");
       return fail();
-    }
-    if (algo != kPl2KingAlgoPopcount) {
-      const uint64_t raw_t_bytes = static_cast<uint64_t>(job->stage[b].sample_ct_padded) * (job->stage[b].variant_cap / 4);
-      if (cudaMalloc(&job->d_raw_t[b], raw_t_bytes) != cudaSuccess) {
-        cudaGetLastError();
-        set_error("pl2gpu_king_begin: insufficient device memory for the sample-major genotype copy");
-        return fail();
-      }
     }
   }
   const uint64_t acc_bytes = static_cast<uint64_t>(job->tiles.tile_ct) * (5ull * job->tile_cols * kTileRows) * sizeof(int32_t);
@@ -530,7 +590,7 @@ static int KingBegin(Pl2GpuCtx* ctx, uint32_t sample_ct, const uint32_t* order, 
     return fail();
   }
   if (algo == kPl2KingAlgoPopcount) {
-    const uint64_t plane_bytes = 3ull * (job->stage[0].variant_cap / 32) * job->stage[0].sample_ct_padded * sizeof(uint32_t);
+    const uint64_t plane_bytes = 3ull * (job->stage.variant_cap / 32) * job->stage.sample_ct_padded * sizeof(uint32_t);
     if (cudaMalloc(&job->d_planes, plane_bytes) != cudaSuccess) {
       cudaGetLastError();
       set_error("pl2gpu_king_begin: insufficient device memory for bit planes");
@@ -566,35 +626,23 @@ int pl2gpu_king_begin_mapped(Pl2GpuCtx* ctx, uint32_t sample_ct, const uint32_t*
   return KingBegin(ctx, sample_ct, order, row_start, row_end, col_end, kPl2KingAlgoTensorTS, max_variants_per_add, job_ptr);
 }
 
-// TS path: the staged block stage[b] holds `cur` variants (rows [0, cur)); pad it, write its sample-major copy
-// and queue the tensor kernel.  Everything up to the kernel runs on the prep stream.
+// TS path: ring slot b holds `cur` variants (rows [0, cur)); pad it, write its sample-major copy and queue the
+// tensor kernel.  Everything up to the kernel runs on the prep stream.
 static int KingTsPrepAndLaunch(Pl2KingJob* job, uint32_t b, uint32_t cur, bool pad_valid_rows) {
   Ctx* c = &job->ctx->c;
-  cudaStream_t prep = c->copy_stream;
-  GenoStage& st = job->stage[b];
-  const uint32_t padded = RoundUpU32(cur, kVariantPad);
-  // pad_valid_rows == false: the valid rows were already padded slice by slice (sharded add); only the tail rows remain
-  if (pad_valid_rows) {
-    PL2_TRY(LaunchPadGenotypes(c, st.d_raw, st.pitch, st.sample_ct, cur, padded, prep));
-  } else if (padded > cur) {
-    PL2_TRY(LaunchPadGenotypes(c, st.d_raw + static_cast<uint64_t>(cur) * st.pitch, st.pitch, st.sample_ct, 0, padded - cur, prep));
-  }
-  if (!job->tiles.tile_ct) {  // nothing to count on this rank: only order later reuse of the buffer behind the gather
-    PL2_CUDA_OK(cudaEventRecord(job->ev_kernel_done[b], prep));
-    job->kernel_pending[b] = true;
-    return 0;
-  }
-  geno_tile_rows_kernel<true><<<dim3(padded / 256, st.sample_ct_padded / 64), 256, 0, prep>>>(st.d_raw, st.pitch, padded / 32, 0, job->d_raw_t[b]);
+  const GenoStage& st = job->ring.stage[b];
+  uint32_t padded;
+  PL2_TRY(job->ring.pad(b, cur, pad_valid_rows, kVariantPad, &padded));
+  if (!job->tiles.tile_ct) return job->ring.mark_busy(b, c->copy_stream);  // nothing to count on this rank
+  geno_tile_rows_kernel<true><<<dim3(padded / 256, st.sample_ct_padded / 64), 256, 0, c->copy_stream>>>(st.d_raw, st.pitch, padded / 32, 0, job->d_raw_t[b]);
   c->launches++;
   PL2_CUDA_OK(cudaGetLastError());
-  PL2_CUDA_OK(cudaEventRecord(job->ev_prep_done[b], prep));
-  PL2_CUDA_OK(cudaStreamWaitEvent(c->stream, job->ev_prep_done[b], 0));
+  PL2_TRY(job->ring.fence(b));
   PL2_CUDA_OK(cudaEventRecord(job->ev_kernel_start[b], c->stream));
   king_b1_kernel<<<job->tiles.tile_ct, kKwThreads, kKb1SmemBytes, c->stream>>>(job->d_raw_t[b], padded, job->tiles.d_tile_order, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->d_raw_acc);
   c->launches++;
   PL2_CUDA_OK(cudaGetLastError());
-  PL2_CUDA_OK(cudaEventRecord(job->ev_kernel_done[b], c->stream));
-  job->kernel_pending[b] = true;
+  PL2_TRY(job->ring.mark_busy(b, c->stream));
   job->last_buf = static_cast<int>(b);
   return 0;
 }
@@ -613,50 +661,38 @@ int pl2gpu_king_add_variants(Pl2KingJob* job, const void* genovecs, uint64_t var
   }
   const uint8_t* src = static_cast<const uint8_t*>(genovecs);
   const bool ts = job->algo == kPl2KingAlgoTensorTS;
-  uint32_t done = 0;
-  while (done < variant_ct) {
-    uint32_t cur = variant_ct - done;
-    if (cur > job->stage[0].variant_cap) cur = job->stage[0].variant_cap;
+  const uint32_t cap = (ts ? job->ring.stage[0] : job->stage).variant_cap;
+  for (uint32_t done = 0; done < variant_ct;) {
+    const uint32_t cur = std::min(cap, variant_ct - done);
     const uint8_t* src_cur = src + static_cast<uint64_t>(done) * variant_stride_bytes;
-    if (ts && job->tiles.tile_ct) {
-      // Double-buffered: copy + pad + row re-tiling on the prep stream while the previous batch's tensor
-      // kernel (which reads the OTHER staged block through its tensor map) is still running.
-      const uint32_t b = job->buf_idx;
-      job->buf_idx ^= 1;
-      GenoStage& st = job->stage[b];
-      cudaStream_t prep = c->copy_stream;
-      if (job->kernel_pending[b]) PL2_CUDA_OK(cudaStreamWaitEvent(prep, job->ev_kernel_done[b], 0));
-      if (src_is_device == 1) {
-        // device source produced by work the caller ordered on the context's stream
-        PL2_CUDA_OK(cudaEventRecord(job->ev_src_ready, c->stream));
-        PL2_CUDA_OK(cudaStreamWaitEvent(prep, job->ev_src_ready, 0));
-      }
+    if (ts) {
+      uint32_t b;
+      PL2_TRY(job->ring.acquire(src_is_device, &b));
+      const GenoStage& st = job->ring.stage[b];
       // a mapped job lands the caller's rows in d_unmapped and gathers them into position order (the prep stream runs
-      // copy and gather in turn, so one unmapped block serves both staged buffers)
-      uint8_t* const land = job->d_order ? job->d_unmapped : st.d_raw;
-      PL2_CUDA_OK(cudaMemcpy2DAsync(land, st.pitch, src_cur, variant_stride_bytes, DivUpU32(st.sample_ct, 4), cur, src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, prep));
-      PL2_CUDA_OK(cudaEventRecord(job->ev_copied, prep));
-      for (uint32_t v0 = 0; job->d_order && v0 < cur; v0 += 32768) {  // grid.y is at most 65,535 rows
+      // copy and gather in turn, so one unmapped block serves both slots); without tiles nothing reads the slot
+      PL2_TRY(job->ring.land(b, job->d_unmapped, src_cur, variant_stride_bytes, cur, src_is_device));
+      for (uint32_t v0 = 0; job->d_order && job->tiles.tile_ct && v0 < cur; v0 += 32768) {  // grid.y is at most 65,535 rows
         const uint32_t rows = std::min(cur - v0, 32768u);
-        geno_gather_kernel<<<dim3(DivUpU32(st.pitch, 256), rows), 256, 0, prep>>>(land + static_cast<uint64_t>(v0) * st.pitch, st.pitch, st.d_raw + static_cast<uint64_t>(v0) * st.pitch, st.pitch, job->d_order, st.sample_ct);
+        geno_gather_kernel<<<dim3(DivUpU32(st.pitch, 256), rows), 256, 0, c->copy_stream>>>(job->d_unmapped + static_cast<uint64_t>(v0) * st.pitch, st.pitch, st.d_raw + static_cast<uint64_t>(v0) * st.pitch, st.pitch, job->d_order, st.sample_ct);
         c->launches++;
         PL2_CUDA_OK(cudaGetLastError());
       }
       PL2_TRY(KingTsPrepAndLaunch(job, b, cur, true));
-      if (!src_is_device) PL2_CUDA_OK(cudaEventSynchronize(job->ev_copied));  // the caller may reuse its buffer; the kernels keep running
+      PL2_TRY(job->ring.release_host_source(src_is_device));
     } else {
       uint32_t padded = 0;
-      PL2_TRY(StageUpload(c, &job->stage[0], src_cur, variant_stride_bytes, cur, src_is_device, &padded));
+      PL2_TRY(StageUpload(c, &job->stage, src_cur, variant_stride_bytes, cur, src_is_device, &padded));
       if (job->tiles.tile_ct) {
         if (job->algo == kPl2KingAlgoPopcount) {
           const uint32_t word_ct = padded / 32;
-          const uint64_t warps = static_cast<uint64_t>(job->stage[0].sample_ct_padded / 32) * word_ct;
-          split_transpose_kernel<<<static_cast<uint32_t>(DivUpU64(warps, 8)), 256, 0, c->stream>>>(job->stage[0].d_raw, job->stage[0].pitch, job->stage[0].sample_ct_padded, word_ct, job->d_planes);
+          const uint64_t warps = static_cast<uint64_t>(job->stage.sample_ct_padded / 32) * word_ct;
+          split_transpose_kernel<<<static_cast<uint32_t>(DivUpU64(warps, 8)), 256, 0, c->stream>>>(job->stage.d_raw, job->stage.pitch, job->stage.sample_ct_padded, word_ct, job->d_planes);
           c->launches++;
-          king_popc_kernel<<<job->tiles.tile_ct * 2, 256, 0, c->stream>>>(job->d_planes, job->stage[0].sample_ct_padded, word_ct, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->d_raw_acc);
+          king_popc_kernel<<<job->tiles.tile_ct * 2, 256, 0, c->stream>>>(job->d_planes, job->stage.sample_ct_padded, word_ct, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->d_raw_acc);
           c->launches++;
         } else {
-          const GenoStage& st = job->stage[0];
+          const GenoStage& st = job->stage;
           geno_tile_rows_kernel<<<dim3(padded / 64, st.sample_ct_padded / 64), 256, 0, c->stream>>>(st.d_raw, st.pitch, padded / 32, 0, job->d_raw_t[0]);
           c->launches++;
           king_wg_kernel<kTileCols><<<2 * job->tiles.tile_ct, kKwThreads, KingWgShape<kTileCols>::kSmemBytes, c->stream>>>(job->d_raw_t[0], padded, job->tiles.d_tile_order, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->d_raw_acc);
@@ -689,8 +725,8 @@ int pl2gpu_king_add_variants_sharded(Pl2KingJob* job, const void* slice, uint64_
     return 1;
   }
   const uint64_t total64 = static_cast<uint64_t>(slice_variant_ct) * c->comm_world;
-  if (!slice_variant_ct || total64 > job->stage[0].variant_cap) {
-    set_error("pl2gpu_king_add_variants_sharded: %u variants x %d ranks exceed the stage capacity %u", slice_variant_ct, c->comm_world, job->stage[0].variant_cap);
+  if (!slice_variant_ct || total64 > job->ring.stage[0].variant_cap) {
+    set_error("pl2gpu_king_add_variants_sharded: %u variants x %d ranks exceed the stage capacity %u", slice_variant_ct, c->comm_world, job->ring.stage[0].variant_cap);
     return 1;
   }
   if (variant_stride_bytes < DivUpU32(job->sample_ct, 4)) {
@@ -698,24 +734,11 @@ int pl2gpu_king_add_variants_sharded(Pl2KingJob* job, const void* slice, uint64_
     return 1;
   }
   const uint32_t total = static_cast<uint32_t>(total64);
-  const uint32_t b = job->buf_idx;
-  job->buf_idx ^= 1;
-  GenoStage& st = job->stage[b];
-  cudaStream_t prep = c->copy_stream;
-  if (job->kernel_pending[b]) PL2_CUDA_OK(cudaStreamWaitEvent(prep, job->ev_kernel_done[b], 0));
-  if (src_is_device == 1) {
-    PL2_CUDA_OK(cudaEventRecord(job->ev_src_ready, c->stream));
-    PL2_CUDA_OK(cudaStreamWaitEvent(prep, job->ev_src_ready, 0));
-  }
-  // this rank's variants land at rows [rank * slice, (rank + 1) * slice) of the staged block, are padded
-  // there, and ONE in-place all-gather of the genotype column tile makes the block complete on every GPU
-  uint8_t* mine = st.d_raw + static_cast<uint64_t>(c->comm_rank) * slice_variant_ct * st.pitch;
-  PL2_CUDA_OK(cudaMemcpy2DAsync(mine, st.pitch, slice, variant_stride_bytes, DivUpU32(st.sample_ct, 4), slice_variant_ct, src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, prep));
-  PL2_CUDA_OK(cudaEventRecord(job->ev_copied, prep));
-  PL2_TRY(LaunchPadGenotypes(c, mine, st.pitch, st.sample_ct, slice_variant_ct, slice_variant_ct, prep));
-  PL2_TRY(CommAllGatherInPlace(c, st.d_raw, static_cast<uint64_t>(slice_variant_ct) * st.pitch, prep));
+  uint32_t b;
+  PL2_TRY(job->ring.acquire(src_is_device, &b));
+  PL2_TRY(job->ring.land_slice(b, slice, variant_stride_bytes, slice_variant_ct, src_is_device));
   PL2_TRY(KingTsPrepAndLaunch(job, b, total, false));
-  if (!src_is_device) PL2_CUDA_OK(cudaEventSynchronize(job->ev_copied));
+  PL2_TRY(job->ring.release_host_source(src_is_device));
   job->variants_added += total;
   return 0;
 }
@@ -868,8 +891,8 @@ int pl2gpu_king_last_kernel_ms(Pl2KingJob* job, float* ms) {
     return 1;
   }
   PL2_CUDA_OK(cudaSetDevice(job->ctx->c.device));
-  PL2_CUDA_OK(cudaEventSynchronize(job->ev_kernel_done[job->last_buf]));
-  PL2_CUDA_OK(cudaEventElapsedTime(ms, job->ev_kernel_start[job->last_buf], job->ev_kernel_done[job->last_buf]));
+  PL2_CUDA_OK(cudaEventSynchronize(job->ring.ev_free[job->last_buf]));
+  PL2_CUDA_OK(cudaEventElapsedTime(ms, job->ev_kernel_start[job->last_buf], job->ring.ev_free[job->last_buf]));
   return 0;
 }
 
@@ -880,14 +903,11 @@ int pl2gpu_king_end(Pl2KingJob* job) {
     cudaStreamSynchronize(job->ctx->c.stream);
     if (job->ctx->c.copy_stream) cudaStreamSynchronize(job->ctx->c.copy_stream);
   }
-  if (job->ev_copied) cudaEventDestroy(job->ev_copied);
-  if (job->ev_src_ready) cudaEventDestroy(job->ev_src_ready);
   FreeTileList(&job->tiles);
+  job->ring.free();
+  StageFree(&job->stage);
   for (int b = 0; b < 2; ++b) {
-    if (job->ev_prep_done[b]) cudaEventDestroy(job->ev_prep_done[b]);
     if (job->ev_kernel_start[b]) cudaEventDestroy(job->ev_kernel_start[b]);
-    if (job->ev_kernel_done[b]) cudaEventDestroy(job->ev_kernel_done[b]);
-    StageFree(&job->stage[b]);
     cudaFree(job->d_raw_t[b]);
   }
   cudaFree(job->d_order);
