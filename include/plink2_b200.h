@@ -287,6 +287,29 @@ int pl2gpu_score_add_variants(Pl2ScoreJob* job, const void* genovecs, uint64_t v
 int pl2gpu_score_get(Pl2ScoreJob* job, double* score_sums, uint64_t* named_dosage_sums, uint32_t* missing_cts);
 /* Idempotent; accepts NULL. */
 int pl2gpu_score_end(Pl2ScoreJob* job);
+/* Sex chromosomes and MT (CalcScoreThread :6682-6845, per-entry bookkeeping in ScoreReport :7792-8037).  Each entry
+ * of pl2gpu_score_add_variants_ploidy has a ploidy class:
+ *   kPl2ScoreDiploid           every sample uses weights4_diploid (autosomes, XY, chrX under --xchr-model 2);
+ *   kPl2ScoreHaploidAll        every sample uses weights4_haploid (MT);
+ *   kPl2ScoreChrY              males use weights4_haploid, unknown-sex samples weights4_diploid with no dosage counted
+ *                              (the reference zeroes every nonmale's chrY dosage), females are skipped (no weight,
+ *                              dosage or missing call); missing calls of males and unknown-sex samples count haploid;
+ *   kPl2ScoreChrXMaleHaploid   males use weights4_haploid, nonmales weights4_diploid (chrX under --xchr-model 1).
+ * Both tables are laid out [entry][score_ct][4] as weights4 above; weights4_haploid may be NULL when every entry is
+ * diploid.  Entries of the last three classes must be additive (named_dosages 0x24 / 0x06), and chrY / chrX entries
+ * need the sample sexes, given once per job by pl2gpu_score_set_sex (sample_sex[sample]: 0 unknown, 1 male,
+ * 2 female).  pl2gpu_score_get_ploidy returns the score sums as pl2gpu_score_get, the named-allele dosage sums in
+ * half allele units (a haploid call of the named allele counts 1, a diploid copy 2; ddosage / 16384 in the reference's
+ * terms), and the missing calls of samples scored as diploid and as haploid (ALLELE_CT = DENOM - 2 x diploid -
+ * haploid, :8581).  Runs of consecutive diploid entries are scored exactly as pl2gpu_score_add_variants scores them
+ * (a diploid-only job gives bit-identical sums); the other classes go through a kernel that picks each sample's table
+ * from the sex masks, with partials reduced in the same fixed order.  After entries of the other classes,
+ * pl2gpu_score_get's dosage sums and missing counts cover only part of them: read them with pl2gpu_score_get_ploidy. */
+enum { kPl2ScoreDiploid = 0, kPl2ScoreHaploidAll = 1, kPl2ScoreChrY = 2, kPl2ScoreChrXMaleHaploid = 3 };
+int pl2gpu_score_set_sex(Pl2ScoreJob* job, const uint8_t* sample_sex);
+int pl2gpu_score_add_variants_ploidy(Pl2ScoreJob* job, const void* genovecs, uint64_t variant_stride_bytes, uint32_t variant_ct, int src_is_device, const uint8_t* ploidy_classes, const double* weights4_diploid,
+                                     const double* weights4_haploid, const uint8_t* named_dosages);
+int pl2gpu_score_get_ploidy(Pl2ScoreJob* job, double* score_sums, uint64_t* named_half_dosage_sums, uint32_t* missing_diploid_cts, uint32_t* missing_haploid_cts);
 
 /* ---- measured tensor peak: two warpgroups per SM issue back-to-back wgmmas with A fragments in registers and B in
  * shared memory, as the KING/GRM kernels use them, for at least min_seconds.  form 1: int8 (M = 64, N = n_cols in

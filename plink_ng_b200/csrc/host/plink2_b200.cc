@@ -100,6 +100,8 @@ struct Cmd {
   bool score_header = false, score_header_read = false, score_no_meanimpute = false, score_zs = false, score_center = false, score_varstd = false, score_dominant = false, score_recessive = false, score_list_variants = false;
   bool sc_fid_maybe = true, sc_fid = false, sc_sid_maybe = true, sc_sid = false, sc_pheno1 = false, sc_phenos = true, sc_nallele = true, sc_denom = false, sc_dosagesum = true, sc_avgs = true, sc_sums = false;
   std::string vscore_file;                // --variant-score <file> ['zs'] ['cols=' chrom,pos,ref,alt,maybeprovref,provref,altfreq]
+  uint32_t xchr_model = 2;                // --xchr-model {1,2}: chrX males haploid (1) or coded 0..2 like an autosome (2)
+  bool xchr_model_given = false;
   bool vscore_zs = false, vs_chrom = true, vs_pos = true, vs_ref = true, vs_alt = true, vs_maybeprovref = true, vs_provref = false, vs_altfreq = false;
   std::string king_cutoff_table;          // --king-cutoff-table <.kin0 file> <threshold>
   double king_cutoff_table_thresh = -1;
@@ -481,6 +483,12 @@ int ParseArgs(int argc, char** argv, Cmd* c) {
     } else if (flag == "--score-col-nums" || flag == "--vscore-col-nums") {
       const bool vs = flag == "--vscore-col-nums";
       if (int rc = ParseColNums(flag, prm, nparam, vs ? &c->vscore_col_nums : &c->score_col_nums)) return rc;
+    } else if (flag == "--xchr-model") {
+      if (nparam != 1) return Usage("--xchr-model requires exactly one argument.");
+      const std::string m = prm[0];
+      if (m.size() != 1 || m[0] < '0' || m[0] > '2') return Usage(("Invalid --xchr-model argument '" + m + "'.").c_str());
+      c->xchr_model = static_cast<uint32_t>(m[0] - '0');
+      c->xchr_model_given = true;
     } else if (flag == "--variant-score" || flag == "--vscore") {
       if (nparam < 1) return Usage("--variant-score requires a filename.");
       c->vscore_file = prm[0];
@@ -743,6 +751,11 @@ int ParseArgs(int argc, char** argv, Cmd* c) {
   // --score / --score-col-nums / --vscore-col-nums, in the reference's order (plink2.cc:11573-11582, :12566-12574,
   // :12955; column overlaps 2.0/plink2_matrix_calc.cc:7186-7234)
   if (!c->vscore_col_nums.empty() && c->vscore_file.empty()) return Usage("--vscore-col-nums must be used with --variant-score.");
+  if (c->xchr_model_given && c->score_file.empty() && c->vscore_file.empty()) return Usage("--xchr-model must be used with --glm, --score[-list], or\n--variant-score.");
+  if (c->xchr_model_given && c->xchr_model == 0) {
+    logprintf("Error: --xchr-model 0 (skip chrX) is not supported by plink2_b200; use --not-chr X to leave chrX out.\n");
+    return kRetNotYetSupported;
+  }
   if (!c->score_col_nums.empty()) {
     if (c->score_file.empty()) return Usage("--score-col-nums must be used with --score[-list].");
     if (c->score_numeric_params == 3) return Usage("--score-col-nums cannot be used when three numeric arguments are\nprovided to --score.");
@@ -2966,10 +2979,18 @@ bool TypePheno(const std::string& name, const std::vector<std::string>& tok, Phe
   return any;
 }
 
-// `--score` (ScoreReport, 2.0/plink2_matrix_calc.cc:6892-9270) for diploid hard calls: default report columns plus
+std::vector<uint32_t> AllVariants(const Dataset& ds) {
+  std::vector<uint32_t> vidx(ds.variants.size());
+  for (uint32_t v = 0; v < vidx.size(); ++v) vidx[v] = v;
+  return vidx;
+}
+int SexChrRefFreqs(Dataset* ds, Pl2GpuCtx* ctx, const std::vector<uint32_t>& vidx, std::vector<double>* ref_freqs);
+
+// `--score` (ScoreReport, 2.0/plink2_matrix_calc.cc:6892-9270) for hard calls: default report columns plus
 // denom / scoresums, 'header' / 'header-read', 'no-mean-imputation', and any number of coefficient columns
-// (--score-col-nums).  The per-sample sums of every column come from one device pass (pl2gpu_score_*); the file
-// parsing, allele matching, mean-imputation weights and the report are here.
+// (--score-col-nums).  chrX, chrY and MT entries are scored with the reference's sex-dependent ploidy (--xchr-model 2:
+// chrX like an autosome; 1: chrX males haploid).  The per-sample sums of every column come from one device pass
+// (pl2gpu_score_*); the file parsing, allele matching, mean-imputation weights and the report are here.
 int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   const SampleInfo& S = ds->samples;
   const VariantInfo& V = ds->variants;
@@ -2993,6 +3014,7 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   std::vector<Entry> entries;
   std::vector<double> coefs;
   std::vector<uint8_t> seen(2ull * V.size(), 0);
+  const bool y_prohibited = !c.score_no_meanimpute && std::find(S.sex.begin(), S.sex.end(), 0) != S.sex.end();
   uint64_t missing_id = 0, missing_allele = 0;
   // coefficient columns in file order (1-based); without --score-col-nums the one column --score names
   const std::vector<uint32_t> score_cols = c.score_col_nums.empty() ? std::vector<uint32_t>{c.score_coef_col} : c.score_col_nums;
@@ -3064,9 +3086,19 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
       }
       coefs.push_back(coef);
     }
-    if (V.chr_code[v] == 23 || V.chr_code[v] == 24 || V.chr_code[v] == 26) {
-      logprintf("Error: --score on chrX / chrY / chrMT variants (sex-dependent ploidy) is not supported by plink2_b200 yet ('%s').\n", id.c_str());
-      return kRetNotYetSupported;
+    // the reference's refusals for haploid chromosomes (:7794-7814)
+    const uint32_t chr = V.chr_code[v];
+    if ((chr == 23 || chr == 24 || chr == 26) && (c.score_dominant || c.score_recessive)) {
+      logprintf("Error: --score[-list] 'dominant' and 'recessive' modifiers cannot be used with\nhaploid chromosomes.\n");
+      return kRetInconsistentInput;
+    }
+    if ((chr == 23 || chr == 26) && c.score_varstd) {
+      logprintf("Error: --score[-list] 'variance-standardize' cannot be used with chrX or MT.\n");
+      return kRetInconsistentInput;
+    }
+    if (chr == 24 && y_prohibited) {
+      logprintf("Error: When both chrY variants and unknown-sex samples are present,\n--score[-list] can only be run with the 'no-mean-imputation' modifier.\n");
+      return kRetInconsistentInput;
     }
     entries.push_back({v, aidx, entries.size()});
   }
@@ -3099,8 +3131,18 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
     int rc = 0;
     bool have = FounderRefFreqs(ds, ctx, vidx, &ref_freqs, &rc, true);
     if (rc) return rc;
+    if ((rc = SexChrRefFreqs(ds, ctx, vidx, &ref_freqs))) return rc;
     ApplyReadFreq(*ds, vidx, &ref_freqs, have);
   }
+  // ploidy class of each entry (pl2gpu_score_add_variants_ploidy); a job with diploid entries only keeps the plain path
+  auto ploidy_class = [&](uint32_t v) -> uint8_t {
+    const uint32_t chr = V.chr_code[v];
+    if (chr == 24) return kPl2ScoreChrY;
+    if (chr == 26) return kPl2ScoreHaploidAll;
+    return (chr == 23 && c.xchr_model == 1) ? kPl2ScoreChrXMaleHaploid : kPl2ScoreDiploid;
+  };
+  bool ploidy_job = false;
+  for (const Entry& e : entries) ploidy_job = ploidy_job || ploidy_class(e.v) != kPl2ScoreDiploid;
   Pl2ScoreJob* job = nullptr;
   if (score_ct == 1) {  // the one-column job (same device work as pl2gpu_score_begin_cols with one column)
     if (pl2gpu_score_begin(ctx, n, &job)) return GpuFail("pl2gpu_score_begin");
@@ -3111,11 +3153,12 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
     Pl2ScoreJob* j;
     ~JobGuard() { pl2gpu_score_end(j); }
   } guard{job};
+  if (ploidy_job && pl2gpu_score_set_sex(job, S.sex.data())) return GpuFail("pl2gpu_score_set_sex");
   BlockStreamer bs(ds, &vidx, n, 16384);
   if (!bs.Init()) return GpuFail("pl2gpu_host_alloc");
-  std::vector<double> w4;
-  std::vector<uint8_t> d4;
-  std::vector<int64_t> repeat_miss(n, 0);
+  std::vector<double> w4, w4h;  // diploid and haploid tables
+  std::vector<uint8_t> d4, cls;
+  std::vector<int64_t> repeat_miss(n, 0), repeat_miss_hap(n, 0);
   size_t base = 0;
   for (;;) {
     const int got = bs.Next(&err);
@@ -3125,27 +3168,32 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
     }
     if (!got) break;
     w4.resize(4ull * score_ct * got);
+    w4h.resize(4ull * score_ct * got);
     d4.resize(got);
+    cls.resize(got);
     for (int k = 0; k < got; ++k) {
       const Entry& e = entries[base + k];
+      const uint8_t pc = cls[k] = ploidy_class(e.v);
       const double f_named = e.aidx ? (1.0 - ref_freqs[base + k]) : ref_freqs[base + k];
       // genotype code = ALT allele count; named-allele dosage of codes 0, 1, 2.  The tables below do not depend on
       // the column; each column scales them by its coefficient.  'center' / 'variance-standardize'
-      // (:8003-8033): dosage x slope + intercept with intercept = -2 f slope and slope = 1 / sqrt(2 f (1 - f)) (0 when
-      // the variance is not above 2^-44).  A missing call contributes 2 f slope WITHOUT the intercept in the reference
-      // (missing_effect, :6756-6762) - kept, since the outputs are compared with its files.
+      // (:8003-8033): dosage x slope + intercept with intercept = -p f slope and slope = 1 / sqrt(p / 2 x 2 f (1 - f))
+      // (0 when the variance is not above 2^-44), p the variant's ploidy: 1 on chrY and MT, else 2 (chrX too, whatever
+      // the model).  A missing call contributes (sample ploidy) f slope WITHOUT the intercept in the reference
+      // (missing_effect, :6756-6762, :6795-6836) - kept, since the outputs are compared with its files.
       const uint32_t d0 = e.aidx ? 0 : 2, d2 = e.aidx ? 2 : 0;
+      const bool haploid_variant = pc == kPl2ScoreChrY || pc == kPl2ScoreHaploidAll;
       double slope = 1.0, icpt = 0.0;
       if (c.score_center) {
         if (c.score_varstd) {
-          const double variance = 2.0 * f_named * (1.0 - f_named);
+          const double variance = (haploid_variant ? 0.5 : 1.0) * (2.0 * f_named * (1.0 - f_named));
           if (!(variance > 1.0 / 17592186044416.0)) {
             slope = 0.0;  // the reference additionally insists that such a variant is monomorphic (:8013-8027); a weight of 0 scores it the same
           } else {
             slope = 1.0 / sqrt(variance);
           }
         }
-        icpt = (-2.0 * f_named) * slope;
+        icpt = ((haploid_variant ? -1.0 : -2.0) * f_named) * slope;
       }
       // 'dominant' / 'recessive' (:6747-6762): copies -> min(copies, 1) / max(copies - 1, 0), a missing call -> ONE x f
       uint32_t e0 = d0, e1 = 1, e2 = d2;
@@ -3158,6 +3206,8 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
         miss_dosage = f_named;
       }
       const double t0 = static_cast<double>(e0) * slope + icpt, t1 = static_cast<double>(e1) * slope + icpt, t2 = static_cast<double>(e2) * slope + icpt, t3 = miss_dosage * slope;
+      // a haploid sample (chrY nonfemales, MT, chrX males under --xchr-model 1) holds half the dosage of each code
+      const double h0 = (0.5 * e0) * slope + icpt, h1 = (0.5 * e1) * slope + icpt, h2 = (0.5 * e2) * slope + icpt, h3 = f_named * slope;
       for (uint32_t j = 0; j < score_ct; ++j) {
         const double coef = coefs[e.coef_row * score_ct + j];
         double* w = &w4[4ull * (static_cast<uint64_t>(k) * score_ct + j)];
@@ -3165,28 +3215,54 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
         w[1] = coef * t1;
         w[2] = coef * t2;
         w[3] = c.score_no_meanimpute ? 0.0 : coef * t3;
+        if (pc == kPl2ScoreChrY) {  // the first table serves unknown-sex samples, whose chrY dosage the reference zeroes
+          w[0] = w[1] = w[2] = coef * icpt;
+          w[3] = c.score_no_meanimpute ? 0.0 : coef * h3;
+        }
+        double* wh = &w4h[4ull * (static_cast<uint64_t>(k) * score_ct + j)];
+        wh[0] = coef * h0;
+        wh[1] = coef * h1;
+        wh[2] = coef * h2;
+        wh[3] = c.score_no_meanimpute ? 0.0 : coef * h3;
       }
       d4[k] = static_cast<uint8_t>(e0 | (e1 << 2) | (e2 << 4));
       // a file that names both alleles of a variant (PC projection with allele weights): the device counts the missing
       // calls of both entries, the reference counts them once per variant (:7788), so the second entry's are taken
-      // back out here
+      // back out here, from the diploid or haploid count the sample's class put them in
       if (base + k > 0 && entries[base + k - 1].v == e.v) {
         const uint64_t* row = bs.buf + static_cast<uint64_t>(k) * bs.words;
         for (uint32_t w = 0; w < bs.words; ++w) {
           uint64_t ms = row[w] & (row[w] >> 1) & 0x5555555555555555ull;
           if (32ull * (w + 1) > n) ms &= (1ull << (2 * (n - 32 * w))) - 1;
-          for (; ms; ms &= ms - 1) --repeat_miss[32 * w + __builtin_ctzll(ms) / 2];
+          for (; ms; ms &= ms - 1) {
+            const uint32_t s = 32 * w + __builtin_ctzll(ms) / 2;
+            const uint8_t sex = S.sex[s];
+            if (pc == kPl2ScoreDiploid || (pc == kPl2ScoreChrXMaleHaploid && sex != 1)) --repeat_miss[s];
+            else if (pc != kPl2ScoreChrY || sex != 2) --repeat_miss_hap[s];  // chrY females are not counted
+          }
         }
       }
     }
-    if (pl2gpu_score_add_variants(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0, w4.data(), d4.data())) return GpuFail("pl2gpu_score_add_variants");
+    if (ploidy_job) {
+      if (pl2gpu_score_add_variants_ploidy(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0, cls.data(), w4.data(), w4h.data(), d4.data())) return GpuFail("pl2gpu_score_add_variants_ploidy");
+    } else if (pl2gpu_score_add_variants(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0, w4.data(), d4.data())) {
+      return GpuFail("pl2gpu_score_add_variants");
+    }
     base += static_cast<size_t>(got);
   }
   std::vector<double> sums(static_cast<uint64_t>(n) * score_ct);  // [sample][score_ct]
-  std::vector<uint64_t> dos(n);
-  std::vector<uint32_t> miss(n);
-  if (pl2gpu_score_get(job, sums.data(), dos.data(), miss.data())) return GpuFail("pl2gpu_score_get");
-  for (uint32_t k = 0; k < n; ++k) miss[k] = static_cast<uint32_t>(miss[k] + repeat_miss[k]);
+  std::vector<uint64_t> hdos(n);                                  // named-allele dosage sums in half allele units
+  std::vector<uint32_t> miss(n), miss_hap(n, 0);
+  if (ploidy_job) {
+    if (pl2gpu_score_get_ploidy(job, sums.data(), hdos.data(), miss.data(), miss_hap.data())) return GpuFail("pl2gpu_score_get_ploidy");
+  } else {
+    if (pl2gpu_score_get(job, sums.data(), hdos.data(), miss.data())) return GpuFail("pl2gpu_score_get");
+    for (uint64_t& d : hdos) d *= 2;
+  }
+  for (uint32_t k = 0; k < n; ++k) {
+    miss[k] = static_cast<uint32_t>(miss[k] + repeat_miss[k]);
+    miss_hap[k] = static_cast<uint32_t>(miss_hap[k] + repeat_miss_hap[k]);
+  }
   logprintf("--score: %zu variant%s processed.\n", entries.size(), entries.size() == 1 ? "" : "s");
   if (c.score_list_variants) {
     OutFile fv;
@@ -3227,14 +3303,22 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
     for (const std::string& nm : score_names) hdr += "\t" + nm + "_SUM";
   hdr += "\n";
   f.Puts(hdr.c_str());
-  uint32_t scored_variants = 0;
-  for (size_t k = 0; k < entries.size(); ++k) scored_variants += !k || entries[k - 1].v != entries[k].v;
-  const uint32_t denom_full = 2 * scored_variants;
+  // DENOM = base + nonfemale x chrY variants - male x chrX variants under --xchr-model 1 (:8581); base counts 2 per
+  // diploid variant and 1 per MT variant
+  uint32_t denom_base = 0, y_incr = 0, x_decr = 0;
+  for (size_t k = 0; k < entries.size(); ++k) {
+    if (k && entries[k - 1].v == entries[k].v) continue;
+    const uint8_t pc = ploidy_class(entries[k].v);
+    denom_base += pc == kPl2ScoreHaploidAll ? 1 : pc == kPl2ScoreChrY ? 0 : 2;
+    y_incr += pc == kPl2ScoreChrY;
+    x_decr += pc == kPl2ScoreChrXMaleHaploid;
+  }
   char num[64];
   for (uint32_t k = 0; k < n; ++k) {
     std::string row = FmtId(S, k, idf);
     for (const PhenoOut& po : phenos) row += "\t" + po.text[k];
-    const uint32_t nallele = denom_full - 2 * miss[k];
+    const uint32_t denom_full = denom_base + (S.sex[k] != 2 ? y_incr : 0) - (S.sex[k] == 1 ? x_decr : 0);
+    const uint32_t nallele = denom_full - 2 * miss[k] - miss_hap[k];
     const uint32_t denom = c.score_no_meanimpute ? nallele : denom_full;
     if (c.sc_nallele) {
       *u32toa(nallele, num) = '\0';
@@ -3244,7 +3328,7 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
       *u32toa(denom, num) = '\0';
       row += std::string("\t") + num;
     }
-    if (c.sc_dosagesum) row += "\t" + std::to_string(dos[k]);
+    if (c.sc_dosagesum) row += "\t" + std::to_string(hdos[k] / 2) + ((hdos[k] & 1) ? ".5" : "");
     const double* ks = &sums[static_cast<uint64_t>(k) * score_ct];
     if (c.sc_avgs) {
       for (uint32_t j = 0; j < score_ct; ++j) {
@@ -3269,10 +3353,17 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
 // `--variant-score` (VscoreReport, 2.0/plink2_matrix_calc.cc:9274-10100): sample weights from a file ([#FID] IID [SID]
 // + named weight columns, or headerless FID IID + VSCORE1..), per variant the weighted sum of ALT dosages with a missing
 // call replaced by 2 x ALT frequency.  The sums are one pass of the approx-PCA tensor tile path (pl2gpu_pca_vscore).
+// chrY and MT dosages count half (slope 0.5), chrY only for males, and chrX males count half under --xchr-model 1
+// (VscoreThread :8831-8868, :9158-9200): the product is linear in the weights, so those variants run as jobs of their
+// own with the weight matrix rescaled or masked that way.
 int RunVscore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   const SampleInfo& S = ds->samples;
   const VariantInfo& V = ds->variants;
   const uint32_t n = S.size(), m = V.size();
+  if (std::find(V.chr_code.begin(), V.chr_code.end(), 24u) != V.chr_code.end() && std::find(S.sex.begin(), S.sex.end(), 0) != S.sex.end()) {  // :9297-9301
+    logprintf("Error: When chrY is present, --variant-score cannot be used with unknown-sex\nsamples.\n");
+    return kRetInconsistentInput;
+  }
   std::vector<std::string> lines;
   std::string err;
   if (!ReadLines(c.vscore_file, &lines, &err)) {
@@ -3390,51 +3481,65 @@ int RunVscore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
     return kRetDegenerateData;
   }
   logprintf("--variant-score: %u score-vector%s loaded for %u sample%s.\n", cols, cols == 1 ? "" : "s", loaded, loaded == 1 ? "" : "s");
-  for (uint32_t v = 0; v < m; ++v) {
-    if (V.chr_code[v] == 23 || V.chr_code[v] == 24 || V.chr_code[v] == 26) {
-      logprintf("Error: --variant-score on chrX / chrY / chrMT variants (sex-dependent ploidy) is not supported by plink2_b200 yet.\n");
-      return kRetNotYetSupported;
-    }
-  }
-  std::vector<uint32_t> vidx(m);
-  for (uint32_t v = 0; v < m; ++v) vidx[v] = v;
+  const std::vector<uint32_t> vidx = AllVariants(*ds);
   std::vector<double> ref_freqs;
   int rc = 0;
   {
     const bool have = FounderRefFreqs(ds, ctx, vidx, &ref_freqs, &rc, true);
     if (rc) return rc;
+    if ((rc = SexChrRefFreqs(ds, ctx, vidx, &ref_freqs))) return rc;
     ApplyReadFreq(*ds, vidx, &ref_freqs, have);
   }
-  // the matrix is kept resident in pieces that fit comfortably; every piece is one pl2gpu_pca job
+  // variant classes by weight matrix: 0 as given (autosomes, XY, chrX under --xchr-model 2), 1 chrX under
+  // --xchr-model 1 (male weights halved), 2 chrY (male weights halved, others zero), 3 MT (all weights halved)
+  std::vector<uint32_t> cls_vidx[4];
+  for (uint32_t v = 0; v < m; ++v) {
+    const uint32_t chr = V.chr_code[v];
+    cls_vidx[chr == 26 ? 3 : chr == 24 ? 2 : (chr == 23 && c.xchr_model == 1) ? 1 : 0].push_back(v);
+  }
   std::vector<double> scores(static_cast<uint64_t>(m) * cols);
-  const uint32_t piece = 262144;
-  for (uint32_t p0 = 0; p0 < m; p0 += piece) {
-    const uint32_t p1 = std::min(m, p0 + piece);
-    Pl2PcaJob* job = nullptr;
-    if (pl2gpu_pca_begin_shard(ctx, n, p1 - p0, 0, &job)) return GpuFail("pl2gpu_pca_begin_shard");  // pc_ct 0: a --variant-score job
-    struct Guard {
-      Pl2PcaJob* j;
-      ~Guard() { pl2gpu_pca_end(j); }
-    } guard{job};
-    std::vector<uint32_t> sub(vidx.begin() + p0, vidx.begin() + p1);
-    BlockStreamer bs(ds, &sub, n, 32768);
-    if (!bs.Init()) return GpuFail("pl2gpu_host_alloc");
-    size_t base = p0;
-    for (;;) {
-      const int got = bs.Next(&err);
-      if (got < 0) {
-        logprintf("Error: %s\n", err.c_str());
-        return kRetMalformedInput;
-      }
-      if (!got) break;
-      const int arc = pl2gpu_pca_add_variants(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0, ref_freqs.data() + base);
-      if (arc) {
-        logprintf("Error: %s\n", pl2gpu_last_error());
-        return arc == 2 ? kRetDegenerateData : kRetGpuFail;
-      }
-      base += static_cast<size_t>(got);
+  for (int cl = 0; cl < 4; ++cl) {
+    const std::vector<uint32_t>& list = cls_vidx[cl];
+    if (list.empty()) continue;
+    std::vector<double> wc(w);
+    for (uint32_t k = 0; cl && k < n; ++k) {
+      const double f = (cl == 3 || S.sex[k] == 1) ? 0.5 : cl == 2 ? 0.0 : 1.0;
+      for (uint32_t cc = 0; cc < cols; ++cc) wc[static_cast<uint64_t>(k) * cols + cc] *= f;
     }
-    if (pl2gpu_pca_vscore(job, w.data(), cols, scores.data() + static_cast<uint64_t>(p0) * cols)) return GpuFail("pl2gpu_pca_vscore");
+    // the matrix is kept resident in pieces that fit comfortably; every piece is one pl2gpu_pca job
+    const uint32_t lm = static_cast<uint32_t>(list.size()), piece = 262144;
+    for (uint32_t p0 = 0; p0 < lm; p0 += piece) {
+      const uint32_t p1 = std::min(lm, p0 + piece);
+      Pl2PcaJob* job = nullptr;
+      if (pl2gpu_pca_begin_shard(ctx, n, p1 - p0, 0, &job)) return GpuFail("pl2gpu_pca_begin_shard");  // pc_ct 0: a --variant-score job
+      struct Guard {
+        Pl2PcaJob* j;
+        ~Guard() { pl2gpu_pca_end(j); }
+      } guard{job};
+      std::vector<uint32_t> sub(list.begin() + p0, list.begin() + p1);
+      std::vector<double> sub_freqs(sub.size());
+      for (size_t k = 0; k < sub.size(); ++k) sub_freqs[k] = ref_freqs[sub[k]];
+      BlockStreamer bs(ds, &sub, n, 32768);
+      if (!bs.Init()) return GpuFail("pl2gpu_host_alloc");
+      size_t base = 0;
+      for (;;) {
+        const int got = bs.Next(&err);
+        if (got < 0) {
+          logprintf("Error: %s\n", err.c_str());
+          return kRetMalformedInput;
+        }
+        if (!got) break;
+        const int arc = pl2gpu_pca_add_variants(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0, sub_freqs.data() + base);
+        if (arc) {
+          logprintf("Error: %s\n", pl2gpu_last_error());
+          return arc == 2 ? kRetDegenerateData : kRetGpuFail;
+        }
+        base += static_cast<size_t>(got);
+      }
+      std::vector<double> out(static_cast<uint64_t>(sub.size()) * cols);
+      if (pl2gpu_pca_vscore(job, wc.data(), cols, out.data())) return GpuFail("pl2gpu_pca_vscore");
+      for (size_t k = 0; k < sub.size(); ++k) std::copy_n(out.data() + k * cols, cols, scores.data() + static_cast<uint64_t>(sub[k]) * cols);
+    }
   }
   // report (:9900-10060): #CHROM POS ID REF ALT [PROVISIONAL_REF?] [ALT_FREQ] <score names>
   const bool provref_col = c.vs_provref || (c.vs_maybeprovref && V.provisional_ref && c.vs_ref);
@@ -3481,11 +3586,12 @@ int RunVscore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
 // `--freq` (WriteAlleleFreqs, 2.0/plink2_misc.cc:3573; counts from the LoadAlleleAndGenoCounts pass,
 // 2.0/plink2.cc:2280): founder ALT allele frequencies of biallelic hard calls -> <out>.afreq.
 // Founder allele "ddosage" totals per variant, in 1/32768 units as the reference accumulates them: alt_dd[v] / tot_dd[v]
-// is the ALT frequency `--freq` prints and every later command consumes (allele_freqs, plink2.cc:2301).
-int FounderAlleleDosages(Dataset* ds, Pl2GpuCtx* ctx, std::vector<uint64_t>* alt_dd_out, std::vector<uint64_t>* tot_dd_out, bool all_samples = false) {
+// is the ALT frequency `--freq` prints and every later command consumes (allele_freqs, plink2.cc:2301).  Computed for
+// the variants vidx (view indices); the outputs follow vidx's order.
+int FounderAlleleDosages(Dataset* ds, Pl2GpuCtx* ctx, const std::vector<uint32_t>& vidx, std::vector<uint64_t>* alt_dd_out, std::vector<uint64_t>* tot_dd_out, bool all_samples = false) {
   const SampleInfo& S = ds->samples;
   const VariantInfo& V = ds->variants;
-  const uint32_t n = S.size(), m = V.size();
+  const uint32_t n = S.size(), m = static_cast<uint32_t>(vidx.size());
   uint32_t founder_ct = 0, male_ct = 0, nonfemale_ct = 0;
   std::vector<uint64_t> inc((n + 63) / 64, 0), inc_male((n + 63) / 64, 0), inc_nonfemale((n + 63) / 64, 0);
   for (uint32_t k = 0; k < n; ++k) {
@@ -3528,22 +3634,22 @@ int FounderAlleleDosages(Dataset* ds, Pl2GpuCtx* ctx, std::vector<uint64_t>* alt
     }
     return 0;
   };
-  std::vector<uint32_t> all(m), xv, yv;
-  for (uint32_t v = 0; v < m; ++v) {
-    all[v] = v;
+  std::vector<uint32_t> xv, yv;
+  for (const uint32_t v : vidx) {
     if (V.chr_code[v] == 23) xv.push_back(v);
     else if (V.chr_code[v] == 24) yv.push_back(v);
   }
   std::vector<uint32_t> counts, xmale, ynonfemale;
-  int rc = count_pass(all, inc.data(), founder_ct, &counts);
+  int rc = count_pass(vidx, inc.data(), founder_ct, &counts);
   if (!rc) rc = count_pass(xv, inc_male.data(), male_ct, &xmale);
   if (!rc) rc = count_pass(yv, inc_nonfemale.data(), nonfemale_ct, &ynonfemale);
   if (rc) return rc;
   alt_dd_out->assign(m, 0);
   tot_dd_out->assign(m, 0);
   size_t xi = 0, yi = 0;
-  for (uint32_t v = 0; v < m; ++v) {
-    const uint64_t n0 = counts[4ull * v], n1 = counts[4ull * v + 1], n2 = counts[4ull * v + 2], n3 = counts[4ull * v + 3];
+  for (uint32_t k = 0; k < m; ++k) {
+    const uint32_t v = vidx[k];
+    const uint64_t n0 = counts[4ull * k], n1 = counts[4ull * k + 1], n2 = counts[4ull * k + 2], n3 = counts[4ull * k + 3];
     // allele "ddosages" in 1/32768 units, as the reference accumulates them (plink2_data.cc:2420-2690): diploid x2;
     // MT and chrY (nonfemale founders) haploid, a het counting half; chrX nonmales twice, males once
     uint64_t alt_dd, tot_dd;
@@ -3564,9 +3670,30 @@ int FounderAlleleDosages(Dataset* ds, Pl2GpuCtx* ctx, std::vector<uint64_t>* alt
       alt_dd = (n1 + 2 * n2) * 32768ull;
       tot_dd = 2 * (n0 + n1 + n2) * 32768ull;
     }
-    (*alt_dd_out)[v] = alt_dd;
-    (*tot_dd_out)[v] = tot_dd;
+    (*alt_dd_out)[k] = alt_dd;
+    (*tot_dd_out)[k] = tot_dd;
   }
+  return 0;
+}
+
+// --score / --variant-score: the REF frequencies of the chrX, chrY and MT variants among vidx from the per-class
+// founder counting above (ComputeAlleleFreqs), written over FounderRefFreqs' all-diploid values; the other variants
+// keep theirs.  Nothing to do without such variants, or without founders (FounderRefFreqs' 0.5 then stands).
+int SexChrRefFreqs(Dataset* ds, Pl2GpuCtx* ctx, const std::vector<uint32_t>& vidx, std::vector<double>* ref_freqs) {
+  const VariantInfo& V = ds->variants;
+  std::vector<uint32_t> pos, sub;
+  for (size_t k = 0; k < vidx.size(); ++k) {
+    const uint32_t chr = V.chr_code[vidx[k]];
+    if (chr == 23 || chr == 24 || chr == 26) {
+      pos.push_back(static_cast<uint32_t>(k));
+      sub.push_back(vidx[k]);
+    }
+  }
+  const std::vector<uint8_t>& fo = ds->samples.is_founder;
+  if (sub.empty() || std::find(fo.begin(), fo.end(), 1) == fo.end()) return 0;
+  std::vector<uint64_t> alt_dd, tot_dd;
+  if (const int rc = FounderAlleleDosages(ds, ctx, sub, &alt_dd, &tot_dd)) return rc;
+  for (size_t k = 0; k < sub.size(); ++k) (*ref_freqs)[pos[k]] = tot_dd[k] ? static_cast<double>(tot_dd[k] - alt_dd[k]) * (1.0 / static_cast<double>(tot_dd[k])) : 0.5;
   return 0;
 }
 
@@ -3578,7 +3705,7 @@ int RunFreq(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
     return kRetNotYetSupported;
   }
   std::vector<uint64_t> alt_dds, tot_dds;
-  const int rc = FounderAlleleDosages(ds, ctx, &alt_dds, &tot_dds, c.nonfounders);
+  const int rc = FounderAlleleDosages(ds, ctx, AllVariants(*ds), &alt_dds, &tot_dds, c.nonfounders);
   if (rc) return rc;
   if (c.freq_counts && !c.nonfounders) {  // plink2.cc:2102
     for (uint8_t fo : ds->samples.is_founder) {
@@ -4624,7 +4751,7 @@ int main(int argc, char** argv) {
     // (the --read-freq mechanism), then drop the samples from the view.
     if (later_gpu_command) {
       std::vector<uint64_t> alt_dd, tot_dd;
-      rc = FounderAlleleDosages(&ds, ctx, &alt_dd, &tot_dd);
+      rc = FounderAlleleDosages(&ds, ctx, AllVariants(ds), &alt_dd, &tot_dd);
       if (rc) return rc;
       if (ds.read_ref_freq.empty()) ds.read_ref_freq.assign(ds.variants.size(), std::numeric_limits<double>::quiet_NaN());
       for (uint32_t v = 0; v < ds.variants.size(); ++v) {

@@ -444,6 +444,37 @@ def score_sums_cols(ctx: GpuContext, genovecs: np.ndarray, sample_ct: int, weigh
         lib.pl2gpu_score_end(h)
 
 
+SCORE_DIPLOID, SCORE_HAPLOID_ALL, SCORE_CHR_Y, SCORE_CHR_X_MALE_HAPLOID = 0, 1, 2, 3  # kPl2Score* ploidy classes
+
+
+def score_sums_ploidy(ctx: GpuContext, genovecs: np.ndarray, sample_ct: int, sample_sex: np.ndarray, ploidy_classes: np.ndarray, weights4_diploid: np.ndarray, weights4_haploid: np.ndarray, named_dosages: np.ndarray):
+    """`--score` with sex-dependent ploidy (pl2gpu_score_set_sex / _add_variants_ploidy / _get_ploidy): sample_sex
+    [sample_ct] (0 unknown, 1 male, 2 female), ploidy_classes [entries] (SCORE_*), both tables [entries, score_ct, 4]
+    -> (score sums [sample_ct, score_ct], named-allele dosage sums in half allele units, diploid missing counts,
+    haploid missing counts)."""
+    g = np.ascontiguousarray(genovecs)
+    wd = np.ascontiguousarray(weights4_diploid, dtype=np.float64)
+    wh = np.ascontiguousarray(weights4_haploid, dtype=np.float64)
+    pc = np.ascontiguousarray(ploidy_classes, dtype=np.uint8)
+    sx = np.ascontiguousarray(sample_sex, dtype=np.uint8)
+    d = np.ascontiguousarray(named_dosages, dtype=np.uint8)
+    assert wd.ndim == 3 and wd.shape == wh.shape and wd.shape[0] == g.shape[0] and wd.shape[2] == 4 and d.shape == pc.shape == (g.shape[0],) and sx.shape == (sample_ct,)
+    score_ct = wd.shape[1]
+    h = C.c_void_p()
+    check(lib.pl2gpu_score_begin_cols(ctx.handle, sample_ct, score_ct, C.byref(h)), "pl2gpu_score_begin_cols")
+    try:
+        check(lib.pl2gpu_score_set_sex(h, sx.ctypes.data), "pl2gpu_score_set_sex")
+        check(lib.pl2gpu_score_add_variants_ploidy(h, g.ctypes.data, g.strides[0], g.shape[0], 0, pc.ctypes.data, wd.ctypes.data, wh.ctypes.data, d.ctypes.data), "pl2gpu_score_add_variants_ploidy")
+        sums = np.empty((sample_ct, score_ct), dtype=np.float64)
+        hdos = np.empty(sample_ct, dtype=np.uint64)
+        miss_d = np.empty(sample_ct, dtype=np.uint32)
+        miss_h = np.empty(sample_ct, dtype=np.uint32)
+        check(lib.pl2gpu_score_get_ploidy(h, sums.ctypes.data, hdos.ctypes.data, miss_d.ctypes.data, miss_h.ctypes.data), "pl2gpu_score_get_ploidy")
+        return sums, hdos, miss_d, miss_h
+    finally:
+        lib.pl2gpu_score_end(h)
+
+
 def variant_scores(ctx: GpuContext, genovecs: np.ndarray, sample_ct: int, weights: np.ndarray, ref_freqs=None) -> np.ndarray:
     """`--variant-score` sums (pl2gpu_pca_vscore) for an in-memory block: weights [sample_ct, cols] -> [variants, cols]."""
     g = np.ascontiguousarray(genovecs)
