@@ -145,6 +145,9 @@ uint64_t pl2gpu_king_variants_added(Pl2KingJob* job);
 /* Device time of the most recent pair-count tensor kernel launch (CUDA events recorded around that launch on
  * the context's stream; blocks until it has finished).  bench.py's roofline uses it. */
 int pl2gpu_king_last_kernel_ms(Pl2KingJob* job, float* ms);
+/* Diagnostic: copies the first `bytes` bytes of the column plane copy that the most recent default-algorithm launch
+ * read (its layout: geno_tile.cuh) to host memory `dst`; blocks until that launch has finished. */
+int pl2gpu_king_last_planes(Pl2KingJob* job, void* dst, uint64_t bytes);
 /* Idempotent; accepts NULL. */
 int pl2gpu_king_end(Pl2KingJob* job);
 

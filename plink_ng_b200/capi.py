@@ -55,6 +55,7 @@ SIGNATURES = {
     "pl2gpu_king_get_filtered": (C.c_int, [vp, C.c_uint32, C.c_uint32, C.c_double, C.c_uint64, vp, vp, vp, C.POINTER(C.c_uint64)]),
     "pl2gpu_king_variants_added": (C.c_uint64, [vp]),
     "pl2gpu_king_last_kernel_ms": (C.c_int, [vp, C.POINTER(C.c_float)]),
+    "pl2gpu_king_last_planes": (C.c_int, [vp, vp, C.c_uint64]),
     "pl2gpu_king_end": (C.c_int, [vp]),
     "pl2gpu_king_pairs_begin": (C.c_int, [vp, C.c_uint32, vp, C.c_uint64, C.POINTER(vp)]),
     "pl2gpu_king_pairs_add_variants": (C.c_int, [vp, vp, C.c_uint64, C.c_uint32, C.c_int]),

@@ -74,12 +74,15 @@ struct TileList {
   uint32_t* d_tile_tc = nullptr;       // [tile_ct] col-tile index
   uint32_t* d_rowtile_offset = nullptr;  // [row_tile_ct + 1] first tile of each row tile
   uint32_t* d_tile_order = nullptr;      // [tile_ct] launch order: 12 x 12 tile blocks so co-resident CTAs share L2 lines
+  uint32_t pair_tile_ct = 0;             // row_pairs lists: d_tile_order starts with this many tiles, pairs (rt, ct), (rt + 1, ct)
   std::vector<uint32_t> h_rowtile_offset;  // host copy of the same
 };
 
 // col_end: tiles that lie entirely at or past this column are left out (a KING job cut at a column bound)
 uint64_t CountTiles(uint32_t row_start, uint32_t row_end, bool include_diag, uint32_t tile_cols = kTileCols, uint32_t col_end = 0xFFFFFFFFu);
-int BuildTileList(uint32_t row_start, uint32_t row_end, bool include_diag, TileList* tl, uint32_t tile_cols = kTileCols, uint32_t col_end = 0xFFFFFFFFu);
+// row_pairs: the launch order starts with the tiles (rt, ct), (rt + 1, ct) of row-tile pairs counted from the first
+// row tile, two by two, and ends with the tiles that have no such partner
+int BuildTileList(uint32_t row_start, uint32_t row_end, bool include_diag, TileList* tl, uint32_t tile_cols = kTileCols, uint32_t col_end = 0xFFFFFFFFu, bool row_pairs = false);
 void FreeTileList(TileList* tl);
 
 // ---- staged genotype block on the device (implemented in pl2gpu.cu) ----

@@ -12,6 +12,8 @@ constexpr uint32_t kTsSamplePad = 640;  // lcm(128, 80)
 // 128 x 64 pair tiles (the default KING tiling); its blocks keep the 640-sample padding.
 constexpr uint32_t kKingTsCols = 64;
 static_assert(kTsSamplePad % 128 == 0 && kTsSamplePad % kKingTsCols == 0, "padded samples: whole row and column tiles");
+// One plane image: the four bit planes T | H | R | A of one 64-sample column tile over one k256 step (king_b1_kernel).
+constexpr uint32_t kKingPlaneStepBytes = 4 * kKingTsCols * 32;
 
 // ---- operand re-tiling of the staged block raw[variant][pitch] (2-bit, variant-major) -------------
 // kSplitBits = false (GRM, PCA and king_wg_kernel):
@@ -25,10 +27,16 @@ static_assert(kTsSamplePad % 128 == 0 && kTsSamplePad % kKingTsCols == 0, "padde
 //   0, 4, 1, 5, 2, 6, 3, 7, so 16-byte chunk c holds words c and c + 4: the two k32 steps that thread c of a quad
 //   needs for its binary wgmma A fragment registers of one row.  Same size as the 2-bit form.
 //   One CTA = 256 variants (one k256 step) x 64 samples, so each sample's 64-byte piece is written whole.
+//   The same CTA also writes the plane image of its 64 samples (one column tile of the default KING kernel) and step:
+//   planes[sample / 64][k256 step][plane T | H | R | A][sample % 64 / 8][core matrix h][sample % 8][16 B], with
+//   T = lo & ~hi, H = ~lo, R = ~(lo | hi), A = ~lo & hi, core matrix h = k32 words 4 h .. 4 h + 3 as the 16-byte
+//   little-endian image of their 32-bit words: the K-major, no-swizzle shared-memory layout of a wgmma B operand
+//   (LBO 128 B, SBO 256 B), copied to shared memory as is.  Code 3 (missing, padding) is zero in every plane.
+//   Twice the size of the split copy.
 // Only samples [s_base, s_base + 64 * gridDim.y) are written (a job re-tiles its own row tiles only);
 // row tile s_base / 128 is stored at index 0.
 template <bool kSplitBits = false>
-static __global__ void __launch_bounds__(256) geno_tile_rows_kernel(const uint8_t* __restrict__ raw, uint32_t pitch, uint32_t kstep_ct, uint32_t s_base, uint8_t* __restrict__ raw_i) {
+static __global__ void __launch_bounds__(256) geno_tile_rows_kernel(const uint8_t* __restrict__ raw, uint32_t pitch, uint32_t kstep_ct, uint32_t s_base, uint8_t* __restrict__ raw_i, uint8_t* __restrict__ planes = nullptr) {
   const uint32_t t = threadIdx.x;
   if constexpr (kSplitBits) {
     // codes[v][word ^ ((v >> 5) & 3)]: the 64 samples of variant v as four 32-bit words of 16 samples each.  The
@@ -60,6 +68,14 @@ static __global__ void __launch_bounds__(256) geno_tile_rows_kernel(const uint8_
     }
     const uint32_t s = s0 + sl;
     *reinterpret_cast<uint4*>(raw_i + (static_cast<uint64_t>((s - s_base) >> 7) * (kstep_ct / 8) + blockIdx.x) * 8192 + (s & 127) * 64 + 16 * c) = make_uint4(lo[0], hi[0], lo[1], hi[1]);
+    // word c of core matrix h is k32 word c + 4 h: a quad writes a sample's 16 bytes, a warp 8 samples' 128 bytes
+    uint8_t* img = planes + (static_cast<uint64_t>((s - s_base) >> 6) * (kstep_ct / 8) + blockIdx.x) * kKingPlaneStepBytes + (sl >> 3) * 256 + (sl & 7) * 16 + 4 * c;
+#pragma unroll
+    for (uint32_t h = 0; h < 2; ++h) {
+      const uint32_t pl[4] = {lo[h] & ~hi[h], ~lo[h], ~(lo[h] | hi[h]), ~lo[h] & hi[h]};
+#pragma unroll
+      for (uint32_t p = 0; p < 4; ++p) *reinterpret_cast<uint32_t*>(img + p * (kKingPlaneStepBytes / 4) + h * 128) = pl[p];
+    }
   } else {
     __shared__ uint8_t tile[64][68];
     const uint32_t v0 = blockIdx.x * 64, s0 = s_base + blockIdx.y * 64;

@@ -1763,10 +1763,11 @@ int RunKing(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, std::vector<uint8_t>* cut
   }
   uint64_t budget = free_b - free_b / 10;
   if (c.gpu_memory_mib && (c.gpu_memory_mib << 20) < budget) budget = c.gpu_memory_mib << 20;
-  // variants per staged block: the full 65,536 unless the cap is so small that the two staged blocks would
-  // eat most of it (then halve until they fit in a quarter of the budget)
+  // variants per staged block: the full 65,536 unless the cap is so small that the two staged blocks, their
+  // sample-major copies and their column plane copies (8 block sizes in all) would eat most of it (then halve until
+  // they fit in a quarter of the budget)
   uint32_t batch = 65536;
-  while (batch > 2048 && 4ull * batch * ((n + 639) / 640 * 160) > budget / 4) batch /= 2;
+  while (batch > 2048 && 8ull * batch * ((n + 639) / 640 * 160) > budget / 4) batch /= 2;
   auto pass_fits = [&](uint32_t a, uint32_t b) {
     const std::vector<uint32_t> sb = TileAlignedBounds(a, b, G, false);
     for (uint32_t g = 0; g < G; ++g) {

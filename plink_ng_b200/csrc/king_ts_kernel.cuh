@@ -243,13 +243,14 @@ king_wg_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
 
 // ---------------------------------------------------------------------------------------------------------------
 // king_b1_kernel: the KING counts as AND-popcounts of bit planes on the binary tensor pipe (wgmma .b1 AND.POPC,
-// m64nNk256).  From the low and high bits (lo, hi) of each 2-bit code, which the split form of the sample-major copy
-// (geno_tile_rows_kernel<true>) already holds as two 32-variant halves of each word:
+// m64nNk256).  From the low and high bits (lo, hi) of each 2-bit code:
 //   T = lo & ~hi (het),  H = ~lo (hom),  R = ~lo & ~hi (hom-REF),  A = ~lo & hi (hom-ALT);
-// missing data and padding (code 3) are zero in every plane.  One CTA = one whole 128 x 64 pair tile, three warpgroups:
-//   warpgroup 0:  producer.  Warp 0 brings a stage's raw words into a slot of the ring with bulk copies onto the
-//                 slot's `load` mbarrier as soon as the slot is free; warps 2 and 3 turn the column words into the
-//                 four planes T | H | R | A (K-major, no swizzle; one core matrix = 8 samples x 128 variants).
+// missing data and padding (code 3) are zero in every plane.  The prep stream writes two copies of each staged block
+// (geno_tile_rows_kernel<true>): the split sample-major copy (row side, {lo32, hi32} words) and the column planes,
+// one 8 KB image per 64-sample column tile and k256 step, byte for byte what the B descriptor reads.  So the kernel
+// is a pure bulk-copy -> wgmma pipeline.  One CTA = one whole 128 x 64 pair tile, three warpgroups:
+//   warpgroup 0:  producer.  Thread 0 refills a slot of the ring as soon as the consumers have handed it back: the
+//                 stage's row words and its plane images, bulk copies onto the slot's `full` mbarrier (tx count).
 //   warpgroups 1, 2:  consumer c owns rows 64 c .. 64 c + 63.  Per k256 step it turns its own row words straight
 //                 into fragment registers and issues   T_I x [T_J | H_J] (n128) -> TT | TH,
 //                 H_I x [T_J | H_J] (n128) -> HT | HH,   R_I x A_J + A_I x R_J (n64, one accumulator) -> IBS0:
@@ -257,34 +258,39 @@ king_wg_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
 //                 (40) to the consumers (232).  The row words of the next k256 step are loaded while this step's
 //                 group is being issued, so only LOP3s stand between a retired group and the next one.
 // The epilogue writes SS = HH - 2 IBS0 (= the int8 form's S_I x S_J with S = R - A), so the raw accumulator layout
-// {TT, TH, HT, HH, SS} is that of king_wg_kernel.  Hand-off as in king_wg_kernel: `full` (64 producer arrivals
-// after the fence), `empty` (256 consumer arrivals once `wgmma.wait_group 1` has retired the stage), one wgmma group
-// in flight across stage boundaries.  A stage holds kKb1Ks k256 steps; the last one may be short (the block is padded
-// to 256 variants only): its missing steps are neither copied nor split, and run on zero planes.
-// The sample-major copy keeps each sample's 256 variants of a k256 step as one 64-byte piece, 16-byte chunk c = k32
-// words c and c + 4 (geno_tile.cuh), so the row words of a k256 step are one contiguous 8 KB and the 64 column
-// samples one contiguous 4 KB (half of a 128-sample block).
+// {TT, TH, HT, HH, SS} is that of king_wg_kernel.  `empty` collects one arrival per consumer warp once
+// `wgmma.wait_group 1` has retired the stage; one wgmma group stays in flight across stage boundaries.  A stage holds
+// kKb1Ks k256 steps; the last one may be short (the block is padded to 256 variants only): its missing steps are not
+// copied, and their row fragments are zero, so whatever the slot holds there adds nothing.
+//
+// kCluster = 2: the CTAs of a cluster run tiles (rt, ct) and (rt + 1, ct), which read the same plane images.  Each
+// CTA copies its own row words and half of every plane image, multicast into both CTAs, so a tile still reads
+// 12 KB from L2 per k256 step (8 KB of rows, 4 KB of planes).  A CTA's `full` barrier therefore also counts the
+// partner's bytes, and a producer may refill a slot only once the consumers of both CTAs have released it: every
+// consumer warp arrives on `empty` of both CTAs.  The tiles without a partner run with kCluster = 1.
 constexpr uint32_t kKb1Ks = 2;       // k256 steps per stage
-constexpr uint32_t kKb1Stages = 5;
-constexpr uint32_t kKb1Sbo = 2 * kKb1Ks * kKwChunkBytes;                 // next group of 8 samples
+constexpr uint32_t kKb1Stages = 7;
+constexpr uint32_t kKb1Sbo = 2 * kKwChunkBytes;                          // next group of 8 samples of a plane image
 constexpr uint32_t kKb1PlaneBytes = (kKingTsCols / 8) * kKb1Sbo;         // one plane of the 64 column samples
-constexpr uint32_t kKb1BBytes = 4 * kKb1PlaneBytes;                      // T | H | R | A
+constexpr uint32_t kKb1BStepBytes = 4 * kKb1PlaneBytes;                  // T | H | R | A of one k256 step
 constexpr uint32_t kKb1SampleBytes = 64;                                 // one sample's words of one k256 step
 constexpr uint32_t kKb1AStepBytes = kTileRows * kKb1SampleBytes;         // row words of one k256 step
-constexpr uint32_t kKb1WStepBytes = kKingTsCols * kKb1SampleBytes;       // column words of one k256 step
+constexpr uint32_t kKb1BBytes = kKb1Ks * kKb1BStepBytes;                 // [k256 step][plane image]
 constexpr uint32_t kKb1ABytes = kKb1Ks * kKb1AStepBytes;                 // [k256 step][128 rows][64 B]
-constexpr uint32_t kKb1WBytes = kKb1Ks * kKb1WStepBytes;                 // [k256 step][64 samples][64 B]
-constexpr uint32_t kKb1StageBytes = kKb1BBytes + kKb1ABytes + kKb1WBytes;
-constexpr uint32_t kKb1SmemBytes = kKb1Stages * kKb1StageBytes + 128 + 3 * kKb1Stages * 8;  // + alignment + mbarriers
-constexpr uint32_t kKb1SplitThreads = kKingTsCols;  // producer warps 2, 3: one column sample each
-static_assert(kKwProducerThreads == 2 * kKingTsCols, "producer warps: copier, idle, two split warps");
+constexpr uint32_t kKb1StageBytes = kKb1BBytes + kKb1ABytes;
+constexpr uint32_t kKb1SmemBytes = kKb1Stages * kKb1StageBytes + 128 + 2 * kKb1Stages * 8;  // + alignment + mbarriers
+constexpr uint32_t kKb1ConsumerWarps = kKwConsumerThreads / 32;
+static_assert(kKb1BStepBytes == kKingPlaneStepBytes, "plane image of geno_tile_rows_kernel<true>");
 static_assert(kKb1SmemBytes <= kKwSmemLimit, "exceeds the 227 KB shared-memory opt-in limit");
 
-// raw_t: sample-major copy of the whole padded block (sample 0 at row tile 0) in the split form of
-// geno_tile_rows_kernel<true>: [sample / 128][k256 step][sample % 128][64 B], each 8-byte word {lo32, hi32} of 32
-// variants; grid: one CTA per tile.
+// raw_t: split sample-major copy of the whole padded block (sample 0 at row tile 0),
+// [sample / 128][k256 step][sample % 128][64 B], each 8-byte word {lo32, hi32} of 32 variants; planes: its plane
+// images, [sample / 64][k256 step][8 KB] (geno_tile.cuh).  Grid: one CTA per tile, consecutive pairs of CTAs form a
+// cluster when kCluster = 2 (tile_order lists the two tiles of a pair next to each other).
+template <uint32_t kCluster>
 __global__ void __launch_bounds__(kKwThreads, 1)
-king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* multiple of 256 */, const uint32_t* __restrict__ tile_order, const uint32_t* __restrict__ tile_rt, const uint32_t* __restrict__ tile_tc, int32_t* __restrict__ raw_acc) {
+king_b1_kernel(const uint8_t* __restrict__ raw_t, const uint8_t* __restrict__ planes, uint32_t variant_ct_padded /* multiple of 256 */, const uint32_t* __restrict__ tile_order, const uint32_t* __restrict__ tile_rt, const uint32_t* __restrict__ tile_tc, int32_t* __restrict__ raw_acc) {
+  static_assert(kCluster == 1 || kCluster == 2, "a tile pair at most");
   extern __shared__ __align__(128) uint8_t smem[];
   const uint32_t tid = threadIdx.x;
   const uint32_t wg = tid >> 7;
@@ -293,104 +299,54 @@ king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
   const uint32_t ct = tile_tc[tile];
   const uint32_t k256_ct = variant_ct_padded / 256;
   const uint32_t stage_ct = (k256_ct + kKb1Ks - 1) / kKb1Ks;
+  // the same offset in every CTA of the cluster: multicast copies and remote arrivals address the partner with it
   const uint32_t smem_base = (static_cast<uint32_t>(__cvta_generic_to_shared(smem)) + 127u) & ~127u;
   const uint32_t bar_full = smem_base + kKb1Stages * kKb1StageBytes;  // full[s] = bar_full + 8 s
   const uint32_t bar_empty = bar_full + kKb1Stages * 8;
-  const uint32_t bar_load = bar_empty + kKb1Stages * 8;
   if (tid == 0) {
     for (uint32_t s = 0; s < kKb1Stages; ++s) {
-      mbar_init(bar_full + 8 * s, kKb1SplitThreads);
-      mbar_init(bar_empty + 8 * s, kKwConsumerThreads);
-      mbar_init(bar_load + 8 * s, 1);
+      mbar_init(bar_full + 8 * s, 1);
+      mbar_init(bar_empty + 8 * s, kCluster * kKb1ConsumerWarps);
     }
     mbar_init_fence();
   }
-  __syncthreads();
+  // the partner copies into this CTA and arrives on its barriers only after they are initialised
+  if constexpr (kCluster > 1) {
+    cluster_sync();
+  } else {
+    __syncthreads();
+  }
 
   if (wg == 0) {
     setmaxnreg_dec<40>();
-    // ---- producer
-    const uint32_t pw = tid >> 5;
-    if (pw == 0) {
-      // copier warp: the row words of a stage (one contiguous piece, [k256 step][128 rows][64 B]) and the column
-      // words of this tile (4 KB per k256 step), one bulk copy per lane onto the slot's `load` mbarrier.  It refills
-      // a slot as soon as the consumers have handed it back, so every slot but the one being read has its copies in
-      // flight.  These threads never split planes: the proxy fence after the split waits for every memory access
-      // of the thread still in flight, bulk copies included, which would hold the split up by a whole copy latency.
+    if (tid == 0) {
+      // ---- producer: row words [k256 step][128 rows][64 B] of row tile rt, plane images of column tile ct
+      const uint32_t rank = kCluster > 1 ? cluster_cta_rank() : 0;
+      constexpr uint32_t kBPart = kKb1BStepBytes / kCluster;  // this CTA's part of each plane image
       const uint8_t* a_src = raw_t + static_cast<uint64_t>(rt) * k256_ct * kKb1AStepBytes;
-      // column samples 64 ct .. 64 ct + 63: half (ct & 1) of 128-sample block ct >> 1
-      const uint8_t* w_src = raw_t + static_cast<uint64_t>(ct >> 1) * k256_ct * kKb1AStepBytes + (ct & 1) * kKb1WStepBytes;
-      const uint32_t lane = tid & 31;
+      const uint8_t* b_src = planes + static_cast<uint64_t>(ct) * k256_ct * kKb1BStepBytes + rank * kBPart;
       for (uint32_t st = 0; st < stage_ct; ++st) {
         const uint32_t slot = st % kKb1Stages;
         // the first pass over the ring finds every slot free (parity 1 = the phase before a fresh barrier's first)
-        mbar_wait(bar_empty + 8 * slot, ((st / kKb1Stages) & 1) ^ 1);
+        const uint32_t parity = ((st / kKb1Stages) & 1) ^ 1;
+        mbar_wait(bar_empty + 8 * slot, parity);
         const uint32_t base = smem_base + slot * kKb1StageBytes;
-        const uint32_t bar = bar_load + 8 * slot;
+        const uint32_t bar = bar_full + 8 * slot;
         const uint32_t steps = min(kKb1Ks, k256_ct - st * kKb1Ks);
-        const uint64_t off = static_cast<uint64_t>(st) * kKb1Ks * kKb1AStepBytes;
-        if (lane == 0) mbar_arrive_expect_tx(bar, steps * (kKb1AStepBytes + kKb1WStepBytes));
-        if (lane < steps) bulk_copy_g2s(base + kKb1BBytes + kKb1ABytes + lane * kKb1WStepBytes, w_src + off + lane * kKb1AStepBytes, kKb1WStepBytes, bar);
-        if (lane == 31) bulk_copy_g2s(base + kKb1BBytes, a_src + off, steps * kKb1AStepBytes, bar);
-        __syncwarp();
-      }
-    } else if (pw >= 2) {
-      // split warps 2, 3: column sample n = tid % 64; for each k256 step j and half h, k32 steps 8 j + 4 h ..
-      // 8 j + 4 h + 3, i.e. the 16-byte half h of row n of each plane's core matrices for step j.
-      // Sample n's 64 bytes of step j sit at n * 64, chunk m (k32 words m, m + 4) at + 16 m: banks 16 (n & 1) + 4 m
-      // .. + 3.  An LDS.128 serves 8 threads per wavefront; if the 8 threads n = 8 a .. 8 a + 7 all read the same
-      // chunk m, the four even (and the four odd) ones land on the same four banks: 4 wavefronts instead of 1.  So
-      // load i reads chunk (i + (n >> 1)) & 3: the four even threads then take four different chunks, the 8 threads
-      // cover the 32 banks once, and the chunks are rotated back into order in registers.
-      const uint32_t n = tid & (kKingTsCols - 1);
-      const uint32_t rot = (n >> 1) & 3;
-      for (uint32_t st = 0; st < stage_ct; ++st) {
-        const uint32_t slot = st % kKb1Stages, phase = (st / kKb1Stages) & 1;
-        const uint32_t base = smem_base + slot * kKb1StageBytes;
-        const uint32_t steps = min(kKb1Ks, k256_ct - st * kKb1Ks);
-        // the copies into this slot were issued once it was free; the planes go in after the same wait
-        if (st >= kKb1Stages) mbar_wait(bar_empty + 8 * slot, phase ^ 1);
-        mbar_wait(bar_load + 8 * slot, phase);
-#pragma unroll
-        for (uint32_t j = 0; j < kKb1Ks; ++j) {
-          uint32_t w[4][4];  // w[m] = chunk m = {lo, hi of k32 word m, lo, hi of word m + 4}
-#pragma unroll
-          for (uint32_t m = 0; m < 4; ++m) w[m][0] = w[m][1] = w[m][2] = w[m][3] = ~0u;  // missing step: code 3, zero planes
-          if (j < steps) {
-#pragma unroll
-            for (uint32_t i = 0; i < 4; ++i)
-              asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(w[i][0]), "=r"(w[i][1]), "=r"(w[i][2]), "=r"(w[i][3]) : "r"(base + kKb1BBytes + kKb1ABytes + j * kKb1WStepBytes + n * kKb1SampleBytes + 16 * ((i + rot) & 3)) : "memory");
-          }
-          // w[i] holds chunk (i + rot) & 3: rotate by rot & 1, then by rot & 2
-#pragma unroll
-          for (uint32_t r = 1; r <= 2; r <<= 1) {
-            const bool on = rot & r;
-            uint32_t t[4][4];
-#pragma unroll
-            for (uint32_t m = 0; m < 4; ++m)
-#pragma unroll
-              for (uint32_t e = 0; e < 4; ++e) t[m][e] = on ? w[(m - r) & 3][e] : w[m][e];
-#pragma unroll
-            for (uint32_t m = 0; m < 4; ++m)
-#pragma unroll
-              for (uint32_t e = 0; e < 4; ++e) w[m][e] = t[m][e];
-          }
-#pragma unroll
-          for (uint32_t h = 0; h < 2; ++h) {
-            uint32_t lo[4], hi[4];  // k32 words 4 h + q
-#pragma unroll
-            for (uint32_t q = 0; q < 4; ++q) lo[q] = w[q][2 * h], hi[q] = w[q][2 * h + 1];
-            const uint32_t addr = base + (n >> 3) * kKb1Sbo + (2 * j + h) * kKwChunkBytes + (n & 7) * 16;
-            asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr), "r"(lo[0] & ~hi[0]), "r"(lo[1] & ~hi[1]), "r"(lo[2] & ~hi[2]), "r"(lo[3] & ~hi[3]) : "memory");
-            asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + kKb1PlaneBytes), "r"(~lo[0]), "r"(~lo[1]), "r"(~lo[2]), "r"(~lo[3]) : "memory");
-            asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + 2 * kKb1PlaneBytes), "r"(~(lo[0] | hi[0])), "r"(~(lo[1] | hi[1])), "r"(~(lo[2] | hi[2])), "r"(~(lo[3] | hi[3])) : "memory");
-            asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(addr + 3 * kKb1PlaneBytes), "r"(~lo[0] & hi[0]), "r"(~lo[1] & hi[1]), "r"(~lo[2] & hi[2]), "r"(~lo[3] & hi[3]) : "memory");
-          }
+        const uint64_t k0 = static_cast<uint64_t>(st) * kKb1Ks;
+        mbar_arrive_expect_tx(bar, steps * (kKb1AStepBytes + kKb1BStepBytes));
+        bulk_copy_g2s(base + kKb1BBytes, a_src + k0 * kKb1AStepBytes, steps * kKb1AStepBytes, bar);
+        if constexpr (kCluster > 1) {
+          for (uint32_t j = 0; j < steps; ++j)
+            bulk_copy_g2s_multicast(base + j * kKb1BStepBytes + rank * kBPart, b_src + (k0 + j) * kKb1BStepBytes, kBPart, bar, (1u << kCluster) - 1);
+        } else {
+          bulk_copy_g2s(base, b_src + k0 * kKb1BStepBytes, steps * kKb1BStepBytes, bar);
         }
-        fence_proxy_async_smem();  // this thread's st.shared -> visible to the consumers' wgmma operand fetch
-        mbar_arrive(bar_full + 8 * slot);
       }
     }
+    // the partner may still copy into this CTA and arrive on its barriers until it has passed the same point
+    __syncwarp();
+    if constexpr (kCluster > 1) cluster_sync();
     return;
   }
 
@@ -428,7 +384,7 @@ king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
     const uint32_t steps = min(kKb1Ks, k256_ct - st * kKb1Ks);
     const uint32_t next_slot = slot + 1 == kKb1Stages ? 0 : slot + 1;
     const uint32_t next_phase = slot + 1 == kKb1Stages ? phase ^ 1 : phase;
-    const uint64_t desc = make_wg_desc(base, kKwChunkBytes, kKb1Sbo);
+    const uint64_t desc = make_wg_desc(base, kKwChunkBytes, kKb1Sbo);  // plane image of step j: + j * kKb1BStepBytes
 #pragma unroll
     for (uint32_t j = 0; j < kKb1Ks; ++j) {
       const uint32_t lo[4] = {w[0].x, w[1].x, w[0].z, w[1].z}, hi[4] = {w[0].y, w[1].y, w[0].w, w[1].w};
@@ -440,7 +396,7 @@ king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
         fr[q] = ~(lo[q] | hi[q]);
         fa[q] = ~lo[q] & hi[q];
       }
-      const uint64_t dk = desc + ((j * 2 * kKwChunkBytes) >> 4);
+      const uint64_t dk = desc + ((j * kKb1BStepBytes) >> 4);
       wgmma_fence();
       wgmma_b1_rs<2 * kKingTsCols>(acc_t, ft, dk);                               // x [T_J | H_J]
       wgmma_b1_rs<2 * kKingTsCols>(acc_h, fh, dk);                               // x [T_J | H_J]
@@ -458,8 +414,19 @@ king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
         load_words(smem_base + next_slot * kKb1StageBytes, 0);
       }
       wgmma_wait<1>();
-      // every group but the one just issued has retired, the previous stage's last one included: hand that slot back
-      if (j == 0 && st > 0) mbar_arrive(bar_empty + 8 * prev_slot);
+      // every group but the one just issued has retired, the previous stage's last one included: hand that slot back,
+      // to the producers of both CTAs of a cluster
+      if (j == 0 && st > 0) {
+        __syncwarp();
+        if (lane == 0) {
+          if constexpr (kCluster > 1) {
+#pragma unroll
+            for (uint32_t cta = 0; cta < kCluster; ++cta) mbar_arrive_cluster(bar_empty + 8 * prev_slot, cta);
+          } else {
+            mbar_arrive(bar_empty + 8 * prev_slot);
+          }
+        }
+      }
     }
     prev_slot = slot;
     slot = next_slot, phase = next_phase;
@@ -477,6 +444,7 @@ king_b1_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
   king_acc_add<2 * kKingTsCols>(acc_tile, acc_t, r_lo, c);                                                   // TT | TH
   king_acc_add<2 * kKingTsCols>(acc_tile + static_cast<uint64_t>(2 * kKingTsCols) * kTileRows, acc_h, r_lo, c);  // HT | HH
   king_acc_add<kKingTsCols>(acc_tile + static_cast<uint64_t>(4 * kKingTsCols) * kTileRows, acc_i, r_lo, c);      // SS
+  if constexpr (kCluster > 1) cluster_sync();
 }
 
 }  // namespace pl2

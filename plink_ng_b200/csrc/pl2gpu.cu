@@ -46,7 +46,7 @@ uint64_t CountTiles(uint32_t row_start, uint32_t row_end, bool include_diag, uin
   return n;
 }
 
-int BuildTileList(uint32_t row_start, uint32_t row_end, bool include_diag, TileList* tl, uint32_t tile_cols, uint32_t col_end) {
+int BuildTileList(uint32_t row_start, uint32_t row_end, bool include_diag, TileList* tl, uint32_t tile_cols, uint32_t col_end, bool row_pairs) {
   std::vector<uint32_t> rt_v, tc_v, off_v;
   tl->row_tile_first = row_start / kTileRows;
   uint32_t rt = tl->row_tile_first;
@@ -73,22 +73,36 @@ int BuildTileList(uint32_t row_start, uint32_t row_end, bool include_diag, TileL
   PL2_CUDA_OK(cudaMemcpy(tl->d_rowtile_offset, off_v.data(), off_v.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
   tl->h_rowtile_offset = off_v;
   // launch order: blocks of kBand x kBand tiles (144, about one wave on the 132 SMs of an H100 SXM) so that the
-  // CTAs resident at the same time stream the same few row/column sample ranges and hit in L2
+  // CTAs resident at the same time stream the same few row/column sample ranges and hit in L2.  With row_pairs the
+  // row tiles of a block go two at a time (kBand is even, so a pair never straddles two blocks): a column tile both
+  // rows have becomes a pair, next to each other in the order; the rest, the second row's last column tiles at the
+  // triangle edge and a last unpaired row, go to the end in the same blocked order.
   constexpr uint32_t kBand = 12;
-  std::vector<uint32_t> order;
+  std::vector<uint32_t> order, lone;
   order.reserve(rt_v.size());
   const uint32_t n_rt = tl->row_tile_ct;
+  const uint32_t r_step = row_pairs ? 2 : 1;
   for (uint32_t rb = 0; rb < n_rt; rb += kBand) {
     const uint32_t rb_end = std::min(n_rt, rb + kBand);
     uint32_t max_cols = 0;
     for (uint32_t r = rb; r < rb_end; ++r) max_cols = std::max(max_cols, off_v[r + 1] - off_v[r]);
     for (uint32_t cb = 0; cb < max_cols; cb += kBand) {
-      for (uint32_t r = rb; r < rb_end; ++r) {
-        const uint32_t ncols = off_v[r + 1] - off_v[r];
-        for (uint32_t c = cb; c < std::min(ncols, cb + kBand); ++c) order.push_back(off_v[r] + c);
+      for (uint32_t r = rb; r < rb_end; r += r_step) {
+        const uint32_t n0 = off_v[r + 1] - off_v[r];
+        const uint32_t n1 = row_pairs && r + 1 < rb_end ? off_v[r + 2] - off_v[r + 1] : 0;
+        for (uint32_t c = cb; c < std::min(std::max(n0, n1), cb + kBand); ++c) {
+          if (c < n0 && c < n1) {
+            order.push_back(off_v[r] + c);
+            order.push_back(off_v[r + 1] + c);
+          } else {
+            (row_pairs ? lone : order).push_back(c < n0 ? off_v[r] + c : off_v[r + 1] + c);
+          }
+        }
       }
     }
   }
+  tl->pair_tile_ct = row_pairs ? static_cast<uint32_t>(order.size()) : 0;
+  order.insert(order.end(), lone.begin(), lone.end());
   PL2_CUDA_OK(cudaMalloc(&tl->d_tile_order, nb));
   if (!order.empty()) PL2_CUDA_OK(cudaMemcpy(tl->d_tile_order, order.data(), order.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
   return 0;
@@ -302,6 +316,7 @@ struct Pl2KingJob {
   StageRing ring;   // TS path: the row re-tiling of each slot also runs on the prep stream
   GenoStage stage;  // the other algorithms: one block on the compute stream
   uint8_t* d_raw_t[2] = {nullptr, nullptr};  // tensor paths: sample-major copy of the staged block (geno_tile.cuh; split form on the TS path)
+  uint8_t* d_col_planes[2] = {nullptr, nullptr};  // TS path: the column plane images of the staged block (geno_tile.cuh)
   cudaEvent_t ev_kernel_start[2] = {nullptr, nullptr};  // with the ring's ev_free, the timed pair around the tensor kernel (pl2gpu_king_last_kernel_ms)
   int last_buf = -1;
   uint32_t* d_planes = nullptr;  // popcount path only
@@ -354,7 +369,8 @@ int pl2gpu_ctx_create(int device_idx, Pl2GpuCtx** ctx_ptr) {
     PL2_CUDA_OK(cudaStreamCreateWithPriority(&ctx->c.copy_stream, cudaStreamNonBlocking, prio_hi));
   }
   PL2_CUDA_OK(cudaFuncSetAttribute(king_wg_kernel<kTileCols>, cudaFuncAttributeMaxDynamicSharedMemorySize, KingWgShape<kTileCols>::kSmemBytes));
-  PL2_CUDA_OK(cudaFuncSetAttribute(king_b1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kKb1SmemBytes));
+  PL2_CUDA_OK(cudaFuncSetAttribute(king_b1_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kKb1SmemBytes));
+  PL2_CUDA_OK(cudaFuncSetAttribute(king_b1_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kKb1SmemBytes));
   *ctx_ptr = ctx;
   return 0;
 }
@@ -502,10 +518,11 @@ uint64_t pl2gpu_king_mem_required(uint32_t sample_ct, uint32_t row_start, uint32
   const uint64_t tiles = CountTiles(row_start, row_end, false);
   const uint64_t npad = RoundUpU32(sample_ct, kSamplePad);
   const uint64_t need_ss = tiles * kKingTileAccWords * 4 + cap * (npad / 4) + 3ull * (cap / 32) * npad * 4 + tiles * 16;
-  // 128 x 64 tiles (the default): two raw blocks + two sample-major copies
+  // 128 x 64 tiles (the default): two raw blocks + two sample-major copies (each the size of a raw block) + two copies
+  // of the column planes (twice that size)
   const uint64_t tiles_ts = CountTiles(row_start, row_end, false, kKingTsCols);
   const uint64_t npad_ts = RoundUpU32(sample_ct, kTsSamplePad);
-  const uint64_t need_ts = tiles_ts * kKingTsTileAccWords * 4 + 4 * cap * (npad_ts / 4) + tiles_ts * 16;
+  const uint64_t need_ts = tiles_ts * kKingTsTileAccWords * 4 + 8 * cap * (npad_ts / 4) + tiles_ts * 16;
   return (need_ss > need_ts ? need_ss : need_ts) + kKingOutStageBytes + slack;
 }
 
@@ -515,11 +532,12 @@ int pl2gpu_king_begin(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start, ui
 
 uint64_t pl2gpu_king_mapped_mem_required(uint32_t sample_ct, uint32_t row_start, uint32_t row_end, uint32_t col_end, uint32_t max_variants_per_add) {
   // what pl2gpu_king_begin_mapped allocates: the TS accumulators of the cut tile list, two raw blocks + two sample-major
-  // copies, the unmapped block, the position map, the output staging buffer, plus slack for allocator granularity
+  // copies + two copies of the column planes (twice their size), the unmapped block, the position map, the output
+  // staging buffer, plus slack for allocator granularity
   const uint64_t cap = ClampStageCap(max_variants_per_add);
   const uint64_t tiles_ts = CountTiles(row_start, row_end, false, kKingTsCols, col_end);
   const uint64_t npad_ts = RoundUpU32(sample_ct, kTsSamplePad);
-  return tiles_ts * kKingTsTileAccWords * 4 + 5 * cap * (npad_ts / 4) + tiles_ts * 16 + 4ull * sample_ct + kKingOutStageBytes + (128ull << 20);
+  return tiles_ts * kKingTsTileAccWords * 4 + 9 * cap * (npad_ts / 4) + tiles_ts * 16 + 4ull * sample_ct + kKingOutStageBytes + (128ull << 20);
 }
 
 static int KingBegin(Pl2GpuCtx* ctx, uint32_t sample_ct, const uint32_t* order, uint32_t row_start, uint32_t row_end, uint32_t col_end, int algo, uint32_t max_variants_per_add, Pl2KingJob** job_ptr) {
@@ -560,7 +578,7 @@ static int KingBegin(Pl2GpuCtx* ctx, uint32_t sample_ct, const uint32_t* order, 
     return fail();
   }
   job->tile_cols = ts ? kKingTsCols : kTileCols;
-  if (BuildTileList(row_start, row_end, false, &job->tiles, job->tile_cols, col_end)) return fail();
+  if (BuildTileList(row_start, row_end, false, &job->tiles, job->tile_cols, col_end, ts)) return fail();
   if (order && (cudaMalloc(&job->d_order, 4ull * sample_ct) != cudaSuccess || cudaMemcpy(job->d_order, order, 4ull * sample_ct, cudaMemcpyHostToDevice) != cudaSuccess)) {
     set_error("pl2gpu_king_begin_mapped: position map upload failed: %s", cudaGetErrorString(cudaGetLastError()));
     return fail();
@@ -576,6 +594,11 @@ static int KingBegin(Pl2GpuCtx* ctx, uint32_t sample_ct, const uint32_t* order, 
     if (cudaMalloc(&job->d_raw_t[b], static_cast<uint64_t>(st0.sample_ct_padded) * (st0.variant_cap / 4)) != cudaSuccess) {
       cudaGetLastError();
       set_error("pl2gpu_king_begin: insufficient device memory for the sample-major genotype copy");
+      return fail();
+    }
+    if (ts && cudaMalloc(&job->d_col_planes[b], static_cast<uint64_t>(st0.sample_ct_padded) * (st0.variant_cap / 2)) != cudaSuccess) {
+      cudaGetLastError();
+      set_error("pl2gpu_king_begin: insufficient device memory for the column plane copy (%.1f GB per staged block); lower the variants per batch", static_cast<double>(st0.sample_ct_padded) * (st0.variant_cap / 2) / 1e9);
       return fail();
     }
   }
@@ -634,13 +657,35 @@ static int KingTsPrepAndLaunch(Pl2KingJob* job, uint32_t b, uint32_t cur, bool p
   uint32_t padded;
   PL2_TRY(job->ring.pad(b, cur, pad_valid_rows, kVariantPad, &padded));
   if (!job->tiles.tile_ct) return job->ring.mark_busy(b, c->copy_stream);  // nothing to count on this rank
-  geno_tile_rows_kernel<true><<<dim3(padded / 256, st.sample_ct_padded / 64), 256, 0, c->copy_stream>>>(st.d_raw, st.pitch, padded / 32, 0, job->d_raw_t[b]);
+  geno_tile_rows_kernel<true><<<dim3(padded / 256, st.sample_ct_padded / 64), 256, 0, c->copy_stream>>>(st.d_raw, st.pitch, padded / 32, 0, job->d_raw_t[b], job->d_col_planes[b]);
   c->launches++;
   PL2_CUDA_OK(cudaGetLastError());
   PL2_TRY(job->ring.fence(b));
   PL2_CUDA_OK(cudaEventRecord(job->ev_kernel_start[b], c->stream));
-  king_b1_kernel<<<job->tiles.tile_ct, kKwThreads, kKb1SmemBytes, c->stream>>>(job->d_raw_t[b], padded, job->tiles.d_tile_order, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->d_raw_acc);
-  c->launches++;
+  // tile pairs as 2-CTA clusters that share their plane copies, then the tiles without a partner
+  const uint8_t* raw_t = job->d_raw_t[b];
+  const uint8_t* planes = job->d_col_planes[b];
+  const uint32_t pair_tiles = job->tiles.pair_tile_ct, lone_tiles = job->tiles.tile_ct - pair_tiles;
+  if (pair_tiles) {
+    cudaLaunchConfig_t cfg = {};
+    cudaLaunchAttribute cluster = {};
+    cluster.id = cudaLaunchAttributeClusterDimension;
+    cluster.val.clusterDim.x = 2;
+    cluster.val.clusterDim.y = cluster.val.clusterDim.z = 1;
+    cfg.gridDim = dim3(pair_tiles);
+    cfg.blockDim = dim3(kKwThreads);
+    cfg.dynamicSmemBytes = kKb1SmemBytes;
+    cfg.stream = c->stream;
+    cfg.attrs = &cluster;
+    cfg.numAttrs = 1;
+    const uint32_t* order = job->tiles.d_tile_order;
+    PL2_CUDA_OK(cudaLaunchKernelEx(&cfg, king_b1_kernel<2>, raw_t, planes, padded, order, static_cast<const uint32_t*>(job->tiles.d_tile_rt), static_cast<const uint32_t*>(job->tiles.d_tile_tc), job->d_raw_acc));
+    c->launches++;
+  }
+  if (lone_tiles) {
+    king_b1_kernel<1><<<lone_tiles, kKwThreads, kKb1SmemBytes, c->stream>>>(raw_t, planes, padded, job->tiles.d_tile_order + pair_tiles, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->d_raw_acc);
+    c->launches++;
+  }
   PL2_CUDA_OK(cudaGetLastError());
   PL2_TRY(job->ring.mark_busy(b, c->stream));
   job->last_buf = static_cast<int>(b);
@@ -896,6 +941,17 @@ int pl2gpu_king_last_kernel_ms(Pl2KingJob* job, float* ms) {
   return 0;
 }
 
+int pl2gpu_king_last_planes(Pl2KingJob* job, void* dst, uint64_t bytes) {
+  if (!job || !dst || job->last_buf < 0 || bytes > static_cast<uint64_t>(job->ring.stage[0].sample_ct_padded) * (job->ring.stage[0].variant_cap / 2)) {
+    set_error("pl2gpu_king_last_planes: no default-algorithm launch recorded, or more bytes than the plane copy holds");
+    return 1;
+  }
+  PL2_CUDA_OK(cudaSetDevice(job->ctx->c.device));
+  PL2_CUDA_OK(cudaEventSynchronize(job->ring.ev_free[job->last_buf]));
+  PL2_CUDA_OK(cudaMemcpy(dst, job->d_col_planes[job->last_buf], bytes, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
 int pl2gpu_king_end(Pl2KingJob* job) {
   if (!job) return 0;
   if (job->ctx) {
@@ -909,6 +965,7 @@ int pl2gpu_king_end(Pl2KingJob* job) {
   for (int b = 0; b < 2; ++b) {
     if (job->ev_kernel_start[b]) cudaEventDestroy(job->ev_kernel_start[b]);
     cudaFree(job->d_raw_t[b]);
+    cudaFree(job->d_col_planes[b]);
   }
   cudaFree(job->d_order);
   cudaFree(job->d_unmapped);

@@ -69,6 +69,33 @@ __device__ __forceinline__ void mbar_arrive_expect_tx(uint32_t bar, uint32_t byt
 __device__ __forceinline__ void bulk_copy_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
 }
+// The same copy written to the same shared-memory offset of every CTA of the cluster in `cta_mask`; each
+// destination's mbarrier at offset `bar` receives the bytes that land in that CTA.
+__device__ __forceinline__ void bulk_copy_g2s_multicast(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint16_t cta_mask) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(dst), "l"(src), "r"(bytes), "r"(bar), "h"(cta_mask) : "memory");
+}
+
+// ---- thread-block clusters
+__device__ __forceinline__ uint32_t cluster_cta_rank() {
+  uint32_t r;
+  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
+  return r;
+}
+// every thread of every CTA of the cluster: writes before -> visible after, in all of them
+__device__ __forceinline__ void cluster_sync() {
+  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
+}
+// arrive on the mbarrier at shared-window offset `bar` of cluster CTA `cta` (this CTA included); release at CTA
+// scope, like mbar_arrive: a cluster-scope release would fence every global access of the thread (MEMBAR.ALL.GPU)
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
+  asm volatile(
+      "{\n\t.reg .b32 remote;\n\t"
+      "mapa.shared::cluster.u32 remote, %0, %1;\n\t"
+      "mbarrier.arrive.shared::cluster.b64 _, [remote];\n\t}" ::"r"(bar),
+      "r"(cta)
+      : "memory");
+}
+
 // move registers between the warpgroups of a warp-specialised kernel (values: multiples of 8 in [24, 256])
 template <uint32_t kRegs>
 __device__ __forceinline__ void setmaxnreg_dec() {

@@ -166,6 +166,12 @@ class KingJob:
         check(lib.pl2gpu_king_last_kernel_ms(self._h, C.byref(ms)), "pl2gpu_king_last_kernel_ms")
         return float(ms.value)
 
+    def last_planes(self, nbytes: int) -> np.ndarray:
+        """The first nbytes of the column plane copy the last default-algorithm launch read (geno_tile.cuh)."""
+        out = np.empty(nbytes, dtype=np.uint8)
+        check(lib.pl2gpu_king_last_planes(self._h, out.ctypes.data, nbytes), "pl2gpu_king_last_planes")
+        return out
+
     def counts(self, row_start: int = None, row_end: int = None) -> np.ndarray:
         r0 = self.row_start if row_start is None else row_start
         r1 = self.row_end if row_end is None else row_end
