@@ -63,7 +63,10 @@ struct KingWgShape {
   static_assert(kSmemBytes <= kKwSmemLimit, "exceeds the 227 KB shared-memory opt-in limit");
 };
 
-template <int N>
+// kRed = false: a load and a store per accumulator; true: one fire-and-forget `red.global.add.s32` instead, so the
+// thread waits for no load round trip (integer addition is exact and order-free; the kernel boundary orders the
+// reductions before anything that reads the counts)
+template <int N, bool kRed = false>
 __device__ __forceinline__ void king_acc_add(int32_t* base, const int32_t (&d)[N / 2], uint32_t r, uint32_t c, int j0 = 0) {
   // base -> accumulator column 0 of this block, row 0 of the tile; fragment (j, i): column 8 j + 2 c + (i & 1),
   // row r + 8 (i >> 1); column groups j < j0 are skipped
@@ -73,7 +76,11 @@ __device__ __forceinline__ void king_acc_add(int32_t* base, const int32_t (&d)[N
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
       int32_t* p = base + static_cast<uint64_t>(8 * j + 2 * c + (i & 1)) * kTileRows + r + 8 * (i >> 1);
-      *p += d[4 * j + i];
+      if constexpr (kRed) {
+        asm volatile("red.global.add.s32 [%0], %1;" ::"l"(p), "r"(d[4 * j + i]) : "memory");
+      } else {
+        *p += d[4 * j + i];
+      }
     }
   }
 }
@@ -267,7 +274,12 @@ king_wg_kernel(const uint8_t* __restrict__ raw_t, uint32_t variant_ct_padded /* 
 // CTA copies its own row words and half of every plane image, multicast into both CTAs, so a tile still reads
 // 12 KB from L2 per k256 step (8 KB of rows, 4 KB of planes).  A CTA's `full` barrier therefore also counts the
 // partner's bytes, and a producer may refill a slot only once the consumers of both CTAs have released it: every
-// consumer warp arrives on `empty` of both CTAs.  The tiles without a partner run with kCluster = 1.
+// consumer warp arrives on `empty` of both CTAs.  The tiles without a partner run with kCluster = 1.  The cluster
+// barrier after the barrier set-up keeps copies and remote arrivals away from a barrier that is not yet initialised;
+// the one before exit keeps a CTA alive while its partner may still copy into it or arrive on it.
+// The epilogue adds the tile's counts with `red.global.add` (king_acc_add<.., true>): nothing waits for a load, and
+// the consumers arrive on the exit barrier before it and wait after it, so the barrier's release fence does not wait
+// for the reductions either.
 constexpr uint32_t kKb1Ks = 2;       // k256 steps per stage
 constexpr uint32_t kKb1Stages = 7;
 constexpr uint32_t kKb1Sbo = 2 * kKwChunkBytes;                          // next group of 8 samples of a plane image
@@ -431,20 +443,23 @@ king_b1_kernel(const uint8_t* __restrict__ raw_t, const uint8_t* __restrict__ pl
     prev_slot = slot;
     slot = next_slot, phase = next_phase;
   }
+  // the exit barrier's arrive: this thread's last remote arrival is behind it, and its release (a fence of every
+  // global access in flight) comes before the epilogue's reductions
+  if constexpr (kCluster > 1) cluster_arrive();
   wgmma_wait<0>();
   wgmma_fence_operand(acc_t);
   wgmma_fence_operand(acc_h);
   wgmma_fence_operand(acc_i);
 
-  // ---- epilogue: registers -> raw accumulators (+=); rows are in natural sample order.  HH column 8 j + .. sits
-  // in acc_h[32 + 4 j + i], the IBS0 of the same pair in acc_i[4 j + i]: SS = HH - 2 IBS0 in place.
+  // ---- epilogue: registers -> raw accumulators (red.global.add); rows are in natural sample order.  HH column
+  // 8 j + .. sits in acc_h[32 + 4 j + i], the IBS0 of the same pair in acc_i[4 j + i]: SS = HH - 2 IBS0 in place.
 #pragma unroll
   for (uint32_t i = 0; i < kKingTsCols / 2; ++i) acc_i[i] = acc_h[kKingTsCols / 2 + i] - 2 * acc_i[i];
   int32_t* acc_tile = raw_acc + static_cast<uint64_t>(tile) * kKingTsTileAccWords;
-  king_acc_add<2 * kKingTsCols>(acc_tile, acc_t, r_lo, c);                                                   // TT | TH
-  king_acc_add<2 * kKingTsCols>(acc_tile + static_cast<uint64_t>(2 * kKingTsCols) * kTileRows, acc_h, r_lo, c);  // HT | HH
-  king_acc_add<kKingTsCols>(acc_tile + static_cast<uint64_t>(4 * kKingTsCols) * kTileRows, acc_i, r_lo, c);      // SS
-  if constexpr (kCluster > 1) cluster_sync();
+  king_acc_add<2 * kKingTsCols, true>(acc_tile, acc_t, r_lo, c);                                                   // TT | TH
+  king_acc_add<2 * kKingTsCols, true>(acc_tile + static_cast<uint64_t>(2 * kKingTsCols) * kTileRows, acc_h, r_lo, c);  // HT | HH
+  king_acc_add<kKingTsCols, true>(acc_tile + static_cast<uint64_t>(4 * kKingTsCols) * kTileRows, acc_i, r_lo, c);      // SS
+  if constexpr (kCluster > 1) cluster_wait();
 }
 
 }  // namespace pl2

@@ -85,6 +85,10 @@ __device__ __forceinline__ uint32_t cluster_cta_rank() {
 __device__ __forceinline__ void cluster_sync() {
   asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
 }
+// the same in two halves: the release in the arrive fences every global access in flight (MEMBAR.ALL.GPU), so work
+// placed between them, such as global reductions, is not waited for
+__device__ __forceinline__ void cluster_arrive() { asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory"); }
+__device__ __forceinline__ void cluster_wait() { asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory"); }
 // arrive on the mbarrier at shared-window offset `bar` of cluster CTA `cta` (this CTA included); release at CTA
 // scope, like mbar_arrive: a cluster-scope release would fence every global access of the thread (MEMBAR.ALL.GPU)
 __device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
