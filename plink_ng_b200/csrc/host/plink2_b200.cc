@@ -23,6 +23,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <limits>
+#include <memory>
 #include <ctime>
 #include <string>
 #include <thread>
@@ -845,6 +846,11 @@ bool WriteIdFile(const std::string& path, const SampleInfo& s, const std::vector
   }
   return f.Close();
 }
+bool WriteAllIds(const std::string& path, const SampleInfo& s, bool header) {
+  std::vector<uint32_t> all(s.size());
+  for (uint32_t k = 0; k < s.size(); ++k) all[k] = k;
+  return WriteIdFile(path, s, all, header);
+}
 
 // ---- genotype block streaming: decode `idx` variants into a pinned host buffer ----
 // host threads for genotype decoding: --threads if given, else min(affinity mask, cgroup CPU quota), at most 64
@@ -877,6 +883,7 @@ struct BlockStreamer {
   size_t pos = 0;
   uint32_t spare = 0;  // extra rows behind the block (filler for sharded uploads)
   uint32_t threads = 0;  // decode threads for this streamer (0: g_decode_threads)
+  double decode_s = 0;  // time spent in Next
   BlockStreamer(Dataset* d, const std::vector<uint32_t>* v, uint32_t n_samples, uint32_t batch, uint32_t spare_rows = 0) : ds(d), vidx(v), sample_ct(n_samples), words(PgenReader::WordsFor(n_samples)), cap(batch), spare(spare_rows) {}
   ~BlockStreamer() { pl2gpu_host_free(buf); }
   bool Init() {
@@ -890,7 +897,9 @@ struct BlockStreamer {
   int Next(std::string* err) {
     const uint32_t n = static_cast<uint32_t>(std::min<size_t>(cap, vidx->size() - pos));
     if (!n) return 0;
+    const auto t = std::chrono::steady_clock::now();
     if (!ds->reader.GetBlock(vidx->data() + pos, n, sample_include, sample_ct, buf, words, threads ? threads : g_decode_threads, err)) return -1;
+    decode_s += g_clock.Since(t);
     pos += n;
     return static_cast<int>(n);
   }
@@ -986,6 +995,199 @@ std::vector<uint32_t> TileAlignedBounds(uint32_t r0, uint32_t r1, uint32_t parts
   }
   return b;
 }
+
+// ------------------------------------------------------------------------------------------ relationship drivers
+// Device jobs end (pl2gpu_*_end) when their owner goes out of scope.  An owner is declared after the GpuTeam whose
+// context its job runs on, so that the job ends before the context is destroyed.
+template <class J, int (*End)(J*)>
+struct JobEnd {
+  void operator()(J* job) const { End(job); }
+};
+using KingJob = std::unique_ptr<Pl2KingJob, JobEnd<Pl2KingJob, pl2gpu_king_end>>;
+using KingPairJob = std::unique_ptr<Pl2KingPairJob, JobEnd<Pl2KingPairJob, pl2gpu_king_pairs_end>>;
+using GrmJob = std::unique_ptr<Pl2GrmJob, JobEnd<Pl2GrmJob, pl2gpu_grm_end>>;
+using PcaJob = std::unique_ptr<Pl2PcaJob, JobEnd<Pl2PcaJob, pl2gpu_pca_end>>;
+
+// The variants KING and the GRM are computed over (KeptForRelationship); `what` names the calculation in the log.
+int RelationshipVariants(const Dataset& ds, const char* what, std::vector<uint32_t>* vidx) {
+  vidx->clear();
+  uint32_t non_auto = 0;
+  for (uint32_t v = 0; v < ds.variants.size(); ++v) {
+    if (KeptForRelationship(ds.variants.chr_code[v])) vidx->push_back(v);
+    else ++non_auto;
+  }
+  if (non_auto) logprintf("Excluding %u variant%s on non-autosomes from %s.\n", non_auto, non_auto == 1 ? "" : "s", what);
+  if (vidx->empty()) {
+    logprintf("Error: No variants remaining for %s.\n", what);
+    return kRetDegenerateData;
+  }
+  return 0;
+}
+
+// f(got) for every block bs decodes from the start of its variant list; a decode error is logged and ends the stream
+// with kRetMalformedInput.  f returns 0 or a kRet* code, which ends the stream too.
+template <class F>
+int StreamBlocks(BlockStreamer* bs, F&& f) {
+  bs->Rewind();
+  std::string err;
+  for (;;) {
+    const int got = bs->Next(&err);
+    if (got < 0) {
+      logprintf("\nError: %s\n", err.c_str());
+      return kRetMalformedInput;
+    }
+    if (!got) return 0;
+    const int rc = f(static_cast<uint32_t>(got));
+    if (rc) return rc;
+  }
+}
+
+// --gpus: device g adds rows [g * per, (g + 1) * per) of the decoded block through add(g, slice, per), one host thread
+// per device, and the library all-gathers the column tile.  The filler rows that top the block up to per * G are
+// all-missing and count nothing (bs has G spare rows behind the block).  Returns ForEachRank's code and error text.
+template <class F>
+int AddSharded(BlockStreamer* bs, uint32_t got, uint32_t G, F&& add, std::string* err) {
+  const uint32_t per = (got + G - 1) / G;
+  memset(bs->buf + static_cast<uint64_t>(got) * bs->words, 0xFF, static_cast<uint64_t>(per * G - got) * bs->words * 8);
+  return ForEachRank(G, [&](uint32_t g) { return add(g, bs->buf + static_cast<uint64_t>(g) * per * bs->words, per); }, err);
+}
+
+// KING pass planning (CountTrianglePasses / NextTrianglePass, :216-255) for rows [r0, r1).  The budget is the least
+// free device memory over `ctxs` less 10 %, capped by --gpu-memory.  Variants per staged block: the full 65,536 unless
+// `block_copies` buffers of that size (the staged blocks and their device-side copies) would take more than a quarter
+// of the budget; then halved until they fit.  Every pass is the largest row block from its start whose device memory,
+// need(a, b, batch), fits the budget.  Returns 0 or a kRet* code after logging.
+template <class Need>
+int PlanKingPasses(const Cmd& c, const std::vector<Pl2GpuCtx*>& ctxs, const char* flagname, uint32_t n, uint32_t r0, uint32_t r1, uint32_t block_copies, Need&& need, uint32_t* batch, std::vector<uint32_t>* bounds) {
+  uint64_t free_b = ~0ull;
+  for (Pl2GpuCtx* cx : ctxs) {
+    uint64_t f = 0, t = 0;
+    if (pl2gpu_ctx_mem_info(cx, &f, &t)) return GpuFail("pl2gpu_ctx_mem_info");
+    free_b = std::min(free_b, f);
+  }
+  uint64_t budget = free_b - free_b / 10;
+  if (c.gpu_memory_mib && (c.gpu_memory_mib << 20) < budget) budget = c.gpu_memory_mib << 20;
+  *batch = 65536;
+  while (*batch > 2048 && static_cast<uint64_t>(block_copies) * *batch * ((n + 639) / 640 * 160) > budget / 4) *batch /= 2;
+  auto fits = [&](uint32_t a, uint32_t b) { return need(a, b, *batch) <= budget; };
+  bounds->assign(1, r0);
+  while (bounds->back() < r1) {
+    const uint32_t r = bounds->back();
+    if (!fits(r, r + 1)) {
+      logprintf("Error: Insufficient GPU memory for %s on %u samples.\n", flagname, n);
+      return kRetNomem;
+    }
+    uint32_t lo = r + 1, hi = r1;
+    while (lo < hi) {
+      const uint32_t mid = lo + (hi - lo + 1) / 2;
+      if (fits(r, mid)) lo = mid;
+      else hi = mid - 1;
+    }
+    bounds->push_back(lo);
+  }
+  const uint32_t pass_ct = static_cast<uint32_t>(bounds->size() - 1);
+  if (pass_ct > 1) logprintf("%s: %u passes over the variants (device accumulators planned against %llu MiB).\n", flagname, pass_ct, static_cast<unsigned long long>(budget >> 20));
+  return 0;
+}
+
+// KING pairs (j, i) with i < min(j, col_end) over the rows j < r
+uint64_t KingPairsBelow(uint64_t r, uint64_t col_end) { return r <= col_end ? (r ? r * (r - 1) / 2 : 0) : (col_end ? col_end * (col_end - 1) / 2 : 0) + (r - col_end) * col_end; }
+
+// The pairs of rows [r0, r1) whose kinship is at least `threshold` (pl2gpu_king_get_filtered), the buffers grown until
+// all of them fit: pair q is (pairs[2q], pairs[2q + 1]) with counts[5q..5q + 4] and kin[q], q < found.
+int FetchKingFiltered(Pl2KingJob* job, uint32_t r0, uint32_t r1, double threshold, std::vector<uint32_t>* pairs, std::vector<uint32_t>* counts, std::vector<double>* kin, uint64_t* found) {
+  uint64_t cap = 1ull << 22;
+  for (;;) {
+    pairs->resize(cap * 2);
+    counts->resize(cap * 5);
+    kin->resize(cap);
+    if (pl2gpu_king_get_filtered(job, r0, r1, threshold, cap, pairs->data(), counts->data(), kin->data(), found)) return GpuFail("pl2gpu_king_get_filtered");
+    if (*found <= cap) return 0;
+    cap = *found;
+  }
+}
+
+// Rows [r0, r1) of a KING job in chunks of at most ~512 MB of counts: f(c0, c1, pair_ct, counts) per chunk, counts =
+// the chunk's counts[pair][5] in the library's pair order (KingPairsBelow), or unfetched when with_counts is false.
+// f returns 0 or a kRet* code.
+template <class F>
+int ForEachKingCountChunk(Pl2KingJob* job, uint32_t r0, uint32_t r1, uint32_t col_end, bool with_counts, F&& f) {
+  const uint64_t max_pairs = (512ull << 20) / 20;
+  std::vector<uint32_t> counts;
+  for (uint32_t c0 = r0; c0 < r1;) {
+    uint32_t c1 = c0 + 1;
+    while (c1 < r1 && KingPairsBelow(c1 + 1, col_end) - KingPairsBelow(c0, col_end) <= max_pairs) ++c1;
+    const uint64_t pair_ct = KingPairsBelow(c1, col_end) - KingPairsBelow(c0, col_end);
+    if (with_counts) {
+      counts.resize(pair_ct * 5);
+      if (pair_ct && pl2gpu_king_get_counts(job, c0, c1, counts.data(), 0)) return GpuFail("pl2gpu_king_get_counts");
+    }
+    const int rc = f(c0, c1, pair_ct, counts.data());
+    if (rc) return rc;
+    c0 = c1;
+  }
+  return 0;
+}
+
+// --make-king / --make-rel matrix writer (shapes triangle, square0, square; encodings text, bin4, bin) fed the rows of
+// the lower triangle in order: Row(j, v, diag) with v[0..j-1] the values left of the diagonal.  `triangle` writes each
+// row through its diagonal when tri_diag is set (REL), else without it (KING, whose triangle starts at row 1);
+// square0 pads every row with zeros to n columns; square keeps the lower triangle with its diagonal, and Finish()
+// writes the mirrored n x n matrix.
+struct TriangleMatrixWriter {
+  OutFile* f;
+  uint32_t n;
+  Cmd::Shape shape;
+  Cmd::Enc enc;
+  bool tri_diag;
+  std::vector<double> full;  // square: row j at j * (j + 1) / 2
+  std::vector<float> rowf;
+  std::vector<double> rowd;
+  TriangleMatrixWriter(OutFile* file, uint32_t n_samples, Cmd::Shape s, Cmd::Enc e, bool diag) : f(file), n(n_samples), shape(s), enc(e), tri_diag(diag), rowf(e == Cmd::kBin4 ? n : 0), rowd(e == Cmd::kBin ? n : 0) {
+    if (shape == Cmd::kSq) full.resize(static_cast<uint64_t>(n) * (n + 1) / 2);
+  }
+  void Row(uint32_t j, const double* v, double diag) {
+    if (shape == Cmd::kSq) {
+      double* dst = &full[static_cast<uint64_t>(j) * (j + 1) / 2];
+      memcpy(dst, v, sizeof(double) * j);
+      dst[j] = diag;
+    } else {
+      Put(v, j, (shape == Cmd::kSq0 || tri_diag) ? &diag : nullptr, shape == Cmd::kSq0 ? n : j + tri_diag);
+    }
+  }
+  void Finish() {
+    if (shape != Cmd::kSq) return;
+    std::vector<double> row(n);
+    for (uint32_t j = 0; j < n; ++j) {
+      for (uint32_t i = 0; i < n; ++i) row[i] = i <= j ? full[static_cast<uint64_t>(j) * (j + 1) / 2 + i] : full[static_cast<uint64_t>(i) * (i + 1) / 2 + j];
+      Put(row.data(), n, nullptr, n);
+    }
+  }
+  // one row of len values: v[0..nv-1], then *diag unless it is null, then zeros
+  void Put(const double* v, uint32_t nv, const double* diag, uint32_t len) {
+    if (!len) return;
+    const uint32_t nd = nv + (diag != nullptr);
+    if (enc == Cmd::kText) {
+      char* w = f->Reserve(static_cast<size_t>(n) * 16 + 64);
+      for (uint32_t i = 0; i < len; ++i) {
+        w = dtoa_g(i < nv ? v[i] : (i < nd ? *diag : 0.0), w);
+        *w++ = '\t';
+      }
+      w[-1] = '\n';
+      f->Advance(w);
+    } else if (enc == Cmd::kBin4) {
+      for (uint32_t i = 0; i < nv; ++i) rowf[i] = static_cast<float>(v[i]);
+      if (diag) rowf[nv] = static_cast<float>(*diag);
+      std::fill(rowf.begin() + nd, rowf.begin() + len, 0.0f);
+      f->Write(rowf.data(), sizeof(float) * len);
+    } else {
+      memcpy(rowd.data(), v, sizeof(double) * nv);
+      if (diag) rowd[nv] = *diag;
+      std::fill(rowd.begin() + nd, rowd.begin() + len, 0.0);
+      f->Write(rowd.data(), sizeof(double) * len);
+    }
+  }
+};
 
 // ------------------------------------------------------------------------------------------ KING
 // KinshipPruneDestructive (2.0/plink2_matrix_calc.cc:278-391): while edges remain, remove the
@@ -1083,6 +1285,28 @@ std::string KingTableHeader(const Cmd& c, const IdFmt& idf) {
   if (c.col_kinship) h += "KINSHIP\t";
   h.back() = '\n';
   return h;
+}
+
+// Opens this --parallel piece's --make-king-table output; the first piece writes the header.
+bool OpenKingTable(const Cmd& c, const IdFmt& idf, OutFile* ftab, std::string* name) {
+  *name = PieceName(c.out + ".kin0", c) + (c.king_table_zs ? ".zst" : "");
+  if (!ftab->Open(*name, c.king_table_zs)) {
+    logprintf("Error: Failed to open %s for writing.\n", name->c_str());
+    return false;
+  }
+  if (!c.parallel_idx) ftab->Puts(KingTableHeader(c, idf).c_str());
+  return true;
+}
+
+// The end of a pair-list or --king-table-require table of pair_ct pairs, `filtered` of them left out by
+// --king-table-filter.
+int CloseKingTable(const Cmd& c, OutFile* ftab, const std::string& name, size_t variant_ct, uint64_t pair_ct, uint64_t filtered) {
+  if (!ftab->Close()) return kRetWriteFail;
+  printf("\r");
+  logprintf("--make-king-table: %u variant%s processed.\n", static_cast<uint32_t>(variant_ct), variant_ct == 1 ? "" : "s");
+  logprintf("Results written to %s .\n", name.c_str());
+  if (c.king_table_filter != -DBL_MAX) logprintf("--king-table-filter: %llu relationship%s reported (%llu filtered out).\n", static_cast<unsigned long long>(pair_ct - filtered), (pair_ct - filtered == 1) ? "" : "s", static_cast<unsigned long long>(filtered));
+  return 0;
 }
 
 // One .kin0 line (:2285-2364 / :3705-3760): cc = {IBS0, HETHET, HET2HOM1, HET1HOM2, HOMHOM}.
@@ -1324,16 +1548,8 @@ int RunKingSubset(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, bool rel_check) {
     return kRetDegenerateData;
   }
   std::vector<uint32_t> vidx;
-  uint32_t non_auto = 0;
-  for (uint32_t v = 0; v < ds->variants.size(); ++v) {
-    if (KeptForRelationship(ds->variants.chr_code[v])) vidx.push_back(v);
-    else ++non_auto;
-  }
-  if (non_auto) logprintf("Excluding %u variant%s on non-autosomes from KING-robust calculation.\n", non_auto, non_auto == 1 ? "" : "s");
-  if (vidx.empty()) {
-    logprintf("Error: No variants remaining for KING-robust calculation.\n");
-    return kRetDegenerateData;
-  }
+  const int vrc = RelationshipVariants(*ds, "KING-robust calculation", &vidx);
+  if (vrc) return vrc;
   std::vector<uint8_t> req;
   if (!c.king_table_require.empty()) {
     const int rrc = LoadKingRequire(c, S, &req);
@@ -1458,38 +1674,23 @@ int RunKingSubset(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, bool rel_check) {
   }
   logprintf("%s: %llu pair%s loaded.\n", c.king_table_subset.empty() ? "--make-king-table rel-check" : "--king-table-subset", static_cast<unsigned long long>(pair_ct), pair_ct == 1 ? "" : "s");
   const IdFmt idf = KingIdFmt(c, S);
-  const std::string tab_name = c.out + (c.king_table_zs ? ".kin0.zst" : ".kin0");
+  std::string tab_name;
   OutFile ftab;
-  if (!ftab.Open(tab_name, c.king_table_zs)) {
-    logprintf("Error: Failed to open %s for writing.\n", tab_name.c_str());
-    return kRetOpenFail;
-  }
-  ftab.Puts(KingTableHeader(c, idf).c_str());
-  Pl2KingPairJob* job = nullptr;
-  if (pl2gpu_king_pairs_begin(ctx, n, pairs.data(), pair_ct, &job)) return GpuFail("pl2gpu_king_pairs_begin");
+  if (!OpenKingTable(c, idf, &ftab, &tab_name)) return kRetOpenFail;
+  Pl2KingPairJob* pair_job = nullptr;
+  if (pl2gpu_king_pairs_begin(ctx, n, pairs.data(), pair_ct, &pair_job)) return GpuFail("pl2gpu_king_pairs_begin");
+  const KingPairJob job(pair_job);
   BlockStreamer bs(ds, &vidx, n, 32768);
-  if (!bs.Init()) {
-    pl2gpu_king_pairs_end(job);
-    return GpuFail("pl2gpu_host_alloc");
-  }
-  std::string err;
+  if (!bs.Init()) return GpuFail("pl2gpu_host_alloc");
   uint32_t done = 0;
-  for (;;) {
-    const int got = bs.Next(&err);
-    if (got < 0) {
-      logprintf("\nError: %s\n", err.c_str());
-      pl2gpu_king_pairs_end(job);
-      return kRetMalformedInput;
-    }
-    if (!got) break;
-    if (pl2gpu_king_pairs_add_variants(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0)) {
-      pl2gpu_king_pairs_end(job);
-      return GpuFail("pl2gpu_king_pairs_add_variants");
-    }
-    done += static_cast<uint32_t>(got);
+  const int src = StreamBlocks(&bs, [&](uint32_t got) -> int {
+    if (pl2gpu_king_pairs_add_variants(job.get(), bs.buf, static_cast<uint64_t>(bs.words) * 8, got, 0)) return GpuFail("pl2gpu_king_pairs_add_variants");
+    done += got;
     printf("\r--make-king-table pass 1: %u variants complete.", done);
     fflush(stdout);
-  }
+    return 0;
+  });
+  if (src) return src;
   printf("\r--make-king-table pass 1: Writing...                   ");
   fflush(stdout);
   std::vector<uint32_t> counts;
@@ -1498,10 +1699,7 @@ int RunKingSubset(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, bool rel_check) {
   for (uint64_t p0 = 0; p0 < pair_ct; p0 += chunk) {
     const uint64_t p1 = std::min(pair_ct, p0 + chunk);
     counts.resize((p1 - p0) * 5);
-    if (pl2gpu_king_pairs_get_counts(job, p0, p1, counts.data(), 0)) {
-      pl2gpu_king_pairs_end(job);
-      return GpuFail("pl2gpu_king_pairs_get_counts");
-    }
+    if (pl2gpu_king_pairs_get_counts(job.get(), p0, p1, counts.data(), 0)) return GpuFail("pl2gpu_king_pairs_get_counts");
     for (uint64_t p = p0; p < p1; ++p) {
       const uint32_t* cc = &counts[(p - p0) * 5];
       const double kinship = KinshipFromCounts(cc);
@@ -1512,15 +1710,7 @@ int RunKingSubset(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, bool rel_check) {
       WriteKingTableRow(c, FmtId(S, pairs[2 * p], idf), FmtId(S, pairs[2 * p + 1], idf), cc, kinship, &ftab);
     }
   }
-  pl2gpu_king_pairs_end(job);
-  if (!ftab.Close()) return kRetWriteFail;
-  printf("\r");
-  logprintf("--make-king-table: %u variant%s processed.\n", static_cast<uint32_t>(vidx.size()), vidx.size() == 1 ? "" : "s");
-  logprintf("Results written to %s .\n", tab_name.c_str());
-  if (c.king_table_filter != -DBL_MAX) {
-    logprintf("--king-table-filter: %llu relationship%s reported (%llu filtered out).\n", static_cast<unsigned long long>(pair_ct - filter_ct), (pair_ct - filter_ct == 1) ? "" : "s", static_cast<unsigned long long>(filter_ct));
-  }
-  return 0;
+  return CloseKingTable(c, &ftab, tab_name, vidx.size(), pair_ct, filter_ct);
 }
 
 // --king-table-require[-xor] without a pair list (GetRelCheckOrKTRequirePairs' require branch, :3045-3160): in natural
@@ -1543,8 +1733,7 @@ int RunKingRequireDense(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, const std::ve
   for (uint32_t k = 0; k < n; ++k)
     if (req[k]) order.push_back(k);
   const uint32_t col_end = c.king_table_require_xor ? n0 : n;
-  auto pairs_below = [col_end](uint64_t r) { return r <= col_end ? (r ? r * (r - 1) / 2 : 0) : (col_end ? static_cast<uint64_t>(col_end) * (col_end - 1) / 2 : 0) + (r - col_end) * col_end; };
-  const uint64_t pair_ct = pairs_below(n) - pairs_below(n0);
+  const uint64_t pair_ct = KingPairsBelow(n, col_end) - KingPairsBelow(n0, col_end);
   const bool filter = c.king_table_filter != -DBL_MAX;
   logprintf("--king-table-require%s: %llu pair%s on the device (rows %u-%u of the sample order with the required samples last).\n", c.king_table_require_xor ? "-xor" : "", static_cast<unsigned long long>(pair_ct), pair_ct == 1 ? "" : "s", n0, n - 1);
   if (!filter) logprintf("--king-table-require%s: the unfiltered table is sorted in host memory (%.1f MB) before it is written.\n", c.king_table_require_xor ? "-xor" : "", pair_ct * 28.0 / 1e6);
@@ -1553,31 +1742,12 @@ int RunKingRequireDense(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, const std::ve
     const std::vector<uint32_t> nat = NaturalSampleOrder(S);
     for (uint32_t r = 0; r < n; ++r) rank[nat[r]] = r;
   }
-  // pass planning against free device memory (or --gpu-memory), as RunKing does; each pass re-streams the variants
-  uint64_t free_b = 0, total_b = 0;
-  if (pl2gpu_ctx_mem_info(ctx, &free_b, &total_b)) return GpuFail("pl2gpu_ctx_mem_info");
-  uint64_t budget = free_b - free_b / 10;
-  if (c.gpu_memory_mib && (c.gpu_memory_mib << 20) < budget) budget = c.gpu_memory_mib << 20;
-  uint32_t batch = 65536;
-  while (batch > 2048 && 5ull * batch * ((n + 639) / 640 * 160) > budget / 4) batch /= 2;
-  auto fits = [&](uint32_t a, uint32_t b) { return pl2gpu_king_mapped_mem_required(n, a, b, col_end, batch) <= budget; };
-  std::vector<uint32_t> bounds{n0};
-  while (bounds.back() < n) {
-    const uint32_t r = bounds.back();
-    if (!fits(r, r + 1)) {
-      logprintf("Error: Insufficient GPU memory for --make-king-table on %u samples.\n", n);
-      return kRetNomem;
-    }
-    uint32_t lo = r + 1, hi = n;
-    while (lo < hi) {
-      const uint32_t mid = lo + (hi - lo + 1) / 2;
-      if (fits(r, mid)) lo = mid;
-      else hi = mid - 1;
-    }
-    bounds.push_back(lo);
-  }
+  // pass planning as in RunKing; each pass re-streams the variants
+  uint32_t batch = 0;
+  std::vector<uint32_t> bounds;
+  const int prc = PlanKingPasses(c, {ctx}, "--make-king-table", n, n0, n, 5, [&](uint32_t a, uint32_t b, uint32_t bt) { return pl2gpu_king_mapped_mem_required(n, a, b, col_end, bt); }, &batch, &bounds);
+  if (prc) return prc;
   const uint32_t pass_ct = static_cast<uint32_t>(bounds.size() - 1);
-  if (pass_ct > 1) logprintf("--make-king-table: %u passes over the variants (device accumulators planned against %llu MiB).\n", pass_ct, static_cast<unsigned long long>(budget >> 20));
   struct Row {
     uint32_t r1, r2;  // natural-order ranks of the sample listed first (the larger) and second
     uint32_t cc[5];
@@ -1603,87 +1773,47 @@ int RunKingRequireDense(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, const std::ve
   if (!bs.Init()) return GpuFail("pl2gpu_host_alloc");
   for (uint32_t pass = 1; pass <= pass_ct; ++pass) {
     const uint32_t p0 = bounds[pass - 1], p1 = bounds[pass];
-    Pl2KingJob* job = nullptr;
-    if (pl2gpu_king_begin_mapped(ctx, n, order.data(), p0, p1, col_end, batch, &job)) return GpuFail("pl2gpu_king_begin_mapped");
-    bs.Rewind();
-    std::string err;
+    Pl2KingJob* mapped_job = nullptr;
+    if (pl2gpu_king_begin_mapped(ctx, n, order.data(), p0, p1, col_end, batch, &mapped_job)) return GpuFail("pl2gpu_king_begin_mapped");
+    const KingJob job(mapped_job);
     uint32_t done = 0;
-    for (;;) {
-      const int got = bs.Next(&err);
-      if (got < 0) {
-        logprintf("\nError: %s\n", err.c_str());
-        pl2gpu_king_end(job);
-        return kRetMalformedInput;
-      }
-      if (!got) break;
-      if (pl2gpu_king_add_variants(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0)) {
-        pl2gpu_king_end(job);
-        return GpuFail("pl2gpu_king_add_variants");
-      }
-      done += static_cast<uint32_t>(got);
+    int rc = StreamBlocks(&bs, [&](uint32_t got) -> int {
+      if (pl2gpu_king_add_variants(job.get(), bs.buf, static_cast<uint64_t>(bs.words) * 8, got, 0)) return GpuFail("pl2gpu_king_add_variants");
+      done += got;
       printf("\r--make-king-table pass %u/%u: %u variants complete.", pass, pass_ct, done);
       fflush(stdout);
-    }
+      return 0;
+    });
+    if (rc) return rc;
     if (filter) {
       std::vector<uint32_t> fp, fc;
       std::vector<double> fk;
-      uint64_t cap = 1ull << 22, found = 0;
-      for (;;) {
-        fp.resize(cap * 2);
-        fc.resize(cap * 5);
-        fk.resize(cap);
-        if (pl2gpu_king_get_filtered(job, p0, p1, c.king_table_filter, cap, fp.data(), fc.data(), fk.data(), &found)) {
-          pl2gpu_king_end(job);
-          return GpuFail("pl2gpu_king_get_filtered");
-        }
-        if (found <= cap) break;
-        cap = found;
-      }
+      uint64_t found = 0;
+      rc = FetchKingFiltered(job.get(), p0, p1, c.king_table_filter, &fp, &fc, &fk, &found);
+      if (rc) return rc;
       for (uint64_t q = 0; q < found; ++q) add_row(fp[2 * q], fp[2 * q + 1], &fc[5 * q]);
     } else {
-      const uint64_t max_pairs = (512ull << 20) / 20;
-      std::vector<uint32_t> counts;
-      for (uint32_t c0 = p0; c0 < p1;) {
-        uint32_t c1 = c0 + 1;
-        while (c1 < p1 && pairs_below(c1 + 1) - pairs_below(c0) <= max_pairs) ++c1;
-        counts.resize((pairs_below(c1) - pairs_below(c0)) * 5);
-        if (!counts.empty() && pl2gpu_king_get_counts(job, c0, c1, counts.data(), 0)) {
-          pl2gpu_king_end(job);
-          return GpuFail("pl2gpu_king_get_counts");
-        }
-        const uint32_t* cc = counts.data();
+      rc = ForEachKingCountChunk(job.get(), p0, p1, col_end, true, [&](uint32_t c0, uint32_t c1, uint64_t, const uint32_t* cc) {
         for (uint32_t pj = c0; pj < c1; ++pj)
           for (uint32_t pi = 0; pi < std::min(pj, col_end); ++pi, cc += 5) add_row(pj, pi, cc);
-        c0 = c1;
-      }
+        return 0;
+      });
+      if (rc) return rc;
     }
-    pl2gpu_king_end(job);
   }
   printf("\r--make-king-table: Writing...                   ");
   fflush(stdout);
   std::sort(rows.begin(), rows.end(), [](const Row& a, const Row& b) { return a.r1 != b.r1 ? a.r1 < b.r1 : a.r2 < b.r2; });
   const IdFmt idf = KingIdFmt(c, S);
-  const std::string tab_name = c.out + (c.king_table_zs ? ".kin0.zst" : ".kin0");
+  std::string tab_name;
   OutFile ftab;
-  if (!ftab.Open(tab_name, c.king_table_zs)) {
-    logprintf("Error: Failed to open %s for writing.\n", tab_name.c_str());
-    return kRetOpenFail;
-  }
-  ftab.Puts(KingTableHeader(c, idf).c_str());
+  if (!OpenKingTable(c, idf, &ftab, &tab_name)) return kRetOpenFail;
   {
     std::vector<uint32_t> by_rank(n);
     for (uint32_t k = 0; k < n; ++k) by_rank[rank[k]] = k;
     for (const Row& row : rows) WriteKingTableRow(c, FmtId(S, by_rank[row.r1], idf), FmtId(S, by_rank[row.r2], idf), row.cc, KinshipFromCounts(row.cc), &ftab);
   }
-  if (!ftab.Close()) return kRetWriteFail;
-  printf("\r");
-  logprintf("--make-king-table: %u variant%s processed.\n", static_cast<uint32_t>(vidx.size()), vidx.size() == 1 ? "" : "s");
-  logprintf("Results written to %s .\n", tab_name.c_str());
-  if (filter) {
-    const uint64_t kept = rows.size();
-    logprintf("--king-table-filter: %llu relationship%s reported (%llu filtered out).\n", static_cast<unsigned long long>(kept), kept == 1 ? "" : "s", static_cast<unsigned long long>(pair_ct - kept));
-  }
-  return 0;
+  return CloseKingTable(c, &ftab, tab_name, vidx.size(), pair_ct, pair_ct - rows.size());
 }
 
 int RunKing(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, std::vector<uint8_t>* cutoff_removed) {
@@ -1695,22 +1825,13 @@ int RunKing(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, std::vector<uint8_t>* cut
     return kRetDegenerateData;
   }
   std::vector<uint32_t> vidx;
-  uint32_t non_auto = 0;
-  for (uint32_t v = 0; v < ds->variants.size(); ++v) {
-    if (KeptForRelationship(ds->variants.chr_code[v])) vidx.push_back(v);
-    else ++non_auto;
-  }
-  if (non_auto) logprintf("Excluding %u variant%s on non-autosomes from KING-robust calculation.\n", non_auto, non_auto == 1 ? "" : "s");
-  if (vidx.empty()) {
-    logprintf("Error: No variants remaining for KING-robust calculation.\n");
-    return kRetDegenerateData;
-  }
+  const int vrc = RelationshipVariants(*ds, "KING-robust calculation", &vidx);
+  if (vrc) return vrc;
   uint32_t grand_r0, grand_r1;
   ParallelBounds(n, 1, c.parallel_idx, c.parallel_tot, &grand_r0, &grand_r1);
   const bool want_table = c.make_king_table;
   const bool want_matrix = c.make_king;
-  const bool square_text_full = want_matrix && c.king_shape == Cmd::kSq;  // needs the mirrored upper triangle
-  if (square_text_full && c.parallel_tot != 1) {
+  if (want_matrix && c.king_shape == Cmd::kSq && c.parallel_tot != 1) {
     logprintf("Error: --make-king square output cannot be combined with --parallel; use square0 or triangle.\n");
     return kRetInvalidCmdline;
   }
@@ -1731,17 +1852,15 @@ int RunKing(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, std::vector<uint8_t>* cut
   const IdFmt idf = KingIdFmt(c, S);
   std::vector<std::string> fmtids;
   if (want_table) {
-    tab_name = PieceName(c.out + ".kin0", c) + (c.king_table_zs ? ".zst" : "");
-    if (!ftab.Open(tab_name, c.king_table_zs)) {
-      logprintf("Error: Failed to open %s for writing.\n", tab_name.c_str());
-      return kRetOpenFail;
-    }
-    if (!c.parallel_idx) ftab.Puts(KingTableHeader(c, idf).c_str());
+    if (!OpenKingTable(c, idf, &ftab, &tab_name)) return kRetOpenFail;
     fmtids.resize(n);
     for (uint32_t k = 0; k < n; ++k) fmtids[k] = FmtId(S, k, idf);
   }
-  std::vector<double> full_kin;  // lower triangle, only for `square` output
-  if (square_text_full) full_kin.resize(static_cast<uint64_t>(n) * (n - 1) / 2);
+  // the matrix's rows start at 1 (ParallelBounds with start 1); sample 0's row, the diagonal 0.5 alone, goes first
+  // with the first --parallel piece (:2129-2132)
+  TriangleMatrixWriter mat(&fmat, n, c.king_shape, c.king_enc, false);
+  const double half = 0.5;
+  if (want_matrix && !c.parallel_idx) mat.Row(0, &half, half);
 
   // multi-GPU team (--gpus): every pass's row block is cut into one tile-aligned slab per device
   GpuTeam team;
@@ -1753,286 +1872,121 @@ int RunKing(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, std::vector<uint8_t>* cut
     if (trc) return trc;
   }
   const uint32_t G = team.size();
-  // pass planning (CountTrianglePasses / NextTrianglePass, :216-255): largest row block whose
-  // device accumulators fit (on every device of the team)
-  uint64_t free_b = ~0ull;
-  for (uint32_t g = 0; g < G; ++g) {
-    uint64_t f = 0, t = 0;
-    if (pl2gpu_ctx_mem_info(team.ctx[g], &f, &t)) return GpuFail("pl2gpu_ctx_mem_info");
-    free_b = std::min(free_b, f);
-  }
-  uint64_t budget = free_b - free_b / 10;
-  if (c.gpu_memory_mib && (c.gpu_memory_mib << 20) < budget) budget = c.gpu_memory_mib << 20;
-  // variants per staged block: the full 65,536 unless the cap is so small that the two staged blocks, their
-  // sample-major copies and their column plane copies (8 block sizes in all) would eat most of it (then halve until
-  // they fit in a quarter of the budget)
-  uint32_t batch = 65536;
-  while (batch > 2048 && 8ull * batch * ((n + 639) / 640 * 160) > budget / 4) batch /= 2;
-  auto pass_fits = [&](uint32_t a, uint32_t b) {
+  // pass planning: every device holds the accumulators of its slab of the pass; the two staged blocks, their
+  // sample-major copies and their column plane copies take 8 block sizes
+  uint32_t batch = 0;
+  std::vector<uint32_t> bounds;
+  int rc = PlanKingPasses(c, team.ctx, flagname, n, grand_r0, grand_r1, 8, [&](uint32_t a, uint32_t b, uint32_t bt) {
     const std::vector<uint32_t> sb = TileAlignedBounds(a, b, G, false);
+    uint64_t need = 0;
     for (uint32_t g = 0; g < G; ++g) {
-      if (sb[g + 1] > sb[g] && pl2gpu_king_mem_required(n, sb[g], sb[g + 1], batch) > budget) return false;
+      if (sb[g + 1] > sb[g]) need = std::max(need, pl2gpu_king_mem_required(n, sb[g], sb[g + 1], bt));
     }
-    return true;
-  };
-  auto next_pass_end = [&](uint32_t r) {  // largest e in (r, grand_r1] that fits
-    uint32_t lo = r + 1, hi = grand_r1;
-    while (lo < hi) {
-      const uint32_t mid = lo + (hi - lo + 1) / 2;
-      if (pass_fits(r, mid)) lo = mid;
-      else hi = mid - 1;
-    }
-    return lo;
-  };
-  uint32_t pass_ct = 0;
-  for (uint32_t r = grand_r0; r < grand_r1; ++pass_ct) {
-    if (pl2gpu_king_mem_required(n, r, r + 1, batch) > budget) {
-      logprintf("Error: Insufficient GPU memory for %s on %u samples.\n", flagname, n);
-      return kRetNomem;
-    }
-    r = next_pass_end(r);
-  }
-  if (pass_ct > 1) logprintf("%s: %u passes over the variants (device accumulators planned against %llu MiB).\n", flagname, pass_ct, static_cast<unsigned long long>(budget >> 20));
+    return need;
+  }, &batch, &bounds);
+  if (rc) return rc;
+  const uint32_t pass_ct = static_cast<uint32_t>(bounds.size() - 1);
   BlockStreamer bs(ds, &vidx, n, batch, G);  // G spare rows: a sharded batch is topped up to a multiple of G
   if (!bs.Init()) return GpuFail("pl2gpu_host_alloc");
-  if (want_matrix && c.king_shape == Cmd::kSq0 && !c.parallel_idx) {
-    // square0 output starts with sample 0's row: the diagonal 0.5 followed by zeros (:2129-2132)
-    if (c.king_enc == Cmd::kText) {
-      std::string row0 = "0.5";
-      for (uint32_t i = 1; i < n; ++i) row0 += "\t0";
-      row0 += "\n";
-      fmat.Puts(row0.c_str());
-    } else if (c.king_enc == Cmd::kBin4) {
-      std::vector<float> row(n, 0.0f);
-      row[0] = 0.5f;
-      fmat.Write(row.data(), sizeof(float) * n);
-    } else {
-      std::vector<double> row(n, 0.0);
-      row[0] = 0.5;
-      fmat.Write(row.data(), sizeof(double) * n);
-    }
-  }
+  // --make-king-table with --king-table-filter and nothing else to produce: filter on the device and fetch only the
+  // surviving rows (the unfiltered table is 20 bytes x N^2/2)
+  const bool device_filter = want_table && !want_matrix && c.king_cutoff < 0 && c.king_table_filter != -DBL_MAX;
   uint64_t filter_ct = 0;
-  struct Slab {
-    Pl2KingJob* job = nullptr;
-    uint32_t r0 = 0, r1 = 0;
-  };
   // NSNP compatibility with the reference's rare-variant pre-scan (SparseNsnpFix); only the table shows NSNP
-  const bool nsnp_fix_on = want_table && (c.col_nsnp || !c.king_counts) && !getenv("PL2_KING_DENSE_NSNP");
+  const bool nsnp_fix_on = want_table && (c.col_nsnp || !c.king_counts);
   SparseNsnpFix nsnp_fix;
-  uint32_t pass_r1 = grand_r0;
   for (uint32_t pass = 1; pass <= pass_ct; ++pass) {
-    const uint32_t pass_r0 = pass_r1;
-    pass_r1 = next_pass_end(pass_r0);
+    const uint32_t pass_r0 = bounds[pass - 1], pass_r1 = bounds[pass];
     const std::vector<uint32_t> sbounds = TileAlignedBounds(pass_r0, pass_r1, G, false);
-    std::vector<Slab> slabs(G);
-    auto end_jobs = [&]() {
-      for (Slab& sl : slabs) {
-        pl2gpu_king_end(sl.job);
-        sl.job = nullptr;
-      }
-    };
+    std::vector<KingJob> jobs(G);
     for (uint32_t g = 0; g < G; ++g) {
-      slabs[g].r0 = sbounds[g];
-      slabs[g].r1 = sbounds[g + 1];
       // an empty slab still takes part in the all-gathers (rank g of the communicator)
-      if (pl2gpu_king_begin_ex(team.ctx[g], n, slabs[g].r0, slabs[g].r1, kPl2KingAlgoAuto, batch, &slabs[g].job)) {
-        end_jobs();
-        return GpuFail("pl2gpu_king_begin_ex");
-      }
+      Pl2KingJob* job = nullptr;
+      if (pl2gpu_king_begin_ex(team.ctx[g], n, sbounds[g], sbounds[g + 1], kPl2KingAlgoAuto, batch, &job)) return GpuFail("pl2gpu_king_begin_ex");
+      jobs[g].reset(job);
     }
     g_clock.Mark("king: begin (device alloc)");
-    bs.Rewind();
-    std::string err;
     uint32_t done = 0;
-    double t_decode = 0, t_add = 0;
-    for (;;) {
-      const auto td = std::chrono::steady_clock::now();
-      const int got = bs.Next(&err);
-      t_decode += g_clock.Since(td);
-      if (got < 0) {
-        logprintf("\nError: %s\n", err.c_str());
-        end_jobs();
-        return kRetMalformedInput;
-      }
-      if (!got) break;
-      if (nsnp_fix_on) nsnp_fix.Scan(bs.buf, static_cast<uint32_t>(got), bs.words, grand_r1, pass_r0, pass_r1, g_decode_threads);
+    double t_add = 0;
+    const double decode0 = bs.decode_s;
+    rc = StreamBlocks(&bs, [&](uint32_t got) -> int {
+      if (nsnp_fix_on) nsnp_fix.Scan(bs.buf, got, bs.words, grand_r1, pass_r0, pass_r1, g_decode_threads);
       const auto ta = std::chrono::steady_clock::now();
       if (G == 1) {
-        if (pl2gpu_king_add_variants(slabs[0].job, bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0)) {
-          end_jobs();
-          return GpuFail("pl2gpu_king_add_variants");
-        }
+        if (pl2gpu_king_add_variants(jobs[0].get(), bs.buf, static_cast<uint64_t>(bs.words) * 8, got, 0)) return GpuFail("pl2gpu_king_add_variants");
       } else {
-        // device g uploads rows [g * per, (g + 1) * per) of the decoded block; NCCL all-gathers the column tile.
-        // Filler rows that top the block up to per * G are all-missing and count nothing.
-        const uint32_t per = (static_cast<uint32_t>(got) + G - 1) / G;
-        memset(bs.buf + static_cast<uint64_t>(got) * bs.words, 0xFF, static_cast<uint64_t>(per * G - static_cast<uint32_t>(got)) * bs.words * 8);
         std::string gerr;
-        if (ForEachRank(G, [&](uint32_t g) { return pl2gpu_king_add_variants_sharded(slabs[g].job, bs.buf + static_cast<uint64_t>(g) * per * bs.words, static_cast<uint64_t>(bs.words) * 8, per, 0); }, &gerr)) {
+        if (AddSharded(&bs, got, G, [&](uint32_t g, const uint64_t* slice, uint32_t per) { return pl2gpu_king_add_variants_sharded(jobs[g].get(), slice, static_cast<uint64_t>(bs.words) * 8, per, 0); }, &gerr)) {
           logprintf("\nError: pl2gpu_king_add_variants_sharded: %s\n", gerr.c_str());
-          end_jobs();
           return kRetGpuFail;
         }
       }
       t_add += g_clock.Since(ta);
-      done += static_cast<uint32_t>(got);
+      done += got;
       printf("\r%s pass %u/%u: %u variants complete.", flagname, pass, pass_ct, done);
       fflush(stdout);
-    }
+      return 0;
+    });
+    if (rc) return rc;
     printf("\r%s pass %u/%u: Writing...                   ", flagname, pass, pass_ct);
     fflush(stdout);
-    if (g_clock.on) fprintf(stderr, "[timing]   decode (PgrGet) %.3f s, pl2gpu_king_add_variants %.3f s\n", t_decode, t_add);
+    if (g_clock.on) fprintf(stderr, "[timing]   decode (PgrGet) %.3f s, pl2gpu_king_add_variants %.3f s\n", bs.decode_s - decode0, t_add);
     g_clock.Mark("king: decode + add_variants");
-    for (Slab& sl : slabs) {
-    Pl2KingJob* const job = sl.job;
-    const uint32_t row_start = sl.r0, row_end = sl.r1;
-    if (row_start >= row_end) continue;
-    // --make-king-table with --king-table-filter and nothing else to produce: filter on the device and
-    // fetch only the surviving rows (the unfiltered table is 20 bytes x N^2/2)
-    const bool device_filter = want_table && !want_matrix && c.king_cutoff < 0 && c.king_table_filter != -DBL_MAX;
-    if (device_filter) {
-      std::vector<uint32_t> fp, fc;
-      std::vector<double> fk;
-      uint64_t cap = 1ull << 22, found = 0;
-      for (;;) {
-        fp.resize(cap * 2);
-        fc.resize(cap * 5);
-        fk.resize(cap);
-        if (pl2gpu_king_get_filtered(job, row_start, row_end, c.king_table_filter, cap, fp.data(), fc.data(), fk.data(), &found)) {
-          end_jobs();
-          return GpuFail("pl2gpu_king_get_filtered");
-        }
-        if (found <= cap) break;
-        cap = found;
+    for (uint32_t g = 0; g < G; ++g) {
+      Pl2KingJob* const job = jobs[g].get();
+      const uint32_t row_start = sbounds[g], row_end = sbounds[g + 1];
+      if (row_start >= row_end) continue;
+      if (device_filter) {
+        std::vector<uint32_t> fp, fc;
+        std::vector<double> fk;
+        uint64_t found = 0;
+        rc = FetchKingFiltered(job, row_start, row_end, c.king_table_filter, &fp, &fc, &fk, &found);
+        if (rc) return rc;
+        for (uint64_t q = 0; q < found; ++q) WriteKingTableRow(c, fmtids[fp[2 * q]], fmtids[fp[2 * q + 1]], &fc[5 * q], fk[q], &ftab, nsnp_fix.Get(fp[2 * q], fp[2 * q + 1]));
+        filter_ct += KingPairsBelow(row_end, n) - KingPairsBelow(row_start, n) - found;
+        continue;
       }
-      for (uint64_t q = 0; q < found; ++q) WriteKingTableRow(c, fmtids[fp[2 * q]], fmtids[fp[2 * q + 1]], &fc[5 * q], fk[q], &ftab, nsnp_fix.Get(fp[2 * q], fp[2 * q + 1]));
-      auto tri = [](uint64_t r) { return r ? r * (r - 1) / 2 : 0ull; };
-      filter_ct += tri(row_end) - tri(row_start) - found;
-    }
-    // results in row chunks of <= ~512 MB
-    const uint64_t max_pairs = (512ull << 20) / 20;
-    std::vector<uint32_t> counts;
-    std::vector<double> kin;
-    for (uint32_t c0 = row_start; c0 < row_end && !device_filter;) {
-      uint32_t c1 = c0 + 1;
-      auto tri = [](uint64_t r) { return r ? r * (r - 1) / 2 : 0ull; };
-      while (c1 < row_end && tri(c1 + 1) - tri(c0) <= max_pairs) ++c1;
-      const uint64_t pairs = tri(c1) - tri(c0);
-      if (want_table) {
-        counts.resize(pairs * 5);
-        if (pairs && pl2gpu_king_get_counts(job, c0, c1, counts.data(), 0)) {
-          end_jobs();
-          return GpuFail("pl2gpu_king_get_counts");
+      std::vector<double> kin;
+      rc = ForEachKingCountChunk(job, row_start, row_end, n, want_table, [&](uint32_t c0, uint32_t c1, uint64_t pairs, const uint32_t* counts) {
+        if (want_matrix || c.king_cutoff >= 0 || !want_table) {
+          kin.resize(pairs);
+          if (pairs && pl2gpu_king_get_kinship(job, c0, c1, kin.data(), 0)) return GpuFail("pl2gpu_king_get_kinship");
         }
-      }
-      if (want_matrix || c.king_cutoff >= 0 || !want_table) {
-        kin.resize(pairs);
-        if (pairs && pl2gpu_king_get_kinship(job, c0, c1, kin.data(), 0)) {
-          end_jobs();
-          return GpuFail("pl2gpu_king_get_kinship");
-        }
-      }
-      uint64_t p = 0;
-      for (uint32_t j = c0; j < c1; ++j) {
-        const uint64_t row_p = p;
-        // --king-cutoff bit matrix (:2148-2151)
-        if (c.king_cutoff >= 0) {
-          for (uint32_t i = 0; i < j; ++i) {
-            if (kin[row_p + i] > c.king_cutoff) {
-              kin_table[static_cast<uint64_t>(j) * wl + i / 64] |= 1ull << (i % 64);
-              kin_table[static_cast<uint64_t>(i) * wl + j / 64] |= 1ull << (j % 64);
-            }
-          }
-        }
-        if (want_matrix) {
-          if (square_text_full) {
-            memcpy(&full_kin[tri(j)], &kin[row_p], sizeof(double) * j);
-          } else if (c.king_enc == Cmd::kText) {
-            // triangle: row j = kin(j,0..j-1); square0: + "0.5" + zeros (:2133-2184)
-            char* w = fmat.Reserve(static_cast<size_t>(n) * 16 + 64);
+        uint64_t p = 0;
+        for (uint32_t j = c0; j < c1; ++j) {
+          // --king-cutoff bit matrix (:2148-2151)
+          if (c.king_cutoff >= 0) {
             for (uint32_t i = 0; i < j; ++i) {
-              w = dtoa_g(kin[row_p + i], w);
-              *w++ = '\t';
-            }
-            if (c.king_shape == Cmd::kSq0) {
-              memcpy(w, "0.5", 3);
-              w += 3;
-              for (uint32_t i = j + 1; i < n; ++i) {
-                *w++ = '\t';
-                *w++ = '0';
+              if (kin[p + i] > c.king_cutoff) {
+                kin_table[static_cast<uint64_t>(j) * wl + i / 64] |= 1ull << (i % 64);
+                kin_table[static_cast<uint64_t>(i) * wl + j / 64] |= 1ull << (j % 64);
               }
-              *w++ = '\n';
-            } else {
-              if (j) w[-1] = '\n';
-              else *w++ = '\n';
-            }
-            fmat.Advance(w);
-          } else {
-            const bool f4 = c.king_enc == Cmd::kBin4;
-            const uint32_t row_len = (c.king_shape == Cmd::kTri) ? j : n;
-            if (f4) {
-              std::vector<float> rowf(row_len, 0.0f);
-              for (uint32_t i = 0; i < j; ++i) rowf[i] = static_cast<float>(kin[row_p + i]);
-              if (c.king_shape != Cmd::kTri) rowf[j] = 0.5f;
-              fmat.Write(rowf.data(), sizeof(float) * row_len);
-            } else {
-              std::vector<double> rowd(row_len, 0.0);
-              for (uint32_t i = 0; i < j; ++i) rowd[i] = kin[row_p + i];
-              if (c.king_shape != Cmd::kTri) rowd[j] = 0.5;
-              fmat.Write(rowd.data(), sizeof(double) * row_len);
             }
           }
-        }
-        if (want_table) {
-          for (uint32_t i = 0; i < j; ++i) {
-            const uint32_t* cc = &counts[(row_p + i) * 5];
-            const double kinship = KinshipFromCounts(cc);
-            if (c.king_table_filter != -DBL_MAX && kinship < c.king_table_filter) {
-              ++filter_ct;
-              continue;
+          if (want_matrix) mat.Row(j, &kin[p], half);
+          if (want_table) {
+            for (uint32_t i = 0; i < j; ++i) {
+              const uint32_t* cc = &counts[(p + i) * 5];
+              const double kinship = KinshipFromCounts(cc);
+              if (c.king_table_filter != -DBL_MAX && kinship < c.king_table_filter) {
+                ++filter_ct;
+                continue;
+              }
+              WriteKingTableRow(c, fmtids[j], fmtids[i], cc, kinship, &ftab, nsnp_fix.Get(j, i));
             }
-            WriteKingTableRow(c, fmtids[j], fmtids[i], cc, kinship, &ftab, nsnp_fix.Get(j, i));
           }
+          p += j;
         }
-        p += j;
-      }
-      c0 = c1;
+        return 0;
+      });
+      if (rc) return rc;
     }
-    }  // slabs
     nsnp_fix.extra.clear();
     g_clock.Mark("king: fetch results + write");
-    end_jobs();
+    jobs.clear();
     g_clock.Mark("king: end (device free)");
   }
-  if (square_text_full) {
-    auto tri = [](uint64_t r) { return r ? r * (r - 1) / 2 : 0ull; };
-    auto at = [&](uint32_t a, uint32_t b) { return a > b ? full_kin[tri(a) + b] : full_kin[tri(b) + a]; };
-    for (uint32_t j = 0; j < n; ++j) {
-      if (c.king_enc == Cmd::kText) {
-        char* w = fmat.Reserve(static_cast<size_t>(n) * 16 + 64);
-        for (uint32_t i = 0; i < n; ++i) {
-          if (i == j) {
-            memcpy(w, "0.5", 3);
-            w += 3;
-          } else {
-            w = dtoa_g(at(j, i), w);
-          }
-          *w++ = '\t';
-        }
-        w[-1] = '\n';
-        fmat.Advance(w);
-      } else if (c.king_enc == Cmd::kBin4) {
-        std::vector<float> row(n);
-        for (uint32_t i = 0; i < n; ++i) row[i] = (i == j) ? 0.5f : static_cast<float>(at(j, i));
-        fmat.Write(row.data(), sizeof(float) * n);
-      } else {
-        std::vector<double> row(n);
-        for (uint32_t i = 0; i < n; ++i) row[i] = (i == j) ? 0.5 : at(j, i);
-        fmat.Write(row.data(), sizeof(double) * n);
-      }
-    }
-  }
+  if (want_matrix) mat.Finish();
   printf("\r                                              \r");
   logprintf("%s: %u variants processed.\n", flagname, static_cast<uint32_t>(vidx.size()));
   if (want_matrix) {
@@ -2042,9 +1996,7 @@ int RunKing(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, std::vector<uint8_t>* cut
     }
     std::string idname = c.out + ".king.id";
     if (!c.parallel_idx) {
-      std::vector<uint32_t> all(n);
-      for (uint32_t k = 0; k < n; ++k) all[k] = k;
-      if (!WriteIdFile(idname, S, all, true)) return kRetWriteFail;
+      if (!WriteAllIds(idname, S, true)) return kRetWriteFail;
       logprintf("Results written to %s and %s .\n", mat_name.c_str(), idname.c_str());
     } else {
       logprintf("Results written to %s .\n", mat_name.c_str());
@@ -2497,21 +2449,12 @@ bool FounderRefFreqs(Dataset* ds, Pl2GpuCtx* ctx, const std::vector<uint32_t>& v
   return true;
 }
 
-int RunGrm(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, bool keep_for_pca, Pl2GrmJob** kept_job, std::vector<uint32_t>* used_vidx) {
+int RunGrm(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, bool keep_for_pca, GrmJob* kept_job) {
   const SampleInfo& S = ds->samples;
   const uint32_t n = S.size();
-  std::vector<uint32_t>& vidx = *used_vidx;
-  vidx.clear();
-  uint32_t non_auto = 0;
-  for (uint32_t v = 0; v < ds->variants.size(); ++v) {
-    if (KeptForRelationship(ds->variants.chr_code[v])) vidx.push_back(v);
-    else ++non_auto;
-  }
-  if (non_auto) logprintf("Excluding %u variant%s on non-autosomes from GRM construction.\n", non_auto, non_auto == 1 ? "" : "s");
-  if (vidx.empty()) {
-    logprintf("Error: No variants remaining for GRM construction.\n");
-    return kRetDegenerateData;
-  }
+  std::vector<uint32_t> vidx;
+  const int vrc = RelationshipVariants(*ds, "GRM construction", &vidx);
+  if (vrc) return vrc;
   uint32_t r0, r1;
   ParallelBounds(n, 0, c.parallel_idx, c.parallel_tot, &r0, &r1);
   std::vector<double> ref_freqs;
@@ -2532,100 +2475,79 @@ int RunGrm(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, bool keep_for_pca, Pl2GrmJ
   }
   const uint32_t G = team.size();
   const std::vector<uint32_t> sbounds = TileAlignedBounds(r0, r1, G, true);
-  std::vector<Pl2GrmJob*> jobs(G, nullptr);
-  auto end_jobs = [&]() {
-    for (auto& j : jobs) {
-      pl2gpu_grm_end(j);
-      j = nullptr;
-    }
-  };
+  std::vector<GrmJob> jobs(G);
   for (uint32_t g = 0; g < G; ++g) {
-    if (pl2gpu_grm_begin(team.ctx[g], n, sbounds[g], sbounds[g + 1], flags, &jobs[g])) {
-      end_jobs();
-      return GpuFail("pl2gpu_grm_begin");
-    }
+    Pl2GrmJob* job = nullptr;
+    if (pl2gpu_grm_begin(team.ctx[g], n, sbounds[g], sbounds[g + 1], flags, &job)) return GpuFail("pl2gpu_grm_begin");
+    jobs[g].reset(job);
   }
   BlockStreamer bs(ds, &vidx, n, 32768, G);
   if (!bs.Init()) return GpuFail("pl2gpu_host_alloc");
   logprintf("Constructing GRM: ");
-  std::string err;
   size_t base = 0;
-  for (;;) {
-    const int got = bs.Next(&err);
-    if (got < 0) {
-      logprintf("\nError: %s\n", err.c_str());
-      end_jobs();
-      return kRetMalformedInput;
-    }
-    if (!got) break;
+  rc = StreamBlocks(&bs, [&](uint32_t got) -> int {
     int arc;
     std::string gerr;
     const double* batch_freqs = have_freqs ? ref_freqs.data() + base : nullptr;
     if (G == 1) {
-      arc = pl2gpu_grm_add_variants(jobs[0], bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0, batch_freqs);
+      arc = pl2gpu_grm_add_variants(jobs[0].get(), bs.buf, static_cast<uint64_t>(bs.words) * 8, got, 0, batch_freqs);
       if (arc) gerr = pl2gpu_last_error();
     } else {
-      const uint32_t per = (static_cast<uint32_t>(got) + G - 1) / G;
-      memset(bs.buf + static_cast<uint64_t>(got) * bs.words, 0xFF, static_cast<uint64_t>(per * G - static_cast<uint32_t>(got)) * bs.words * 8);
-      arc = ForEachRank(G, [&](uint32_t g) { return pl2gpu_grm_add_variants_sharded(jobs[g], bs.buf + static_cast<uint64_t>(g) * per * bs.words, static_cast<uint64_t>(bs.words) * 8, per, static_cast<uint32_t>(got), 0, batch_freqs); }, &gerr);
+      arc = AddSharded(&bs, got, G, [&](uint32_t g, const uint64_t* slice, uint32_t per) { return pl2gpu_grm_add_variants_sharded(jobs[g].get(), slice, static_cast<uint64_t>(bs.words) * 8, per, got, 0, batch_freqs); }, &gerr);
     }
     if (arc) {
       logprintf("\nError: %s\n", gerr.c_str());
-      end_jobs();
       return arc == 2 ? kRetDegenerateData : kRetGpuFail;
     }
-    base += static_cast<size_t>(got);
+    base += got;
     printf("\rConstructing GRM: %u%%", static_cast<uint32_t>(base * 100 / vidx.size()));
     fflush(stdout);
-  }
+    return 0;
+  });
+  if (rc) return rc;
   printf("\r");
   logprintf("Constructing GRM: done.\n");
-  // writers
+  // writers: f(j, g, obs) for rows j of [r0, r1) in order, with row j's values and observation counts; fetched in
+  // chunks of rows that never straddle two devices' slabs
   const uint64_t stride = r1;
   const uint64_t max_rows = std::max<uint64_t>(1, (384ull << 20) / (stride * 12));
   std::vector<double> g;
   std::vector<float> obs;
-  auto slab_of = [&](uint32_t row) {
-    uint32_t sg = 0;
-    while (sg + 1 < G && row >= sbounds[sg + 1]) ++sg;
-    return sg;
+  auto for_each_row = [&](auto&& f) -> int {
+    for (uint32_t a = r0, sg = 0; a < r1;) {
+      while (a >= sbounds[sg + 1]) ++sg;
+      const uint32_t b = static_cast<uint32_t>(std::min<uint64_t>(a + max_rows, sbounds[sg + 1]));
+      g.assign(static_cast<uint64_t>(b - a) * stride, 0.0);
+      obs.assign(static_cast<uint64_t>(b - a) * stride, 0.0f);
+      if (pl2gpu_grm_get_rows(jobs[sg].get(), a, b, g.data(), obs.data(), stride, 0)) return GpuFail("pl2gpu_grm_get_rows");
+      for (uint32_t j = a; j < b; ++j) f(j, &g[static_cast<uint64_t>(j - a) * stride], &obs[static_cast<uint64_t>(j - a) * stride]);
+      a = b;
+    }
+    return 0;
   };
-  // row chunks handed to the writers never straddle two devices' slabs
-  auto chunk_end = [&](uint32_t a) { return static_cast<uint32_t>(std::min<uint64_t>(std::min<uint64_t>(r1, a + max_rows), sbounds[slab_of(a) + 1])); };
-  auto fetch = [&](uint32_t a, uint32_t b) -> bool {
-    g.assign(static_cast<uint64_t>(b - a) * stride, 0.0);
-    obs.assign(static_cast<uint64_t>(b - a) * stride, 0.0f);
-    return pl2gpu_grm_get_rows(jobs[slab_of(a)], a, b, g.data(), obs.data(), stride, 0) == 0;
+  // "<msg> ." in the log, with " , and IDs to <idname>" after the first --parallel piece has written that file
+  auto report = [&](std::string msg, const std::string& idname, bool header) -> int {
+    if (!c.parallel_idx) {
+      if (!WriteAllIds(idname, S, header)) return kRetWriteFail;
+      msg += " , and IDs to " + idname;
+    }
+    logprintf("%s .\n", msg.c_str());
+    return 0;
   };
+  const std::string piece = c.parallel_tot != 1 ? "component " : "";
   if (c.make_grm_bin) {
     const std::string gname = PieceName(c.out + ".grm.bin", c), nname = PieceName(c.out + ".grm.N.bin", c);
     OutFile fg, fn;
     if (!fg.Open(gname) || !fn.Open(nname)) return kRetOpenFail;
-    std::vector<float> rowf(r1);
-    for (uint32_t a = r0; a < r1;) {
-      const uint32_t b = chunk_end(a);
-      if (!fetch(a, b)) {
-        end_jobs();
-        return GpuFail("pl2gpu_grm_get_rows");
-      }
-      for (uint32_t j = a; j < b; ++j) {
-        const double* gr = &g[static_cast<uint64_t>(j - a) * stride];
-        for (uint32_t i = 0; i <= j; ++i) rowf[i] = static_cast<float>(gr[i]);
-        fg.Write(rowf.data(), sizeof(float) * (j + 1));
-        fn.Write(&obs[static_cast<uint64_t>(j - a) * stride], sizeof(float) * (j + 1));
-      }
-      a = b;
-    }
+    TriangleMatrixWriter gmat(&fg, n, Cmd::kTri, Cmd::kBin4, true);
+    rc = for_each_row([&](uint32_t j, const double* gr, const float* orow) {
+      gmat.Row(j, gr, gr[j]);
+      fn.Write(orow, sizeof(float) * (j + 1));
+    });
+    if (rc) return rc;
     if (!fg.Close() || !fn.Close()) return kRetWriteFail;
-    std::string msg = std::string("--make-grm-bin: GRM ") + (c.parallel_tot != 1 ? "component " : "") + "written to " + gname + " , observation counts to " + nname;
-    if (!c.parallel_idx) {
-      const std::string idname = c.out + ".grm.id";
-      std::vector<uint32_t> all(n);
-      for (uint32_t k = 0; k < n; ++k) all[k] = k;
-      if (!WriteIdFile(idname, S, all, c.grm_id_header)) return kRetWriteFail;
-      msg += " , and IDs to " + idname;
-    }
-    logprintf("%s .\n", msg.c_str());
+    rc = report("--make-grm-bin: GRM " + piece + "written to " + gname + " , observation counts to " + nname, c.out + ".grm.id", c.grm_id_header);
+    if (rc) return rc;
   }
   if (c.make_grm_list) {
     // `.grm`: one line per pair i <= j, "j+1 <tab> i+1 <tab> observation count <tab> value" (2.0/plink2_matrix_calc.cc:5082-5106)
@@ -2634,40 +2556,24 @@ int RunGrm(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, bool keep_for_pca, Pl2GrmJ
     if (!fg.Open(gname, c.grm_zs)) return kRetOpenFail;
     std::string line;
     char num[64];
-    for (uint32_t a = r0; a < r1;) {
-      const uint32_t b = chunk_end(a);
-      if (!fetch(a, b)) {
-        end_jobs();
-        return GpuFail("pl2gpu_grm_get_rows");
+    rc = for_each_row([&](uint32_t j, const double* gr, const float* orow) {
+      line.clear();
+      for (uint32_t i = 0; i <= j; ++i) {
+        line.append(num, u32toa(j + 1, num) - num);
+        line.push_back('\t');
+        line.append(num, u32toa(i + 1, num) - num);
+        line.push_back('\t');
+        line.append(num, u32toa(static_cast<uint32_t>(orow[i]), num) - num);
+        line.push_back('\t');
+        line.append(num, dtoa_g(gr[i], num) - num);
+        line.push_back('\n');
       }
-      for (uint32_t j = a; j < b; ++j) {
-        const double* gr = &g[static_cast<uint64_t>(j - a) * stride];
-        const float* orow = &obs[static_cast<uint64_t>(j - a) * stride];
-        line.clear();
-        for (uint32_t i = 0; i <= j; ++i) {
-          line.append(num, u32toa(j + 1, num) - num);
-          line.push_back('\t');
-          line.append(num, u32toa(i + 1, num) - num);
-          line.push_back('\t');
-          line.append(num, u32toa(static_cast<uint32_t>(orow[i]), num) - num);
-          line.push_back('\t');
-          line.append(num, dtoa_g(gr[i], num) - num);
-          line.push_back('\n');
-        }
-        fg.Write(line.data(), line.size());
-      }
-      a = b;
-    }
+      fg.Write(line.data(), line.size());
+    });
+    if (rc) return rc;
     if (!fg.Close()) return kRetWriteFail;
-    std::string msg = std::string("--make-grm-list: GRM ") + (c.parallel_tot != 1 ? "component " : "") + "written to " + gname;
-    if (!c.parallel_idx) {
-      const std::string idname = c.out + ".grm.id";
-      std::vector<uint32_t> all(n);
-      for (uint32_t k = 0; k < n; ++k) all[k] = k;
-      if (!WriteIdFile(idname, S, all, c.grm_id_header)) return kRetWriteFail;
-      msg += " , and IDs to " + idname;
-    }
-    logprintf("%s .\n", msg.c_str());
+    rc = report("--make-grm-list: GRM " + piece + "written to " + gname, c.out + ".grm.id", c.grm_id_header);
+    if (rc) return rc;
   }
   if (c.make_grm_sparse) {
     // `.grm.sp` (GCTA sparse GRM): "j <tab> i <tab> value" (0-based, 8 significant digits) for every i <= j whose
@@ -2675,38 +2581,23 @@ int RunGrm(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, bool keep_for_pca, Pl2GrmJ
     const std::string gname = PieceName(c.out + ".grm.sp", c) + (c.grm_zs ? ".zst" : "");
     OutFile fg;
     if (!fg.Open(gname, c.grm_zs)) return kRetOpenFail;
-    for (uint32_t a = r0; a < r1;) {
-      const uint32_t b = chunk_end(a);
-      if (!fetch(a, b)) {
-        end_jobs();
-        return GpuFail("pl2gpu_grm_get_rows");
+    rc = for_each_row([&](uint32_t j, const double* gr, const float*) {
+      for (uint32_t i = 0; i <= j; ++i) {
+        if (gr[i] < c.grm_sparse_cutoff) continue;
+        char* w = fg.Reserve(64);
+        w = u32toa(j, w);
+        *w++ = '\t';
+        w = u32toa(i, w);
+        *w++ = '\t';
+        w = dtoa_g_p8(gr[i], w);
+        *w++ = '\n';
+        fg.Advance(w);
       }
-      for (uint32_t j = a; j < b; ++j) {
-        const double* gr = &g[static_cast<uint64_t>(j - a) * stride];
-        for (uint32_t i = 0; i <= j; ++i) {
-          if (gr[i] < c.grm_sparse_cutoff) continue;
-          char* w = fg.Reserve(64);
-          w = u32toa(j, w);
-          *w++ = '\t';
-          w = u32toa(i, w);
-          *w++ = '\t';
-          w = dtoa_g_p8(gr[i], w);
-          *w++ = '\n';
-          fg.Advance(w);
-        }
-      }
-      a = b;
-    }
+    });
+    if (rc) return rc;
     if (!fg.Close()) return kRetWriteFail;
-    std::string msg = std::string("--make-grm-sparse: GRM ") + (c.parallel_tot != 1 ? "component " : "") + "written to " + gname;
-    if (!c.parallel_idx) {
-      const std::string idname = c.out + ".grm.id";
-      std::vector<uint32_t> all(n);
-      for (uint32_t k = 0; k < n; ++k) all[k] = k;
-      if (!WriteIdFile(idname, S, all, c.grm_id_header)) return kRetWriteFail;
-      msg += " , and IDs to " + idname;
-    }
-    logprintf("%s .\n", msg.c_str());
+    rc = report("--make-grm-sparse: GRM " + piece + "written to " + gname, c.out + ".grm.id", c.grm_id_header);
+    if (rc) return rc;
   }
   if (c.make_rel) {
     const std::string base_name = c.out + (c.rel_enc == Cmd::kText ? ".rel" : ".rel.bin");
@@ -2718,85 +2609,15 @@ int RunGrm(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, bool keep_for_pca, Pl2GrmJ
     }
     OutFile fr;
     if (!fr.Open(rname, rel_zs)) return kRetOpenFail;
-    std::vector<double> full;  // square: whole lower triangle incl. diagonal
-    auto tri1 = [](uint64_t r) { return r * (r + 1) / 2; };
-    if (c.rel_shape == Cmd::kSq) full.resize(tri1(n));
-    for (uint32_t a = r0; a < r1;) {
-      const uint32_t b = chunk_end(a);
-      if (!fetch(a, b)) {
-        end_jobs();
-        return GpuFail("pl2gpu_grm_get_rows");
-      }
-      for (uint32_t j = a; j < b; ++j) {
-        const double* gr = &g[static_cast<uint64_t>(j - a) * stride];
-        if (c.rel_shape == Cmd::kSq) {
-          memcpy(&full[tri1(j)], gr, sizeof(double) * (j + 1));
-          continue;
-        }
-        if (c.rel_enc == Cmd::kText) {
-          char* w = fr.Reserve(static_cast<size_t>(n) * 16 + 64);
-          for (uint32_t i = 0; i <= j; ++i) {
-            w = dtoa_g(gr[i], w);
-            *w++ = '\t';
-          }
-          if (c.rel_shape == Cmd::kSq0) {
-            for (uint32_t i = j + 1; i < n; ++i) {
-              *w++ = '0';
-              *w++ = '\t';
-            }
-          }
-          w[-1] = '\n';
-          fr.Advance(w);
-        } else {
-          const uint32_t len = (c.rel_shape == Cmd::kTri) ? j + 1 : n;
-          if (c.rel_enc == Cmd::kBin4) {
-            std::vector<float> row(len, 0.0f);
-            for (uint32_t i = 0; i <= j; ++i) row[i] = static_cast<float>(gr[i]);
-            fr.Write(row.data(), sizeof(float) * len);
-          } else {
-            std::vector<double> row(len, 0.0);
-            memcpy(row.data(), gr, sizeof(double) * (j + 1));
-            fr.Write(row.data(), sizeof(double) * len);
-          }
-        }
-      }
-      a = b;
-    }
-    if (c.rel_shape == Cmd::kSq) {
-      auto at = [&](uint32_t x, uint32_t y) { return x >= y ? full[tri1(x) + y] : full[tri1(y) + x]; };
-      for (uint32_t j = 0; j < n; ++j) {
-        if (c.rel_enc == Cmd::kText) {
-          char* w = fr.Reserve(static_cast<size_t>(n) * 16 + 64);
-          for (uint32_t i = 0; i < n; ++i) {
-            w = dtoa_g(at(j, i), w);
-            *w++ = '\t';
-          }
-          w[-1] = '\n';
-          fr.Advance(w);
-        } else if (c.rel_enc == Cmd::kBin4) {
-          std::vector<float> row(n);
-          for (uint32_t i = 0; i < n; ++i) row[i] = static_cast<float>(at(j, i));
-          fr.Write(row.data(), sizeof(float) * n);
-        } else {
-          std::vector<double> row(n);
-          for (uint32_t i = 0; i < n; ++i) row[i] = at(j, i);
-          fr.Write(row.data(), sizeof(double) * n);
-        }
-      }
-    }
+    TriangleMatrixWriter mat(&fr, n, c.rel_shape, c.rel_enc, true);
+    rc = for_each_row([&](uint32_t j, const double* gr, const float*) { mat.Row(j, gr, gr[j]); });
+    if (rc) return rc;
+    mat.Finish();
     if (!fr.Close()) return kRetWriteFail;
-    std::string msg = "--make-rel: GRM " + std::string(c.parallel_tot != 1 ? "component " : "") + "written to " + rname;
-    if (!c.parallel_idx) {
-      const std::string idname = c.out + ".rel.id";
-      std::vector<uint32_t> all(n);
-      for (uint32_t k = 0; k < n; ++k) all[k] = k;
-      if (!WriteIdFile(idname, S, all, true)) return kRetWriteFail;
-      msg += " , and IDs to " + idname;
-    }
-    logprintf("%s .\n", msg.c_str());
+    rc = report("--make-rel: GRM " + piece + "written to " + rname, c.out + ".rel.id", true);
+    if (rc) return rc;
   }
-  if (keep_for_pca) *kept_job = jobs[0];  // G == 1 in that case
-  else end_jobs();
+  if (keep_for_pca) *kept_job = std::move(jobs[0]);  // G == 1 in that case
   return 0;
 }
 
@@ -2845,43 +2666,35 @@ int RunPca(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, Pl2GrmJob* grm_job) {
     }
     const uint32_t G = team.size();
     const uint32_t shard = static_cast<uint32_t>(((vidx.size() + G - 1) / G + 127) / 128 * 128);
-    std::vector<Pl2PcaJob*> jobs(G, nullptr);
-    auto end_jobs = [&]() {
-      for (Pl2PcaJob* j : jobs) pl2gpu_pca_end(j);
-    };
+    std::vector<PcaJob> jobs(G);
     for (uint32_t r = 0; r < G; ++r) {
       const size_t s0 = std::min<size_t>(vidx.size(), static_cast<size_t>(r) * shard), s1 = std::min<size_t>(vidx.size(), s0 + shard);
       if (s0 == s1) {
         logprintf("Error: --gpus %u leaves a device without variants.\n", G);
-        end_jobs();
         return kRetInvalidCmdline;
       }
-      rc = G == 1 ? pl2gpu_pca_begin(team.ctx[r], n, static_cast<uint32_t>(vidx.size()), pc_ct, &jobs[r]) : pl2gpu_pca_begin_shard(team.ctx[r], n, static_cast<uint32_t>(s1 - s0), pc_ct, &jobs[r]);
+      Pl2PcaJob* job = nullptr;
+      rc = G == 1 ? pl2gpu_pca_begin(team.ctx[r], n, static_cast<uint32_t>(vidx.size()), pc_ct, &job) : pl2gpu_pca_begin_shard(team.ctx[r], n, static_cast<uint32_t>(s1 - s0), pc_ct, &job);
+      jobs[r].reset(job);
       if (rc) {
         logprintf("Error: %s\n", pl2gpu_last_error());
-        end_jobs();
         return rc == 2 ? kRetDegenerateData : kRetGpuFail;
       }
       std::vector<uint32_t> sub(vidx.begin() + s0, vidx.begin() + s1);
       BlockStreamer bs(ds, &sub, n, 32768);
-      if (!bs.Init()) {
-        end_jobs();
-        return GpuFail("pl2gpu_host_alloc");
-      }
+      if (!bs.Init()) return GpuFail("pl2gpu_host_alloc");
       std::string err;
       size_t base = s0;
       for (;;) {
         const int got = bs.Next(&err);
         if (got < 0) {
           logprintf("Error: %s\n", err.c_str());
-          end_jobs();
           return kRetMalformedInput;
         }
         if (!got) break;
-        const int arc = pl2gpu_pca_add_variants(jobs[r], bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0, have_freqs ? ref_freqs.data() + base : nullptr);
+        const int arc = pl2gpu_pca_add_variants(jobs[r].get(), bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0, have_freqs ? ref_freqs.data() + base : nullptr);
         if (arc) {
           logprintf("Error: %s\n", pl2gpu_last_error());
-          end_jobs();
           return arc == 2 ? kRetDegenerateData : kRetGpuFail;
         }
         base += static_cast<size_t>(got);
@@ -2897,9 +2710,8 @@ int RunPca(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, Pl2GrmJob* grm_job) {
     FillGaussian(static_cast<uint64_t>(n) * pc_ct, c.threads ? c.threads : 1, &rng, g1.data());
     logprintf("Projecting random vectors, computing SVD of Krylov matrix, recovering top PCs... ");
     if (G == 1) {
-      if (pl2gpu_pca_run(jobs[0], g1.data(), eigvals.data(), eigvecs.data())) {
+      if (pl2gpu_pca_run(jobs[0].get(), g1.data(), eigvals.data(), eigvecs.data())) {
         logprintf("\nError: %s\n", pl2gpu_last_error());
-        end_jobs();
         return kRetGpuFail;
       }
     } else {
@@ -2907,15 +2719,13 @@ int RunPca(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx, Pl2GrmJob* grm_job) {
       std::vector<std::vector<double>> vals(G, std::vector<double>(pc_ct)), vecs(G);
       for (uint32_t r = 1; r < G; ++r) vecs[r].resize(static_cast<uint64_t>(pc_ct) * n);
       std::string errtext;
-      const int prc = ForEachRank(G, [&](uint32_t r) { return pl2gpu_pca_run_sharded(jobs[r], g1.data(), vidx.size(), r ? vals[r].data() : eigvals.data(), r ? vecs[r].data() : eigvecs.data()); }, &errtext);
+      const int prc = ForEachRank(G, [&](uint32_t r) { return pl2gpu_pca_run_sharded(jobs[r].get(), g1.data(), vidx.size(), r ? vals[r].data() : eigvals.data(), r ? vecs[r].data() : eigvecs.data()); }, &errtext);
       if (prc) {
         logprintf("\nError: %s\n", errtext.c_str());
-        end_jobs();
         return kRetGpuFail;
       }
     }
     logprintf("done.\n");
-    end_jobs();
   }
   if (!WriteEigen(c.out, S, pc_ct, eigvals.data(), eigvecs.data())) {
     logprintf("Error: File write failure.\n");
@@ -4646,10 +4456,8 @@ int main(int argc, char** argv) {
     logprintf("--write-snplist: Variant IDs written to %s .\n", name.c_str());
   }
   if (c.write_samples) {
-    std::vector<uint32_t> all(ds.samples.size());
-    for (uint32_t k = 0; k < all.size(); ++k) all[k] = k;
     const std::string name = c.out + ".id";
-    if (!WriteIdFile(name, ds.samples, all, true)) return kRetWriteFail;
+    if (!WriteAllIds(name, ds.samples, true)) return kRetWriteFail;
     logprintf("--write-samples: Sample IDs written to %s .\n", name.c_str());
   }
   g_clock.Mark("load .psam/.pvar, open .pgen");
@@ -4779,21 +4587,21 @@ int main(int argc, char** argv) {
     rc = RunVscore(c, &ds, ctx);
     if (rc) return rc;
   }
-  Pl2GrmJob* grm_job = nullptr;
-  std::vector<uint32_t> grm_vidx;
-  const bool exact_pca = c.pca && !c.pca_approx;
-  if (c.make_grm_bin || c.make_grm_list || c.make_grm_sparse || c.make_rel || exact_pca) {
-    if (exact_pca && c.parallel_tot != 1) {
-      logprintf("Error: --pca cannot be used with --parallel.\n");
-      return kRetInvalidCmdline;
+  {
+    GrmJob grm_job;  // exact --pca's matrix, ended before the commands below
+    const bool exact_pca = c.pca && !c.pca_approx;
+    if (c.make_grm_bin || c.make_grm_list || c.make_grm_sparse || c.make_rel || exact_pca) {
+      if (exact_pca && c.parallel_tot != 1) {
+        logprintf("Error: --pca cannot be used with --parallel.\n");
+        return kRetInvalidCmdline;
+      }
+      rc = RunGrm(c, &ds, ctx, exact_pca, &grm_job);
+      if (rc) return rc;
     }
-    rc = RunGrm(c, &ds, ctx, exact_pca, &grm_job, &grm_vidx);
-    if (rc) return rc;
-  }
-  if (c.pca) {
-    rc = RunPca(c, &ds, ctx, grm_job);
-    if (grm_job) pl2gpu_grm_end(grm_job);
-    if (rc) return rc;
+    if (c.pca) {
+      rc = RunPca(c, &ds, ctx, grm_job.get());
+      if (rc) return rc;
+    }
   }
   if (c.indep_pairwise) {
     rc = RunLdPrune(c, &ds, ctx);

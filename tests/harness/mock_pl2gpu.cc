@@ -7,7 +7,10 @@
 // real, exported pl2_ld_prune_walk of libpl2gpu.so (host code) is called.  Autosomal (diploid) chromosomes only.
 // Build: g++ -O2 -std=c++17 -ffp-contract=off -shared -fPIC -o mock_pl2gpu.so mock_pl2gpu.cc
 // PL2_MOCK_DEVICES = number of devices to report; PL2_MOCK_LOG = file that receives one line per entry-point call.
+// Multi-GPU (--gpus): a communicator is a shared block in host memory; the *_add_variants_sharded calls all-gather
+// every rank's slice into it at rank x slice and each rank then adds the whole gathered block, as NCCL would.
 #include <cmath>
+#include <condition_variable>
 #include <cstdint>
 #include <cstdio>
 #include <cstdlib>
@@ -16,8 +19,11 @@
 #include <string>
 #include <vector>
 
+struct MockComm;
 struct Pl2GpuCtx {
   int device;
+  MockComm* comm = nullptr;
+  int rank = 0;
 };
 
 extern "C" int pl2_ld_prune_walk(uint32_t variant_ct, const uint32_t* chr_codes, const uint32_t* variant_bps, uint32_t window_size, uint32_t window_incr, int window_is_bp, const double* maj_freq, const uint8_t* mono,
@@ -36,6 +42,40 @@ void Log(const char* fmt, int a, unsigned b) {
   }
 }
 inline uint32_t Code(const uint8_t* row, uint32_t s) { return (row[s >> 2] >> (2 * (s & 3))) & 3; }
+}  // namespace
+
+struct MockComm {
+  std::mutex mu;
+  std::condition_variable cv;
+  int world = 0;
+  int arrived = 0;  // ranks whose slice has landed in this round
+  int unread = 0;   // ranks still to copy out the previous round's block
+  uint64_t round = 0;
+  std::vector<uint8_t> block;
+};
+namespace {
+// All-gather of equal-sized slices: rank r's bytes land at r x slice_bytes of the shared block; every rank waits until
+// all `world` slices have landed and returns a copy of the whole block.  A new round starts only after every rank
+// has copied out the previous one.
+std::vector<uint8_t> AllGather(Pl2GpuCtx* ctx, const void* slice, uint64_t slice_bytes) {
+  MockComm* c = ctx->comm;
+  std::unique_lock<std::mutex> lock(c->mu);
+  c->cv.wait(lock, [&] { return c->unread == 0; });
+  if (!c->arrived) c->block.assign(static_cast<size_t>(c->world) * slice_bytes, 0);
+  memcpy(&c->block[static_cast<size_t>(ctx->rank) * slice_bytes], slice, slice_bytes);
+  const uint64_t round = c->round;
+  if (++c->arrived == c->world) {
+    c->arrived = 0;
+    c->unread = c->world;
+    ++c->round;
+    c->cv.notify_all();
+  } else {
+    c->cv.wait(lock, [&] { return c->round != round; });
+  }
+  std::vector<uint8_t> out = c->block;
+  if (--c->unread == 0) c->cv.notify_all();
+  return out;
+}
 }  // namespace
 
 extern "C" {
@@ -58,6 +98,26 @@ int pl2gpu_ctx_destroy(Pl2GpuCtx* ctx) {
   delete ctx;
   return 0;
 }
+// the id carries the address of a fresh communicator; every rank's pl2gpu_comm_init joins it
+int pl2gpu_comm_unique_id(uint8_t* id_out) {
+  MockComm* c = new MockComm;
+  memset(id_out, 0, 128);
+  memcpy(id_out, &c, sizeof(c));
+  return 0;
+}
+int pl2gpu_comm_init(Pl2GpuCtx* ctx, int rank, int world, const uint8_t* id) {
+  MockComm* c;
+  memcpy(&c, id, sizeof(c));
+  {
+    std::lock_guard<std::mutex> lock(c->mu);
+    c->world = world;
+  }
+  ctx->comm = c;
+  ctx->rank = rank;
+  Log("comm_init device=%d rank=%u\n", ctx->device, static_cast<unsigned>(rank));
+  return 0;
+}
+int pl2gpu_comm_destroy(Pl2GpuCtx*) { return 0; }
 int pl2gpu_ctx_synchronize(Pl2GpuCtx*) { return 0; }
 int pl2gpu_host_alloc(uint64_t bytes, void** ptr) {
   *ptr = malloc(bytes ? bytes : 1);
@@ -86,6 +146,7 @@ struct Pl2KingJob {
   uint32_t n, r0, r1;
   std::vector<uint8_t> codes;  // [variant][sample]
   uint64_t variants = 0;
+  Pl2GpuCtx* ctx = nullptr;
 };
 namespace {
 void PairCounts(const Pl2KingJob* job, uint32_t j, uint32_t i, uint32_t* c5) {
@@ -118,7 +179,7 @@ uint64_t pl2gpu_king_mem_required(uint32_t sample_ct, uint32_t row_start, uint32
 }
 int pl2gpu_king_begin_ex(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start, uint32_t row_end, int, uint32_t, Pl2KingJob** job_ptr) {
   Log("king_begin device=%d rows=%u\n", ctx->device, row_end - row_start);
-  *job_ptr = new Pl2KingJob{sample_ct, row_start, row_end, {}, 0};
+  *job_ptr = new Pl2KingJob{sample_ct, row_start, row_end, {}, 0, ctx};
   return 0;
 }
 int pl2gpu_king_begin(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start, uint32_t row_end, int algo, Pl2KingJob** job_ptr) { return pl2gpu_king_begin_ex(ctx, sample_ct, row_start, row_end, algo, 0, job_ptr); }
@@ -129,6 +190,10 @@ int pl2gpu_king_add_variants(Pl2KingJob* job, const void* genovecs, uint64_t str
   }
   job->variants += variant_ct;
   return 0;
+}
+int pl2gpu_king_add_variants_sharded(Pl2KingJob* job, const void* slice, uint64_t stride, uint32_t slice_variant_ct, int src) {
+  const std::vector<uint8_t> block = AllGather(job->ctx, slice, stride * slice_variant_ct);
+  return pl2gpu_king_add_variants(job, block.data(), stride, static_cast<uint32_t>(block.size() / stride), src);
 }
 int pl2gpu_king_get_counts(Pl2KingJob* job, uint32_t out_row_start, uint32_t out_row_end, uint32_t* dst, int) {
   for (uint32_t j = out_row_start; j < out_row_end; ++j)
@@ -180,6 +245,7 @@ struct Pl2GrmJob {
   std::vector<uint8_t> codes;   // [variant][sample]
   std::vector<double> ref_freq;  // per variant
   uint64_t variants = 0;
+  Pl2GpuCtx* ctx = nullptr;
 };
 namespace {
 void GrmMatrix(const Pl2GrmJob* job, std::vector<double>* g, std::vector<double>* obs) {
@@ -215,7 +281,7 @@ void GrmMatrix(const Pl2GrmJob* job, std::vector<double>* g, std::vector<double>
 extern "C" {
 int pl2gpu_grm_begin(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start, uint32_t row_end, int flags, Pl2GrmJob** job_ptr) {
   Log("grm_begin device=%d rows=%u\n", ctx->device, row_end - row_start);
-  *job_ptr = new Pl2GrmJob{sample_ct, row_start, row_end, flags, {}, {}, 0};
+  *job_ptr = new Pl2GrmJob{sample_ct, row_start, row_end, flags, {}, {}, 0, ctx};
   return 0;
 }
 int pl2gpu_grm_add_variants(Pl2GrmJob* job, const void* genovecs, uint64_t stride, uint32_t variant_ct, int, const double* ref_freqs) {
@@ -234,6 +300,11 @@ int pl2gpu_grm_add_variants(Pl2GrmJob* job, const void* genovecs, uint64_t strid
   }
   job->variants += variant_ct;
   return 0;
+}
+// the gathered block's first batch_variant_ct rows are the batch; the filler behind them is ignored
+int pl2gpu_grm_add_variants_sharded(Pl2GrmJob* job, const void* slice, uint64_t stride, uint32_t slice_variant_ct, uint32_t batch_variant_ct, int src, const double* ref_freqs) {
+  const std::vector<uint8_t> block = AllGather(job->ctx, slice, stride * slice_variant_ct);
+  return pl2gpu_grm_add_variants(job, block.data(), stride, batch_variant_ct, src, ref_freqs);
 }
 int pl2gpu_grm_get_rows(Pl2GrmJob* job, uint32_t r0, uint32_t r1, double* dst_grm, float* dst_obs, uint64_t row_stride, int) {
   std::vector<double> g, obs;
