@@ -7,6 +7,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <string>
+#include <utility>
 #include <vector>
 
 namespace pl2 {
@@ -31,6 +32,98 @@ const char* get_error();
     }                  \
   } while (0)
 
+// ---- owners of device memory, pinned host memory, events and streams: move-only, released when they go out of
+// scope, null until created.  A failed creation clears the CUDA error, leaves the owner null and records
+// fmt(args..., CUDA error string) as the library error, so a message may end in "%s" to name the CUDA error.
+template <class T, class Traits>
+class CudaOwner {
+ public:
+  CudaOwner() = default;
+  CudaOwner(CudaOwner&& o) noexcept : h_(o.h_) { o.h_ = nullptr; }
+  CudaOwner& operator=(CudaOwner&& o) noexcept {
+    std::swap(h_, o.h_);
+    return *this;
+  }
+  ~CudaOwner() { reset(); }
+  void reset() {
+    if (h_) Traits::release(h_);
+    h_ = nullptr;
+  }
+  T get() const { return h_; }
+  operator T() const { return h_; }  // the handle, for CUDA calls and kernel arguments
+
+ protected:
+  template <class... A>
+  int take(cudaError_t err, T h, const char* fmt, A... args) {
+    reset();
+    if (err != cudaSuccess) {
+      cudaGetLastError();
+      set_error(fmt, args..., cudaGetErrorString(err));
+      return 1;
+    }
+    h_ = h;
+    return 0;
+  }
+
+ private:
+  T h_ = nullptr;
+};
+
+struct DevFree {
+  static void release(void* p) { cudaFree(p); }
+};
+struct HostFree {
+  static void release(void* p) { cudaFreeHost(p); }
+};
+struct EventFree {
+  static void release(cudaEvent_t e) { cudaEventDestroy(e); }
+};
+struct StreamFree {
+  static void release(cudaStream_t s) { cudaStreamDestroy(s); }
+};
+
+// n elements of T in device memory (cudaMalloc of exactly n * sizeof(T) bytes)
+template <class T>
+struct DevArray : CudaOwner<T*, DevFree> {
+  template <class... A>
+  int alloc(uint64_t n, const char* fmt, A... args) {
+    void* p = nullptr;
+    const cudaError_t err = cudaMalloc(&p, n * sizeof(T));
+    return this->take(err, static_cast<T*>(p), fmt, args...);
+  }
+};
+
+// n elements of T in pinned host memory
+template <class T>
+struct PinnedArray : CudaOwner<T*, HostFree> {
+  template <class... A>
+  int alloc(uint64_t n, const char* fmt, A... args) {
+    void* p = nullptr;
+    const cudaError_t err = cudaHostAlloc(&p, n * sizeof(T), cudaHostAllocDefault);
+    return this->take(err, static_cast<T*>(p), fmt, args...);
+  }
+};
+
+struct Event : CudaOwner<cudaEvent_t, EventFree> {
+  // flags: cudaEventDisableTiming, or cudaEventDefault for an event cudaEventElapsedTime reads
+  template <class... A>
+  int create(unsigned flags, const char* fmt, A... args) {
+    cudaEvent_t e = nullptr;
+    const cudaError_t err = cudaEventCreateWithFlags(&e, flags);
+    return this->take(err, e, fmt, args...);
+  }
+};
+
+struct Stream : CudaOwner<cudaStream_t, StreamFree> {
+  // a non-blocking stream; priority 0 is the default priority
+  template <class... A>
+  int create(int priority, const char* fmt, A... args) {
+    cudaStream_t s = nullptr;
+    const cudaError_t err = cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, priority);
+    return this->take(err, s, fmt, args...);
+  }
+};
+
 // ---- pair-tile geometry shared by every N x N kernel ----
 // Output tiles are kTileRows (larger-index samples, "sample 2") x kTileCols (smaller-index
 // samples, "sample 1").  A tensor kernel runs a tile as two CTAs of 64 rows (the wgmma M dimension), each
@@ -50,11 +143,11 @@ __host__ __device__ constexpr uint32_t SampleToPos(uint32_t s) { return (s & 1) 
 
 struct Ctx {
   int device = -1;
-  cudaStream_t stream = nullptr;       // compute stream: every tensor / popcount / finalize kernel
-  cudaStream_t copy_stream = nullptr;  // high-priority prep stream: H2D / D2D copies, all-gathers, padding, re-tiling
+  Stream stream;       // compute stream: every tensor / popcount / finalize kernel
+  Stream copy_stream;  // high-priority prep stream: H2D / D2D copies, all-gathers, padding, re-tiling
   int sm_count = 0;
   uint64_t launches = 0;
-  cudaEvent_t events[16] = {};
+  Event events[16];  // pl2gpu_ctx_event_record, created on first use
   // optional NCCL communicator (one rank per context; pl2gpu_comm_init), loaded lazily with dlopen
   void* comm = nullptr;
   int comm_rank = 0, comm_world = 1;
@@ -70,10 +163,10 @@ struct TileList {
   uint32_t row_tile_first = 0;  // row_start / kTileRows
   uint32_t row_tile_ct = 0;
   uint32_t tile_ct = 0;
-  uint32_t* d_tile_rt = nullptr;       // [tile_ct] row-tile index (absolute)
-  uint32_t* d_tile_tc = nullptr;       // [tile_ct] col-tile index
-  uint32_t* d_rowtile_offset = nullptr;  // [row_tile_ct + 1] first tile of each row tile
-  uint32_t* d_tile_order = nullptr;      // [tile_ct] launch order: 12 x 12 tile blocks so co-resident CTAs share L2 lines
+  DevArray<uint32_t> d_tile_rt;         // [tile_ct] row-tile index (absolute)
+  DevArray<uint32_t> d_tile_tc;         // [tile_ct] col-tile index
+  DevArray<uint32_t> d_rowtile_offset;  // [row_tile_ct + 1] first tile of each row tile
+  DevArray<uint32_t> d_tile_order;      // [tile_ct] launch order: 12 x 12 tile blocks so co-resident CTAs share L2 lines
   uint32_t pair_tile_ct = 0;             // row_pairs lists: d_tile_order starts with this many tiles, pairs (rt, ct), (rt + 1, ct)
   std::vector<uint32_t> h_rowtile_offset;  // host copy of the same
 };
@@ -83,11 +176,10 @@ uint64_t CountTiles(uint32_t row_start, uint32_t row_end, bool include_diag, uin
 // row_pairs: the launch order starts with the tiles (rt, ct), (rt + 1, ct) of row-tile pairs counted from the first
 // row tile, two by two, and ends with the tiles that have no such partner
 int BuildTileList(uint32_t row_start, uint32_t row_end, bool include_diag, TileList* tl, uint32_t tile_cols = kTileCols, uint32_t col_end = 0xFFFFFFFFu, bool row_pairs = false);
-void FreeTileList(TileList* tl);
 
 // ---- staged genotype block on the device (implemented in pl2gpu.cu) ----
 struct GenoStage {
-  uint8_t* d_raw = nullptr;  // [variant_cap][pitch]
+  DevArray<uint8_t> d_raw;  // [variant_cap][pitch]
   uint32_t pitch = 0;        // bytes per variant row = sample_ct_padded / 4
   uint32_t sample_ct = 0;
   uint32_t sample_ct_padded = 0;
@@ -99,7 +191,6 @@ constexpr uint32_t kMaxStageVariantsEx = 1u << 20;   // largest capacity pl2gpu_
 // pad_genotypes_kernel launcher (kernel lives in pl2gpu.cu's translation unit); stream = nullptr: the compute stream
 int LaunchPadGenotypes(Ctx* ctx, uint8_t* dst, uint32_t pitch, uint32_t sample_ct, uint32_t variant_ct, uint32_t variant_ct_padded, cudaStream_t stream = nullptr);
 int StageAlloc(uint32_t sample_ct, uint32_t variant_cap, GenoStage* gs, uint32_t sample_pad = kSamplePad);
-void StageFree(GenoStage* gs);
 // Copies variant_ct (<= variant_cap) rows starting at destination row dst_row and forces padding
 // samples / rows [dst_row + variant_ct, dst_row + padded) to "missing".
 int StageUpload(Ctx* ctx, GenoStage* gs, const void* src, uint64_t src_stride, uint32_t variant_ct, int src_is_device, uint32_t* padded_ct_ptr, uint32_t dst_row = 0, uint32_t pad_to = kVariantPad);
@@ -112,15 +203,14 @@ int StageUpload(Ctx* ctx, GenoStage* gs, const void* src, uint64_t src_stride, u
 struct StageRing {
   Ctx* ctx = nullptr;
   GenoStage stage[2];
-  cudaEvent_t ev_prep_done[2] = {nullptr, nullptr};
-  cudaEvent_t ev_free[2] = {nullptr, nullptr};  // the slot's last reader has finished; timing-enabled for pl2gpu_king_last_kernel_ms
+  Event ev_prep_done[2];
+  Event ev_free[2];  // the slot's last reader has finished; timing-enabled for pl2gpu_king_last_kernel_ms
   bool free_pending[2] = {false, false};
-  uint32_t next = 0;                   // the slot the next acquire returns
-  cudaEvent_t ev_src_ready = nullptr;  // the compute stream has reached the copy of a src_is_device == 1 source
-  cudaEvent_t ev_copied = nullptr;     // the caller's rows have been copied (prep stream)
+  uint32_t next = 0;   // the slot the next acquire returns
+  Event ev_src_ready;  // the compute stream has reached the copy of a src_is_device == 1 source
+  Event ev_copied;     // the caller's rows have been copied (prep stream)
 
   int alloc(Ctx* c, uint32_t sample_ct, uint32_t variant_cap, uint32_t sample_pad);
-  void free();
   int acquire(int src_is_device, uint32_t* slot);
   // `rows` rows into the slot, or into dst (same pitch) when dst is not null
   int land(uint32_t slot, uint8_t* dst, const void* src, uint64_t src_stride, uint32_t rows, int src_is_device);

@@ -66,6 +66,74 @@ static int BlockOrthonormalize(Ctx* c, double* q, uint64_t ld, uint32_t rows, ui
   return 0;
 }
 
+// SymEigTopKKrylov after its size check, with b columns per block and p Krylov steps: the scratch is freed on return,
+// before SymEigTopKKrylov clears the CUDA error state
+static int SymEigTopKKrylovRun(Ctx* c, const double* d_a, uint32_t n, uint32_t k, uint32_t b, uint32_t p, double* eigvals_host, double* d_u, uint32_t* restarts_out, const char** err) {
+  const uint32_t q = b * (p + 1);
+  DevArray<double> d_q, d_aq, d_t, d_tu, d_x, d_ax, d_c, d_cpart, d_tmp, d_res;
+  uint64_t part = DgemmTNPartialDoubles(c, q, q, n);
+  for (uint32_t t = 1; t <= p; ++t) part = std::max(part, DgemmTNPartialDoubles(c, t * b, b, n));
+  const uint64_t nq = static_cast<uint64_t>(n) * q, nb = static_cast<uint64_t>(n) * b;
+  const char* oom = "insufficient device memory for the Krylov basis";
+  if (d_q.alloc(nq, oom) || d_aq.alloc(nq, oom) || d_t.alloc(1ull * q * q, oom) || d_tu.alloc(1ull * q * b, oom) || d_x.alloc(nb, oom) || d_ax.alloc(nb, oom) || d_c.alloc(1ull * q * b, oom) || d_cpart.alloc(part, oom) ||
+      d_tmp.alloc(nb, oom) || d_res.alloc(2ull * b, oom)) {
+    *err = oom;
+    return 1;
+  }
+  {  // deterministic Gaussian start block
+    std::vector<double> x0(nb);
+    std::mt19937_64 gen(20260923);
+    std::normal_distribution<double> nd(0.0, 1.0);
+    for (double& v : x0) v = nd(gen);
+    if (cudaMemcpyAsync(d_x, x0.data(), nb * 8, cudaMemcpyHostToDevice, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) return 1;
+  }
+  std::vector<double> theta(q), res(2ull * b);
+  const double tol = 1e-10;
+  uint32_t it = 0;
+  bool converged = false, failed = false;
+  for (; it < 400 && !converged; ++it) {
+    // Krylov blocks
+    if (cudaMemcpyAsync(d_q, d_x, nb * 8, cudaMemcpyDeviceToDevice, c->stream) != cudaSuccess) { failed = true; break; }
+    for (uint32_t j = 1; j <= p && !failed; ++j) failed = DgemmNN(c, d_a, n, n, n, d_q + static_cast<uint64_t>(j - 1) * nb, n, b, d_q + static_cast<uint64_t>(j) * nb, n, false, nullptr) != 0;
+    if (failed) break;
+    if (BlockOrthonormalize(c, d_q, n, n, b, p + 1, d_c, d_cpart, d_tmp, err)) { failed = true; break; }
+    // Rayleigh-Ritz
+    if (DgemmNN(c, d_a, n, n, n, d_q, n, q, d_aq, n, false, nullptr) || DgemmTN(c, d_q, n, q, d_aq, n, q, n, d_cpart, d_t, q)) { failed = true; break; }
+    if (JacobiSvd(c, d_t, q, q, q, b, theta.data(), d_tu, q, nullptr, err)) { failed = true; break; }
+    if (DgemmNN(c, d_q, n, n, q, d_tu, q, b, d_x, n, false, nullptr) || DgemmNN(c, d_aq, n, n, q, d_tu, q, b, d_ax, n, false, nullptr)) { failed = true; break; }
+    ritz_residual_kernel<<<b, 256, 0, c->stream>>>(d_x, d_ax, n, n, d_res);
+    c->launches++;
+    if (cudaMemcpyAsync(res.data(), d_res, 16ull * b, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) { failed = true; break; }
+    double worst = 0.0;
+    for (uint32_t i = 0; i < k; ++i) worst = std::max(worst, sqrt(res[2 * i + 1]));
+    converged = worst <= tol * fabs(res[0]);
+  }
+  if (failed) {
+    if (!*err) *err = "CUDA failure in the Krylov solver";
+    return 1;
+  }
+  if (!converged) {
+    *err = "Krylov eigensolver did not converge in 400 restarts";
+    return 1;
+  }
+  // the Ritz values came out as singular values of T (|theta|); the Rayleigh quotients carry the sign
+  bool ordered = true;
+  for (uint32_t i = 0; i < k; ++i) {
+    eigvals_host[i] = res[2 * i];
+    ordered = ordered && res[2 * i] > 0.0 && (i == 0 || res[2 * i] <= res[2 * (i - 1)] * (1 + 1e-12));
+  }
+  if (!ordered) {
+    *err = "leading eigenvalues are not positive and descending (indefinite matrix?)";
+    return 1;
+  }
+  if (cudaMemcpyAsync(d_u, d_x, static_cast<uint64_t>(n) * k * 8, cudaMemcpyDeviceToDevice, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
+    *err = "CUDA failure in the Krylov solver";
+    return 1;
+  }
+  if (restarts_out) *restarts_out = it;
+  return 0;
+}
+
 // d_a: symmetric n x n (column-major == row-major), untouched.  eigvals_host[k] descending, d_u: n x k unit eigenvectors
 // (leading dimension n).  Returns 0, or 1 with *err set.
 static int SymEigTopKKrylov(Ctx* c, const double* d_a, uint32_t n, uint32_t k, double* eigvals_host, double* d_u, uint32_t* restarts_out, const char** err) {
@@ -77,83 +145,7 @@ static int SymEigTopKKrylov(Ctx* c, const double* d_a, uint32_t n, uint32_t k, d
     *err = "matrix too small for the Krylov solver";
     return 1;
   }
-  const uint32_t q = b * (p + 1);
-  double *d_q = nullptr, *d_aq = nullptr, *d_t = nullptr, *d_tu = nullptr, *d_x = nullptr, *d_ax = nullptr, *d_c = nullptr, *d_cpart = nullptr, *d_tmp = nullptr, *d_res = nullptr;
-  uint64_t part = DgemmTNPartialDoubles(c, q, q, n);
-  for (uint32_t t = 1; t <= p; ++t) part = std::max(part, DgemmTNPartialDoubles(c, t * b, b, n));
-  int rc = 1;
-  do {
-    const uint64_t nq = static_cast<uint64_t>(n) * q, nb = static_cast<uint64_t>(n) * b;
-    if (cudaMalloc(&d_q, nq * 8) != cudaSuccess || cudaMalloc(&d_aq, nq * 8) != cudaSuccess || cudaMalloc(&d_t, 8ull * q * q) != cudaSuccess || cudaMalloc(&d_tu, 8ull * q * b) != cudaSuccess ||
-        cudaMalloc(&d_x, nb * 8) != cudaSuccess || cudaMalloc(&d_ax, nb * 8) != cudaSuccess || cudaMalloc(&d_c, 8ull * q * b) != cudaSuccess || cudaMalloc(&d_cpart, part * 8) != cudaSuccess ||
-        cudaMalloc(&d_tmp, nb * 8) != cudaSuccess || cudaMalloc(&d_res, 16ull * b) != cudaSuccess) {
-      cudaGetLastError();
-      *err = "insufficient device memory for the Krylov basis";
-      break;
-    }
-    {  // deterministic Gaussian start block
-      std::vector<double> x0(nb);
-      std::mt19937_64 gen(20260923);
-      std::normal_distribution<double> nd(0.0, 1.0);
-      for (double& v : x0) v = nd(gen);
-      if (cudaMemcpyAsync(d_x, x0.data(), nb * 8, cudaMemcpyHostToDevice, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) break;
-    }
-    std::vector<double> theta(q), res(2ull * b);
-    const double tol = 1e-10;
-    uint32_t it = 0;
-    bool converged = false, failed = false;
-    for (; it < 400 && !converged; ++it) {
-      // Krylov blocks
-      if (cudaMemcpyAsync(d_q, d_x, nb * 8, cudaMemcpyDeviceToDevice, c->stream) != cudaSuccess) { failed = true; break; }
-      for (uint32_t j = 1; j <= p && !failed; ++j) failed = DgemmNN(c, d_a, n, n, n, d_q + static_cast<uint64_t>(j - 1) * nb, n, b, d_q + static_cast<uint64_t>(j) * nb, n, false, nullptr) != 0;
-      if (failed) break;
-      if (BlockOrthonormalize(c, d_q, n, n, b, p + 1, d_c, d_cpart, d_tmp, err)) { failed = true; break; }
-      // Rayleigh-Ritz
-      if (DgemmNN(c, d_a, n, n, n, d_q, n, q, d_aq, n, false, nullptr) || DgemmTN(c, d_q, n, q, d_aq, n, q, n, d_cpart, d_t, q)) { failed = true; break; }
-      if (JacobiSvd(c, d_t, q, q, q, b, theta.data(), d_tu, q, nullptr, err)) { failed = true; break; }
-      if (DgemmNN(c, d_q, n, n, q, d_tu, q, b, d_x, n, false, nullptr) || DgemmNN(c, d_aq, n, n, q, d_tu, q, b, d_ax, n, false, nullptr)) { failed = true; break; }
-      ritz_residual_kernel<<<b, 256, 0, c->stream>>>(d_x, d_ax, n, n, d_res);
-      c->launches++;
-      if (cudaMemcpyAsync(res.data(), d_res, 16ull * b, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) { failed = true; break; }
-      double worst = 0.0;
-      for (uint32_t i = 0; i < k; ++i) worst = std::max(worst, sqrt(res[2 * i + 1]));
-      converged = worst <= tol * fabs(res[0]);
-    }
-    if (failed) {
-      if (!*err) *err = "CUDA failure in the Krylov solver";
-      break;
-    }
-    if (!converged) {
-      *err = "Krylov eigensolver did not converge in 400 restarts";
-      break;
-    }
-    // the Ritz values came out as singular values of T (|theta|); the Rayleigh quotients carry the sign
-    bool ordered = true;
-    for (uint32_t i = 0; i < k; ++i) {
-      eigvals_host[i] = res[2 * i];
-      ordered = ordered && res[2 * i] > 0.0 && (i == 0 || res[2 * i] <= res[2 * (i - 1)] * (1 + 1e-12));
-    }
-    if (!ordered) {
-      *err = "leading eigenvalues are not positive and descending (indefinite matrix?)";
-      break;
-    }
-    if (cudaMemcpyAsync(d_u, d_x, static_cast<uint64_t>(n) * k * 8, cudaMemcpyDeviceToDevice, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
-      *err = "CUDA failure in the Krylov solver";
-      break;
-    }
-    if (restarts_out) *restarts_out = it;
-    rc = 0;
-  } while (0);
-  cudaFree(d_q);
-  cudaFree(d_aq);
-  cudaFree(d_t);
-  cudaFree(d_tu);
-  cudaFree(d_x);
-  cudaFree(d_ax);
-  cudaFree(d_c);
-  cudaFree(d_cpart);
-  cudaFree(d_tmp);
-  cudaFree(d_res);
+  const int rc = SymEigTopKKrylovRun(c, d_a, n, k, b, p, eigvals_host, d_u, restarts_out, err);
   cudaGetLastError();
   return rc;
 }

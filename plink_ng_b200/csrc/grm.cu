@@ -2,6 +2,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstring>
+#include <memory>
 #include <vector>
 
 
@@ -20,28 +21,32 @@ constexpr double kSmallEpsilon = 1.0 / 17592186044416.0;  // 2^-44
 }
 
 struct Pl2GrmJob {
-  Pl2GpuCtx* ctx = nullptr;
+  explicit Pl2GrmJob(Pl2GpuCtx* x) : ctx(x) {}
+  ~Pl2GrmJob() {  // the kernels and copies that use the buffers finish before they are freed
+    cudaSetDevice(ctx->c.device);
+    cudaStreamSynchronize(ctx->c.stream);
+    cudaStreamSynchronize(ctx->c.copy_stream);
+  }
+  Pl2GpuCtx* ctx;
   uint32_t sample_ct = 0, row_start = 0, row_end = 0;
   int flags = 0;
   TileList tiles;
   StageRing ring;  // genotype counts, digit tables and row re-tiling of each slot also run on the prep stream
-  uint8_t* d_raw_i[2] = {nullptr, nullptr};  // sample-major copy of the staged block (geno_tile.cuh)
-  uint8_t* d_tab[2] = {nullptr, nullptr};    // digit tables (grm_tables_kernel)
-  double* d_lvals[2] = {nullptr, nullptr};
-  uint32_t* d_counts[2] = {nullptr, nullptr};
-  double* h_lvals[2] = {nullptr, nullptr};     // pinned
-  uint32_t* h_counts[2] = {nullptr, nullptr};  // pinned
-  double* d_acc_g = nullptr;
-  int32_t* d_acc_obs = nullptr;
-  void* d_out_stage = nullptr;
+  DevArray<uint8_t> d_raw_i[2];  // sample-major copy of the staged block (geno_tile.cuh)
+  DevArray<uint8_t> d_tab[2];    // digit tables (grm_tables_kernel)
+  DevArray<double> d_lvals[2];
+  DevArray<uint32_t> d_counts[2];
+  PinnedArray<double> h_lvals[2];
+  PinnedArray<uint32_t> h_counts[2];
+  DevArray<double> d_acc_g;
+  DevArray<int32_t> d_acc_obs;
+  DevArray<double> d_out_stage;
   uint64_t out_stage_bytes = 0;
   uint64_t variants_added = 0;
   uint64_t variants_with_missing = 0;
 };
 
 extern "C" {
-
-int pl2gpu_grm_end(Pl2GrmJob* job);
 
 int pl2gpu_grm_begin(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start, uint32_t row_end, int flags, Pl2GrmJob** job_ptr) {
   *job_ptr = nullptr;
@@ -51,39 +56,31 @@ int pl2gpu_grm_begin(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t row_start, uin
   }
   PL2_CUDA_OK(cudaSetDevice(ctx->c.device));
   PL2_CUDA_OK(cudaFuncSetAttribute(grm_wg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kGwSmemBytes));
-  Pl2GrmJob* job = new Pl2GrmJob();
-  job->ctx = ctx;
+  std::unique_ptr<Pl2GrmJob, int (*)(Pl2GrmJob*)> job(new Pl2GrmJob(ctx), pl2gpu_grm_end);
   job->sample_ct = sample_ct;
   job->row_start = row_start;
   job->row_end = row_end;
   job->flags = flags;
-  auto fail = [&]() {
-    pl2gpu_grm_end(job);
-    return 1;
-  };
-  if (BuildTileList(row_start, row_end, true, &job->tiles, kGrmTileCols)) return fail();
+  PL2_TRY(BuildTileList(row_start, row_end, true, &job->tiles, kGrmTileCols));
   const uint64_t words = static_cast<uint64_t>(job->tiles.tile_ct) * kGrmTileWords;
   job->out_stage_bytes = 256ull << 20;
-  if (job->ring.alloc(&ctx->c, sample_ct, kMaxStageVariants, kGrmSamplePad)) return fail();
+  PL2_TRY(job->ring.alloc(&ctx->c, sample_ct, kMaxStageVariants, kGrmSamplePad));
   const uint64_t cap = job->ring.stage[0].variant_cap;
   const uint64_t raw_i_bytes = static_cast<uint64_t>(job->ring.stage[0].sample_ct_padded) * (cap / 4);
-  bool ok = true;
-  for (int b = 0; b < 2 && ok; ++b) {
-    ok = cudaMalloc(&job->d_raw_i[b], raw_i_bytes ? raw_i_bytes : 16) == cudaSuccess && cudaMalloc(&job->d_tab[b], cap / 16 * kGrmTabChunkBytes) == cudaSuccess &&
-         cudaMalloc(&job->d_lvals[b], cap * 6 * 8) == cudaSuccess && cudaMalloc(&job->d_counts[b], cap * 16) == cudaSuccess &&
-         cudaHostAlloc(reinterpret_cast<void**>(&job->h_lvals[b]), cap * 6 * 8, cudaHostAllocDefault) == cudaSuccess &&
-         cudaHostAlloc(reinterpret_cast<void**>(&job->h_counts[b]), cap * 16, cudaHostAllocDefault) == cudaSuccess;
+  const char* oom = "pl2gpu_grm_begin: insufficient device memory for %u pair tiles (%.1f GB of accumulators); narrow the row range";
+  const uint32_t tile_ct = job->tiles.tile_ct;
+  const double acc_gb = words * 12 / 1e9;
+  for (int b = 0; b < 2; ++b) {
+    if (job->d_raw_i[b].alloc(raw_i_bytes ? raw_i_bytes : 16, oom, tile_ct, acc_gb) || job->d_tab[b].alloc(cap / 16 * kGrmTabChunkBytes, oom, tile_ct, acc_gb) || job->d_lvals[b].alloc(cap * 6, oom, tile_ct, acc_gb) ||
+        job->d_counts[b].alloc(cap * 4, oom, tile_ct, acc_gb) || job->h_lvals[b].alloc(cap * 6, oom, tile_ct, acc_gb) || job->h_counts[b].alloc(cap * 4, oom, tile_ct, acc_gb))
+      return 1;
   }
-  if (!ok || cudaMalloc(&job->d_acc_g, words * 8 + 8) != cudaSuccess || cudaMalloc(&job->d_acc_obs, words * 4 + 4) != cudaSuccess || cudaMalloc(&job->d_out_stage, job->out_stage_bytes) != cudaSuccess) {
-    cudaGetLastError();
-    set_error("pl2gpu_grm_begin: insufficient device memory for %u pair tiles (%.1f GB of accumulators); narrow the row range", job->tiles.tile_ct, words * 12 / 1e9);
-    return fail();
-  }
+  if (job->d_acc_g.alloc(words + 1, oom, tile_ct, acc_gb) || job->d_acc_obs.alloc(words + 1, oom, tile_ct, acc_gb) || job->d_out_stage.alloc(job->out_stage_bytes / 8, oom, tile_ct, acc_gb)) return 1;
   if (cudaMemsetAsync(job->d_acc_g, 0, words * 8, ctx->c.stream) != cudaSuccess || cudaMemsetAsync(job->d_acc_obs, 0, words * 4, ctx->c.stream) != cudaSuccess) {
     set_error("pl2gpu_grm_begin: memset failed");
-    return fail();
+    return 1;
   }
-  *job_ptr = job;
+  *job_ptr = job.release();
   return 0;
 }
 
@@ -260,7 +257,7 @@ int pl2gpu_grm_get_rows(Pl2GrmJob* job, uint32_t r0, uint32_t r1, double* dst_gr
         return 1;
       }
       cur1 = static_cast<uint32_t>(std::min<uint64_t>(r1, cur0 + max_rows));
-      d_g = static_cast<double*>(job->d_out_stage);
+      d_g = job->d_out_stage;
       if (dst_obs) d_o = reinterpret_cast<float*>(d_g + static_cast<uint64_t>(cur1 - cur0) * row_stride);
       PL2_CUDA_OK(cudaMemsetAsync(job->d_out_stage, 0, static_cast<uint64_t>(cur1 - cur0) * per_row, c->stream));
     }
@@ -345,95 +342,67 @@ int pl2gpu_grm_eigen_topk(Pl2GrmJob* job, uint32_t pc_ct, double* eigvals_host, 
   // Top eigenpairs of the symmetric GRM by one-sided Jacobi on the shifted matrix G + mu I (mu = the
   // Gershgorin bound that makes it positive semi-definite, so singular values = eigenvalues + mu in
   // the same order and the unit columns of (G + mu I) V are the eigenvectors).  Replaces dsyevr (:5943-6039).
-  double *d_a = nullptr, *d_u = nullptr, *d_ex = nullptr;
-  int rc = 1;
-  do {
-    if (cudaMalloc(&d_a, static_cast<uint64_t>(n) * n * 8) != cudaSuccess || cudaMalloc(&d_u, static_cast<uint64_t>(n) * pc_ct * 8) != cudaSuccess || cudaMalloc(&d_ex, 8ull * n) != cudaSuccess) {
-      cudaGetLastError();
-      set_error("pl2gpu_grm_eigen_topk: insufficient device memory for a dense %u x %u matrix", n, n);
-      break;
+  DevArray<double> d_a, d_u, d_ex;
+  const char* oom = "pl2gpu_grm_eigen_topk: insufficient device memory for a dense %u x %u matrix";
+  if (d_a.alloc(static_cast<uint64_t>(n) * n, oom, n, n) || d_u.alloc(static_cast<uint64_t>(n) * pc_ct, oom, n, n) || d_ex.alloc(n, oom, n, n)) return 1;
+  if (cudaMemsetAsync(d_a, 0, static_cast<uint64_t>(n) * n * 8, c->stream) != cudaSuccess) return 1;
+  PL2_TRY(pl2gpu_grm_get_rows(job, 0, n, d_a, nullptr, n, 1));  // row-major lower triangle == column-major upper
+  symmetrize_kernel<<<dim3(DivUpU32(n, 256), n), 256, 0, c->stream>>>(d_a, n);
+  gershgorin_kernel<<<n, 256, 0, c->stream>>>(d_a, n, d_ex);
+  c->launches += 2;
+  std::vector<double> ex(n);
+  if (cudaMemcpyAsync(ex.data(), d_ex, 8ull * n, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
+    set_error("pl2gpu_grm_eigen_topk: %s", cudaGetErrorString(cudaGetLastError()));
+    return 1;
+  }
+  double mu = 0.0;
+  bool finite = true;
+  for (uint32_t j = 0; j < n; ++j) {
+    finite = finite && std::isfinite(ex[j]);
+    mu = std::max(mu, ex[j]);
+  }
+  if (!finite) {
+    set_error("pl2gpu_grm_eigen_topk: GRM contains missing values (a sample pair has no jointly observed variant)");
+    return 1;
+  }
+  // Small matrices: one-sided Jacobi on G + mu I (all eigenpairs, O(N^3) per sweep).  Beyond 2,048 samples - or with
+  // PL2_EIGEN=krylov - the leading pairs come from a restarted block Krylov iteration on G itself (eig_krylov.cuh):
+  // (2p + 1)(k + 8) N^2 MACs per restart instead of N^3 per sweep.  PL2_EIGEN=jacobi forces the dense form.
+  const char* eig_env = getenv("PL2_EIGEN");
+  const bool krylov = pc_ct + 8 <= n / 6 && ((eig_env && !strcmp(eig_env, "krylov")) || (!(eig_env && !strcmp(eig_env, "jacobi")) && n > 2048));
+  std::vector<double> sigma(pc_ct);
+  const char* err = nullptr;
+  if (krylov) {
+    uint32_t restarts = 0;
+    if (SymEigTopKKrylov(c, d_a, n, pc_ct, sigma.data(), d_u, &restarts, &err)) {
+      set_error("pl2gpu_grm_eigen_topk: eigendecomposition failed (%s)", err ? err : "?");
+      return 1;
     }
-    if (cudaMemsetAsync(d_a, 0, static_cast<uint64_t>(n) * n * 8, c->stream) != cudaSuccess) break;
-    if (pl2gpu_grm_get_rows(job, 0, n, d_a, nullptr, n, 1)) break;  // row-major lower triangle == column-major upper
-    symmetrize_kernel<<<dim3(DivUpU32(n, 256), n), 256, 0, c->stream>>>(d_a, n);
-    gershgorin_kernel<<<n, 256, 0, c->stream>>>(d_a, n, d_ex);
-    c->launches += 2;
-    std::vector<double> ex(n);
-    if (cudaMemcpyAsync(ex.data(), d_ex, 8ull * n, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
-      set_error("pl2gpu_grm_eigen_topk: %s", cudaGetErrorString(cudaGetLastError()));
-      break;
+    if (getenv("PL2_TIMING")) fprintf(stderr, "[timing]   eigen: block Krylov, %u restarts\n", restarts);
+    mu = 0.0;
+  } else {
+    if (mu > 0.0) {
+      add_diagonal_kernel<<<DivUpU32(n, 256), 256, 0, c->stream>>>(d_a, n, mu);
+      c->launches++;
     }
-    double mu = 0.0;
-    bool finite = true;
-    for (uint32_t j = 0; j < n; ++j) {
-      finite = finite && std::isfinite(ex[j]);
-      mu = std::max(mu, ex[j]);
+    uint32_t sweeps = 0;
+    if (JacobiSvd(c, d_a, n, n, n, pc_ct, sigma.data(), d_u, n, &sweeps, &err)) {
+      set_error("pl2gpu_grm_eigen_topk: eigendecomposition failed (%s)", err ? err : "?");
+      return 1;
     }
-    if (!finite) {
-      set_error("pl2gpu_grm_eigen_topk: GRM contains missing values (a sample pair has no jointly observed variant)");
-      break;
-    }
-    // Small matrices: one-sided Jacobi on G + mu I (all eigenpairs, O(N^3) per sweep).  Beyond 2,048 samples - or with
-    // PL2_EIGEN=krylov - the leading pairs come from a restarted block Krylov iteration on G itself (eig_krylov.cuh):
-    // (2p + 1)(k + 8) N^2 MACs per restart instead of N^3 per sweep.  PL2_EIGEN=jacobi forces the dense form.
-    const char* eig_env = getenv("PL2_EIGEN");
-    const bool krylov = pc_ct + 8 <= n / 6 && ((eig_env && !strcmp(eig_env, "krylov")) || (!(eig_env && !strcmp(eig_env, "jacobi")) && n > 2048));
-    std::vector<double> sigma(pc_ct);
-    const char* err = nullptr;
-    if (krylov) {
-      uint32_t restarts = 0;
-      if (SymEigTopKKrylov(c, d_a, n, pc_ct, sigma.data(), d_u, &restarts, &err)) {
-        set_error("pl2gpu_grm_eigen_topk: eigendecomposition failed (%s)", err ? err : "?");
-        break;
-      }
-      if (getenv("PL2_TIMING")) fprintf(stderr, "[timing]   eigen: block Krylov, %u restarts\n", restarts);
-      mu = 0.0;
-    } else {
-      if (mu > 0.0) {
-        add_diagonal_kernel<<<DivUpU32(n, 256), 256, 0, c->stream>>>(d_a, n, mu);
-        c->launches++;
-      }
-      uint32_t sweeps = 0;
-      if (JacobiSvd(c, d_a, n, n, n, pc_ct, sigma.data(), d_u, n, &sweeps, &err)) {
-        set_error("pl2gpu_grm_eigen_topk: eigendecomposition failed (%s)", err ? err : "?");
-        break;
-      }
-    }
-    if (cudaMemcpyAsync(eigvecs_host, d_u, 8ull * pc_ct * n, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
-      set_error("pl2gpu_grm_eigen_topk: %s", cudaGetErrorString(cudaGetLastError()));
-      break;
-    }
-    for (uint32_t k = 0; k < pc_ct; ++k) eigvals_host[k] = sigma[k] - mu;  // descending (:6024-6039)
-    rc = 0;
-  } while (0);
-  cudaFree(d_a);
-  cudaFree(d_u);
-  cudaFree(d_ex);
-  return rc;
+  }
+  if (cudaMemcpyAsync(eigvecs_host, d_u, 8ull * pc_ct * n, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
+    set_error("pl2gpu_grm_eigen_topk: %s", cudaGetErrorString(cudaGetLastError()));
+    return 1;
+  }
+  for (uint32_t k = 0; k < pc_ct; ++k) eigvals_host[k] = sigma[k] - mu;  // descending (:6024-6039)
+  return 0;
 }
 
 int pl2gpu_grm_end(Pl2GrmJob* job) {
   if (!job) return 0;
-  if (job->ctx) {
-    cudaSetDevice(job->ctx->c.device);
-    cudaStreamSynchronize(job->ctx->c.stream);
-    cudaStreamSynchronize(job->ctx->c.copy_stream);
-  }
-  FreeTileList(&job->tiles);
-  job->ring.free();
-  for (int b = 0; b < 2; ++b) {
-    cudaFree(job->d_raw_i[b]);
-    cudaFree(job->d_tab[b]);
-    cudaFree(job->d_lvals[b]);
-    cudaFree(job->d_counts[b]);
-    if (job->h_lvals[b]) cudaFreeHost(job->h_lvals[b]);
-    if (job->h_counts[b]) cudaFreeHost(job->h_counts[b]);
-  }
-  cudaFree(job->d_acc_g);
-  cudaFree(job->d_acc_obs);
-  cudaFree(job->d_out_stage);
-  cudaGetLastError();
   delete job;
+  cudaGetLastError();
   return 0;
 }
 

@@ -162,16 +162,8 @@ static __global__ void jacobi_gather_kernel(const double* __restrict__ a, uint64
   if (r < rows) out[static_cast<uint64_t>(blockIdx.y) * ldo + r] = a[static_cast<uint64_t>(src) * lda + r] * inv;
 }
 
-// Host driver.  d_a (rows x q, leading dimension lda) is overwritten with U Sigma (unsorted).
-// sigma_host[0..out_cols) = singular values in descending order; d_u (may be nullptr) receives the
-// matching unit left singular vectors as a rows x out_cols column-major matrix (ldu).
-// Returns 0, or 1 with *err set (CUDA failure / no convergence).
-static int JacobiSvd(Ctx* c, double* d_a, uint64_t lda, uint32_t rows, uint32_t q, uint32_t out_cols, double* sigma_host, double* d_u, uint64_t ldu, uint32_t* sweeps_out, const char** err) {
-  *err = nullptr;
-  if (!q || rows < q || out_cols > q) {
-    *err = "JacobiSvd: bad shape";
-    return 1;
-  }
+// JacobiSvd after its shape check: the scratch is freed on return, before JacobiSvd clears the CUDA error state
+static int JacobiSvdRun(Ctx* c, double* d_a, uint64_t lda, uint32_t rows, uint32_t q, uint32_t out_cols, double* sigma_host, double* d_u, uint64_t ldu, uint32_t* sweeps_out, const char** err) {
   const uint32_t qe = (q + 1) & ~1u;
   const uint32_t half = qe / 2, rounds = qe - 1;
   std::vector<int2> sched(static_cast<size_t>(rounds ? rounds : 1) * half);
@@ -194,84 +186,87 @@ static int JacobiSvd(Ctx* c, double* d_a, uint64_t lda, uint32_t rows, uint32_t 
     chunk_rows = std::max<uint32_t>(16384, DivUpU32(rows, kJacobiMaxChunks));
     chunks = DivUpU32(rows, chunk_rows);
   }
-  int2* d_sched = nullptr;
-  double *d_partial = nullptr, *d_norms = nullptr;
-  uint32_t* d_perm = nullptr;
-  int* d_flag = nullptr;
-  int rc = 1;
-  do {
-    if (cudaMalloc(&d_sched, sched.size() * sizeof(int2)) != cudaSuccess || cudaMalloc(&d_partial, static_cast<uint64_t>(half) * chunks * 3 * 8) != cudaSuccess || cudaMalloc(&d_norms, 8ull * q) != cudaSuccess ||
-        cudaMalloc(&d_perm, 4ull * q) != cudaSuccess || cudaMalloc(&d_flag, 4) != cudaSuccess) {
-      cudaGetLastError();
-      *err = "JacobiSvd: insufficient device memory";
-      break;
-    }
-    if (cudaMemcpyAsync(d_sched, sched.data(), sched.size() * sizeof(int2), cudaMemcpyHostToDevice, c->stream) != cudaSuccess) break;
-    const double tol = std::max(1e-15, 4.4408920985006262e-16 * sqrt(static_cast<double>(rows)));
-    uint32_t sweep = 0;
-    bool converged = (q == 1);
-    for (; sweep < 60 && !converged; ++sweep) {
-      if (cudaMemsetAsync(d_flag, 0, 4, c->stream) != cudaSuccess) break;
-      for (uint32_t r = 0; r < rounds; ++r) {
-        const int2* pr = d_sched + static_cast<size_t>(r) * half;
-        if (fused) {
-          jacobi_fused_kernel<<<half, kJacobiThreads, 0, c->stream>>>(d_a, lda, rows, pr, tol, d_flag);
-          c->launches++;
-        } else {
-          jacobi_dots_kernel<<<dim3(half, chunks), kJacobiThreads, 0, c->stream>>>(d_a, lda, rows, pr, chunk_rows, d_partial);
-          jacobi_rotate_kernel<<<dim3(half, chunks), kJacobiThreads, 0, c->stream>>>(d_a, lda, rows, pr, chunk_rows, d_partial, tol, d_flag);
-          c->launches += 2;
-        }
+  DevArray<int2> d_sched;
+  DevArray<double> d_partial, d_norms;
+  DevArray<uint32_t> d_perm;
+  DevArray<int> d_flag;
+  const char* oom = "JacobiSvd: insufficient device memory";
+  if (d_sched.alloc(sched.size(), oom) || d_partial.alloc(static_cast<uint64_t>(half) * chunks * 3, oom) || d_norms.alloc(q, oom) || d_perm.alloc(q, oom) || d_flag.alloc(1, oom)) {
+    *err = oom;
+    return 1;
+  }
+  if (cudaMemcpyAsync(d_sched, sched.data(), sched.size() * sizeof(int2), cudaMemcpyHostToDevice, c->stream) != cudaSuccess) return 1;
+  const double tol = std::max(1e-15, 4.4408920985006262e-16 * sqrt(static_cast<double>(rows)));
+  uint32_t sweep = 0;
+  bool converged = (q == 1);
+  for (; sweep < 60 && !converged; ++sweep) {
+    if (cudaMemsetAsync(d_flag, 0, 4, c->stream) != cudaSuccess) break;
+    for (uint32_t r = 0; r < rounds; ++r) {
+      const int2* pr = d_sched + static_cast<size_t>(r) * half;
+      if (fused) {
+        jacobi_fused_kernel<<<half, kJacobiThreads, 0, c->stream>>>(d_a, lda, rows, pr, tol, d_flag);
+        c->launches++;
+      } else {
+        jacobi_dots_kernel<<<dim3(half, chunks), kJacobiThreads, 0, c->stream>>>(d_a, lda, rows, pr, chunk_rows, d_partial);
+        jacobi_rotate_kernel<<<dim3(half, chunks), kJacobiThreads, 0, c->stream>>>(d_a, lda, rows, pr, chunk_rows, d_partial, tol, d_flag);
+        c->launches += 2;
       }
-      int flag = 1;
-      if (cudaMemcpyAsync(&flag, d_flag, 4, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
-        *err = "JacobiSvd: kernel failure";
-        break;
-      }
-      converged = (flag == 0);
     }
-    if (*err) break;
-    if (!converged) {
-      *err = "JacobiSvd: no convergence in 60 sweeps (non-finite input?)";
-      break;
-    }
-    if (sweeps_out) *sweeps_out = sweep;
-    jacobi_colnorm_kernel<<<q, kJacobiThreads, 0, c->stream>>>(d_a, lda, rows, d_norms);
-    c->launches++;
-    std::vector<double> norms(q);
-    if (cudaMemcpyAsync(norms.data(), d_norms, 8ull * q, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
+    int flag = 1;
+    if (cudaMemcpyAsync(&flag, d_flag, 4, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
       *err = "JacobiSvd: kernel failure";
-      break;
+      return 1;
     }
-    std::vector<uint32_t> perm(q);
-    std::iota(perm.begin(), perm.end(), 0u);
-    std::stable_sort(perm.begin(), perm.end(), [&](uint32_t x, uint32_t y) { return norms[x] > norms[y]; });
-    bool finite = true;
-    for (uint32_t i = 0; i < out_cols; ++i) {
-      sigma_host[i] = norms[perm[i]];
-      finite = finite && std::isfinite(sigma_host[i]);
+    converged = (flag == 0);
+  }
+  if (!converged) {
+    *err = "JacobiSvd: no convergence in 60 sweeps (non-finite input?)";
+    return 1;
+  }
+  if (sweeps_out) *sweeps_out = sweep;
+  jacobi_colnorm_kernel<<<q, kJacobiThreads, 0, c->stream>>>(d_a, lda, rows, d_norms);
+  c->launches++;
+  std::vector<double> norms(q);
+  if (cudaMemcpyAsync(norms.data(), d_norms, 8ull * q, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
+    *err = "JacobiSvd: kernel failure";
+    return 1;
+  }
+  std::vector<uint32_t> perm(q);
+  std::iota(perm.begin(), perm.end(), 0u);
+  std::stable_sort(perm.begin(), perm.end(), [&](uint32_t x, uint32_t y) { return norms[x] > norms[y]; });
+  bool finite = true;
+  for (uint32_t i = 0; i < out_cols; ++i) {
+    sigma_host[i] = norms[perm[i]];
+    finite = finite && std::isfinite(sigma_host[i]);
+  }
+  if (!finite) {
+    *err = "JacobiSvd: non-finite singular values";
+    return 1;
+  }
+  if (d_u && out_cols) {
+    if (cudaMemcpyAsync(d_perm, perm.data(), 4ull * q, cudaMemcpyHostToDevice, c->stream) != cudaSuccess) return 1;
+    jacobi_gather_kernel<<<dim3(DivUpU32(rows, 256), out_cols), 256, 0, c->stream>>>(d_a, lda, rows, d_perm, d_norms, d_u, ldu);
+    c->launches++;
+    if (cudaStreamSynchronize(c->stream) != cudaSuccess) {
+      *err = "JacobiSvd: kernel failure";
+      return 1;
     }
-    if (!finite) {
-      *err = "JacobiSvd: non-finite singular values";
-      break;
-    }
-    if (d_u && out_cols) {
-      if (cudaMemcpyAsync(d_perm, perm.data(), 4ull * q, cudaMemcpyHostToDevice, c->stream) != cudaSuccess) break;
-      jacobi_gather_kernel<<<dim3(DivUpU32(rows, 256), out_cols), 256, 0, c->stream>>>(d_a, lda, rows, d_perm, d_norms, d_u, ldu);
-      c->launches++;
-      if (cudaStreamSynchronize(c->stream) != cudaSuccess) {
-        *err = "JacobiSvd: kernel failure";
-        break;
-      }
-    }
-    rc = 0;
-  } while (0);
+  }
+  return 0;
+}
+
+// Host driver.  d_a (rows x q, leading dimension lda) is overwritten with U Sigma (unsorted).
+// sigma_host[0..out_cols) = singular values in descending order; d_u (may be nullptr) receives the
+// matching unit left singular vectors as a rows x out_cols column-major matrix (ldu).
+// Returns 0, or 1 with *err set (CUDA failure / no convergence).
+static int JacobiSvd(Ctx* c, double* d_a, uint64_t lda, uint32_t rows, uint32_t q, uint32_t out_cols, double* sigma_host, double* d_u, uint64_t ldu, uint32_t* sweeps_out, const char** err) {
+  *err = nullptr;
+  if (!q || rows < q || out_cols > q) {
+    *err = "JacobiSvd: bad shape";
+    return 1;
+  }
+  const int rc = JacobiSvdRun(c, d_a, lda, rows, q, out_cols, sigma_host, d_u, ldu, sweeps_out, err);
   if (rc && !*err) *err = "JacobiSvd: CUDA failure";
-  cudaFree(d_sched);
-  cudaFree(d_partial);
-  cudaFree(d_norms);
-  cudaFree(d_perm);
-  cudaFree(d_flag);
   cudaGetLastError();
   return rc;
 }

@@ -16,23 +16,7 @@ namespace {
 constexpr double kSmallEpsilon = 1.0 / 17592186044416.0;  // 2^-44, 2.0/include/plink2_base.h kSmallEpsilon
 constexpr uint32_t kLdChunkVariants = 16384;
 
-struct DevBuf {
-  void* p = nullptr;
-  ~DevBuf() { cudaFree(p); }
-  void release() {
-    cudaFree(p);
-    p = nullptr;
-  }
-  int alloc(uint64_t bytes) {
-    if (cudaMalloc(&p, bytes ? bytes : 4) != cudaSuccess) {
-      cudaGetLastError();
-      p = nullptr;
-      set_error("insufficient device memory (%.2f GB requested)", bytes / 1e9);
-      return 1;
-    }
-    return 0;
-  }
-};
+constexpr const char* kOom = "insufficient device memory (%.2f GB requested)";
 
 }  // namespace
 
@@ -48,11 +32,8 @@ int pl2gpu_geno_counts(Pl2GpuCtx* ctx, const void* genovecs, uint64_t variant_st
   GenoStage st;
   const uint32_t cap = std::min<uint32_t>(kMaxStageVariants, RoundUpU32(std::max(variant_ct, 1u), kVariantPad));
   PL2_TRY(StageAlloc(sample_ct, cap, &st));
-  DevBuf d_counts;
-  if (d_counts.alloc(16ull * cap)) {
-    StageFree(&st);
-    return 1;
-  }
+  DevArray<uint32_t> d_counts;
+  PL2_TRY(d_counts.alloc(4ull * cap, kOom, 16ull * cap / 1e9));
   const uint8_t* src = static_cast<const uint8_t*>(genovecs);
   int rc = 0;
   for (uint32_t done = 0; done < variant_ct && !rc; done += cap) {
@@ -60,14 +41,13 @@ int pl2gpu_geno_counts(Pl2GpuCtx* ctx, const void* genovecs, uint64_t variant_st
     uint32_t padded;
     rc = StageUpload(c, &st, src + static_cast<uint64_t>(done) * variant_stride_bytes, variant_stride_bytes, cur, src_is_device, &padded);
     if (rc) break;
-    geno_counts_kernel<<<DivUpU32(cur, 8), 256, 0, c->stream>>>(st.d_raw, st.pitch, st.sample_ct, st.sample_ct_padded, cur, static_cast<uint32_t*>(d_counts.p));
+    geno_counts_kernel<<<DivUpU32(cur, 8), 256, 0, c->stream>>>(st.d_raw, st.pitch, st.sample_ct, st.sample_ct_padded, cur, d_counts);
     c->launches++;
-    if (cudaMemcpyAsync(counts_host + 4ull * done, d_counts.p, 16ull * cur, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
+    if (cudaMemcpyAsync(counts_host + 4ull * done, d_counts, 16ull * cur, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
       set_error("pl2gpu_geno_counts: %s", cudaGetErrorString(cudaGetLastError()));
       rc = 1;
     }
   }
-  StageFree(&st);
   return rc;
 }
 
@@ -83,9 +63,10 @@ int pl2gpu_ld_band_flags(Pl2GpuCtx* ctx, const void* genovecs, uint64_t variant_
   // the copy of chunk k+1 (prep stream) overlaps the pair kernel of chunk k; flags come back through two device
   // buffers in the same rhythm
   StageRing ring;
-  DevBuf d_flags[2];
+  DevArray<uint8_t> d_flags[2];
+  const uint64_t flag_bytes = static_cast<uint64_t>(kLdChunkVariants) * band;
   int rc = ring.alloc(c, founder_ct, rows_cap, 64);
-  for (int b = 0; b < 2 && !rc; ++b) rc = d_flags[b].alloc(static_cast<uint64_t>(kLdChunkVariants) * band);
+  for (int b = 0; b < 2 && !rc; ++b) rc = d_flags[b].alloc(flag_bytes, kOom, flag_bytes / 1e9);
   if (!rc && cudaFuncSetAttribute(ld_ts_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kLdtSmemBytes) != cudaSuccess) {
     set_error("pl2gpu_ld_band_flags: %s", cudaGetErrorString(cudaGetLastError()));
     rc = 1;
@@ -98,7 +79,7 @@ int pl2gpu_ld_band_flags(Pl2GpuCtx* ctx, const void* genovecs, uint64_t variant_
   auto drain = [&](int b) -> int {  // flags of the chunk that used buffer b -> host
     if (!pend[b].live) return 0;
     pend[b].live = false;
-    if (cudaMemcpyAsync(flags_host + static_cast<uint64_t>(pend[b].a0) * band, d_flags[b].p, static_cast<uint64_t>(pend[b].a1 - pend[b].a0) * band, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess ||
+    if (cudaMemcpyAsync(flags_host + static_cast<uint64_t>(pend[b].a0) * band, d_flags[b], static_cast<uint64_t>(pend[b].a1 - pend[b].a0) * band, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess ||
         cudaStreamSynchronize(c->stream) != cudaSuccess) {
       set_error("pl2gpu_ld_band_flags: %s", cudaGetErrorString(cudaGetLastError()));
       return 1;
@@ -114,7 +95,7 @@ int pl2gpu_ld_band_flags(Pl2GpuCtx* ctx, const void* genovecs, uint64_t variant_
          ring.pad(b, a1 - lo, true, 64, &padded) || ring.fence(b);
     if (rc) break;
     const GenoStage& st = ring.stage[b];
-    ld_ts_kernel<<<dim3(DivUpU32(a1 - a0, kLdtRows), (kLdtRows - kLdtCols + band_r) / kLdtCols + 1), kLdtThreads, kLdtSmemBytes, c->stream>>>(st.d_raw, st.pitch, st.sample_ct_padded, lo, a0, a1, band, prune_ld_thresh, static_cast<uint8_t*>(d_flags[b].p));
+    ld_ts_kernel<<<dim3(DivUpU32(a1 - a0, kLdtRows), (kLdtRows - kLdtCols + band_r) / kLdtCols + 1), kLdtThreads, kLdtSmemBytes, c->stream>>>(st.d_raw, st.pitch, st.sample_ct_padded, lo, a0, a1, band, prune_ld_thresh, d_flags[b]);
     c->launches++;
     if (cudaGetLastError() != cudaSuccess) {
       set_error("pl2gpu_ld_band_flags: %s", cudaGetErrorString(cudaGetLastError()));
@@ -130,9 +111,8 @@ int pl2gpu_ld_band_flags(Pl2GpuCtx* ctx, const void* genovecs, uint64_t variant_
   for (uint32_t b = 0; b < 2; ++b) {
     if (!rc) rc = drain((ring.next + b) & 1);  // oldest pending first
   }
-  cudaStreamSynchronize(c->stream);
+  cudaStreamSynchronize(c->stream);  // the ring and the flag buffers are freed on return
   cudaStreamSynchronize(c->copy_stream);
-  ring.free();
   return rc;
 }
 
@@ -191,26 +171,28 @@ void PlanSubcontigs(uint32_t variant_ct, const uint32_t* chr_codes, const uint32
 
 // rows [v0, v1) of the caller's block, gathered / het-masked per `map` into a dense device block
 // out[v - v0][out_pitch] (PgrGet layout for out_sample_ct samples)
-int GatherRun(Ctx* c, const uint8_t* src, uint64_t stride, uint32_t founder_ct, uint32_t v0, uint32_t v1, int src_is_device, const std::vector<uint32_t>& map, DevBuf* out, uint32_t* out_pitch_ptr) {
+int GatherRun(Ctx* c, const uint8_t* src, uint64_t stride, uint32_t founder_ct, uint32_t v0, uint32_t v1, int src_is_device, const std::vector<uint32_t>& map, DevArray<uint8_t>* out, uint32_t* out_pitch_ptr) {
   const uint32_t out_ct = static_cast<uint32_t>(map.size());
   const uint32_t out_pitch = DivUpU32(std::max(out_ct, 1u), 32) * 8;
   *out_pitch_ptr = out_pitch;
-  DevBuf d_map, d_in;
-  if (out->alloc(static_cast<uint64_t>(v1 - v0) * out_pitch) || d_map.alloc(4ull * std::max(out_ct, 1u))) return 1;
-  if (out_ct) PL2_CUDA_OK(cudaMemcpyAsync(d_map.p, map.data(), 4ull * out_ct, cudaMemcpyHostToDevice, c->stream));
+  DevArray<uint32_t> d_map;
+  DevArray<uint8_t> d_in;
+  const uint64_t out_bytes = static_cast<uint64_t>(v1 - v0) * out_pitch;
+  if (out->alloc(out_bytes, kOom, out_bytes / 1e9) || d_map.alloc(std::max(out_ct, 1u), kOom, 4ull * std::max(out_ct, 1u) / 1e9)) return 1;
+  if (out_ct) PL2_CUDA_OK(cudaMemcpyAsync(d_map, map.data(), 4ull * out_ct, cudaMemcpyHostToDevice, c->stream));
   const uint32_t in_bytes = DivUpU32(founder_ct, 4);
   constexpr uint32_t kRows = 8192;
-  if (!src_is_device && d_in.alloc(static_cast<uint64_t>(kRows) * in_bytes)) return 1;
+  if (!src_is_device && d_in.alloc(static_cast<uint64_t>(kRows) * in_bytes, kOom, static_cast<uint64_t>(kRows) * in_bytes / 1e9)) return 1;
   for (uint32_t r0 = v0; r0 < v1; r0 += kRows) {
     const uint32_t rows = std::min(kRows, v1 - r0);
     const uint8_t* in = src + static_cast<uint64_t>(r0) * stride;
     uint64_t in_pitch = stride;
     if (!src_is_device) {
-      PL2_CUDA_OK(cudaMemcpy2DAsync(d_in.p, in_bytes, in, stride, in_bytes, rows, cudaMemcpyHostToDevice, c->stream));
-      in = static_cast<const uint8_t*>(d_in.p);
+      PL2_CUDA_OK(cudaMemcpy2DAsync(d_in, in_bytes, in, stride, in_bytes, rows, cudaMemcpyHostToDevice, c->stream));
+      in = d_in;
       in_pitch = in_bytes;
     }
-    geno_gather_kernel<<<dim3(DivUpU32(out_pitch, 256), rows), 256, 0, c->stream>>>(in, in_pitch, static_cast<uint8_t*>(out->p) + static_cast<uint64_t>(r0 - v0) * out_pitch, out_pitch, static_cast<const uint32_t*>(d_map.p), out_ct);
+    geno_gather_kernel<<<dim3(DivUpU32(out_pitch, 256), rows), 256, 0, c->stream>>>(in, in_pitch, out->get() + static_cast<uint64_t>(r0 - v0) * out_pitch, out_pitch, d_map, out_ct);
     c->launches++;
     PL2_CUDA_OK(cudaGetLastError());
     if (!src_is_device) PL2_CUDA_OK(cudaStreamSynchronize(c->stream));  // d_in is reused by the next chunk
@@ -275,7 +257,7 @@ int pl2_indep_pairwise_ex(Pl2GpuCtx* ctx, const void* genovecs, uint64_t variant
     runs.push_back({s, e, cls});
     s = e;
   }
-  std::vector<DevBuf> run_blocks(runs.size());
+  std::vector<DevArray<uint8_t>> run_blocks(runs.size());
   std::vector<uint32_t> run_pitch(runs.size(), 0), run_samples(runs.size(), founder_ct);
   std::vector<uint32_t> cls_counts, ld_counts;
   for (size_t ri = 0; ri < runs.size(); ++ri) {
@@ -287,15 +269,15 @@ int pl2_indep_pairwise_ex(Pl2GpuCtx* ctx, const void* genovecs, uint64_t variant
       run_samples[ri] = static_cast<uint32_t>(map_ld.size());
       if (!map_ld.empty()) {
         PL2_TRY(GatherRun(c, src, variant_stride_bytes, founder_ct, r.v0, r.v1, src_is_device, map_ld, &run_blocks[ri], &run_pitch[ri]));
-        PL2_TRY(pl2gpu_geno_counts(ctx, run_blocks[ri].p, run_pitch[ri], run_samples[ri], len, 1, ld_counts.data()));
+        PL2_TRY(pl2gpu_geno_counts(ctx, run_blocks[ri], run_pitch[ri], run_samples[ri], len, 1, ld_counts.data()));
       }
       const std::vector<uint32_t>* map_f = r.cls == kChrX ? &map_x_male_raw : r.cls == kChrY ? &map_y_raw : nullptr;
       cls_counts.assign(4ull * len, 0);
       if (map_f && !map_f->empty()) {
-        DevBuf tmp;
+        DevArray<uint8_t> tmp;
         uint32_t tp = 0;
         PL2_TRY(GatherRun(c, src, variant_stride_bytes, founder_ct, r.v0, r.v1, src_is_device, *map_f, &tmp, &tp));
-        PL2_TRY(pl2gpu_geno_counts(ctx, tmp.p, tp, static_cast<uint32_t>(map_f->size()), len, 1, cls_counts.data()));
+        PL2_TRY(pl2gpu_geno_counts(ctx, tmp, tp, static_cast<uint32_t>(map_f->size()), len, 1, cls_counts.data()));
       }
     }
     for (uint32_t v = r.v0; v < r.v1; ++v) {
@@ -348,8 +330,8 @@ int pl2_indep_pairwise_ex(Pl2GpuCtx* ctx, const void* genovecs, uint64_t variant
     if (r.cls == kDip) {
       PL2_TRY(pl2gpu_ld_band_flags(ctx, src + static_cast<uint64_t>(r.v0) * variant_stride_bytes, variant_stride_bytes, founder_ct, r.v1 - r.v0, src_is_device, band, thresh, fl));
     } else if (run_samples[ri]) {
-      PL2_TRY(pl2gpu_ld_band_flags(ctx, run_blocks[ri].p, run_pitch[ri], run_samples[ri], r.v1 - r.v0, 1, band, thresh, fl));
-      run_blocks[ri].release();
+      PL2_TRY(pl2gpu_ld_band_flags(ctx, run_blocks[ri], run_pitch[ri], run_samples[ri], r.v1 - r.v0, 1, band, thresh, fl));
+      run_blocks[ri].reset();
     }
   }
   // 4. greedy window walk on the host

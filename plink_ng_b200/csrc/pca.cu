@@ -4,6 +4,7 @@
 // reproduces the reference's SFMT / Box-Muller stream, host/sfmt.cc).
 #include <algorithm>
 #include <cmath>
+#include <memory>
 #include <vector>
 
 #include "../../include/plink2_b200.h"
@@ -22,24 +23,27 @@ constexpr double kSmallEpsilon = 1.0 / 17592186044416.0;
 }  // namespace
 
 struct Pl2PcaJob {
-  Pl2GpuCtx* ctx = nullptr;
+  explicit Pl2PcaJob(Pl2GpuCtx* x) : ctx(x) {}
+  ~Pl2PcaJob() {  // the kernels and copies that use the buffers finish before they are freed
+    cudaSetDevice(ctx->c.device);
+    cudaStreamSynchronize(ctx->c.stream);
+  }
+  Pl2GpuCtx* ctx;
   uint32_t sample_ct = 0, sample_ct_padded = 0, pitch = 0;
   uint32_t variant_cap = 0, variant_ct = 0, pc_ct = 0;
-  uint8_t* d_raw = nullptr;
-  uint32_t* d_counts = nullptr;
+  DevArray<uint8_t> d_raw;
+  DevArray<uint32_t> d_counts;
   std::vector<uint32_t> h_counts;
-  uint8_t* d_raw_i = nullptr;   // sample-major copy [row tile][k-step][128][8 B] of the whole matrix (geno_tile.cuh)
-  double* d_slope = nullptr;    // per variant: inv_stdev (0 for skipped variants)
-  double* d_icpt = nullptr;     // per variant: -2 alt_freq inv_stdev
-  double* d_twof = nullptr;     // per variant: 2 alt_freq (the mean-imputation value of --variant-score)
+  DevArray<uint8_t> d_raw_i;  // sample-major copy [row tile][k-step][128][8 B] of the whole matrix (geno_tile.cuh)
+  DevArray<double> d_slope;   // per variant: inv_stdev (0 for skipped variants)
+  DevArray<double> d_icpt;    // per variant: -2 alt_freq inv_stdev
+  DevArray<double> d_twof;    // per variant: 2 alt_freq (the mean-imputation value of --variant-score)
   std::vector<double> h_slope, h_icpt, h_twof;
   uint32_t retiled_to = 0;      // variants [0, retiled_to) are in d_raw_i (multiple of 64)
   bool vscore_only = false;     // begun with pc_ct = 0: a --variant-score job (no approx-PCA requirements, see the header)
 };
 
 extern "C" {
-
-int pl2gpu_pca_end(Pl2PcaJob* job);
 
 static int PcaBeginImpl(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t variant_ct_total, uint32_t pc_ct, bool shard, Pl2PcaJob** job_ptr) {
   *job_ptr = nullptr;
@@ -59,30 +63,25 @@ static int PcaBeginImpl(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t variant_ct_
     return 1;
   }
   PL2_CUDA_OK(cudaSetDevice(ctx->c.device));
-  Pl2PcaJob* job = new Pl2PcaJob();
-  job->ctx = ctx;
+  std::unique_ptr<Pl2PcaJob, int (*)(Pl2PcaJob*)> job(new Pl2PcaJob(ctx), pl2gpu_pca_end);
   job->sample_ct = sample_ct;
   job->sample_ct_padded = RoundUpU32(sample_ct, 128);
   job->pitch = job->sample_ct_padded / 4;
   job->variant_cap = RoundUpU32(variant_ct_total, 128);
   job->pc_ct = pc_ct;
   job->vscore_only = pc_ct == 0;
-  if (cudaMalloc(&job->d_raw, static_cast<uint64_t>(job->variant_cap) * job->pitch) != cudaSuccess || cudaMalloc(&job->d_counts, 16ull * 65536) != cudaSuccess ||
-      cudaMalloc(&job->d_raw_i, static_cast<uint64_t>(job->sample_ct_padded) * (job->variant_cap / 4)) != cudaSuccess || cudaMalloc(&job->d_slope, 8ull * job->variant_cap) != cudaSuccess ||
-      cudaMalloc(&job->d_icpt, 8ull * job->variant_cap) != cudaSuccess || cudaMalloc(&job->d_twof, 8ull * job->variant_cap) != cudaSuccess) {
-    cudaGetLastError();
-    set_error("pl2gpu_pca_begin: insufficient device memory to keep %u x %u genotypes resident", variant_ct_total, sample_ct);
-    pl2gpu_pca_end(job);
+  const char* oom = "pl2gpu_pca_begin: insufficient device memory to keep %u x %u genotypes resident";
+  if (job->d_raw.alloc(static_cast<uint64_t>(job->variant_cap) * job->pitch, oom, variant_ct_total, sample_ct) || job->d_counts.alloc(4ull * 65536, oom, variant_ct_total, sample_ct) ||
+      job->d_raw_i.alloc(static_cast<uint64_t>(job->sample_ct_padded) * (job->variant_cap / 4), oom, variant_ct_total, sample_ct) || job->d_slope.alloc(job->variant_cap, oom, variant_ct_total, sample_ct) ||
+      job->d_icpt.alloc(job->variant_cap, oom, variant_ct_total, sample_ct) || job->d_twof.alloc(job->variant_cap, oom, variant_ct_total, sample_ct))
     return 1;
-  }
   if (cudaMemsetAsync(job->d_slope, 0, 8ull * job->variant_cap, ctx->c.stream) != cudaSuccess || cudaMemsetAsync(job->d_icpt, 0, 8ull * job->variant_cap, ctx->c.stream) != cudaSuccess ||
       cudaFuncSetAttribute(pca_xa_wg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPxaSmemBytes) != cudaSuccess ||
       cudaFuncSetAttribute(pca_xtb_wg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kPxtSmemBytes) != cudaSuccess) {
     if (!*get_error()) set_error("pl2gpu_pca_begin: %s", cudaGetErrorString(cudaGetLastError()));
-    pl2gpu_pca_end(job);
     return 1;
   }
-  *job_ptr = job;
+  *job_ptr = job.release();
   return 0;
 }
 
@@ -99,7 +98,7 @@ int pl2gpu_pca_add_variants(Pl2PcaJob* job, const void* genovecs, uint64_t varia
   const uint8_t* src = static_cast<const uint8_t*>(genovecs);
   for (uint32_t done = 0; done < variant_ct;) {
     const uint32_t cur = std::min<uint32_t>(65536, variant_ct - done);
-    uint8_t* dst = job->d_raw + static_cast<uint64_t>(job->variant_ct) * job->pitch;
+    uint8_t* dst = job->d_raw.get() + static_cast<uint64_t>(job->variant_ct) * job->pitch;
     PL2_CUDA_OK(cudaMemcpy2DAsync(dst, job->pitch, src + static_cast<uint64_t>(done) * variant_stride_bytes, variant_stride_bytes, DivUpU32(job->sample_ct, 4), cur, src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, c->stream));
     PL2_TRY(LaunchPadGenotypes(c, dst, job->pitch, job->sample_ct, cur, cur));
     geno_counts_kernel<<<DivUpU32(cur, 8), 256, 0, c->stream>>>(dst, job->pitch, job->sample_ct, job->sample_ct_padded, cur, job->d_counts);
@@ -137,9 +136,9 @@ int pl2gpu_pca_add_variants(Pl2PcaJob* job, const void* genovecs, uint64_t varia
       job->h_slope[v] = inv_stdev;
       job->h_icpt[v] = -2 * alt_freq * inv_stdev;
     }
-    PL2_CUDA_OK(cudaMemcpyAsync(job->d_slope + job->variant_ct, job->h_slope.data(), 8ull * cur, cudaMemcpyHostToDevice, c->stream));
-    PL2_CUDA_OK(cudaMemcpyAsync(job->d_icpt + job->variant_ct, job->h_icpt.data(), 8ull * cur, cudaMemcpyHostToDevice, c->stream));
-    PL2_CUDA_OK(cudaMemcpyAsync(job->d_twof + job->variant_ct, job->h_twof.data(), 8ull * cur, cudaMemcpyHostToDevice, c->stream));
+    PL2_CUDA_OK(cudaMemcpyAsync(job->d_slope.get() + job->variant_ct, job->h_slope.data(), 8ull * cur, cudaMemcpyHostToDevice, c->stream));
+    PL2_CUDA_OK(cudaMemcpyAsync(job->d_icpt.get() + job->variant_ct, job->h_icpt.data(), 8ull * cur, cudaMemcpyHostToDevice, c->stream));
+    PL2_CUDA_OK(cudaMemcpyAsync(job->d_twof.get() + job->variant_ct, job->h_twof.data(), 8ull * cur, cudaMemcpyHostToDevice, c->stream));
     PL2_CUDA_OK(cudaStreamSynchronize(c->stream));
     job->variant_ct += cur;
     done += cur;
@@ -162,22 +161,11 @@ constexpr uint32_t kPcaXtbMaxKsteps = (0x7FFFFFFFu / (384u * 32u)) / 4 * 4;  // 
 
 // scratch of one job's products: digit planes, per-column scales, split-K partial sums of Y^T H
 struct PcaTs {
-  uint8_t *gdig = nullptr, *hs = nullptr, *hi = nullptr;
-  double *scale = nullptr, *inv_scale = nullptr, *partial = nullptr;
-  unsigned long long* colmax = nullptr;
+  DevArray<uint8_t> gdig, hs, hi;
+  DevArray<double> scale, inv_scale, partial;
+  DevArray<unsigned long long> colmax;
   uint32_t splits = 0, ksteps_per_split = 0;
 };
-
-static void PcaTsFree(PcaTs* ts) {
-  cudaFree(ts->gdig);
-  cudaFree(ts->hs);
-  cudaFree(ts->hi);
-  cudaFree(ts->scale);
-  cudaFree(ts->inv_scale);
-  cudaFree(ts->colmax);
-  cudaFree(ts->partial);
-  *ts = PcaTs();
-}
 
 // xtb: also the slope.H / icpt.H digit planes and the split-K partial sums.  Split plan of Y^T H: about two CTAs per
 // SM over the 128-sample row tiles, at least 64 k-steps (2,048 variants) per split, a whole number of 4-k-step stages
@@ -188,16 +176,10 @@ static int PcaTsAlloc(const Pl2PcaJob* job, bool xtb, PcaTs* ts) {
   uint32_t splits = std::max(1u, std::min(DivUpU32(2 * static_cast<uint32_t>(c->sm_count), tiles2), kstep_total / 64));
   ts->ksteps_per_split = std::min(kPcaXtbMaxKsteps, RoundUpU32(DivUpU32(kstep_total, splits), 4));
   ts->splits = DivUpU32(kstep_total, ts->ksteps_per_split);
-  if (cudaMalloc(&ts->gdig, static_cast<uint64_t>(npad) * kPcaNMax) != cudaSuccess || cudaMalloc(&ts->scale, 8 * kPcaCgMax) != cudaSuccess || cudaMalloc(&ts->inv_scale, 8 * kPcaCgMax) != cudaSuccess ||
-      cudaMalloc(&ts->colmax, 8 * kPcaCgMax) != cudaSuccess ||
-      (xtb && (cudaMalloc(&ts->hs, static_cast<uint64_t>(job->variant_cap) * kPcaNMax) != cudaSuccess || cudaMalloc(&ts->hi, static_cast<uint64_t>(job->variant_cap) * kPcaNMax) != cudaSuccess ||
-               cudaMalloc(&ts->partial, static_cast<uint64_t>(ts->splits) * npad * kPcaCgMax * 8) != cudaSuccess))) {
-    cudaGetLastError();
-    set_error("pl2gpu_pca: insufficient device memory for the digit planes");
-    PcaTsFree(ts);
-    return 1;
-  }
-  return 0;
+  const char* oom = "pl2gpu_pca: insufficient device memory for the digit planes";
+  return ts->gdig.alloc(static_cast<uint64_t>(npad) * kPcaNMax, oom) || ts->scale.alloc(kPcaCgMax, oom) || ts->inv_scale.alloc(kPcaCgMax, oom) || ts->colmax.alloc(kPcaCgMax, oom) ||
+         (xtb && (ts->hs.alloc(static_cast<uint64_t>(job->variant_cap) * kPcaNMax, oom) || ts->hi.alloc(static_cast<uint64_t>(job->variant_cap) * kPcaNMax, oom) ||
+                  ts->partial.alloc(static_cast<uint64_t>(ts->splits) * npad * kPcaCgMax, oom)));
 }
 
 // rows [variant_ct, variant_cap) must decode to "missing" in both layouts; sample_major: finish the sample-major copy
@@ -205,11 +187,11 @@ static int PcaTsAlloc(const Pl2PcaJob* job, bool xtb, PcaTs* ts) {
 static int PcaFinishLayouts(Pl2PcaJob* job, bool sample_major) {
   Ctx* c = &job->ctx->c;
   const uint32_t m = job->variant_ct;
-  if (job->variant_cap > m) PL2_TRY(LaunchPadGenotypes(c, job->d_raw + static_cast<uint64_t>(m) * job->pitch, job->pitch, job->sample_ct, 0, job->variant_cap - m));
+  if (job->variant_cap > m) PL2_TRY(LaunchPadGenotypes(c, job->d_raw.get() + static_cast<uint64_t>(m) * job->pitch, job->pitch, job->sample_ct, 0, job->variant_cap - m));
   if (sample_major && job->retiled_to < job->variant_cap) {
     const uint32_t from = job->retiled_to;
-    geno_tile_rows_kernel<<<dim3((job->variant_cap - from) / 64, job->sample_ct_padded / 64), 256, 0, c->stream>>>(job->d_raw + static_cast<uint64_t>(from) * job->pitch, job->pitch, job->variant_cap / 32, 0,
-                                                                                                                 job->d_raw_i + static_cast<uint64_t>(from / 32) * 1024);
+    geno_tile_rows_kernel<<<dim3((job->variant_cap - from) / 64, job->sample_ct_padded / 64), 256, 0, c->stream>>>(job->d_raw.get() + static_cast<uint64_t>(from) * job->pitch, job->pitch, job->variant_cap / 32, 0,
+                                                                                                                 job->d_raw_i.get() + static_cast<uint64_t>(from / 32) * 1024);
     c->launches++;
     job->retiled_to = job->variant_cap;
   }
@@ -293,8 +275,6 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
     set_error("pl2gpu_pca_run: need 2k(k+1) = %llu <= min(variants %llu, samples %u)", static_cast<unsigned long long>(q), static_cast<unsigned long long>(total_variant_ct), n);
     return 1;
   }
-  double *d_qq = nullptr, *d_u = nullptr, *d_g1 = nullptr, *d_g2 = nullptr, *d_b = nullptr, *d_gram = nullptr, *d_gram_u = nullptr, *d_gram_partial = nullptr, *d_colscale = nullptr;
-  int rc = 1;
   const double m_recip = 1.0 / static_cast<double>(total_variant_ct);
   PL2_TRY(PcaFinishLayouts(job, true));
   PcaTs ts;
@@ -302,10 +282,10 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
   int ts_rc = 0;
   // PL2_TIMING=1: phase times on stderr (stream-synchronising; development aid)
   const bool timing = getenv("PL2_TIMING") != nullptr;
-  cudaEvent_t ev_t0 = nullptr, ev_t1 = nullptr;
+  Event ev_t0, ev_t1;
   if (timing) {
-    cudaEventCreate(&ev_t0);
-    cudaEventCreate(&ev_t1);
+    ev_t0.create(cudaEventDefault, "pl2gpu_pca_run: cudaEventCreate failed: %s");
+    ev_t1.create(cudaEventDefault, "pl2gpu_pca_run: cudaEventCreate failed: %s");
     cudaEventRecord(ev_t0, c->stream);
   }
   auto mark = [&](const char* what) {
@@ -317,62 +297,62 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
     fprintf(stderr, "[timing] pca_run %-34s %9.2f ms\n", what, ms);
     std::swap(ev_t0, ev_t1);
   };
-  do {
-    if (cudaMalloc(&d_qq, static_cast<uint64_t>(m) * q * 8) != cudaSuccess || cudaMalloc(&d_u, static_cast<uint64_t>(std::max(m, n)) * q * 8) != cudaSuccess || cudaMalloc(&d_g1, static_cast<uint64_t>(npad) * c2 * 8) != cudaSuccess ||
-        cudaMalloc(&d_g2, static_cast<uint64_t>(npad) * c2 * 8) != cudaSuccess || cudaMalloc(&d_b, static_cast<uint64_t>(n) * q * 8) != cudaSuccess ) {
-      cudaGetLastError();
-      set_error("pl2gpu_pca_run: insufficient device memory for the %u x %llu Krylov matrix", m, static_cast<unsigned long long>(q));
-      break;
+  DevArray<double> d_qq, d_u, d_g1, d_g2, d_b;
+  const char* krylov_oom = "pl2gpu_pca_run: insufficient device memory for the %u x %llu Krylov matrix";
+  const unsigned long long q_ull = q;
+  if (d_qq.alloc(static_cast<uint64_t>(m) * q, krylov_oom, m, q_ull) || d_u.alloc(static_cast<uint64_t>(std::max(m, n)) * q, krylov_oom, m, q_ull) || d_g1.alloc(static_cast<uint64_t>(npad) * c2, krylov_oom, m, q_ull) ||
+      d_g2.alloc(static_cast<uint64_t>(npad) * c2, krylov_oom, m, q_ull) || d_b.alloc(static_cast<uint64_t>(n) * q, krylov_oom, m, q_ull))
+    return 1;
+  if (cudaMemsetAsync(d_g1, 0, static_cast<uint64_t>(npad) * c2 * 8, c->stream) != cudaSuccess || cudaMemcpyAsync(d_g1, g1_host, static_cast<uint64_t>(n) * c2 * 8, cudaMemcpyHostToDevice, c->stream) != cudaSuccess) return 1;
+  // k+1 projections; every H_t = Y G_t is kept side by side in qq (column-major M x q)   :5783-5855
+  for (uint32_t iter = 0; iter <= k; ++iter) {
+    double* h_t = d_qq.get() + static_cast<uint64_t>(iter * c2) * m;
+    ts_rc |= PcaLaunchXa(job, &ts, job->d_slope, job->d_icpt, d_g1, c2, h_t, m, c2);
+    if (iter < k) {
+      if (cudaMemsetAsync(d_g2, 0, static_cast<uint64_t>(npad) * c2 * 8, c->stream) != cudaSuccess) break;
+      ts_rc |= PcaLaunchXtb(job, &ts, h_t, m, c2, d_g2, c2, 1);
+      if (sharded && CommAllReduceSumF64(c, d_g2, static_cast<uint64_t>(npad) * c2, c->stream)) break;
+      scale_kernel<<<static_cast<uint32_t>(DivUpU64(static_cast<uint64_t>(npad) * c2, 256)), 256, 0, c->stream>>>(d_g2, static_cast<uint64_t>(npad) * c2, m_recip);
+      c->launches++;
+      std::swap(d_g1, d_g2);
     }
-    if (cudaMemsetAsync(d_g1, 0, static_cast<uint64_t>(npad) * c2 * 8, c->stream) != cudaSuccess || cudaMemcpyAsync(d_g1, g1_host, static_cast<uint64_t>(n) * c2 * 8, cudaMemcpyHostToDevice, c->stream) != cudaSuccess) break;
-    // k+1 projections; every H_t = Y G_t is kept side by side in qq (column-major M x q)   :5783-5855
-    for (uint32_t iter = 0; iter <= k; ++iter) {
-      double* h_t = d_qq + static_cast<uint64_t>(iter * c2) * m;
-      ts_rc |= PcaLaunchXa(job, &ts, job->d_slope, job->d_icpt, d_g1, c2, h_t, m, c2);
-      if (iter < k) {
-        if (cudaMemsetAsync(d_g2, 0, static_cast<uint64_t>(npad) * c2 * 8, c->stream) != cudaSuccess) break;
-        ts_rc |= PcaLaunchXtb(job, &ts, h_t, m, c2, d_g2, c2, 1);
-        if (sharded && CommAllReduceSumF64(c, d_g2, static_cast<uint64_t>(npad) * c2, c->stream)) break;
-        scale_kernel<<<static_cast<uint32_t>(DivUpU64(static_cast<uint64_t>(npad) * c2, 256)), 256, 0, c->stream>>>(d_g2, static_cast<uint64_t>(npad) * c2, m_recip);
-        c->launches++;
-        std::swap(d_g1, d_g2);
-      }
-    }
-    if (cudaGetLastError() != cudaSuccess) {
-      set_error("pl2gpu_pca_run: kernel launch failed");
-      break;
-    }
-    mark("power iterations (Y.G / Yt.H)");
-    // Orthonormal basis Q of the range of the Krylov matrix, built in place in qq   :5860 (the reference takes the left
-    // singular vectors from dgesvd; only their span enters B = Y^T Q and everything after it).  Block classical
-    // Gram-Schmidt over the k + 1 Krylov blocks, three projection passes per block (the blocks span 35 orders of
-    // magnitude - two passes are not enough), each followed by a Jacobi SVD of the M x 2k residual whose unit left
-    // singular vectors replace the block: O(M q^2) in all, what a one-sided Jacobi SVD of the whole M x q matrix costs
-    // per sweep.  The structure PCs match the LAPACK-based restatement to 1e-13; the noise-level eigenvalues differ
-    // from it by 1e-4..1e-3, because the Krylov matrix is numerically rank deficient and every method completes the
-    // basis differently there.
-    std::vector<double> s(q);
-    const char* err = nullptr;
-    double *d_c = nullptr, *d_cpart = nullptr, *d_wg = nullptr, *d_wf = nullptr, *d_uf = nullptr, *d_sizes = nullptr;
+  }
+  if (cudaGetLastError() != cudaSuccess) {
+    set_error("pl2gpu_pca_run: kernel launch failed");
+    return 1;
+  }
+  mark("power iterations (Y.G / Yt.H)");
+  // Orthonormal basis Q of the range of the Krylov matrix, built in place in qq   :5860 (the reference takes the left
+  // singular vectors from dgesvd; only their span enters B = Y^T Q and everything after it).  Block classical
+  // Gram-Schmidt over the k + 1 Krylov blocks, three projection passes per block (the blocks span 35 orders of
+  // magnitude - two passes are not enough), each followed by a Jacobi SVD of the M x 2k residual whose unit left
+  // singular vectors replace the block: O(M q^2) in all, what a one-sided Jacobi SVD of the whole M x q matrix costs
+  // per sweep.  The structure PCs match the LAPACK-based restatement to 1e-13; the noise-level eigenvalues differ
+  // from it by 1e-4..1e-3, because the Krylov matrix is numerically rank deficient and every method completes the
+  // basis differently there.
+  std::vector<double> s(q);
+  const char* err = nullptr;
+  {  // the scratch of the basis construction is freed before the Gram matrix is allocated
+    DevArray<double> d_c, d_cpart, d_wg, d_wf, d_uf, d_sizes;
+    const char* ortho_oom = "Failed to orthonormalise the Krylov matrix (CUDA failure).";
     uint64_t part_doubles = 1;
     for (uint32_t t = 1; t <= k; ++t) part_doubles = std::max(part_doubles, DgemmTNPartialDoubles(c, t * c2, c2, m));
-    bool ok = cudaMalloc(&d_c, q * c2 * 8) == cudaSuccess && cudaMalloc(&d_cpart, part_doubles * 8) == cudaSuccess;
+    bool ok = !d_c.alloc(q * c2, ortho_oom) && !d_cpart.alloc(part_doubles, ortho_oom);
     // sharded: every rank learns the shard sizes (one all-reduce of a world-length vector), blocks are exchanged
     // in slots of the largest shard
     uint64_t m_pad = m;
     if (ok && sharded) {
       std::vector<double> sizes(world, 0.0);
       sizes[rank] = static_cast<double>(m);
-      ok = cudaMalloc(&d_sizes, 8ull * world) == cudaSuccess && cudaMemcpyAsync(d_sizes, sizes.data(), 8ull * world, cudaMemcpyHostToDevice, c->stream) == cudaSuccess &&
-           !CommAllReduceSumF64(c, d_sizes, world, c->stream) && cudaMemcpyAsync(sizes.data(), d_sizes, 8ull * world, cudaMemcpyDeviceToHost, c->stream) == cudaSuccess &&
-           cudaStreamSynchronize(c->stream) == cudaSuccess;
+      ok = !d_sizes.alloc(world, ortho_oom) && cudaMemcpyAsync(d_sizes, sizes.data(), 8ull * world, cudaMemcpyHostToDevice, c->stream) == cudaSuccess && !CommAllReduceSumF64(c, d_sizes, world, c->stream) &&
+           cudaMemcpyAsync(sizes.data(), d_sizes, 8ull * world, cudaMemcpyDeviceToHost, c->stream) == cudaSuccess && cudaStreamSynchronize(c->stream) == cudaSuccess;
       for (uint32_t r = 0; ok && r < world; ++r) m_pad = std::max<uint64_t>(m_pad, static_cast<uint64_t>(sizes[r]));
-      const uint64_t blk = m_pad * c2 * 8;
-      ok = ok && cudaMalloc(&d_wg, blk * world) == cudaSuccess && cudaMalloc(&d_wf, blk * world) == cudaSuccess && cudaMalloc(&d_uf, blk * world) == cudaSuccess;
+      const uint64_t blk = m_pad * c2;
+      ok = ok && !d_wg.alloc(blk * world, ortho_oom) && !d_wf.alloc(blk * world, ortho_oom) && !d_uf.alloc(blk * world, ortho_oom);
     }
     const uint64_t m_full = m_pad * world;
     for (uint32_t t = 0; ok && t <= k; ++t) {
-      double* w = d_qq + static_cast<uint64_t>(t) * c2 * m;
+      double* w = d_qq.get() + static_cast<uint64_t>(t) * c2 * m;
       const uint32_t prev = t * c2;
       for (int rep = 0; ok && rep < 3; ++rep) {
         if (prev) {
@@ -389,97 +369,77 @@ static int PcaRunImpl(Pl2PcaJob* job, const double* g1_host, uint64_t total_vari
         } else {
           // my rows into my slot (zero-padded to m_pad), all-gather, repack to one column-major (world m_pad) x 2k
           // matrix, the same Jacobi SVD on every rank, my rows of the unit left singular vectors back into the block
-          double* slot = d_wg + static_cast<uint64_t>(rank) * m_pad * c2;
+          double* slot = d_wg.get() + static_cast<uint64_t>(rank) * m_pad * c2;
           ok = cudaMemsetAsync(slot, 0, m_pad * c2 * 8, c->stream) == cudaSuccess &&
                cudaMemcpy2DAsync(slot, m_pad * 8, w, static_cast<uint64_t>(m) * 8, static_cast<uint64_t>(m) * 8, c2, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess &&
                !CommAllGatherInPlace(c, d_wg, m_pad * c2 * 8, c->stream);
           for (uint32_t r = 0; ok && r < world; ++r)
-            ok = cudaMemcpy2DAsync(d_wf + static_cast<uint64_t>(r) * m_pad, m_full * 8, d_wg + static_cast<uint64_t>(r) * m_pad * c2, m_pad * 8, m_pad * 8, c2, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
+            ok = cudaMemcpy2DAsync(d_wf.get() + static_cast<uint64_t>(r) * m_pad, m_full * 8, d_wg.get() + static_cast<uint64_t>(r) * m_pad * c2, m_pad * 8, m_pad * 8, c2, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
           if (!ok) break;
           if (JacobiSvd(c, d_wf, m_full, static_cast<uint32_t>(m_full), c2, c2, s.data(), d_uf, m_full, nullptr, &err)) {
             ok = false;
             break;
           }
-          ok = cudaMemcpy2DAsync(w, static_cast<uint64_t>(m) * 8, d_uf + static_cast<uint64_t>(rank) * m_pad, m_full * 8, static_cast<uint64_t>(m) * 8, c2, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
+          ok = cudaMemcpy2DAsync(w, static_cast<uint64_t>(m) * 8, d_uf.get() + static_cast<uint64_t>(rank) * m_pad, m_full * 8, static_cast<uint64_t>(m) * 8, c2, cudaMemcpyDeviceToDevice, c->stream) == cudaSuccess;
         }
       }
     }
-    cudaFree(d_c);
-    cudaFree(d_cpart);
-    cudaFree(d_wg);
-    cudaFree(d_wf);
-    cudaFree(d_uf);
-    cudaFree(d_sizes);
     if (!ok) {
       cudaGetLastError();
-      if (!err && *get_error()) break;  // a collective already recorded its message
+      if (!err && *get_error()) return 1;  // a collective or an allocation already recorded its message
       set_error("Failed to orthonormalise the Krylov matrix (%s).", err ? err : "CUDA failure");
-      break;
+      return 1;
     }
-    mark("orthonormal basis of the Krylov matrix (BCGS)");
-    // B = Y^T Q (N x q, column-major)   :5870-5916
-    if (cudaMemsetAsync(d_b, 0, static_cast<uint64_t>(n) * q * 8, c->stream) != cudaSuccess) break;
-    ts_rc |= PcaLaunchXtb(job, &ts, d_qq, m, static_cast<uint32_t>(q), d_b, 1, n);
-    if (sharded && CommAllReduceSumF64(c, d_b, static_cast<uint64_t>(n) * q, c->stream)) break;
-    mark("B = Yt.Q");
-    // Top-k left singular pairs of B (:5920, dgesvd in the reference).  Only the leading k of q are wanted and they
-    // are the well-conditioned ones, so they come from the q x q Gram matrix: G = B^T B (fp64, fixed-order split
-    // sums), eigenpairs of G by one-sided Jacobi on its columns (G V = V Lambda for a symmetric PSD matrix), then
-    // U_k = B V_k Lambda_k^-1/2.  The relative error of sigma_i is eps (sigma_1 / sigma_i)^2 - 1e-14 here - and no
-    // N x q Jacobi sweep over B is needed (1.2 s at N = 16,384, O(N q^2) per sweep).
-    const uint32_t q32 = static_cast<uint32_t>(q);
-    if (cudaMalloc(&d_gram, q * q * 8) != cudaSuccess || cudaMalloc(&d_gram_u, q * k * 8) != cudaSuccess || cudaMalloc(&d_gram_partial, DgemmTNPartialDoubles(c, q32, q32, n) * 8) != cudaSuccess ||
-        cudaMalloc(&d_colscale, 8ull * k) != cudaSuccess) {
-      cudaGetLastError();
-      set_error("pl2gpu_pca_run: insufficient device memory for the %llu x %llu Gram matrix", static_cast<unsigned long long>(q), static_cast<unsigned long long>(q));
-      break;
-    }
-    if (DgemmTN(c, d_b, n, q32, d_b, n, q32, n, d_gram_partial, d_gram, q)) break;
-    if (JacobiSvd(c, d_gram, q, q32, q32, k, s.data(), d_gram_u, q, nullptr, &err)) {
-      set_error("Failed to compute SVD of final matrix (%s).", err ? err : "?");
-      break;
-    }
-    std::vector<double> inv_sigma(k);
-    ok = true;
-    for (uint32_t p = 0; p < k; ++p) {
-      ok = ok && s[p] > 0.0;
-      s[p] = sqrt(s[p]);  // eigenvalue of B^T B -> singular value of B
-      inv_sigma[p] = ok ? 1.0 / s[p] : 0.0;
-    }
-    if (!ok) {
-      set_error("Failed to compute SVD of final matrix (rank below the requested number of PCs).");
-      break;
-    }
-    if (cudaMemcpyAsync(d_colscale, inv_sigma.data(), 8ull * k, cudaMemcpyHostToDevice, c->stream) != cudaSuccess) break;
-    // d_u, the scratch of the basis construction, is free once B is formed (stream order): reuse it for U_k (N x k,
-    // column-major)
-    if (DgemmNN(c, d_b, n, n, q32, d_gram_u, q, k, d_u, n, false, d_colscale)) break;
-    mark("top-k singular pairs of the N x q matrix B");
-    // the context's stream is non-blocking: order the copy on it (a plain cudaMemcpy would not wait for the kernels)
-    if (cudaMemcpyAsync(eigvecs_host, d_u, 8ull * k * n, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
-      set_error("pl2gpu_pca_run: %s", cudaGetErrorString(cudaGetLastError()));
-      break;
-    }
-    for (uint32_t p = 0; p < k; ++p) eigvals_host[p] = s[p] * s[p] * m_recip;  // :5931
-    rc = 0;
-  } while (0);
-  if (ev_t0) cudaEventDestroy(ev_t0);
-  if (ev_t1) cudaEventDestroy(ev_t1);
-  if (ts_rc && !rc) {
-    set_error("pl2gpu_pca_run: a tensor-path launch failed");
-    rc = 1;
   }
-  PcaTsFree(&ts);
-  cudaFree(d_gram);
-  cudaFree(d_gram_u);
-  cudaFree(d_gram_partial);
-  cudaFree(d_colscale);
-  cudaFree(d_qq);
-  cudaFree(d_u);
-  cudaFree(d_g1);
-  cudaFree(d_g2);
-  cudaFree(d_b);
-  return rc;
+  mark("orthonormal basis of the Krylov matrix (BCGS)");
+  // B = Y^T Q (N x q, column-major)   :5870-5916
+  if (cudaMemsetAsync(d_b, 0, static_cast<uint64_t>(n) * q * 8, c->stream) != cudaSuccess) return 1;
+  ts_rc |= PcaLaunchXtb(job, &ts, d_qq, m, static_cast<uint32_t>(q), d_b, 1, n);
+  if (sharded && CommAllReduceSumF64(c, d_b, static_cast<uint64_t>(n) * q, c->stream)) return 1;
+  mark("B = Yt.Q");
+  // Top-k left singular pairs of B (:5920, dgesvd in the reference).  Only the leading k of q are wanted and they
+  // are the well-conditioned ones, so they come from the q x q Gram matrix: G = B^T B (fp64, fixed-order split
+  // sums), eigenpairs of G by one-sided Jacobi on its columns (G V = V Lambda for a symmetric PSD matrix), then
+  // U_k = B V_k Lambda_k^-1/2.  The relative error of sigma_i is eps (sigma_1 / sigma_i)^2 - 1e-14 here - and no
+  // N x q Jacobi sweep over B is needed (1.2 s at N = 16,384, O(N q^2) per sweep).
+  const uint32_t q32 = static_cast<uint32_t>(q);
+  DevArray<double> d_gram, d_gram_u, d_gram_partial, d_colscale;
+  const char* gram_oom = "pl2gpu_pca_run: insufficient device memory for the %llu x %llu Gram matrix";
+  if (d_gram.alloc(q * q, gram_oom, q_ull, q_ull) || d_gram_u.alloc(q * k, gram_oom, q_ull, q_ull) || d_gram_partial.alloc(DgemmTNPartialDoubles(c, q32, q32, n), gram_oom, q_ull, q_ull) ||
+      d_colscale.alloc(k, gram_oom, q_ull, q_ull))
+    return 1;
+  if (DgemmTN(c, d_b, n, q32, d_b, n, q32, n, d_gram_partial, d_gram, q)) return 1;
+  if (JacobiSvd(c, d_gram, q, q32, q32, k, s.data(), d_gram_u, q, nullptr, &err)) {
+    set_error("Failed to compute SVD of final matrix (%s).", err ? err : "?");
+    return 1;
+  }
+  std::vector<double> inv_sigma(k);
+  bool ok = true;
+  for (uint32_t p = 0; p < k; ++p) {
+    ok = ok && s[p] > 0.0;
+    s[p] = sqrt(s[p]);  // eigenvalue of B^T B -> singular value of B
+    inv_sigma[p] = ok ? 1.0 / s[p] : 0.0;
+  }
+  if (!ok) {
+    set_error("Failed to compute SVD of final matrix (rank below the requested number of PCs).");
+    return 1;
+  }
+  if (cudaMemcpyAsync(d_colscale, inv_sigma.data(), 8ull * k, cudaMemcpyHostToDevice, c->stream) != cudaSuccess) return 1;
+  // d_u, the scratch of the basis construction, is free once B is formed (stream order): reuse it for U_k (N x k,
+  // column-major)
+  if (DgemmNN(c, d_b, n, n, q32, d_gram_u, q, k, d_u, n, false, d_colscale)) return 1;
+  mark("top-k singular pairs of the N x q matrix B");
+  // the context's stream is non-blocking: order the copy on it (a plain cudaMemcpy would not wait for the kernels)
+  if (cudaMemcpyAsync(eigvecs_host, d_u, 8ull * k * n, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
+    set_error("pl2gpu_pca_run: %s", cudaGetErrorString(cudaGetLastError()));
+    return 1;
+  }
+  for (uint32_t p = 0; p < k; ++p) eigvals_host[p] = s[p] * s[p] * m_recip;  // :5931
+  if (ts_rc) {
+    set_error("pl2gpu_pca_run: a tensor-path launch failed");
+    return 1;
+  }
+  return 0;
 }
 
 extern "C" {
@@ -501,47 +461,32 @@ int pl2gpu_pca_products(Pl2PcaJob* job, const double* g_host, uint32_t g_cols, d
   PL2_TRY(PcaFinishLayouts(job, h_cols != 0));
   PcaTs ts;
   PL2_TRY(PcaTsAlloc(job, h_cols != 0, &ts));
-  double *d_g = nullptr, *d_yg = nullptr, *d_h = nullptr, *d_yth = nullptr;
-  int rc = 1;
-  do {
-    if (g_cols) {
-      if (cudaMalloc(&d_g, static_cast<uint64_t>(npad) * g_cols * 8) != cudaSuccess || cudaMalloc(&d_yg, static_cast<uint64_t>(m) * g_cols * 8) != cudaSuccess) {
-        cudaGetLastError();
-        set_error("pl2gpu_pca_products: insufficient device memory for %u columns of Y G", g_cols);
-        break;
-      }
-      if (cudaMemsetAsync(d_g, 0, static_cast<uint64_t>(npad) * g_cols * 8, c->stream) != cudaSuccess ||
-          cudaMemcpyAsync(d_g, g_host, static_cast<uint64_t>(n) * g_cols * 8, cudaMemcpyHostToDevice, c->stream) != cudaSuccess || PcaLaunchXa(job, &ts, job->d_slope, job->d_icpt, d_g, g_cols, d_yg, m, g_cols) ||
-          cudaMemcpyAsync(yg_host, d_yg, static_cast<uint64_t>(m) * g_cols * 8, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess) {
-        set_error("pl2gpu_pca_products: Y G: %s", cudaGetErrorString(cudaGetLastError()));
-        break;
-      }
+  DevArray<double> d_g, d_yg, d_h, d_yth;
+  if (g_cols) {
+    const char* oom = "pl2gpu_pca_products: insufficient device memory for %u columns of Y G";
+    if (d_g.alloc(static_cast<uint64_t>(npad) * g_cols, oom, g_cols) || d_yg.alloc(static_cast<uint64_t>(m) * g_cols, oom, g_cols)) return 1;
+    if (cudaMemsetAsync(d_g, 0, static_cast<uint64_t>(npad) * g_cols * 8, c->stream) != cudaSuccess ||
+        cudaMemcpyAsync(d_g, g_host, static_cast<uint64_t>(n) * g_cols * 8, cudaMemcpyHostToDevice, c->stream) != cudaSuccess || PcaLaunchXa(job, &ts, job->d_slope, job->d_icpt, d_g, g_cols, d_yg, m, g_cols) ||
+        cudaMemcpyAsync(yg_host, d_yg, static_cast<uint64_t>(m) * g_cols * 8, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess) {
+      set_error("pl2gpu_pca_products: Y G: %s", cudaGetErrorString(cudaGetLastError()));
+      return 1;
     }
-    if (h_cols) {
-      if (cudaMalloc(&d_h, static_cast<uint64_t>(m) * h_cols * 8) != cudaSuccess || cudaMalloc(&d_yth, static_cast<uint64_t>(n) * h_cols * 8) != cudaSuccess) {
-        cudaGetLastError();
-        set_error("pl2gpu_pca_products: insufficient device memory for %u columns of Y^T H", h_cols);
-        break;
-      }
-      if (cudaMemcpyAsync(d_h, h_host, static_cast<uint64_t>(m) * h_cols * 8, cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
-          cudaMemsetAsync(d_yth, 0, static_cast<uint64_t>(n) * h_cols * 8, c->stream) != cudaSuccess || PcaLaunchXtb(job, &ts, d_h, m, h_cols, d_yth, h_cols, 1) ||
-          cudaMemcpyAsync(yth_host, d_yth, static_cast<uint64_t>(n) * h_cols * 8, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess) {
-        set_error("pl2gpu_pca_products: Y^T H: %s", cudaGetErrorString(cudaGetLastError()));
-        break;
-      }
+  }
+  if (h_cols) {
+    const char* oom = "pl2gpu_pca_products: insufficient device memory for %u columns of Y^T H";
+    if (d_h.alloc(static_cast<uint64_t>(m) * h_cols, oom, h_cols) || d_yth.alloc(static_cast<uint64_t>(n) * h_cols, oom, h_cols)) return 1;
+    if (cudaMemcpyAsync(d_h, h_host, static_cast<uint64_t>(m) * h_cols * 8, cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
+        cudaMemsetAsync(d_yth, 0, static_cast<uint64_t>(n) * h_cols * 8, c->stream) != cudaSuccess || PcaLaunchXtb(job, &ts, d_h, m, h_cols, d_yth, h_cols, 1) ||
+        cudaMemcpyAsync(yth_host, d_yth, static_cast<uint64_t>(n) * h_cols * 8, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess) {
+      set_error("pl2gpu_pca_products: Y^T H: %s", cudaGetErrorString(cudaGetLastError()));
+      return 1;
     }
-    if (cudaStreamSynchronize(c->stream) != cudaSuccess || cudaGetLastError() != cudaSuccess) {
-      set_error("pl2gpu_pca_products: %s", cudaGetErrorString(cudaGetLastError()));
-      break;
-    }
-    rc = 0;
-  } while (0);
-  PcaTsFree(&ts);
-  cudaFree(d_g);
-  cudaFree(d_yg);
-  cudaFree(d_h);
-  cudaFree(d_yth);
-  return rc;
+  }
+  if (cudaStreamSynchronize(c->stream) != cudaSuccess || cudaGetLastError() != cudaSuccess) {
+    set_error("pl2gpu_pca_products: %s", cudaGetErrorString(cudaGetLastError()));
+    return 1;
+  }
+  return 0;
 }
 
 // `--variant-score` (VscoreReport, 2.0/plink2_matrix_calc.cc:9274): per variant the dot product of sample weights with
@@ -574,60 +519,36 @@ int pl2gpu_pca_vscore(Pl2PcaJob* job, const double* weights_host, uint32_t cols,
   PL2_TRY(PcaFinishLayouts(job, false));
   PcaTs ts;
   PL2_TRY(PcaTsAlloc(job, false, &ts));
-  double *d_w = nullptr, *d_h = nullptr, *d_wtot = nullptr, *d_out = nullptr, *d_slope = nullptr, *d_icpt = nullptr;
-  int rc = 1;
-  do {
-    if (cudaMalloc(&d_w, static_cast<uint64_t>(npad) * cols * 8) != cudaSuccess || cudaMalloc(&d_h, static_cast<uint64_t>(m) * cols * 8) != cudaSuccess ||
-        cudaMalloc(&d_wtot, 8ull * cols) != cudaSuccess || cudaMalloc(&d_out, static_cast<uint64_t>(m) * cols * 8) != cudaSuccess || cudaMalloc(&d_slope, 8ull * m) != cudaSuccess ||
-        cudaMalloc(&d_icpt, 8ull * m) != cudaSuccess) {
-      cudaGetLastError();
-      set_error("pl2gpu_pca_vscore: insufficient device memory for %u score columns", cols);
-      break;
-    }
-    std::vector<double> wtot(cols, 0.0);
-    for (uint32_t s = 0; s < n; ++s)
-      for (uint32_t cc = 0; cc < cols; ++cc) wtot[cc] += weights_host[static_cast<uint64_t>(s) * cols + cc];
-    if (cudaMemsetAsync(d_w, 0, static_cast<uint64_t>(npad) * cols * 8, c->stream) != cudaSuccess || cudaMemcpyAsync(d_w, weights_host, static_cast<uint64_t>(n) * cols * 8, cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
-        cudaMemcpyAsync(d_wtot, wtot.data(), 8ull * cols, cudaMemcpyHostToDevice, c->stream) != cudaSuccess)
-      break;
-    vscore_centre_kernel<<<DivUpU32(m, 256), 256, 0, c->stream>>>(job->d_twof, m, d_slope, d_icpt);
-    c->launches++;
-    if (PcaLaunchXa(job, &ts, d_slope, d_icpt, d_w, cols, d_h, m, cols) || cudaGetLastError() != cudaSuccess) {
-      set_error("pl2gpu_pca_vscore: kernel launch failed");
-      break;
-    }
-    vscore_finish_kernel<<<static_cast<uint32_t>(DivUpU64(static_cast<uint64_t>(m) * cols, 256)), 256, 0, c->stream>>>(d_h, m, m, cols, job->d_twof, d_wtot, d_out);
-    c->launches++;
-    if (cudaMemcpyAsync(out_host, d_out, static_cast<uint64_t>(m) * cols * 8, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
-      set_error("pl2gpu_pca_vscore: %s", cudaGetErrorString(cudaGetLastError()));
-      break;
-    }
-    rc = 0;
-  } while (0);
-  PcaTsFree(&ts);
-  cudaFree(d_w);
-  cudaFree(d_h);
-  cudaFree(d_wtot);
-  cudaFree(d_out);
-  cudaFree(d_slope);
-  cudaFree(d_icpt);
-  return rc;
+  DevArray<double> d_w, d_h, d_wtot, d_out, d_slope, d_icpt;
+  const char* oom = "pl2gpu_pca_vscore: insufficient device memory for %u score columns";
+  if (d_w.alloc(static_cast<uint64_t>(npad) * cols, oom, cols) || d_h.alloc(static_cast<uint64_t>(m) * cols, oom, cols) || d_wtot.alloc(cols, oom, cols) || d_out.alloc(static_cast<uint64_t>(m) * cols, oom, cols) ||
+      d_slope.alloc(m, oom, cols) || d_icpt.alloc(m, oom, cols))
+    return 1;
+  std::vector<double> wtot(cols, 0.0);
+  for (uint32_t s = 0; s < n; ++s)
+    for (uint32_t cc = 0; cc < cols; ++cc) wtot[cc] += weights_host[static_cast<uint64_t>(s) * cols + cc];
+  if (cudaMemsetAsync(d_w, 0, static_cast<uint64_t>(npad) * cols * 8, c->stream) != cudaSuccess || cudaMemcpyAsync(d_w, weights_host, static_cast<uint64_t>(n) * cols * 8, cudaMemcpyHostToDevice, c->stream) != cudaSuccess ||
+      cudaMemcpyAsync(d_wtot, wtot.data(), 8ull * cols, cudaMemcpyHostToDevice, c->stream) != cudaSuccess)
+    return 1;
+  vscore_centre_kernel<<<DivUpU32(m, 256), 256, 0, c->stream>>>(job->d_twof, m, d_slope, d_icpt);
+  c->launches++;
+  if (PcaLaunchXa(job, &ts, d_slope, d_icpt, d_w, cols, d_h, m, cols) || cudaGetLastError() != cudaSuccess) {
+    set_error("pl2gpu_pca_vscore: kernel launch failed");
+    return 1;
+  }
+  vscore_finish_kernel<<<static_cast<uint32_t>(DivUpU64(static_cast<uint64_t>(m) * cols, 256)), 256, 0, c->stream>>>(d_h, m, m, cols, job->d_twof, d_wtot, d_out);
+  c->launches++;
+  if (cudaMemcpyAsync(out_host, d_out, static_cast<uint64_t>(m) * cols * 8, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
+    set_error("pl2gpu_pca_vscore: %s", cudaGetErrorString(cudaGetLastError()));
+    return 1;
+  }
+  return 0;
 }
 
 int pl2gpu_pca_end(Pl2PcaJob* job) {
   if (!job) return 0;
-  if (job->ctx) {
-    cudaSetDevice(job->ctx->c.device);
-    cudaStreamSynchronize(job->ctx->c.stream);
-  }
-  cudaFree(job->d_raw);
-  cudaFree(job->d_raw_i);
-  cudaFree(job->d_slope);
-  cudaFree(job->d_icpt);
-  cudaFree(job->d_twof);
-  cudaFree(job->d_counts);
-  cudaGetLastError();
   delete job;
+  cudaGetLastError();
   return 0;
 }
 

@@ -5,6 +5,7 @@
 #include <algorithm>
 #include <cstdarg>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <vector>
 
@@ -62,10 +63,10 @@ int BuildTileList(uint32_t row_start, uint32_t row_end, bool include_diag, TileL
   off_v.push_back(static_cast<uint32_t>(rt_v.size()));
   tl->row_tile_ct = rt - tl->row_tile_first;
   tl->tile_ct = static_cast<uint32_t>(rt_v.size());
-  const size_t nb = (rt_v.size() + 1) * sizeof(uint32_t);
-  PL2_CUDA_OK(cudaMalloc(&tl->d_tile_rt, nb));
-  PL2_CUDA_OK(cudaMalloc(&tl->d_tile_tc, nb));
-  PL2_CUDA_OK(cudaMalloc(&tl->d_rowtile_offset, off_v.size() * sizeof(uint32_t)));
+  const char* oom = "BuildTileList: insufficient device memory for the tile list of %u tiles: %s";
+  PL2_TRY(tl->d_tile_rt.alloc(rt_v.size() + 1, oom, tl->tile_ct));
+  PL2_TRY(tl->d_tile_tc.alloc(rt_v.size() + 1, oom, tl->tile_ct));
+  PL2_TRY(tl->d_rowtile_offset.alloc(off_v.size(), oom, tl->tile_ct));
   if (!rt_v.empty()) {
     PL2_CUDA_OK(cudaMemcpy(tl->d_tile_rt, rt_v.data(), rt_v.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
     PL2_CUDA_OK(cudaMemcpy(tl->d_tile_tc, tc_v.data(), tc_v.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
@@ -103,18 +104,9 @@ int BuildTileList(uint32_t row_start, uint32_t row_end, bool include_diag, TileL
   }
   tl->pair_tile_ct = row_pairs ? static_cast<uint32_t>(order.size()) : 0;
   order.insert(order.end(), lone.begin(), lone.end());
-  PL2_CUDA_OK(cudaMalloc(&tl->d_tile_order, nb));
+  PL2_TRY(tl->d_tile_order.alloc(rt_v.size() + 1, oom, tl->tile_ct));
   if (!order.empty()) PL2_CUDA_OK(cudaMemcpy(tl->d_tile_order, order.data(), order.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
   return 0;
-}
-
-void FreeTileList(TileList* tl) {
-  cudaFree(tl->d_tile_rt);
-  cudaFree(tl->d_tile_tc);
-  cudaFree(tl->d_rowtile_offset);
-  cudaFree(tl->d_tile_order);
-  tl->d_tile_order = nullptr;
-  tl->d_tile_rt = tl->d_tile_tc = tl->d_rowtile_offset = nullptr;
 }
 
 // ---- NCCL, loaded on first use: the library has no link-time dependency on it, and inside a process that
@@ -185,13 +177,7 @@ int StageAlloc(uint32_t sample_ct, uint32_t variant_cap, GenoStage* gs, uint32_t
   gs->sample_ct_padded = RoundUpU32(sample_ct, sample_pad);
   gs->pitch = gs->sample_ct_padded / 4;
   gs->variant_cap = RoundUpU32(variant_cap, kVariantPad);
-  if (cudaMalloc(&gs->d_raw, static_cast<uint64_t>(gs->variant_cap) * gs->pitch) != cudaSuccess) {
-    cudaGetLastError();
-    gs->d_raw = nullptr;
-    set_error("insufficient device memory for a %u-variant x %u-sample genotype stage", gs->variant_cap, sample_ct);
-    return 1;
-  }
-  return 0;
+  return gs->d_raw.alloc(static_cast<uint64_t>(gs->variant_cap) * gs->pitch, "insufficient device memory for a %u-variant x %u-sample genotype stage", gs->variant_cap, sample_ct);
 }
 
 int LaunchPadGenotypes(Ctx* ctx, uint8_t* dst, uint32_t pitch, uint32_t sample_ct, uint32_t variant_ct, uint32_t variant_ct_padded, cudaStream_t stream) {
@@ -202,11 +188,6 @@ int LaunchPadGenotypes(Ctx* ctx, uint8_t* dst, uint32_t pitch, uint32_t sample_c
   return 0;
 }
 
-void StageFree(GenoStage* gs) {
-  cudaFree(gs->d_raw);
-  gs->d_raw = nullptr;
-}
-
 int StageUpload(Ctx* ctx, GenoStage* gs, const void* src, uint64_t src_stride, uint32_t variant_ct, int src_is_device, uint32_t* padded_ct_ptr, uint32_t dst_row, uint32_t pad_to) {
   const uint32_t padded = RoundUpU32(variant_ct, pad_to);
   if (dst_row + padded > gs->variant_cap) {
@@ -214,7 +195,7 @@ int StageUpload(Ctx* ctx, GenoStage* gs, const void* src, uint64_t src_stride, u
     return 1;
   }
   const uint32_t width = DivUpU32(gs->sample_ct, 4);
-  uint8_t* dst = gs->d_raw + static_cast<uint64_t>(dst_row) * gs->pitch;
+  uint8_t* dst = gs->d_raw.get() + static_cast<uint64_t>(dst_row) * gs->pitch;
   if (variant_ct) {
     PL2_CUDA_OK(cudaMemcpy2DAsync(dst, gs->pitch, src, src_stride, width, variant_ct, src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->stream));
   }
@@ -229,24 +210,14 @@ int StageUpload(Ctx* ctx, GenoStage* gs, const void* src, uint64_t src_stride, u
 
 int StageRing::alloc(Ctx* c, uint32_t sample_ct, uint32_t variant_cap, uint32_t sample_pad) {
   ctx = c;
+  const char* fail = "StageRing: cudaEventCreate failed: %s";
   for (int s = 0; s < 2; ++s) {
     PL2_TRY(StageAlloc(sample_ct, variant_cap, &stage[s], sample_pad));
-    PL2_CUDA_OK(cudaEventCreateWithFlags(&ev_prep_done[s], cudaEventDisableTiming));
-    PL2_CUDA_OK(cudaEventCreate(&ev_free[s]));
+    PL2_TRY(ev_prep_done[s].create(cudaEventDisableTiming, fail));
+    PL2_TRY(ev_free[s].create(cudaEventDefault, fail));
   }
-  PL2_CUDA_OK(cudaEventCreateWithFlags(&ev_src_ready, cudaEventDisableTiming));
-  PL2_CUDA_OK(cudaEventCreateWithFlags(&ev_copied, cudaEventDisableTiming));
-  return 0;
-}
-
-void StageRing::free() {
-  for (int s = 0; s < 2; ++s) {
-    StageFree(&stage[s]);
-    if (ev_prep_done[s]) cudaEventDestroy(ev_prep_done[s]);
-    if (ev_free[s]) cudaEventDestroy(ev_free[s]);
-  }
-  if (ev_src_ready) cudaEventDestroy(ev_src_ready);
-  if (ev_copied) cudaEventDestroy(ev_copied);
+  PL2_TRY(ev_src_ready.create(cudaEventDisableTiming, fail));
+  return ev_copied.create(cudaEventDisableTiming, fail);
 }
 
 int StageRing::acquire(int src_is_device, uint32_t* slot) {
@@ -263,14 +234,14 @@ int StageRing::acquire(int src_is_device, uint32_t* slot) {
 
 int StageRing::land(uint32_t slot, uint8_t* dst, const void* src, uint64_t src_stride, uint32_t rows, int src_is_device) {
   const GenoStage& st = stage[slot];
-  PL2_CUDA_OK(cudaMemcpy2DAsync(dst ? dst : st.d_raw, st.pitch, src, src_stride, DivUpU32(st.sample_ct, 4), rows, src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->copy_stream));
+  PL2_CUDA_OK(cudaMemcpy2DAsync(dst ? dst : st.d_raw.get(), st.pitch, src, src_stride, DivUpU32(st.sample_ct, 4), rows, src_is_device ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, ctx->copy_stream));
   PL2_CUDA_OK(cudaEventRecord(ev_copied, ctx->copy_stream));
   return 0;
 }
 
 int StageRing::land_slice(uint32_t slot, const void* src, uint64_t src_stride, uint32_t slice_rows, int src_is_device) {
   const GenoStage& st = stage[slot];
-  uint8_t* mine = st.d_raw + static_cast<uint64_t>(ctx->comm_rank) * slice_rows * st.pitch;
+  uint8_t* mine = st.d_raw.get() + static_cast<uint64_t>(ctx->comm_rank) * slice_rows * st.pitch;
   PL2_TRY(land(slot, mine, src, src_stride, slice_rows, src_is_device));
   PL2_TRY(LaunchPadGenotypes(ctx, mine, st.pitch, st.sample_ct, slice_rows, slice_rows, ctx->copy_stream));
   return CommAllGatherInPlace(ctx, st.d_raw, static_cast<uint64_t>(slice_rows) * st.pitch, ctx->copy_stream);
@@ -280,7 +251,7 @@ int StageRing::pad(uint32_t slot, uint32_t cur, bool pad_valid_rows, uint32_t pa
   const GenoStage& st = stage[slot];
   *padded = RoundUpU32(cur, pad_to);
   if (pad_valid_rows) return LaunchPadGenotypes(ctx, st.d_raw, st.pitch, st.sample_ct, cur, *padded, ctx->copy_stream);
-  if (*padded > cur) return LaunchPadGenotypes(ctx, st.d_raw + static_cast<uint64_t>(cur) * st.pitch, st.pitch, st.sample_ct, 0, *padded - cur, ctx->copy_stream);
+  if (*padded > cur) return LaunchPadGenotypes(ctx, st.d_raw.get() + static_cast<uint64_t>(cur) * st.pitch, st.pitch, st.sample_ct, 0, *padded - cur, ctx->copy_stream);
   return 0;
 }
 
@@ -306,23 +277,29 @@ int StageRing::release_host_source(int src_is_device) {
 using namespace pl2;
 
 struct Pl2KingJob {
-  Pl2GpuCtx* ctx = nullptr;
+  explicit Pl2KingJob(Pl2GpuCtx* x) : ctx(x) {}
+  ~Pl2KingJob() {  // the kernels and copies that use the buffers finish before they are freed
+    cudaSetDevice(ctx->c.device);
+    cudaStreamSynchronize(ctx->c.stream);
+    cudaStreamSynchronize(ctx->c.copy_stream);
+  }
+  Pl2GpuCtx* ctx;
   uint32_t sample_ct = 0, row_start = 0, row_end = 0;
   uint32_t col_end = 0;              // pairs with a column at or past this are never returned (sample_ct: none cut)
-  uint32_t* d_order = nullptr;       // mapped job: device position -> sample index; null = identity
-  uint8_t* d_unmapped = nullptr;     // mapped job: the block as the caller gave it, before the gather into position order
+  DevArray<uint32_t> d_order;        // mapped job: device position -> sample index; null = identity
+  DevArray<uint8_t> d_unmapped;      // mapped job: the block as the caller gave it, before the gather into position order
   int algo = kPl2KingAlgoTensor;
   TileList tiles;
   StageRing ring;   // TS path: the row re-tiling of each slot also runs on the prep stream
   GenoStage stage;  // the other algorithms: one block on the compute stream
-  uint8_t* d_raw_t[2] = {nullptr, nullptr};  // tensor paths: sample-major copy of the staged block (geno_tile.cuh; split form on the TS path)
-  uint8_t* d_col_planes[2] = {nullptr, nullptr};  // TS path: the column plane images of the staged block (geno_tile.cuh)
-  cudaEvent_t ev_kernel_start[2] = {nullptr, nullptr};  // with the ring's ev_free, the timed pair around the tensor kernel (pl2gpu_king_last_kernel_ms)
+  DevArray<uint8_t> d_raw_t[2];       // tensor paths: sample-major copy of the staged block (geno_tile.cuh; split form on the TS path)
+  DevArray<uint8_t> d_col_planes[2];  // TS path: the column plane images of the staged block (geno_tile.cuh)
+  Event ev_kernel_start[2];           // with the ring's ev_free, the timed pair around the tensor kernel (pl2gpu_king_last_kernel_ms)
   int last_buf = -1;
-  uint32_t* d_planes = nullptr;  // popcount path only
+  DevArray<uint32_t> d_planes;  // popcount path only
   uint32_t tile_cols = kTileCols;
-  int32_t* d_raw_acc = nullptr;
-  void* d_out_stage = nullptr;   // bounded staging for host downloads
+  DevArray<int32_t> d_raw_acc;
+  DevArray<uint8_t> d_out_stage;  // bounded staging for host downloads
   uint64_t out_stage_bytes = 0;
   uint64_t variants_added = 0;
 };
@@ -357,21 +334,19 @@ int pl2gpu_ctx_create(int device_idx, Pl2GpuCtx** ctx_ptr) {
     return 1;
   }
   PL2_CUDA_OK(cudaSetDevice(device_idx));
-  Pl2GpuCtx* ctx = new Pl2GpuCtx();
+  std::unique_ptr<Pl2GpuCtx> ctx(new Pl2GpuCtx());
   ctx->c.device = device_idx;
   ctx->c.sm_count = prop.multiProcessorCount;
-  PL2_CUDA_OK(cudaStreamCreateWithFlags(&ctx->c.stream, cudaStreamNonBlocking));
-  {
-    // the prep stream outranks the compute stream: its short copy / pad / re-tile / all-gather kernels must get
-    // SM slots while a long tensor kernel keeps every SM busy
-    int prio_lo = 0, prio_hi = 0;
-    PL2_CUDA_OK(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
-    PL2_CUDA_OK(cudaStreamCreateWithPriority(&ctx->c.copy_stream, cudaStreamNonBlocking, prio_hi));
-  }
+  // the prep stream outranks the compute stream (default priority 0): its short copy / pad / re-tile / all-gather
+  // kernels must get SM slots while a long tensor kernel keeps every SM busy
+  int prio_lo = 0, prio_hi = 0;
+  PL2_TRY(ctx->c.stream.create(0, "pl2gpu_ctx_create: cudaStreamCreate failed: %s"));
+  PL2_CUDA_OK(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
+  PL2_TRY(ctx->c.copy_stream.create(prio_hi, "pl2gpu_ctx_create: cudaStreamCreate failed: %s"));
   PL2_CUDA_OK(cudaFuncSetAttribute(king_wg_kernel<kTileCols>, cudaFuncAttributeMaxDynamicSharedMemorySize, KingWgShape<kTileCols>::kSmemBytes));
   PL2_CUDA_OK(cudaFuncSetAttribute(king_b1_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, kKb1SmemBytes));
   PL2_CUDA_OK(cudaFuncSetAttribute(king_b1_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, kKb1SmemBytes));
-  *ctx_ptr = ctx;
+  *ctx_ptr = ctx.release();
   return 0;
 }
 
@@ -379,10 +354,6 @@ int pl2gpu_ctx_destroy(Pl2GpuCtx* ctx) {
   if (!ctx) return 0;
   cudaSetDevice(ctx->c.device);
   pl2gpu_comm_destroy(ctx);
-  if (ctx->c.stream) cudaStreamDestroy(ctx->c.stream);
-  if (ctx->c.copy_stream) cudaStreamDestroy(ctx->c.copy_stream);
-  for (auto& e : ctx->c.events)
-    if (e) cudaEventDestroy(e);
   delete ctx;
   return 0;
 }
@@ -427,7 +398,7 @@ int pl2gpu_ctx_event_record(Pl2GpuCtx* ctx, int slot) {
     return 1;
   }
   PL2_CUDA_OK(cudaSetDevice(ctx->c.device));
-  if (!ctx->c.events[slot]) PL2_CUDA_OK(cudaEventCreate(&ctx->c.events[slot]));
+  if (!ctx->c.events[slot]) PL2_TRY(ctx->c.events[slot].create(cudaEventDefault, "pl2gpu_ctx_event_record: cudaEventCreate failed: %s"));
   PL2_CUDA_OK(cudaEventRecord(ctx->c.events[slot], ctx->c.stream));
   return 0;
 }
@@ -560,73 +531,43 @@ static int KingBegin(Pl2GpuCtx* ctx, uint32_t sample_ct, const uint32_t* order, 
     return 1;
   }
   PL2_CUDA_OK(cudaSetDevice(ctx->c.device));
-  Pl2KingJob* job = new Pl2KingJob();
-  job->ctx = ctx;
+  std::unique_ptr<Pl2KingJob, int (*)(Pl2KingJob*)> job(new Pl2KingJob(ctx), pl2gpu_king_end);
   job->sample_ct = sample_ct;
   job->row_start = row_start;
   job->row_end = row_end;
   job->col_end = col_end;
   job->algo = algo;
-  auto fail = [&]() {
-    pl2gpu_king_end(job);
-    return 1;
-  };
   const bool ts = algo == kPl2KingAlgoTensorTS;
   const uint32_t cap = ClampStageCap(max_variants_per_add);
-  if (cudaEventCreate(&job->ev_kernel_start[0]) != cudaSuccess || cudaEventCreate(&job->ev_kernel_start[1]) != cudaSuccess) {
-    set_error("pl2gpu_king_begin: cudaEventCreate failed");
-    return fail();
-  }
+  for (Event& ev : job->ev_kernel_start) PL2_TRY(ev.create(cudaEventDefault, "pl2gpu_king_begin: cudaEventCreate failed"));
   job->tile_cols = ts ? kKingTsCols : kTileCols;
-  if (BuildTileList(row_start, row_end, false, &job->tiles, job->tile_cols, col_end, ts)) return fail();
-  if (order && (cudaMalloc(&job->d_order, 4ull * sample_ct) != cudaSuccess || cudaMemcpy(job->d_order, order, 4ull * sample_ct, cudaMemcpyHostToDevice) != cudaSuccess)) {
-    set_error("pl2gpu_king_begin_mapped: position map upload failed: %s", cudaGetErrorString(cudaGetLastError()));
-    return fail();
+  PL2_TRY(BuildTileList(row_start, row_end, false, &job->tiles, job->tile_cols, col_end, ts));
+  if (order) {
+    const char* fail = "pl2gpu_king_begin_mapped: position map upload failed: %s";
+    PL2_TRY(job->d_order.alloc(sample_ct, fail));
+    if (cudaMemcpy(job->d_order, order, 4ull * sample_ct, cudaMemcpyHostToDevice) != cudaSuccess) {
+      set_error(fail, cudaGetErrorString(cudaGetLastError()));
+      return 1;
+    }
   }
-  if (ts ? job->ring.alloc(&ctx->c, sample_ct, cap, kTsSamplePad) : StageAlloc(sample_ct, cap, &job->stage, kSamplePad)) return fail();
+  PL2_TRY(ts ? job->ring.alloc(&ctx->c, sample_ct, cap, kTsSamplePad) : StageAlloc(sample_ct, cap, &job->stage, kSamplePad));
   const GenoStage& st0 = ts ? job->ring.stage[0] : job->stage;
-  if (order && cudaMalloc(&job->d_unmapped, static_cast<uint64_t>(st0.variant_cap) * st0.pitch) != cudaSuccess) {
-    cudaGetLastError();
-    set_error("pl2gpu_king_begin_mapped: insufficient device memory for the unmapped genotype block");
-    return fail();
-  }
+  if (order) PL2_TRY(job->d_unmapped.alloc(static_cast<uint64_t>(st0.variant_cap) * st0.pitch, "pl2gpu_king_begin_mapped: insufficient device memory for the unmapped genotype block"));
   for (int b = 0; b < (ts ? 2 : 1) && algo != kPl2KingAlgoPopcount; ++b) {
-    if (cudaMalloc(&job->d_raw_t[b], static_cast<uint64_t>(st0.sample_ct_padded) * (st0.variant_cap / 4)) != cudaSuccess) {
-      cudaGetLastError();
-      set_error("pl2gpu_king_begin: insufficient device memory for the sample-major genotype copy");
-      return fail();
-    }
-    if (ts && cudaMalloc(&job->d_col_planes[b], static_cast<uint64_t>(st0.sample_ct_padded) * (st0.variant_cap / 2)) != cudaSuccess) {
-      cudaGetLastError();
-      set_error("pl2gpu_king_begin: insufficient device memory for the column plane copy (%.1f GB per staged block); lower the variants per batch", static_cast<double>(st0.sample_ct_padded) * (st0.variant_cap / 2) / 1e9);
-      return fail();
-    }
+    PL2_TRY(job->d_raw_t[b].alloc(static_cast<uint64_t>(st0.sample_ct_padded) * (st0.variant_cap / 4), "pl2gpu_king_begin: insufficient device memory for the sample-major genotype copy"));
+    const uint64_t plane_bytes = static_cast<uint64_t>(st0.sample_ct_padded) * (st0.variant_cap / 2);
+    if (ts) PL2_TRY(job->d_col_planes[b].alloc(plane_bytes, "pl2gpu_king_begin: insufficient device memory for the column plane copy (%.1f GB per staged block); lower the variants per batch", plane_bytes / 1e9));
   }
-  const uint64_t acc_bytes = static_cast<uint64_t>(job->tiles.tile_ct) * (5ull * job->tile_cols * kTileRows) * sizeof(int32_t);
-  if (cudaMalloc(&job->d_raw_acc, acc_bytes ? acc_bytes : 4) != cudaSuccess) {
-    cudaGetLastError();
-    set_error("pl2gpu_king_begin: insufficient device memory for %u pair tiles (%.1f GB of accumulators); narrow the row range", job->tiles.tile_ct, acc_bytes / 1e9);
-    return fail();
-  }
-  if (cudaMemsetAsync(job->d_raw_acc, 0, acc_bytes, ctx->c.stream) != cudaSuccess) {
+  const uint64_t acc_words = static_cast<uint64_t>(job->tiles.tile_ct) * (5ull * job->tile_cols * kTileRows);
+  PL2_TRY(job->d_raw_acc.alloc(acc_words ? acc_words : 1, "pl2gpu_king_begin: insufficient device memory for %u pair tiles (%.1f GB of accumulators); narrow the row range", job->tiles.tile_ct, acc_words * 4 / 1e9));
+  if (cudaMemsetAsync(job->d_raw_acc, 0, acc_words * 4, ctx->c.stream) != cudaSuccess) {
     set_error("pl2gpu_king_begin: cudaMemsetAsync failed: %s", cudaGetErrorString(cudaGetLastError()));
-    return fail();
+    return 1;
   }
-  if (algo == kPl2KingAlgoPopcount) {
-    const uint64_t plane_bytes = 3ull * (job->stage.variant_cap / 32) * job->stage.sample_ct_padded * sizeof(uint32_t);
-    if (cudaMalloc(&job->d_planes, plane_bytes) != cudaSuccess) {
-      cudaGetLastError();
-      set_error("pl2gpu_king_begin: insufficient device memory for bit planes");
-      return fail();
-    }
-  }
+  if (algo == kPl2KingAlgoPopcount) PL2_TRY(job->d_planes.alloc(3ull * (job->stage.variant_cap / 32) * job->stage.sample_ct_padded, "pl2gpu_king_begin: insufficient device memory for bit planes"));
   job->out_stage_bytes = kKingOutStageBytes;
-  if (cudaMalloc(&job->d_out_stage, job->out_stage_bytes) != cudaSuccess) {
-    cudaGetLastError();
-    set_error("pl2gpu_king_begin: insufficient device memory for output staging");
-    return fail();
-  }
-  *job_ptr = job;
+  PL2_TRY(job->d_out_stage.alloc(job->out_stage_bytes, "pl2gpu_king_begin: insufficient device memory for output staging"));
+  *job_ptr = job.release();
   return 0;
 }
 
@@ -876,56 +817,46 @@ int pl2gpu_king_get_filtered(Pl2KingJob* job, uint32_t r0, uint32_t r1, double m
   Ctx* c = &job->ctx->c;
   PL2_CUDA_OK(cudaSetDevice(c->device));
   if (!job->tiles.tile_ct || r0 == r1) return 0;
-  unsigned long long* d_found = nullptr;
-  uint32_t *d_pairs = nullptr, *d_counts = nullptr;
-  double* d_kin = nullptr;
+  DevArray<unsigned long long> d_found;
+  DevArray<uint32_t> d_pairs, d_counts;
+  DevArray<double> d_kin;
   const uint64_t cap = max_out ? max_out : 1;
-  int rc = 1;
-  do {
-    if (cudaMalloc(&d_found, 8) != cudaSuccess || cudaMalloc(&d_pairs, cap * 8) != cudaSuccess || cudaMalloc(&d_counts, cap * 20) != cudaSuccess || cudaMalloc(&d_kin, cap * 8) != cudaSuccess) {
-      cudaGetLastError();
-      set_error("pl2gpu_king_get_filtered: insufficient device memory for %llu result slots", static_cast<unsigned long long>(max_out));
-      break;
-    }
-    if (cudaMemsetAsync(d_found, 0, 8, c->stream) != cudaSuccess) break;
-    if (job->tile_cols == kKingTsCols) {
-      king_filter_kernel<kKingTsCols><<<job->tiles.tile_ct, kTileRows, 0, c->stream>>>(job->d_raw_acc, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->sample_ct, job->col_end, r0, r1, min_kinship, max_out, d_found, d_pairs, d_counts, d_kin);
-    } else {
-      king_filter_kernel<kTileCols><<<job->tiles.tile_ct, kTileRows, 0, c->stream>>>(job->d_raw_acc, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->sample_ct, job->col_end, r0, r1, min_kinship, max_out, d_found, d_pairs, d_counts, d_kin);
-    }
-    c->launches++;
-    unsigned long long found = 0;
-    if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&found, d_found, 8, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
+  const char* oom = "pl2gpu_king_get_filtered: insufficient device memory for %llu result slots";
+  const unsigned long long max_out_ull = max_out;
+  if (d_found.alloc(1, oom, max_out_ull) || d_pairs.alloc(cap * 2, oom, max_out_ull) || d_counts.alloc(cap * 5, oom, max_out_ull) || d_kin.alloc(cap, oom, max_out_ull)) return 1;
+  if (cudaMemsetAsync(d_found, 0, 8, c->stream) != cudaSuccess) return 1;
+  if (job->tile_cols == kKingTsCols) {
+    king_filter_kernel<kKingTsCols><<<job->tiles.tile_ct, kTileRows, 0, c->stream>>>(job->d_raw_acc, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->sample_ct, job->col_end, r0, r1, min_kinship, max_out, d_found, d_pairs, d_counts, d_kin);
+  } else {
+    king_filter_kernel<kTileCols><<<job->tiles.tile_ct, kTileRows, 0, c->stream>>>(job->d_raw_acc, job->tiles.d_tile_rt, job->tiles.d_tile_tc, job->sample_ct, job->col_end, r0, r1, min_kinship, max_out, d_found, d_pairs, d_counts, d_kin);
+  }
+  c->launches++;
+  unsigned long long found = 0;
+  if (cudaGetLastError() != cudaSuccess || cudaMemcpyAsync(&found, d_found, 8, cudaMemcpyDeviceToHost, c->stream) != cudaSuccess || cudaStreamSynchronize(c->stream) != cudaSuccess) {
+    set_error("pl2gpu_king_get_filtered: %s", cudaGetErrorString(cudaGetLastError()));
+    return 1;
+  }
+  *n_found = found;
+  const uint64_t k = found < max_out ? found : max_out;
+  if (k) {
+    std::vector<uint32_t> hp(2 * k), hc(5 * k);
+    std::vector<double> hk(k);
+    if (cudaMemcpy(hp.data(), d_pairs, k * 8, cudaMemcpyDeviceToHost) != cudaSuccess || cudaMemcpy(hc.data(), d_counts, k * 20, cudaMemcpyDeviceToHost) != cudaSuccess || cudaMemcpy(hk.data(), d_kin, k * 8, cudaMemcpyDeviceToHost) != cudaSuccess) {
       set_error("pl2gpu_king_get_filtered: %s", cudaGetErrorString(cudaGetLastError()));
-      break;
+      return 1;
     }
-    *n_found = found;
-    const uint64_t k = found < max_out ? found : max_out;
-    if (k) {
-      std::vector<uint32_t> hp(2 * k), hc(5 * k);
-      std::vector<double> hk(k);
-      if (cudaMemcpy(hp.data(), d_pairs, k * 8, cudaMemcpyDeviceToHost) != cudaSuccess || cudaMemcpy(hc.data(), d_counts, k * 20, cudaMemcpyDeviceToHost) != cudaSuccess || cudaMemcpy(hk.data(), d_kin, k * 8, cudaMemcpyDeviceToHost) != cudaSuccess) {
-        set_error("pl2gpu_king_get_filtered: %s", cudaGetErrorString(cudaGetLastError()));
-        break;
-      }
-      std::vector<uint64_t> order(k);
-      for (uint64_t q = 0; q < k; ++q) order[q] = q;
-      std::sort(order.begin(), order.end(), [&](uint64_t a, uint64_t b) { return hp[2 * a] != hp[2 * b] ? hp[2 * a] < hp[2 * b] : hp[2 * a + 1] < hp[2 * b + 1]; });
-      for (uint64_t q = 0; q < k; ++q) {
-        const uint64_t src = order[q];
-        pairs_out[2 * q] = hp[2 * src];
-        pairs_out[2 * q + 1] = hp[2 * src + 1];
-        memcpy(counts_out + 5 * q, &hc[5 * src], 20);
-        kinship_out[q] = hk[src];
-      }
+    std::vector<uint64_t> order(k);
+    for (uint64_t q = 0; q < k; ++q) order[q] = q;
+    std::sort(order.begin(), order.end(), [&](uint64_t a, uint64_t b) { return hp[2 * a] != hp[2 * b] ? hp[2 * a] < hp[2 * b] : hp[2 * a + 1] < hp[2 * b + 1]; });
+    for (uint64_t q = 0; q < k; ++q) {
+      const uint64_t src = order[q];
+      pairs_out[2 * q] = hp[2 * src];
+      pairs_out[2 * q + 1] = hp[2 * src + 1];
+      memcpy(counts_out + 5 * q, &hc[5 * src], 20);
+      kinship_out[q] = hk[src];
     }
-    rc = 0;
-  } while (0);
-  cudaFree(d_found);
-  cudaFree(d_pairs);
-  cudaFree(d_counts);
-  cudaFree(d_kin);
-  return rc;
+  }
+  return 0;
 }
 
 uint64_t pl2gpu_king_variants_added(Pl2KingJob* job) { return job ? job->variants_added : 0; }
@@ -954,39 +885,26 @@ int pl2gpu_king_last_planes(Pl2KingJob* job, void* dst, uint64_t bytes) {
 
 int pl2gpu_king_end(Pl2KingJob* job) {
   if (!job) return 0;
-  if (job->ctx) {
-    cudaSetDevice(job->ctx->c.device);
-    cudaStreamSynchronize(job->ctx->c.stream);
-    if (job->ctx->c.copy_stream) cudaStreamSynchronize(job->ctx->c.copy_stream);
-  }
-  FreeTileList(&job->tiles);
-  job->ring.free();
-  StageFree(&job->stage);
-  for (int b = 0; b < 2; ++b) {
-    if (job->ev_kernel_start[b]) cudaEventDestroy(job->ev_kernel_start[b]);
-    cudaFree(job->d_raw_t[b]);
-    cudaFree(job->d_col_planes[b]);
-  }
-  cudaFree(job->d_order);
-  cudaFree(job->d_unmapped);
-  cudaFree(job->d_planes);
-  cudaFree(job->d_raw_acc);
-  cudaFree(job->d_out_stage);
-  cudaGetLastError();
   delete job;
+  cudaGetLastError();
   return 0;
 }
 
 // ------------------------------------------------------------------------------------------ pair list
 
 struct Pl2KingPairJob {
-  Pl2GpuCtx* ctx = nullptr;
+  explicit Pl2KingPairJob(Pl2GpuCtx* x) : ctx(x) {}
+  ~Pl2KingPairJob() {
+    cudaSetDevice(ctx->c.device);
+    cudaStreamSynchronize(ctx->c.stream);
+  }
+  Pl2GpuCtx* ctx;
   uint32_t sample_ct = 0;
   uint64_t pair_ct = 0;
   GenoStage stage;
-  uint8_t* d_raw_t = nullptr;   // sample-major 2-bit copy of the staged block
-  uint32_t* d_pairs = nullptr;  // [pair][2]
-  uint32_t* d_counts = nullptr; // [pair][5]
+  DevArray<uint8_t> d_raw_t;    // sample-major 2-bit copy of the staged block
+  DevArray<uint32_t> d_pairs;   // [pair][2]
+  DevArray<uint32_t> d_counts;  // [pair][5]
 };
 
 int pl2gpu_king_pairs_begin(Pl2GpuCtx* ctx, uint32_t sample_ct, const uint32_t* pairs_host, uint64_t pair_ct, Pl2KingPairJob** job_ptr) {
@@ -1002,28 +920,22 @@ int pl2gpu_king_pairs_begin(Pl2GpuCtx* ctx, uint32_t sample_ct, const uint32_t* 
     }
   }
   PL2_CUDA_OK(cudaSetDevice(ctx->c.device));
-  Pl2KingPairJob* job = new Pl2KingPairJob();
-  job->ctx = ctx;
+  std::unique_ptr<Pl2KingPairJob, int (*)(Pl2KingPairJob*)> job(new Pl2KingPairJob(ctx), pl2gpu_king_pairs_end);
   job->sample_ct = sample_ct;
   job->pair_ct = pair_ct;
-  auto fail = [&]() {
-    pl2gpu_king_pairs_end(job);
-    return 1;
-  };
-  if (StageAlloc(sample_ct, kMaxStageVariants, &job->stage, 64)) return fail();
+  PL2_TRY(StageAlloc(sample_ct, kMaxStageVariants, &job->stage, 64));
   const uint64_t n_alloc = pair_ct ? pair_ct : 1;
-  if (cudaMalloc(&job->d_raw_t, static_cast<uint64_t>(job->stage.sample_ct_padded) * (job->stage.variant_cap / 4)) != cudaSuccess || cudaMalloc(&job->d_pairs, n_alloc * 8) != cudaSuccess ||
-      cudaMalloc(&job->d_counts, n_alloc * 20) != cudaSuccess) {
-    cudaGetLastError();
-    set_error("pl2gpu_king_pairs_begin: insufficient device memory for %llu pairs", static_cast<unsigned long long>(pair_ct));
-    return fail();
-  }
+  const char* oom = "pl2gpu_king_pairs_begin: insufficient device memory for %llu pairs";
+  const unsigned long long pair_ct_ull = pair_ct;
+  if (job->d_raw_t.alloc(static_cast<uint64_t>(job->stage.sample_ct_padded) * (job->stage.variant_cap / 4), oom, pair_ct_ull) || job->d_pairs.alloc(n_alloc * 2, oom, pair_ct_ull) ||
+      job->d_counts.alloc(n_alloc * 5, oom, pair_ct_ull))
+    return 1;
   if (cudaMemcpyAsync(job->d_pairs, pairs_host, pair_ct * 8, cudaMemcpyHostToDevice, ctx->c.stream) != cudaSuccess || cudaMemsetAsync(job->d_counts, 0, n_alloc * 20, ctx->c.stream) != cudaSuccess ||
       cudaStreamSynchronize(ctx->c.stream) != cudaSuccess) {
     set_error("pl2gpu_king_pairs_begin: %s", cudaGetErrorString(cudaGetLastError()));
-    return fail();
+    return 1;
   }
-  *job_ptr = job;
+  *job_ptr = job.release();
   return 0;
 }
 
@@ -1075,16 +987,8 @@ int pl2gpu_king_pairs_get_counts(Pl2KingPairJob* job, uint64_t pair_start, uint6
 
 int pl2gpu_king_pairs_end(Pl2KingPairJob* job) {
   if (!job) return 0;
-  if (job->ctx) {
-    cudaSetDevice(job->ctx->c.device);
-    cudaStreamSynchronize(job->ctx->c.stream);
-  }
-  StageFree(&job->stage);
-  cudaFree(job->d_raw_t);
-  cudaFree(job->d_pairs);
-  cudaFree(job->d_counts);
-  cudaGetLastError();
   delete job;
+  cudaGetLastError();
   return 0;
 }
 
@@ -1097,11 +1001,11 @@ int pl2gpu_int8_peak(Pl2GpuCtx* ctx, uint32_t n_cols, int form, double min_secon
   }
   Ctx* c = &ctx->c;
   PL2_CUDA_OK(cudaSetDevice(c->device));
-  int32_t* d_sink = nullptr;
-  PL2_CUDA_OK(cudaMalloc(&d_sink, 256 * sizeof(int32_t)));
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  PL2_CUDA_OK(cudaEventCreate(&e0));
-  PL2_CUDA_OK(cudaEventCreate(&e1));
+  DevArray<int32_t> d_sink;
+  Event e0, e1;
+  PL2_TRY(d_sink.alloc(256, "pl2gpu_int8_peak: cudaMalloc failed: %s"));
+  PL2_TRY(e0.create(cudaEventDefault, "pl2gpu_int8_peak: cudaEventCreate failed: %s"));
+  PL2_TRY(e1.create(cudaEventDefault, "pl2gpu_int8_peak: cudaEventCreate failed: %s"));
   const uint32_t blocks = 4096;  // x 32 wgmmas x 2 warpgroups per SM
   const double k_per_wgmma = form == 2 ? 256 : 32;
   const double ops_per_launch = 2.0 * 64 * n_cols * k_per_wgmma * 32.0 * 2 * blocks * c->sm_count;
@@ -1131,9 +1035,6 @@ int pl2gpu_int8_peak(Pl2GpuCtx* ctx, uint32_t n_cols, int form, double min_secon
     total_ops += ops_per_launch * per_batch;
     if (min_seconds <= 0) break;
   }
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
-  cudaFree(d_sink);
   *tops_out = total_ops / total_s / 1e12;
   if (seconds_out) *seconds_out = total_s;
   return 0;
@@ -1153,22 +1054,19 @@ int pl2gpu_bulk_read_rate(Pl2GpuCtx* ctx, uint64_t working_set_bytes, uint32_t i
   // about 64 MB per SM and launch
   const uint32_t rounds = std::max<uint32_t>(2, (64u << 20) / inflight_bytes);
   const double bytes_per_launch = static_cast<double>(kFeedChunk) * chunks * rounds * c->sm_count;
-  uint8_t* d_src = nullptr;
-  PL2_CUDA_OK(cudaMalloc(&d_src, static_cast<uint64_t>(ws_chunks) * kFeedChunk));
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  auto release = [&]() {
-    cudaFree(d_src);
-    if (e0) cudaEventDestroy(e0);
-    if (e1) cudaEventDestroy(e1);
-  };
-  auto fail = [&]() {
-    release();
+  DevArray<uint8_t> d_src;
+  Event e0, e1;
+  const char* setup_failed = "pl2gpu_bulk_read_rate: set-up failed: %s";
+  PL2_TRY(d_src.alloc(static_cast<uint64_t>(ws_chunks) * kFeedChunk, "pl2gpu_bulk_read_rate: cudaMalloc failed: %s"));
+  if (cudaMemsetAsync(d_src, 0x5A, static_cast<uint64_t>(ws_chunks) * kFeedChunk, c->stream) != cudaSuccess) {
+    set_error(setup_failed, cudaGetErrorString(cudaGetLastError()));
     return 1;
-  };
-  if (cudaMemsetAsync(d_src, 0x5A, static_cast<uint64_t>(ws_chunks) * kFeedChunk, c->stream) != cudaSuccess || cudaEventCreate(&e0) != cudaSuccess || cudaEventCreate(&e1) != cudaSuccess ||
-      cudaFuncSetAttribute(bulk_read_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
-    set_error("pl2gpu_bulk_read_rate: set-up failed: %s", cudaGetErrorString(cudaGetLastError()));
-    return fail();
+  }
+  PL2_TRY(e0.create(cudaEventDefault, setup_failed));
+  PL2_TRY(e1.create(cudaEventDefault, setup_failed));
+  if (cudaFuncSetAttribute(bulk_read_probe_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) != cudaSuccess) {
+    set_error(setup_failed, cudaGetErrorString(cudaGetLastError()));
+    return 1;
   }
   auto launch = [&]() {
     bulk_read_probe_kernel<<<c->sm_count, 32, smem, c->stream>>>(d_src, ws_chunks, chunks, rounds);
@@ -1178,18 +1076,17 @@ int pl2gpu_bulk_read_rate(Pl2GpuCtx* ctx, uint64_t working_set_bytes, uint32_t i
   double total_s = 0, total_bytes = 0;
   const uint32_t per_batch = 4;
   while (true) {
-    if (cudaEventRecord(e0, c->stream) != cudaSuccess) return fail();
+    if (cudaEventRecord(e0, c->stream) != cudaSuccess) return 1;
     for (uint32_t k = 0; k < per_batch; ++k) launch();
     float ms = 0;
     if (cudaEventRecord(e1, c->stream) != cudaSuccess || cudaEventSynchronize(e1) != cudaSuccess || cudaGetLastError() != cudaSuccess || cudaEventElapsedTime(&ms, e0, e1) != cudaSuccess) {
       set_error("pl2gpu_bulk_read_rate: probe run failed: %s", cudaGetErrorString(cudaGetLastError()));
-      return fail();
+      return 1;
     }
     total_s += ms * 1e-3;
     total_bytes += bytes_per_launch * per_batch;
     if (total_s >= min_seconds) break;
   }
-  release();
   *tbps_out = total_bytes / total_s / 1e12;
   if (seconds_out) *seconds_out = total_s;
   return 0;
@@ -1215,22 +1112,22 @@ int pl2gpu_selftest_umma(Pl2GpuCtx* ctx, int verbose) {
   };
   for (auto& v : a) v = rnd();
   for (auto& v : b) v = rnd();
-  int8_t *d_a = nullptr, *d_b = nullptr;
-  int32_t* d_d = nullptr;
+  const char* oom = "pl2gpu_selftest_umma: cudaMalloc failed: %s";
   std::vector<int32_t> d(M * N);
-  PL2_CUDA_OK(cudaMalloc(&d_a, M * K));
-  PL2_CUDA_OK(cudaMalloc(&d_b, N * K));
-  PL2_CUDA_OK(cudaMalloc(&d_d, 4ull * M * N));
-  PL2_CUDA_OK(cudaMemcpyAsync(d_a, a.data(), M * K, cudaMemcpyHostToDevice, c->stream));
-  PL2_CUDA_OK(cudaMemcpyAsync(d_b, b.data(), N * K, cudaMemcpyHostToDevice, c->stream));
-  wgmma_probe_kernel<<<1, 128, 0, c->stream>>>(d_a, d_b, d_d);
-  c->launches++;
-  PL2_CUDA_OK(cudaGetLastError());
-  PL2_CUDA_OK(cudaMemcpyAsync(d.data(), d_d, 4ull * M * N, cudaMemcpyDeviceToHost, c->stream));
-  PL2_CUDA_OK(cudaStreamSynchronize(c->stream));
-  cudaFree(d_a);
-  cudaFree(d_b);
-  cudaFree(d_d);
+  {
+    DevArray<int8_t> d_a, d_b;
+    DevArray<int32_t> d_d;
+    PL2_TRY(d_a.alloc(M * K, oom));
+    PL2_TRY(d_b.alloc(N * K, oom));
+    PL2_TRY(d_d.alloc(M * N, oom));
+    PL2_CUDA_OK(cudaMemcpyAsync(d_a, a.data(), M * K, cudaMemcpyHostToDevice, c->stream));
+    PL2_CUDA_OK(cudaMemcpyAsync(d_b, b.data(), N * K, cudaMemcpyHostToDevice, c->stream));
+    wgmma_probe_kernel<<<1, 128, 0, c->stream>>>(d_a, d_b, d_d);
+    c->launches++;
+    PL2_CUDA_OK(cudaGetLastError());
+    PL2_CUDA_OK(cudaMemcpyAsync(d.data(), d_d, 4ull * M * N, cudaMemcpyDeviceToHost, c->stream));
+    PL2_CUDA_OK(cudaStreamSynchronize(c->stream));
+  }
   uint32_t bad = 0;
   for (uint32_t m = 0; m < M; ++m)
     for (uint32_t n = 0; n < N; ++n) {
@@ -1251,20 +1148,20 @@ int pl2gpu_selftest_umma(Pl2GpuCtx* ctx, int verbose) {
   for (auto& v : ab) v = (seed = seed * 1664525u + 1013904223u);
   for (auto& v : bb) v = (seed = seed * 1664525u + 1013904223u) ^ (seed >> 13);
   std::vector<int32_t> db(M * kB1N);
-  uint32_t *d_ab = nullptr, *d_bb = nullptr;
-  PL2_CUDA_OK(cudaMalloc(&d_ab, 4ull * ab.size()));
-  PL2_CUDA_OK(cudaMalloc(&d_bb, 4ull * bb.size()));
-  PL2_CUDA_OK(cudaMalloc(&d_d, 4ull * db.size()));
-  PL2_CUDA_OK(cudaMemcpyAsync(d_ab, ab.data(), 4ull * ab.size(), cudaMemcpyHostToDevice, c->stream));
-  PL2_CUDA_OK(cudaMemcpyAsync(d_bb, bb.data(), 4ull * bb.size(), cudaMemcpyHostToDevice, c->stream));
-  wgmma_b1_probe_kernel<<<1, 128, 0, c->stream>>>(d_ab, d_bb, d_d);
-  c->launches++;
-  PL2_CUDA_OK(cudaGetLastError());
-  PL2_CUDA_OK(cudaMemcpyAsync(db.data(), d_d, 4ull * db.size(), cudaMemcpyDeviceToHost, c->stream));
-  PL2_CUDA_OK(cudaStreamSynchronize(c->stream));
-  cudaFree(d_ab);
-  cudaFree(d_bb);
-  cudaFree(d_d);
+  {
+    DevArray<uint32_t> d_ab, d_bb;
+    DevArray<int32_t> d_d;
+    PL2_TRY(d_ab.alloc(ab.size(), oom));
+    PL2_TRY(d_bb.alloc(bb.size(), oom));
+    PL2_TRY(d_d.alloc(db.size(), oom));
+    PL2_CUDA_OK(cudaMemcpyAsync(d_ab, ab.data(), 4ull * ab.size(), cudaMemcpyHostToDevice, c->stream));
+    PL2_CUDA_OK(cudaMemcpyAsync(d_bb, bb.data(), 4ull * bb.size(), cudaMemcpyHostToDevice, c->stream));
+    wgmma_b1_probe_kernel<<<1, 128, 0, c->stream>>>(d_ab, d_bb, d_d);
+    c->launches++;
+    PL2_CUDA_OK(cudaGetLastError());
+    PL2_CUDA_OK(cudaMemcpyAsync(db.data(), d_d, 4ull * db.size(), cudaMemcpyDeviceToHost, c->stream));
+    PL2_CUDA_OK(cudaStreamSynchronize(c->stream));
+  }
   for (uint32_t m = 0; m < M; ++m)
     for (uint32_t n = 0; n < kB1N; ++n) {
       int32_t ref = 0;

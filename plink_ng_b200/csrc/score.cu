@@ -15,6 +15,8 @@
 // variants and writes per-chunk partial sums; a second kernel adds the partials in chunk order, so results do not
 // depend on scheduling.  The fp64 adds go through a two-variant lookup table, the integer sums are bit-parallel.
 #include <algorithm>
+#include <memory>
+#include <utility>
 #include <vector>
 
 #include "../../include/plink2_b200.h"
@@ -427,47 +429,33 @@ void LaunchPloidyGroup(uint32_t nc, const ScoreLaunch& a, const PloidyLaunch& p,
 }  // namespace
 
 struct Pl2ScoreJob {
-  Pl2GpuCtx* ctx = nullptr;
+  explicit Pl2ScoreJob(Pl2GpuCtx* x) : ctx(x) {}
+  ~Pl2ScoreJob() {  // the kernels and copies that use the buffers finish before they are freed
+    cudaSetDevice(ctx->c.device);
+    cudaStreamSynchronize(ctx->c.stream);
+  }
+  Pl2GpuCtx* ctx;
   uint32_t sample_ct = 0, score_ct = 1;
   uint32_t stage_variants = kScoreStageVariants;  // entries per staged batch
   GenoStage stage;
-  double *d_w4 = nullptr, *d_part_sum = nullptr, *d_acc_sum = nullptr;
-  uint8_t* d_d4 = nullptr;
-  uint32_t *d_part_dos = nullptr, *d_part_miss = nullptr, *d_acc_miss = nullptr;
-  unsigned long long* d_acc_dos = nullptr;
+  DevArray<double> d_w4, d_part_sum, d_acc_sum;
+  DevArray<uint8_t> d_d4;
+  DevArray<uint32_t> d_part_dos, d_part_miss, d_acc_miss;
+  DevArray<unsigned long long> d_acc_dos;
   uint64_t entries = 0;
   // entries of the haploid / sex-dependent classes (pl2gpu_score_add_variants_ploidy), allocated on first use
-  uint32_t *d_male2 = nullptr, *d_female2 = nullptr;  // [word] 2-bit-field sex masks (pl2gpu_score_set_sex)
-  double* d_w4h = nullptr;
-  uint32_t *d_part_miss_hap = nullptr, *d_acc_miss_hap = nullptr;
-  unsigned long long* d_acc_hdos = nullptr;
+  DevArray<uint32_t> d_male2, d_female2;  // [word] 2-bit-field sex masks (pl2gpu_score_set_sex)
+  DevArray<double> d_w4h;
+  DevArray<uint32_t> d_part_miss_hap, d_acc_miss_hap;
+  DevArray<unsigned long long> d_acc_hdos;
 };
 
 extern "C" {
 
 int pl2gpu_score_end(Pl2ScoreJob* job) {
   if (!job) return 0;
-  if (job->ctx) {
-    cudaSetDevice(job->ctx->c.device);
-    cudaStreamSynchronize(job->ctx->c.stream);
-  }
-  StageFree(&job->stage);
-  cudaFree(job->d_w4);
-  cudaFree(job->d_d4);
-  cudaFree(job->d_part_sum);
-  cudaFree(job->d_part_dos);
-  cudaFree(job->d_part_miss);
-  cudaFree(job->d_acc_sum);
-  cudaFree(job->d_acc_dos);
-  cudaFree(job->d_acc_miss);
-  cudaFree(job->d_male2);
-  cudaFree(job->d_female2);
-  cudaFree(job->d_w4h);
-  cudaFree(job->d_part_miss_hap);
-  cudaFree(job->d_acc_miss_hap);
-  cudaFree(job->d_acc_hdos);
-  cudaGetLastError();
   delete job;
+  cudaGetLastError();
   return 0;
 }
 
@@ -478,41 +466,30 @@ int pl2gpu_score_begin_cols(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t score_c
     return 1;
   }
   PL2_CUDA_OK(cudaSetDevice(ctx->c.device));
-  Pl2ScoreJob* job = new Pl2ScoreJob();
-  job->ctx = ctx;
+  std::unique_ptr<Pl2ScoreJob, int (*)(Pl2ScoreJob*)> job(new Pl2ScoreJob(ctx), pl2gpu_score_end);
   job->sample_ct = sample_ct;
   job->score_ct = score_ct;
-  auto fail = [&]() {
-    pl2gpu_score_end(job);
-    return 1;
-  };
-  if (StageAlloc(sample_ct, kScoreStageVariants, &job->stage, 64)) return fail();
+  PL2_TRY(StageAlloc(sample_ct, kScoreStageVariants, &job->stage, 64));
   const uint64_t np = job->stage.sample_ct_padded;
   const uint64_t group = std::min(score_ct, kScoreGroup);
-  if (cudaMalloc(&job->d_d4, kScoreStageVariants) != cudaSuccess || cudaMalloc(&job->d_part_sum, 8 * np * kScoreMaxChunks * group) != cudaSuccess || cudaMalloc(&job->d_part_dos, 4 * np * kScoreMaxChunks) != cudaSuccess ||
-      cudaMalloc(&job->d_part_miss, 4 * np * kScoreMaxChunks) != cudaSuccess || cudaMalloc(&job->d_acc_sum, 8 * np * score_ct) != cudaSuccess || cudaMalloc(&job->d_acc_dos, 8 * np) != cudaSuccess ||
-      cudaMalloc(&job->d_acc_miss, 4 * np) != cudaSuccess) {
-    cudaGetLastError();
-    set_error("pl2gpu_score_begin_cols: insufficient device memory for %u samples x %u score columns", sample_ct, score_ct);
-    return fail();
-  }
+  const char* oom = "pl2gpu_score_begin_cols: insufficient device memory for %u samples x %u score columns";
+  if (job->d_d4.alloc(kScoreStageVariants, oom, sample_ct, score_ct) || job->d_part_sum.alloc(np * kScoreMaxChunks * group, oom, sample_ct, score_ct) || job->d_part_dos.alloc(np * kScoreMaxChunks, oom, sample_ct, score_ct) ||
+      job->d_part_miss.alloc(np * kScoreMaxChunks, oom, sample_ct, score_ct) || job->d_acc_sum.alloc(np * score_ct, oom, sample_ct, score_ct) || job->d_acc_dos.alloc(np, oom, sample_ct, score_ct) ||
+      job->d_acc_miss.alloc(np, oom, sample_ct, score_ct))
+    return 1;
   // the staged weights ([entry][score_ct][4]) are the one buffer that grows with the column count and the batch: when
   // they do not fit, batches get fewer entries (then the chunk plan, and so the last bits of a sum, can differ from a
   // job with fewer columns)
-  while (cudaMalloc(&job->d_w4, 32ull * score_ct * job->stage_variants) != cudaSuccess) {
-    cudaGetLastError();
-    if (job->stage_variants <= kScoreTile) {
-      set_error("pl2gpu_score_begin_cols: insufficient device memory for the weights of %u score columns", score_ct);
-      return fail();
-    }
+  while (job->d_w4.alloc(4ull * score_ct * job->stage_variants, "pl2gpu_score_begin_cols: insufficient device memory for the weights of %u score columns", score_ct)) {
+    if (job->stage_variants <= kScoreTile) return 1;
     job->stage_variants /= 2;
   }
   if (cudaMemsetAsync(job->d_acc_sum, 0, 8 * np * score_ct, ctx->c.stream) != cudaSuccess || cudaMemsetAsync(job->d_acc_dos, 0, 8 * np, ctx->c.stream) != cudaSuccess ||
       cudaMemsetAsync(job->d_acc_miss, 0, 4 * np, ctx->c.stream) != cudaSuccess) {
     set_error("pl2gpu_score_begin_cols: %s", cudaGetErrorString(cudaGetLastError()));
-    return fail();
+    return 1;
   }
-  *job_ptr = job;
+  *job_ptr = job.release();
   return 0;
 }
 
@@ -577,20 +554,24 @@ bool ValidNamedDosages(const uint8_t* named_dosages, uint32_t variant_ct, const 
   return true;
 }
 
-// the buffers only entries of the haploid / sex-dependent classes use
+// the buffers only entries of the haploid / sex-dependent classes use: all of them or none
 int ScoreAllocPloidy(Pl2ScoreJob* job) {
-  if (job->d_acc_hdos) return 0;  // allocated last; whatever a failed attempt left is freed by pl2gpu_score_end
+  if (job->d_acc_hdos) return 0;
   Ctx* c = &job->ctx->c;
   const uint64_t np = job->stage.sample_ct_padded;
-  if ((!job->d_w4h && cudaMalloc(&job->d_w4h, 32ull * job->score_ct * job->stage_variants) != cudaSuccess) || (!job->d_part_miss_hap && cudaMalloc(&job->d_part_miss_hap, 4 * np * kScoreMaxChunks) != cudaSuccess) ||
-      (!job->d_acc_miss_hap && cudaMalloc(&job->d_acc_miss_hap, 4 * np) != cudaSuccess) || cudaMalloc(&job->d_acc_hdos, 8 * np) != cudaSuccess) {
-    cudaGetLastError();
-    job->d_acc_hdos = nullptr;
-    set_error("pl2gpu_score_add_variants_ploidy: insufficient device memory for the haploid tables of %u samples x %u score columns", job->sample_ct, job->score_ct);
+  const char* oom = "pl2gpu_score_add_variants_ploidy: insufficient device memory for the haploid tables of %u samples x %u score columns";
+  DevArray<double> w4h;
+  DevArray<uint32_t> part_miss_hap, acc_miss_hap;
+  DevArray<unsigned long long> acc_hdos;
+  if (w4h.alloc(4ull * job->score_ct * job->stage_variants, oom, job->sample_ct, job->score_ct) || part_miss_hap.alloc(np * kScoreMaxChunks, oom, job->sample_ct, job->score_ct) ||
+      acc_miss_hap.alloc(np, oom, job->sample_ct, job->score_ct) || acc_hdos.alloc(np, oom, job->sample_ct, job->score_ct))
     return 1;
-  }
-  PL2_CUDA_OK(cudaMemsetAsync(job->d_acc_miss_hap, 0, 4 * np, c->stream));
-  PL2_CUDA_OK(cudaMemsetAsync(job->d_acc_hdos, 0, 8 * np, c->stream));
+  PL2_CUDA_OK(cudaMemsetAsync(acc_miss_hap, 0, 4 * np, c->stream));
+  PL2_CUDA_OK(cudaMemsetAsync(acc_hdos, 0, 8 * np, c->stream));
+  job->d_w4h = std::move(w4h);
+  job->d_part_miss_hap = std::move(part_miss_hap);
+  job->d_acc_miss_hap = std::move(acc_miss_hap);
+  job->d_acc_hdos = std::move(acc_hdos);
   return 0;
 }
 
@@ -625,12 +606,11 @@ int pl2gpu_score_set_sex(Pl2ScoreJob* job, const uint8_t* sample_sex) {
   }
   Ctx* c = &job->ctx->c;
   PL2_CUDA_OK(cudaSetDevice(c->device));
-  if (!job->d_male2) {
-    if (cudaMalloc(&job->d_male2, 4ull * words) != cudaSuccess || cudaMalloc(&job->d_female2, 4ull * words) != cudaSuccess) {
-      cudaGetLastError();
-      set_error("pl2gpu_score_set_sex: insufficient device memory");
-      return 1;
-    }
+  if (!job->d_male2) {  // both masks or neither
+    DevArray<uint32_t> d_male2, d_female2;
+    if (d_male2.alloc(words, "pl2gpu_score_set_sex: insufficient device memory") || d_female2.alloc(words, "pl2gpu_score_set_sex: insufficient device memory")) return 1;
+    job->d_male2 = std::move(d_male2);
+    job->d_female2 = std::move(d_female2);
   }
   PL2_CUDA_OK(cudaMemcpyAsync(job->d_male2, male2.data(), 4ull * words, cudaMemcpyHostToDevice, c->stream));
   PL2_CUDA_OK(cudaMemcpyAsync(job->d_female2, female2.data(), 4ull * words, cudaMemcpyHostToDevice, c->stream));
