@@ -313,6 +313,21 @@ int pl2gpu_score_set_sex(Pl2ScoreJob* job, const uint8_t* sample_sex);
 int pl2gpu_score_add_variants_ploidy(Pl2ScoreJob* job, const void* genovecs, uint64_t variant_stride_bytes, uint32_t variant_ct, int src_is_device, const uint8_t* ploidy_classes, const double* weights4_diploid,
                                      const double* weights4_haploid, const uint8_t* named_dosages);
 int pl2gpu_score_get_ploidy(Pl2ScoreJob* job, double* score_sums, uint64_t* named_half_dosage_sums, uint32_t* missing_diploid_cts, uint32_t* missing_haploid_cts);
+/* Classes (--q-score-range: the entries whose p-values lie in the same set of ranges).  A job begun with
+ * pl2gpu_score_begin_classes keeps class_ct separate accumulator sets (score sums, named-allele dosage sums, diploid
+ * and haploid missing counts: class_ct x (8 score_ct + 24) bytes per sample, padded to 64; the begin call fails, naming
+ * the class count, when they do not fit).  pl2gpu_score_add_variants_classes takes, next to the tables of
+ * pl2gpu_score_add_variants_ploidy, the class of each entry (entry_classes[e] < class_ct); ploidy_classes may be NULL
+ * (every entry diploid).  Each staged batch is uploaded once, grouped by class on the device (stably), and every
+ * (class, ploidy class) run goes through the kernels and launch plan of the plain path into its class's accumulators:
+ * each entry is added once per column, whatever the class count.  A call whose entries all share one class scores them
+ * exactly as pl2gpu_score_add_variants_ploidy (or, with ploidy_classes NULL, pl2gpu_score_add_variants) does.
+ * pl2gpu_score_get_class returns one class's sums in the form of pl2gpu_score_get_ploidy.  The existing begin calls
+ * make one-class jobs: pl2gpu_score_get_ploidy is pl2gpu_score_get_class of class 0. */
+int pl2gpu_score_begin_classes(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t score_ct, uint32_t class_ct, Pl2ScoreJob** job_ptr);
+int pl2gpu_score_add_variants_classes(Pl2ScoreJob* job, const void* genovecs, uint64_t variant_stride_bytes, uint32_t variant_ct, int src_is_device, const uint32_t* entry_classes, const uint8_t* ploidy_classes,
+                                      const double* weights4_diploid, const double* weights4_haploid, const uint8_t* named_dosages);
+int pl2gpu_score_get_class(Pl2ScoreJob* job, uint32_t class_idx, double* score_sums, uint64_t* named_half_dosage_sums, uint32_t* missing_diploid_cts, uint32_t* missing_haploid_cts);
 
 /* ---- measured tensor peak: two warpgroups per SM issue back-to-back wgmmas with A fragments in registers and B in
  * shared memory, as the KING/GRM kernels use them, for at least min_seconds.  form 1: int8 (M = 64, N = n_cols in

@@ -23,6 +23,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <limits>
+#include <map>
 #include <memory>
 #include <ctime>
 #include <string>
@@ -97,6 +98,10 @@ struct Cmd {
   std::string score_file;
   uint32_t score_id_col = 1, score_allele_col = 2, score_coef_col = 3, score_numeric_params = 0;
   std::vector<uint32_t> score_col_nums;   // --score-col-nums: 1-based coefficient columns, increasing, no duplicates
+  // --q-score-range <range file> <data file> [i] [j] ['header'] ['min']: variant IDs from column i, p-values from j
+  std::string qsr_range_file, qsr_data_file;
+  uint32_t qsr_id_col = 1, qsr_val_col = 2;
+  bool qsr_header = false, qsr_min = false;
   std::vector<uint32_t> vscore_col_nums;  // --vscore-col-nums: 1-based weight columns, increasing, no duplicates
   bool score_header = false, score_header_read = false, score_no_meanimpute = false, score_zs = false, score_center = false, score_varstd = false, score_dominant = false, score_recessive = false, score_list_variants = false;
   bool sc_fid_maybe = true, sc_fid = false, sc_sid_maybe = true, sc_sid = false, sc_pheno1 = false, sc_phenos = true, sc_nallele = true, sc_denom = false, sc_dosagesum = true, sc_avgs = true, sc_sums = false;
@@ -481,6 +486,28 @@ int ParseArgs(int argc, char** argv, Cmd* c) {
       }
       if (c->score_header && c->score_header_read) return Usage("--score 'header' and 'header-read' modifiers cannot be used together.");
       if ((c->score_dominant || c->score_recessive) && (c->score_center || (c->score_dominant && c->score_recessive))) return Usage("--score 'dominant' / 'recessive' cannot be combined with each other or with 'center' / 'variance-standardize'.");
+    } else if (flag == "--q-score-range") {
+      // plink2.cc:10746-10792
+      if (nparam > 6) return Usage("--q-score-range accepts at most 6 arguments.");
+      if (nparam < 2) return Usage("--q-score-range requires at least 2 arguments.");
+      c->qsr_range_file = prm[0];
+      c->qsr_data_file = prm[1];
+      uint32_t cols[2] = {0, 0}, nnum = 0;
+      for (int k = 2; k < nparam; ++k) {
+        const std::string m = prm[k];
+        if (m == "header") c->qsr_header = true;
+        else if (m == "min") c->qsr_min = true;
+        else {
+          uint32_t v;
+          if (!ParseU32(prm[k], &v) || !v || v > 0x3FFFFFFFu) return Usage(("Invalid --q-score-range argument '" + m + "'.").c_str());
+          if (nnum == 2) return Usage("--q-score-range takes at most two numeric arguments.");
+          cols[nnum] = v;
+          if (nnum && cols[0] == cols[1]) return Usage("Identical --q-score-range column indexes.");
+          ++nnum;
+        }
+      }
+      if (nnum) c->qsr_id_col = cols[0];
+      c->qsr_val_col = nnum == 2 ? cols[1] : c->qsr_id_col + 1;
     } else if (flag == "--score-col-nums" || flag == "--vscore-col-nums") {
       const bool vs = flag == "--vscore-col-nums";
       if (int rc = ParseColNums(flag, prm, nparam, vs ? &c->vscore_col_nums : &c->score_col_nums)) return rc;
@@ -757,6 +784,7 @@ int ParseArgs(int argc, char** argv, Cmd* c) {
     logprintf("Error: --xchr-model 0 (skip chrX) is not supported by plink2_b200; use --not-chr X to leave chrX out.\n");
     return kRetNotYetSupported;
   }
+  if (!c->qsr_range_file.empty() && c->score_file.empty()) return Usage("--q-score-range cannot be used without --score[-list].");
   if (!c->score_col_nums.empty()) {
     if (c->score_file.empty()) return Usage("--score-col-nums must be used with --score[-list].");
     if (c->score_numeric_params == 3) return Usage("--score-col-nums cannot be used when three numeric arguments are\nprovided to --score.");
@@ -2797,6 +2825,108 @@ std::vector<uint32_t> AllVariants(const Dataset& ds) {
 }
 int SexChrRefFreqs(Dataset* ds, Pl2GpuCtx* ctx, const std::vector<uint32_t>& vidx, std::vector<double>* ref_freqs);
 
+// --q-score-range (ScoreReport, 2.0/plink2_matrix_calc.cc:6960-7170).  Range file: name, lower and upper bound per
+// line; lines without two numeric bounds are skipped.  Data file: a variant ID and a p-value per line, from columns
+// qsr_id_col / qsr_val_col.  Lines whose ID is not in the dataset, or is duplicated there, are skipped and counted; NA
+// p-values are skipped silently.  A variant lies in a range when lb <= p <= ub.  Line numbers count nonempty lines.
+struct QsrRange {
+  std::string name;
+  double lb, ub;
+};
+// the 'NA' / 'nan' tokens (any case) the reference tolerates as p-values (IsNanStr)
+bool QsrNaToken(const std::string& t) {
+  if (t.size() != 2 && t.size() != 3) return false;
+  if ((t[0] | 0x20) != 'n' || (t[1] | 0x20) != 'a') return false;
+  return t.size() == 2 || (t[2] | 0x20) == 'n';
+}
+int LoadQsr(const Cmd& c, const VariantInfo& V, const std::unordered_map<std::string, uint32_t>& by_id, const std::unordered_map<std::string, uint32_t>& dup, std::vector<QsrRange>* ranges, std::vector<double>* pval,
+            std::vector<uint8_t>* seen) {
+  std::vector<std::string> lines;
+  std::string err;
+  if (!ReadLines(c.qsr_range_file, &lines, &err)) {
+    logprintf("Error: %s\n", err.c_str());
+    return kRetOpenFail;
+  }
+  size_t line_idx = 0;
+  for (const std::string& ln : lines) {
+    const std::vector<std::string> t = SplitWs(ln);
+    if (t.empty()) continue;
+    ++line_idx;
+    double lb, ub;
+    if (t.size() < 3 || !ParseDouble(t[1].c_str(), &lb) || !ParseDouble(t[2].c_str(), &ub)) continue;
+    if (lb > ub) {
+      logprintf("Error: Upper bound < lower bound on line %zu of --q-score-range range file.\n", line_idx);
+      return kRetMalformedInput;
+    }
+    ranges->push_back({t[0], lb, ub});
+  }
+  if (ranges->empty()) {
+    logprintf("Error: Empty --q-score-range range file.\n");
+    return kRetInconsistentInput;
+  }
+  lines.clear();
+  if (!ReadLines(c.qsr_data_file, &lines, &err)) {
+    logprintf("Error: %s\n", err.c_str());
+    return kRetOpenFail;
+  }
+  pval->assign(V.size(), 0.0);
+  seen->assign(V.size(), 0);
+  line_idx = 0;
+  bool header = c.qsr_header;
+  uint64_t miss_ct = 0;
+  uint32_t loaded = 0;
+  const uint32_t need = std::max(c.qsr_id_col, c.qsr_val_col);
+  for (const std::string& ln : lines) {
+    const std::vector<std::string> t = SplitWs(ln);
+    if (t.empty()) continue;
+    ++line_idx;
+    if (header) {
+      header = false;
+      continue;
+    }
+    if (t.size() < need) {
+      logprintf("Error: Line %zu of --q-score-range data file has fewer tokens than expected.\n", line_idx);
+      return kRetInconsistentInput;
+    }
+    const std::string& id = t[c.qsr_id_col - 1];
+    const auto it = by_id.find(id);
+    if (it == by_id.end() || dup.count(id)) {
+      ++miss_ct;
+      continue;
+    }
+    const std::string& val = t[c.qsr_val_col - 1];
+    double p;
+    if (QsrNaToken(val)) continue;
+    if (!ParseDouble(val.c_str(), &p)) {
+      logprintf("Error: Invalid value '%s' on line %zu of --q-score-range data file.\n", val.c_str(), line_idx);
+      return kRetMalformedInput;
+    }
+    const uint32_t v = it->second;
+    if ((*seen)[v]) {
+      if (!c.qsr_min) {
+        logprintf("Error: Duplicate variant ID '%s' in --q-score-range data file. (Add the 'min' modifier if this is a multiallelic variant that you want to use the minimum p-value for.)\n", id.c_str());
+        return kRetMalformedInput;
+      }
+      if ((*pval)[v] <= p) continue;
+    } else {
+      ++loaded;
+    }
+    (*seen)[v] = 1;
+    (*pval)[v] = p;
+  }
+  if (c.qsr_header && line_idx == 0) {
+    logprintf("Error: Empty --q-score-range data file.\n");
+    return kRetMalformedInput;
+  }
+  if (!loaded) {
+    logprintf("Error: No valid entries in --q-score-range data file.\n");
+    return kRetInconsistentInput;
+  }
+  logprintf("--q-score-range: %zu range%s and %u variant%s loaded.\n", ranges->size(), ranges->size() == 1 ? "" : "s", loaded, loaded == 1 ? "" : "s");
+  if (miss_ct) logprintf("Warning: %llu line%s skipped in --q-score-range data file.\n", static_cast<unsigned long long>(miss_ct), miss_ct == 1 ? "" : "s");
+  return 0;
+}
+
 // `--score` (ScoreReport, 2.0/plink2_matrix_calc.cc:6892-9270) for hard calls: default report columns plus
 // denom / scoresums, 'header' / 'header-read', 'no-mean-imputation', and any number of coefficient columns
 // (--score-col-nums).  chrX, chrY and MT entries are scored with the reference's sex-dependent ploidy (--xchr-model 2:
@@ -2817,6 +2947,14 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   by_id.reserve(static_cast<size_t>(V.size()) * 2);
   for (uint32_t v = 0; v < V.size(); ++v)
     if (!by_id.emplace(V.id[v], v).second) dup.emplace(V.id[v], v);
+  // --q-score-range: the ranges and the data file's p-values, read before the score file as the reference does
+  const bool qsr = !c.qsr_range_file.empty();
+  std::vector<QsrRange> ranges;
+  std::vector<double> qsr_p;
+  std::vector<uint8_t> qsr_seen;
+  if (qsr) {
+    if (int rc = LoadQsr(c, V, by_id, dup, &ranges, &qsr_p, &qsr_seen)) return rc;
+  }
   struct Entry {
     uint32_t v;
     uint8_t aidx;  // 0 = REF named, 1 = ALT named
@@ -2934,6 +3072,31 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   }
   // device passes run in variant order (sums are order-independent up to fp64 rounding; the device adds in a fixed order)
   std::stable_sort(entries.begin(), entries.end(), [](const Entry& a, const Entry& b) { return a.v < b.v; });
+  const size_t processed_ct = entries.size();
+  // --q-score-range classes: entries whose variant lies in the same set of ranges share a class (numbered in variant
+  // order); each range is the union of its classes.  Entries in no range are dropped here.
+  std::vector<uint32_t> entry_class;                // per entry
+  std::vector<std::vector<uint8_t>> class_ranges;  // per class: 1 for each range it lies in
+  if (qsr) {
+    std::map<std::vector<uint8_t>, uint32_t> class_of;
+    std::vector<Entry> kept;
+    for (const Entry& e : entries) {
+      if (!qsr_seen[e.v]) continue;
+      std::vector<uint8_t> in(ranges.size(), 0);
+      bool any = false;
+      for (size_t r = 0; r < ranges.size(); ++r) {
+        in[r] = !(qsr_p[e.v] < ranges[r].lb || qsr_p[e.v] > ranges[r].ub);
+        any = any || in[r];
+      }
+      if (!any) continue;
+      const auto it = class_of.emplace(in, static_cast<uint32_t>(class_ranges.size()));
+      if (it.second) class_ranges.push_back(in);
+      entry_class.push_back(it.first->second);
+      kept.push_back(e);
+    }
+    entries.swap(kept);
+  }
+  const uint32_t class_ct = qsr ? std::max<uint32_t>(1, static_cast<uint32_t>(class_ranges.size())) : 1;
   std::vector<uint32_t> vidx(entries.size());
   for (size_t k = 0; k < entries.size(); ++k) vidx[k] = entries[k].v;
   // named-allele frequencies for the mean imputation: founders (ComputeAlleleFreqs), --read-freq values first
@@ -2955,7 +3118,9 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   bool ploidy_job = false;
   for (const Entry& e : entries) ploidy_job = ploidy_job || ploidy_class(e.v) != kPl2ScoreDiploid;
   Pl2ScoreJob* job = nullptr;
-  if (score_ct == 1) {  // the one-column job (same device work as pl2gpu_score_begin_cols with one column)
+  if (qsr) {
+    if (pl2gpu_score_begin_classes(ctx, n, score_ct, class_ct, &job)) return GpuFail("pl2gpu_score_begin_classes");
+  } else if (score_ct == 1) {  // the one-column job (same device work as pl2gpu_score_begin_cols with one column)
     if (pl2gpu_score_begin(ctx, n, &job)) return GpuFail("pl2gpu_score_begin");
   } else if (pl2gpu_score_begin_cols(ctx, n, score_ct, &job)) {
     return GpuFail("pl2gpu_score_begin_cols");
@@ -2969,7 +3134,8 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   if (!bs.Init()) return GpuFail("pl2gpu_host_alloc");
   std::vector<double> w4, w4h;  // diploid and haploid tables
   std::vector<uint8_t> d4, cls;
-  std::vector<int64_t> repeat_miss(n, 0), repeat_miss_hap(n, 0);
+  std::vector<uint32_t> ecls;
+  std::vector<int64_t> repeat_miss(static_cast<uint64_t>(class_ct) * n, 0), repeat_miss_hap(static_cast<uint64_t>(class_ct) * n, 0);  // [class][sample]
   size_t base = 0;
   for (;;) {
     const int got = bs.Next(&err);
@@ -2982,8 +3148,10 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
     w4h.resize(4ull * score_ct * got);
     d4.resize(got);
     cls.resize(got);
+    ecls.resize(got);
     for (int k = 0; k < got; ++k) {
       const Entry& e = entries[base + k];
+      const uint64_t cbase = qsr ? static_cast<uint64_t>(ecls[k] = entry_class[base + k]) * n : 0;
       const uint8_t pc = cls[k] = ploidy_class(e.v);
       const double f_named = e.aidx ? (1.0 - ref_freqs[base + k]) : ref_freqs[base + k];
       // genotype code = ALT allele count; named-allele dosage of codes 0, 1, 2.  The tables below do not depend on
@@ -3048,33 +3216,43 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
           for (; ms; ms &= ms - 1) {
             const uint32_t s = 32 * w + __builtin_ctzll(ms) / 2;
             const uint8_t sex = S.sex[s];
-            if (pc == kPl2ScoreDiploid || (pc == kPl2ScoreChrXMaleHaploid && sex != 1)) --repeat_miss[s];
-            else if (pc != kPl2ScoreChrY || sex != 2) --repeat_miss_hap[s];  // chrY females are not counted
+            if (pc == kPl2ScoreDiploid || (pc == kPl2ScoreChrXMaleHaploid && sex != 1)) --repeat_miss[cbase + s];
+            else if (pc != kPl2ScoreChrY || sex != 2) --repeat_miss_hap[cbase + s];  // chrY females are not counted
           }
         }
       }
     }
-    if (ploidy_job) {
+    if (qsr) {
+      if (pl2gpu_score_add_variants_classes(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0, ecls.data(), ploidy_job ? cls.data() : nullptr, w4.data(), w4h.data(), d4.data()))
+        return GpuFail("pl2gpu_score_add_variants_classes");
+    } else if (ploidy_job) {
       if (pl2gpu_score_add_variants_ploidy(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0, cls.data(), w4.data(), w4h.data(), d4.data())) return GpuFail("pl2gpu_score_add_variants_ploidy");
     } else if (pl2gpu_score_add_variants(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0, w4.data(), d4.data())) {
       return GpuFail("pl2gpu_score_add_variants");
     }
     base += static_cast<size_t>(got);
   }
-  std::vector<double> sums(static_cast<uint64_t>(n) * score_ct);  // [sample][score_ct]
-  std::vector<uint64_t> hdos(n);                                  // named-allele dosage sums in half allele units
-  std::vector<uint32_t> miss(n), miss_hap(n, 0);
-  if (ploidy_job) {
+  // per class: score sums [sample][score_ct], named-allele dosage sums in half allele units, diploid and haploid
+  // missing calls (with the second entries of variants named by both alleles taken back out)
+  std::vector<double> sums(static_cast<uint64_t>(class_ct) * n * score_ct);
+  std::vector<uint64_t> hdos(static_cast<uint64_t>(class_ct) * n);
+  std::vector<uint32_t> miss(static_cast<uint64_t>(class_ct) * n), miss_hap(static_cast<uint64_t>(class_ct) * n, 0);
+  if (qsr) {
+    for (uint32_t k = 0; k < class_ct; ++k) {
+      const uint64_t o = static_cast<uint64_t>(k) * n;
+      if (pl2gpu_score_get_class(job, k, sums.data() + o * score_ct, hdos.data() + o, miss.data() + o, miss_hap.data() + o)) return GpuFail("pl2gpu_score_get_class");
+    }
+  } else if (ploidy_job) {
     if (pl2gpu_score_get_ploidy(job, sums.data(), hdos.data(), miss.data(), miss_hap.data())) return GpuFail("pl2gpu_score_get_ploidy");
   } else {
     if (pl2gpu_score_get(job, sums.data(), hdos.data(), miss.data())) return GpuFail("pl2gpu_score_get");
     for (uint64_t& d : hdos) d *= 2;
   }
-  for (uint32_t k = 0; k < n; ++k) {
+  for (uint64_t k = 0; k < miss.size(); ++k) {
     miss[k] = static_cast<uint32_t>(miss[k] + repeat_miss[k]);
     miss_hap[k] = static_cast<uint32_t>(miss_hap[k] + repeat_miss_hap[k]);
   }
-  logprintf("--score: %zu variant%s processed.\n", entries.size(), entries.size() == 1 ? "" : "s");
+  logprintf("--score: %zu variant%s processed.\n", processed_ct, processed_ct == 1 ? "" : "s");
   if (c.score_list_variants) {
     OutFile fv;
     const std::string vname = c.out + ".sscore.vars";
@@ -3086,6 +3264,17 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
     if (!fv.Close()) return kRetWriteFail;
     logprintf("Variant list written to %s .\n", vname.c_str());
   }
+  // DENOM = base + nonfemale x chrY variants - male x chrX variants under --xchr-model 1 (:8581); base counts 2 per
+  // diploid variant and 1 per MT variant.  Per class here; a range's terms are the sums over its classes (:8389).
+  std::vector<uint32_t> denom_base(class_ct, 0), y_incr(class_ct, 0), x_decr(class_ct, 0);
+  for (size_t k = 0; k < entries.size(); ++k) {
+    if (k && entries[k - 1].v == entries[k].v) continue;
+    const uint8_t pc = ploidy_class(entries[k].v);
+    const uint32_t cl = qsr ? entry_class[k] : 0;
+    denom_base[cl] += pc == kPl2ScoreHaploidAll ? 1 : pc == kPl2ScoreChrY ? 0 : 2;
+    y_incr[cl] += pc == kPl2ScoreChrY;
+    x_decr[cl] += pc == kPl2ScoreChrXMaleHaploid;
+  }
   // report (:8470-8625)
   std::vector<PhenoOut> phenos;
   if (c.sc_phenos || c.sc_pheno1) {
@@ -3096,9 +3285,6 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
     }
   }
   const IdFmt idf{c.sc_fid || (c.sc_fid_maybe && S.fid_present), c.sc_sid || (c.sc_sid_maybe && S.sid_present)};
-  const std::string name = c.out + (c.score_zs ? ".sscore.zst" : ".sscore");
-  OutFile f;
-  if (!f.Open(name, c.score_zs)) return kRetOpenFail;
   std::string hdr = "#";
   if (idf.fid) hdr += "FID\t";
   hdr += "IID";
@@ -3113,51 +3299,76 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   if (c.sc_sums)
     for (const std::string& nm : score_names) hdr += "\t" + nm + "_SUM";
   hdr += "\n";
-  f.Puts(hdr.c_str());
-  // DENOM = base + nonfemale x chrY variants - male x chrX variants under --xchr-model 1 (:8581); base counts 2 per
-  // diploid variant and 1 per MT variant
-  uint32_t denom_base = 0, y_incr = 0, x_decr = 0;
-  for (size_t k = 0; k < entries.size(); ++k) {
-    if (k && entries[k - 1].v == entries[k].v) continue;
-    const uint8_t pc = ploidy_class(entries[k].v);
-    denom_base += pc == kPl2ScoreHaploidAll ? 1 : pc == kPl2ScoreChrY ? 0 : 2;
-    y_incr += pc == kPl2ScoreChrY;
-    x_decr += pc == kPl2ScoreChrXMaleHaploid;
-  }
-  char num[64];
-  for (uint32_t k = 0; k < n; ++k) {
-    std::string row = FmtId(S, k, idf);
-    for (const PhenoOut& po : phenos) row += "\t" + po.text[k];
-    const uint32_t denom_full = denom_base + (S.sex[k] != 2 ? y_incr : 0) - (S.sex[k] == 1 ? x_decr : 0);
-    const uint32_t nallele = denom_full - 2 * miss[k] - miss_hap[k];
-    const uint32_t denom = c.score_no_meanimpute ? nallele : denom_full;
-    if (c.sc_nallele) {
-      *u32toa(nallele, num) = '\0';
-      row += std::string("\t") + num;
+  // one report: the classes with in_report[class] set, added in ascending class order
+  auto write_report = [&](const std::string& name, const std::vector<uint8_t>& in_report) -> int {
+    std::vector<double> rs(static_cast<uint64_t>(n) * score_ct, 0.0);
+    std::vector<uint64_t> rhdos(n, 0);
+    std::vector<uint32_t> rmiss(n, 0), rmiss_hap(n, 0);
+    uint32_t rbase = 0, ry = 0, rx = 0;
+    for (uint32_t k = 0; k < class_ct; ++k) {
+      if (!in_report[k]) continue;
+      const uint64_t o = static_cast<uint64_t>(k) * n;
+      for (uint64_t i = 0; i < rs.size(); ++i) rs[i] += sums[o * score_ct + i];
+      for (uint32_t s = 0; s < n; ++s) {
+        rhdos[s] += hdos[o + s];
+        rmiss[s] += miss[o + s];
+        rmiss_hap[s] += miss_hap[o + s];
+      }
+      rbase += denom_base[k];
+      ry += y_incr[k];
+      rx += x_decr[k];
     }
-    if (c.sc_denom) {
-      *u32toa(denom, num) = '\0';
-      row += std::string("\t") + num;
-    }
-    if (c.sc_dosagesum) row += "\t" + std::to_string(hdos[k] / 2) + ((hdos[k] & 1) ? ".5" : "");
-    const double* ks = &sums[static_cast<uint64_t>(k) * score_ct];
-    if (c.sc_avgs) {
-      for (uint32_t j = 0; j < score_ct; ++j) {
-        *dtoa_g(ks[j] * (1.0 / static_cast<double>(denom)), num) = '\0';
+    OutFile f;
+    if (!f.Open(name, c.score_zs)) return kRetOpenFail;
+    f.Puts(hdr.c_str());
+    char num[64];
+    for (uint32_t k = 0; k < n; ++k) {
+      std::string row = FmtId(S, k, idf);
+      for (const PhenoOut& po : phenos) row += "\t" + po.text[k];
+      const uint32_t denom_full = rbase + (S.sex[k] != 2 ? ry : 0) - (S.sex[k] == 1 ? rx : 0);
+      const uint32_t nallele = denom_full - 2 * rmiss[k] - rmiss_hap[k];
+      const uint32_t denom = c.score_no_meanimpute ? nallele : denom_full;
+      if (c.sc_nallele) {
+        *u32toa(nallele, num) = '\0';
         row += std::string("\t") + num;
       }
-    }
-    if (c.sc_sums) {
-      for (uint32_t j = 0; j < score_ct; ++j) {
-        *dtoa_g(ks[j], num) = '\0';
+      if (c.sc_denom) {
+        *u32toa(denom, num) = '\0';
         row += std::string("\t") + num;
       }
+      if (c.sc_dosagesum) row += "\t" + std::to_string(rhdos[k] / 2) + ((rhdos[k] & 1) ? ".5" : "");
+      const double* ks = &rs[static_cast<uint64_t>(k) * score_ct];
+      if (c.sc_avgs) {
+        for (uint32_t j = 0; j < score_ct; ++j) {
+          *dtoa_g(ks[j] * (1.0 / static_cast<double>(denom)), num) = '\0';
+          row += std::string("\t") + num;
+        }
+      }
+      if (c.sc_sums) {
+        for (uint32_t j = 0; j < score_ct; ++j) {
+          *dtoa_g(ks[j], num) = '\0';
+          row += std::string("\t") + num;
+        }
+      }
+      row += "\n";
+      f.Write(row.data(), row.size());
     }
-    row += "\n";
-    f.Write(row.data(), row.size());
+    return f.Close() ? 0 : kRetWriteFail;
+  };
+  const char* ext = c.score_zs ? ".sscore.zst" : ".sscore";
+  if (!qsr) {
+    const std::string name = c.out + ext;
+    if (int rc = write_report(name, std::vector<uint8_t>(1, 1))) return rc;
+    logprintf("--score: Results written to %s .\n", name.c_str());
+    return 0;
   }
-  if (!f.Close()) return kRetWriteFail;
-  logprintf("--score: Results written to %s .\n", name.c_str());
+  // one report per range, in range-file order; a range no entry lies in gets one of zero sums
+  for (size_t r = 0; r < ranges.size(); ++r) {
+    std::vector<uint8_t> in_report(class_ct, 0);
+    for (uint32_t k = 0; k < class_ranges.size(); ++k) in_report[k] = class_ranges[k][r];
+    if (int rc = write_report(c.out + "." + ranges[r].name + ext, in_report)) return rc;
+  }
+  logprintf("--score + --q-score-range: Results written to %s.<range name>%s .\n", c.out.c_str(), ext);
   return 0;
 }
 

@@ -10,6 +10,9 @@
 // chrX (--xchr-model 1), chrY and MT entries (pl2gpu_score_add_variants_ploidy) run through score_ploidy_kernel, which
 // picks per sample a diploid or haploid table (or none: chrY females) from the sex masks and counts dosages in half
 // allele units with diploid and haploid missing calls apart; runs of diploid entries keep score_kernel and its plan.
+// A job may keep several accumulator sets, one per class (--q-score-range: the entries whose p-values lie in the same
+// set of ranges): each staged batch is gathered into class-major order on the device (score_row_gather_kernel), and
+// each (class, ploidy class) run goes through the same kernels and launch plan into its class's accumulators.
 //
 // Streaming: every 32-bit word of a variant row (16 samples) is read once.  A CTA covers 128 words x a chunk of
 // variants and writes per-chunk partial sums; a second kernel adds the partials in chunk order, so results do not
@@ -426,6 +429,14 @@ void LaunchPloidyGroup(uint32_t nc, const ScoreLaunch& a, const PloidyLaunch& p,
   }
 }
 
+// Class jobs (pl2gpu_score_add_variants_classes): row r of out is row perm[r] of in, so each class's entries of a
+// staged batch lie next to each other and run through the kernels above as one block.  pitch16: 16-byte words per row.
+__global__ void __launch_bounds__(256) score_row_gather_kernel(const uint4* __restrict__ in, uint4* __restrict__ out, uint32_t pitch16, const uint32_t* __restrict__ perm) {
+  const uint4* src = in + static_cast<uint64_t>(perm[blockIdx.y]) * pitch16;
+  uint4* dst = out + static_cast<uint64_t>(blockIdx.y) * pitch16;
+  for (uint32_t i = blockIdx.x * 256 + threadIdx.x; i < pitch16; i += gridDim.x * 256) dst[i] = src[i];
+}
+
 }  // namespace
 
 struct Pl2ScoreJob {
@@ -436,6 +447,8 @@ struct Pl2ScoreJob {
   }
   Pl2GpuCtx* ctx;
   uint32_t sample_ct = 0, score_ct = 1;
+  uint32_t class_ct = 1;  // accumulator sets (pl2gpu_score_begin_classes): class k's start k x samples_padded (x score_ct) in
+                          // d_acc_sum, d_acc_dos, d_acc_miss, d_acc_hdos and d_acc_miss_hap
   uint32_t stage_variants = kScoreStageVariants;  // entries per staged batch
   GenoStage stage;
   DevArray<double> d_w4, d_part_sum, d_acc_sum;
@@ -448,6 +461,9 @@ struct Pl2ScoreJob {
   DevArray<double> d_w4h;
   DevArray<uint32_t> d_part_miss_hap, d_acc_miss_hap;
   DevArray<unsigned long long> d_acc_hdos;
+  // batches whose entries span several classes: the class-major copy of the stage and its row order, on first use
+  DevArray<uint8_t> d_raw_grouped;
+  DevArray<uint32_t> d_perm;
 };
 
 extern "C" {
@@ -459,39 +475,61 @@ int pl2gpu_score_end(Pl2ScoreJob* job) {
   return 0;
 }
 
-int pl2gpu_score_begin_cols(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t score_ct, Pl2ScoreJob** job_ptr) {
+}  // extern "C"
+
+namespace {
+
+// class_ct accumulator sets; a job of several classes (fn = pl2gpu_score_begin_classes) also gets the haploid
+// accumulators from the start, so that every per-class buffer is sized before the first entry
+int ScoreBegin(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t score_ct, uint32_t class_ct, const char* fn, Pl2ScoreJob** job_ptr) {
   if (job_ptr) *job_ptr = nullptr;
-  if (!ctx || !job_ptr || !sample_ct || !score_ct) {
-    set_error("pl2gpu_score_begin_cols: bad arguments");
+  if (!ctx || !job_ptr || !sample_ct || !score_ct || !class_ct) {
+    set_error("%s: bad arguments", fn);
     return 1;
   }
   PL2_CUDA_OK(cudaSetDevice(ctx->c.device));
   std::unique_ptr<Pl2ScoreJob, int (*)(Pl2ScoreJob*)> job(new Pl2ScoreJob(ctx), pl2gpu_score_end);
   job->sample_ct = sample_ct;
   job->score_ct = score_ct;
+  job->class_ct = class_ct;
   PL2_TRY(StageAlloc(sample_ct, kScoreStageVariants, &job->stage, 64));
   const uint64_t np = job->stage.sample_ct_padded;
   const uint64_t group = std::min(score_ct, kScoreGroup);
-  const char* oom = "pl2gpu_score_begin_cols: insufficient device memory for %u samples x %u score columns";
-  if (job->d_d4.alloc(kScoreStageVariants, oom, sample_ct, score_ct) || job->d_part_sum.alloc(np * kScoreMaxChunks * group, oom, sample_ct, score_ct) || job->d_part_dos.alloc(np * kScoreMaxChunks, oom, sample_ct, score_ct) ||
-      job->d_part_miss.alloc(np * kScoreMaxChunks, oom, sample_ct, score_ct) || job->d_acc_sum.alloc(np * score_ct, oom, sample_ct, score_ct) || job->d_acc_dos.alloc(np, oom, sample_ct, score_ct) ||
-      job->d_acc_miss.alloc(np, oom, sample_ct, score_ct))
+  const char* oom = "%s: insufficient device memory for %u samples x %u score columns";
+  if (job->d_d4.alloc(kScoreStageVariants, oom, fn, sample_ct, score_ct) || job->d_part_sum.alloc(np * kScoreMaxChunks * group, oom, fn, sample_ct, score_ct) || job->d_part_dos.alloc(np * kScoreMaxChunks, oom, fn, sample_ct, score_ct) ||
+      job->d_part_miss.alloc(np * kScoreMaxChunks, oom, fn, sample_ct, score_ct))
     return 1;
+  // the accumulators: class_ct x (8 score_ct + 24) bytes per padded sample
+  const char* oom_acc = "%s: insufficient device memory for the accumulators of %u classes x %u score columns x %u samples (%llu bytes)";
+  const unsigned long long acc_bytes = class_ct * np * (8ull * score_ct + (class_ct > 1 ? 24 : 12));
+  if (job->d_acc_sum.alloc(np * score_ct * class_ct, oom_acc, fn, class_ct, score_ct, sample_ct, acc_bytes) || job->d_acc_dos.alloc(np * class_ct, oom_acc, fn, class_ct, score_ct, sample_ct, acc_bytes) ||
+      job->d_acc_miss.alloc(np * class_ct, oom_acc, fn, class_ct, score_ct, sample_ct, acc_bytes))
+    return 1;
+  if (class_ct > 1 && (job->d_acc_hdos.alloc(np * class_ct, oom_acc, fn, class_ct, score_ct, sample_ct, acc_bytes) || job->d_acc_miss_hap.alloc(np * class_ct, oom_acc, fn, class_ct, score_ct, sample_ct, acc_bytes))) return 1;
   // the staged weights ([entry][score_ct][4]) are the one buffer that grows with the column count and the batch: when
   // they do not fit, batches get fewer entries (then the chunk plan, and so the last bits of a sum, can differ from a
   // job with fewer columns)
-  while (job->d_w4.alloc(4ull * score_ct * job->stage_variants, "pl2gpu_score_begin_cols: insufficient device memory for the weights of %u score columns", score_ct)) {
+  while (job->d_w4.alloc(4ull * score_ct * job->stage_variants, "%s: insufficient device memory for the weights of %u score columns", fn, score_ct)) {
     if (job->stage_variants <= kScoreTile) return 1;
     job->stage_variants /= 2;
   }
-  if (cudaMemsetAsync(job->d_acc_sum, 0, 8 * np * score_ct, ctx->c.stream) != cudaSuccess || cudaMemsetAsync(job->d_acc_dos, 0, 8 * np, ctx->c.stream) != cudaSuccess ||
-      cudaMemsetAsync(job->d_acc_miss, 0, 4 * np, ctx->c.stream) != cudaSuccess) {
-    set_error("pl2gpu_score_begin_cols: %s", cudaGetErrorString(cudaGetLastError()));
+  if (cudaMemsetAsync(job->d_acc_sum, 0, 8 * np * score_ct * class_ct, ctx->c.stream) != cudaSuccess || cudaMemsetAsync(job->d_acc_dos, 0, 8 * np * class_ct, ctx->c.stream) != cudaSuccess ||
+      cudaMemsetAsync(job->d_acc_miss, 0, 4 * np * class_ct, ctx->c.stream) != cudaSuccess ||
+      (job->d_acc_hdos && (cudaMemsetAsync(job->d_acc_hdos, 0, 8 * np * class_ct, ctx->c.stream) != cudaSuccess || cudaMemsetAsync(job->d_acc_miss_hap, 0, 4 * np * class_ct, ctx->c.stream) != cudaSuccess))) {
+    set_error("%s: %s", fn, cudaGetErrorString(cudaGetLastError()));
     return 1;
   }
   *job_ptr = job.release();
   return 0;
 }
+
+}  // namespace
+
+extern "C" {
+
+int pl2gpu_score_begin_cols(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t score_ct, Pl2ScoreJob** job_ptr) { return ScoreBegin(ctx, sample_ct, score_ct, 1, "pl2gpu_score_begin_cols", job_ptr); }
+
+int pl2gpu_score_begin_classes(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t score_ct, uint32_t class_ct, Pl2ScoreJob** job_ptr) { return ScoreBegin(ctx, sample_ct, score_ct, class_ct, "pl2gpu_score_begin_classes", job_ptr); }
 
 int pl2gpu_score_begin(Pl2GpuCtx* ctx, uint32_t sample_ct, Pl2ScoreJob** job_ptr) { return pl2gpu_score_begin_cols(ctx, sample_ct, 1, job_ptr); }
 
@@ -499,11 +537,44 @@ int pl2gpu_score_begin(Pl2GpuCtx* ctx, uint32_t sample_ct, Pl2ScoreJob** job_ptr
 
 namespace {
 
-// Stages and scores variant_ct entries of one ploidy class: class kPl2ScoreDiploid through score_kernel exactly as
-// pl2gpu_score_add_variants always has, the others through score_ploidy_kernel with their haploid tables w_hap.
-int ScoreAddRun(Pl2ScoreJob* job, const uint8_t* src, uint64_t variant_stride_bytes, uint32_t variant_ct, int src_is_device, const double* weights4, const double* w_hap, const uint8_t* named_dosages, uint32_t ploidy_class) {
+// Scores variant_ct staged rows (raw, the stage's pitch) of one ploidy class into the accumulators of class cls: class
+// kPl2ScoreDiploid through score_kernel, the others through score_ploidy_kernel.  w4 / w4h / d4: the rows' device tables.
+int ScoreLaunchRun(Pl2ScoreJob* job, const uint8_t* raw, uint32_t variant_ct, const double* w4, const double* w4h, const uint8_t* d4, uint32_t ploidy_class, uint32_t cls) {
   Ctx* c = &job->ctx->c;
   const uint32_t np = job->stage.sample_ct_padded, words = np / 16;
+  const uint64_t acc = static_cast<uint64_t>(cls) * np;
+  // enough chunks to fill the GPU, each a multiple of the shared-memory tile; the plan does not depend on the column
+  // count, so every column is added in the order of a one-column job
+  const uint32_t col_ctas = DivUpU32(words, kScoreThreads);
+  uint32_t chunks = std::max(1u, std::min({kScoreMaxChunks, DivUpU32(7 * static_cast<uint32_t>(c->sm_count), col_ctas), DivUpU32(variant_ct, kScoreTile)}));
+  const uint32_t chunk_variants = RoundUpU32(DivUpU32(variant_ct, chunks), kScoreTile);
+  chunks = DivUpU32(variant_ct, chunk_variants);
+  ScoreLaunch a{raw, job->stage.pitch, words, variant_ct, chunk_variants, chunks, col_ctas, job->score_ct, 0, np, job->sample_ct, w4, d4, job->d_part_sum, job->d_part_dos, job->d_part_miss,
+                job->d_acc_sum + acc * job->score_ct, job->d_acc_dos + acc, job->d_acc_miss + acc};
+  const PloidyLaunch p{ploidy_class, job->d_male2, job->d_female2, w4h, job->d_part_miss_hap, job->d_acc_hdos + (job->d_acc_hdos ? acc : 0), job->d_acc_miss_hap + (job->d_acc_miss_hap ? acc : 0)};
+  // column groups over the resident batch; the first also adds the integer sums
+  for (uint32_t col0 = 0; col0 < job->score_ct; col0 += kScoreGroup) {
+    a.col0 = col0;
+    const uint32_t nc = std::min(kScoreGroup, job->score_ct - col0);
+    if (ploidy_class == kPl2ScoreDiploid) {
+      if (col0 == 0) LaunchScoreGroup<true>(nc, a, c->stream);
+      else LaunchScoreGroup<false>(nc, a, c->stream);
+      c->launches += 2;
+    } else {
+      if (col0 == 0) LaunchPloidyGroup<true>(nc, a, p, c->stream);
+      else LaunchPloidyGroup<false>(nc, a, p, c->stream);
+      c->launches += col0 == 0 ? 3 : 2;
+    }
+  }
+  PL2_CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// Stages and scores variant_ct entries of one ploidy class into class cls: class kPl2ScoreDiploid exactly as
+// pl2gpu_score_add_variants always has, the others with their haploid tables w_hap.
+int ScoreAddRun(Pl2ScoreJob* job, const uint8_t* src, uint64_t variant_stride_bytes, uint32_t variant_ct, int src_is_device, const double* weights4, const double* w_hap, const uint8_t* named_dosages, uint32_t ploidy_class,
+                uint32_t cls = 0) {
+  Ctx* c = &job->ctx->c;
   const uint64_t w_row = 4ull * job->score_ct;  // doubles of weights per entry
   for (uint32_t done = 0; done < variant_ct;) {
     const uint32_t cur = std::min(job->stage_variants, variant_ct - done);
@@ -512,30 +583,7 @@ int ScoreAddRun(Pl2ScoreJob* job, const uint8_t* src, uint64_t variant_stride_by
     PL2_CUDA_OK(cudaMemcpyAsync(job->d_w4, weights4 + w_row * done, 8 * w_row * cur, cudaMemcpyHostToDevice, c->stream));
     if (ploidy_class != kPl2ScoreDiploid) PL2_CUDA_OK(cudaMemcpyAsync(job->d_w4h, w_hap + w_row * done, 8 * w_row * cur, cudaMemcpyHostToDevice, c->stream));
     PL2_CUDA_OK(cudaMemcpyAsync(job->d_d4, named_dosages + done, cur, cudaMemcpyHostToDevice, c->stream));
-    // enough chunks to fill the GPU, each a multiple of the shared-memory tile; the plan does not depend on the column
-    // count, so every column is added in the order of a one-column job
-    const uint32_t col_ctas = DivUpU32(words, kScoreThreads);
-    uint32_t chunks = std::max(1u, std::min({kScoreMaxChunks, DivUpU32(7 * static_cast<uint32_t>(c->sm_count), col_ctas), DivUpU32(cur, kScoreTile)}));
-    const uint32_t chunk_variants = RoundUpU32(DivUpU32(cur, chunks), kScoreTile);
-    chunks = DivUpU32(cur, chunk_variants);
-    ScoreLaunch a{job->stage.d_raw, job->stage.pitch, words, cur, chunk_variants, chunks, col_ctas, job->score_ct, 0, np, job->sample_ct, job->d_w4, job->d_d4, job->d_part_sum, job->d_part_dos, job->d_part_miss,
-                  job->d_acc_sum, job->d_acc_dos, job->d_acc_miss};
-    const PloidyLaunch p{ploidy_class, job->d_male2, job->d_female2, job->d_w4h, job->d_part_miss_hap, job->d_acc_hdos, job->d_acc_miss_hap};
-    // column groups over the resident batch; the first also adds the integer sums
-    for (uint32_t col0 = 0; col0 < job->score_ct; col0 += kScoreGroup) {
-      a.col0 = col0;
-      const uint32_t nc = std::min(kScoreGroup, job->score_ct - col0);
-      if (ploidy_class == kPl2ScoreDiploid) {
-        if (col0 == 0) LaunchScoreGroup<true>(nc, a, c->stream);
-        else LaunchScoreGroup<false>(nc, a, c->stream);
-        c->launches += 2;
-      } else {
-        if (col0 == 0) LaunchPloidyGroup<true>(nc, a, p, c->stream);
-        else LaunchPloidyGroup<false>(nc, a, p, c->stream);
-        c->launches += col0 == 0 ? 3 : 2;
-      }
-    }
-    PL2_CUDA_OK(cudaGetLastError());
+    PL2_TRY(ScoreLaunchRun(job, job->stage.d_raw, cur, job->d_w4, job->d_w4h, job->d_d4, ploidy_class, cls));
     PL2_CUDA_OK(cudaStreamSynchronize(c->stream));  // host tables and a host source may be reused by the caller
     job->entries += cur;
     done += cur;
@@ -555,23 +603,67 @@ bool ValidNamedDosages(const uint8_t* named_dosages, uint32_t variant_ct, const 
 }
 
 // the buffers only entries of the haploid / sex-dependent classes use: all of them or none
+// (a job of several classes has its haploid accumulators from the start)
 int ScoreAllocPloidy(Pl2ScoreJob* job) {
-  if (job->d_acc_hdos) return 0;
+  if (job->d_w4h) return 0;
   Ctx* c = &job->ctx->c;
   const uint64_t np = job->stage.sample_ct_padded;
   const char* oom = "pl2gpu_score_add_variants_ploidy: insufficient device memory for the haploid tables of %u samples x %u score columns";
   DevArray<double> w4h;
-  DevArray<uint32_t> part_miss_hap, acc_miss_hap;
-  DevArray<unsigned long long> acc_hdos;
-  if (w4h.alloc(4ull * job->score_ct * job->stage_variants, oom, job->sample_ct, job->score_ct) || part_miss_hap.alloc(np * kScoreMaxChunks, oom, job->sample_ct, job->score_ct) ||
-      acc_miss_hap.alloc(np, oom, job->sample_ct, job->score_ct) || acc_hdos.alloc(np, oom, job->sample_ct, job->score_ct))
-    return 1;
-  PL2_CUDA_OK(cudaMemsetAsync(acc_miss_hap, 0, 4 * np, c->stream));
-  PL2_CUDA_OK(cudaMemsetAsync(acc_hdos, 0, 8 * np, c->stream));
+  DevArray<uint32_t> part_miss_hap;
+  if (w4h.alloc(4ull * job->score_ct * job->stage_variants, oom, job->sample_ct, job->score_ct) || part_miss_hap.alloc(np * kScoreMaxChunks, oom, job->sample_ct, job->score_ct)) return 1;
+  if (!job->d_acc_hdos) {
+    DevArray<uint32_t> acc_miss_hap;
+    DevArray<unsigned long long> acc_hdos;
+    if (acc_miss_hap.alloc(np, oom, job->sample_ct, job->score_ct) || acc_hdos.alloc(np, oom, job->sample_ct, job->score_ct)) return 1;
+    PL2_CUDA_OK(cudaMemsetAsync(acc_miss_hap, 0, 4 * np, c->stream));
+    PL2_CUDA_OK(cudaMemsetAsync(acc_hdos, 0, 8 * np, c->stream));
+    job->d_acc_miss_hap = std::move(acc_miss_hap);
+    job->d_acc_hdos = std::move(acc_hdos);
+  }
   job->d_w4h = std::move(w4h);
   job->d_part_miss_hap = std::move(part_miss_hap);
-  job->d_acc_miss_hap = std::move(acc_miss_hap);
-  job->d_acc_hdos = std::move(acc_hdos);
+  return 0;
+}
+
+// the checks of pl2gpu_score_add_variants_ploidy on its ploidy classes (fn names the entry point in the messages)
+bool ValidPloidyClasses(const Pl2ScoreJob* job, const uint8_t* ploidy_classes, uint32_t variant_ct, const double* weights4_haploid, const uint8_t* named_dosages, const char* fn) {
+  for (uint32_t v = 0; v < variant_ct; ++v) {
+    const uint8_t pc = ploidy_classes[v];
+    if (pc > kPl2ScoreChrXMaleHaploid) {
+      set_error("%s: entry %u has ploidy class %u", fn, v, pc);
+      return false;
+    }
+    if (pc == kPl2ScoreDiploid) continue;
+    if (!weights4_haploid) {
+      set_error("%s: entry %u is haploid for some samples but weights4_haploid is NULL", fn, v);
+      return false;
+    }
+    if (named_dosages[v] != 0x24 && named_dosages[v] != 0x06) {
+      set_error("%s: entry %u of ploidy class %u is not additive (named-allele dosages 0x%02x)", fn, v, pc, named_dosages[v]);
+      return false;
+    }
+    if (pc != kPl2ScoreHaploidAll && !job->d_male2) {
+      set_error("%s: entry %u of ploidy class %u needs the sample sexes (pl2gpu_score_set_sex)", fn, v, pc);
+      return false;
+    }
+  }
+  return true;
+}
+
+// runs of consecutive entries of one ploidy class into class cls; a diploid-only call is one run of the plain score path
+int ScoreAddPloidyRuns(Pl2ScoreJob* job, const uint8_t* src, uint64_t variant_stride_bytes, uint32_t variant_ct, int src_is_device, const uint8_t* ploidy_classes, const double* weights4_diploid, const double* weights4_haploid,
+                       const uint8_t* named_dosages, uint32_t cls) {
+  const uint64_t w_row = 4ull * job->score_ct;
+  for (uint32_t r0 = 0; r0 < variant_ct;) {
+    const uint32_t pc = ploidy_classes ? ploidy_classes[r0] : kPl2ScoreDiploid;
+    uint32_t r1 = r0 + 1;
+    while (r1 < variant_ct && (ploidy_classes ? ploidy_classes[r1] : kPl2ScoreDiploid) == pc) ++r1;
+    if (pc != kPl2ScoreDiploid && ScoreAllocPloidy(job)) return 1;
+    PL2_TRY(ScoreAddRun(job, src + static_cast<uint64_t>(r0) * variant_stride_bytes, variant_stride_bytes, r1 - r0, src_is_device, weights4_diploid + w_row * r0, pc == kPl2ScoreDiploid ? nullptr : weights4_haploid + w_row * r0,
+                        named_dosages + r0, pc, cls));
+    r0 = r1;
+  }
   return 0;
 }
 
@@ -625,39 +717,120 @@ int pl2gpu_score_add_variants_ploidy(Pl2ScoreJob* job, const void* genovecs, uin
     return 1;
   }
   if (!ValidNamedDosages(named_dosages, variant_ct, "pl2gpu_score_add_variants_ploidy")) return 1;
+  if (!ValidPloidyClasses(job, ploidy_classes, variant_ct, weights4_haploid, named_dosages, "pl2gpu_score_add_variants_ploidy")) return 1;
+  PL2_CUDA_OK(cudaSetDevice(job->ctx->c.device));
+  return ScoreAddPloidyRuns(job, static_cast<const uint8_t*>(genovecs), variant_stride_bytes, variant_ct, src_is_device, ploidy_classes, weights4_diploid, weights4_haploid, named_dosages, 0);
+}
+
+int pl2gpu_score_add_variants_classes(Pl2ScoreJob* job, const void* genovecs, uint64_t variant_stride_bytes, uint32_t variant_ct, int src_is_device, const uint32_t* entry_classes, const uint8_t* ploidy_classes,
+                                      const double* weights4_diploid, const double* weights4_haploid, const uint8_t* named_dosages) {
+  const char* fn = "pl2gpu_score_add_variants_classes";
+  if (!job || (variant_ct && (!genovecs || !entry_classes || !weights4_diploid || !named_dosages))) {
+    set_error("%s: bad arguments", fn);
+    return 1;
+  }
+  if (!ValidNamedDosages(named_dosages, variant_ct, fn)) return 1;
+  if (ploidy_classes && !ValidPloidyClasses(job, ploidy_classes, variant_ct, weights4_haploid, named_dosages, fn)) return 1;
   for (uint32_t v = 0; v < variant_ct; ++v) {
-    const uint8_t pc = ploidy_classes[v];
-    if (pc > kPl2ScoreChrXMaleHaploid) {
-      set_error("pl2gpu_score_add_variants_ploidy: entry %u has ploidy class %u", v, pc);
-      return 1;
-    }
-    if (pc == kPl2ScoreDiploid) continue;
-    if (!weights4_haploid) {
-      set_error("pl2gpu_score_add_variants_ploidy: entry %u is haploid for some samples but weights4_haploid is NULL", v);
-      return 1;
-    }
-    if (named_dosages[v] != 0x24 && named_dosages[v] != 0x06) {
-      set_error("pl2gpu_score_add_variants_ploidy: entry %u of ploidy class %u is not additive (named-allele dosages 0x%02x)", v, pc, named_dosages[v]);
-      return 1;
-    }
-    if (pc != kPl2ScoreHaploidAll && !job->d_male2) {
-      set_error("pl2gpu_score_add_variants_ploidy: entry %u of ploidy class %u needs the sample sexes (pl2gpu_score_set_sex)", v, pc);
+    if (entry_classes[v] >= job->class_ct) {
+      set_error("%s: entry %u has class %u of a job of %u classes", fn, v, entry_classes[v], job->class_ct);
       return 1;
     }
   }
   PL2_CUDA_OK(cudaSetDevice(job->ctx->c.device));
   const uint8_t* src = static_cast<const uint8_t*>(genovecs);
-  const uint64_t w_row = 4ull * job->score_ct;
-  // runs of consecutive entries of one class; a diploid-only call is one run of the plain score path
-  for (uint32_t r0 = 0; r0 < variant_ct;) {
-    const uint32_t pc = ploidy_classes[r0];
-    uint32_t r1 = r0 + 1;
-    while (r1 < variant_ct && ploidy_classes[r1] == pc) ++r1;
-    if (pc != kPl2ScoreDiploid && ScoreAllocPloidy(job)) return 1;
-    PL2_TRY(ScoreAddRun(job, src + static_cast<uint64_t>(r0) * variant_stride_bytes, variant_stride_bytes, r1 - r0, src_is_device, weights4_diploid + w_row * r0, pc == kPl2ScoreDiploid ? nullptr : weights4_haploid + w_row * r0,
-                        named_dosages + r0, pc));
-    r0 = r1;
+  // one class for every entry: the ploidy runs of the plain path, into that class
+  if (std::all_of(entry_classes, entry_classes + variant_ct, [&](uint32_t k) { return k == entry_classes[0]; }))
+    return ScoreAddPloidyRuns(job, src, variant_stride_bytes, variant_ct, src_is_device, ploidy_classes, weights4_diploid, weights4_haploid, named_dosages, variant_ct ? entry_classes[0] : 0);
+  Ctx* c = &job->ctx->c;
+  if (ploidy_classes && std::any_of(ploidy_classes, ploidy_classes + variant_ct, [](uint8_t pc) { return pc != kPl2ScoreDiploid; }) && ScoreAllocPloidy(job)) return 1;
+  if (!job->d_raw_grouped) {
+    DevArray<uint8_t> raw;
+    DevArray<uint32_t> perm;
+    if (raw.alloc(static_cast<uint64_t>(job->stage.variant_cap) * job->stage.pitch, "%s: insufficient device memory for a class-major copy of the %u-sample genotype stage", fn, job->sample_ct) ||
+        perm.alloc(job->stage_variants, "%s: insufficient device memory", fn))
+      return 1;
+    job->d_raw_grouped = std::move(raw);
+    job->d_perm = std::move(perm);
   }
+  const uint64_t w_row = 4ull * job->score_ct;
+  const uint32_t pitch16 = job->stage.pitch / 16;
+  std::vector<uint32_t> perm, first(job->class_ct + 1);
+  std::vector<double> w4, w4h;
+  std::vector<uint8_t> d4, pcs;
+  for (uint32_t done = 0; done < variant_ct;) {
+    // one staged batch in the caller's order; its entries grouped by class on the device, stably, with the tables
+    // in the same order
+    const uint32_t cur = std::min(job->stage_variants, variant_ct - done);
+    const uint32_t* cls = entry_classes + done;
+    std::fill(first.begin(), first.end(), 0u);
+    for (uint32_t e = 0; e < cur; ++e) ++first[cls[e] + 1];
+    for (uint32_t k = 0; k < job->class_ct; ++k) first[k + 1] += first[k];
+    perm.resize(cur);
+    {
+      std::vector<uint32_t> next(first.begin(), first.end() - 1);
+      for (uint32_t e = 0; e < cur; ++e) perm[next[cls[e]]++] = done + e;
+    }
+    w4.resize(w_row * cur);
+    d4.resize(cur);
+    pcs.assign(cur, kPl2ScoreDiploid);
+    const bool any_hap = ploidy_classes && std::any_of(ploidy_classes + done, ploidy_classes + done + cur, [](uint8_t pc) { return pc != kPl2ScoreDiploid; });
+    if (any_hap) w4h.assign(w_row * cur, 0.0);
+    for (uint32_t r = 0; r < cur; ++r) {
+      const uint32_t e = perm[r];
+      std::copy_n(weights4_diploid + w_row * e, w_row, w4.data() + w_row * r);
+      d4[r] = named_dosages[e];
+      if (ploidy_classes) pcs[r] = ploidy_classes[e];
+      if (any_hap && pcs[r] != kPl2ScoreDiploid) std::copy_n(weights4_haploid + w_row * e, w_row, w4h.data() + w_row * r);
+      perm[r] = e - done;
+    }
+    uint32_t padded = 0;
+    PL2_TRY(StageUpload(c, &job->stage, src + static_cast<uint64_t>(done) * variant_stride_bytes, variant_stride_bytes, cur, src_is_device, &padded));
+    PL2_CUDA_OK(cudaMemcpyAsync(job->d_perm, perm.data(), 4ull * cur, cudaMemcpyHostToDevice, c->stream));
+    PL2_CUDA_OK(cudaMemcpyAsync(job->d_w4, w4.data(), 8 * w_row * cur, cudaMemcpyHostToDevice, c->stream));
+    if (any_hap) PL2_CUDA_OK(cudaMemcpyAsync(job->d_w4h, w4h.data(), 8 * w_row * cur, cudaMemcpyHostToDevice, c->stream));
+    PL2_CUDA_OK(cudaMemcpyAsync(job->d_d4, d4.data(), cur, cudaMemcpyHostToDevice, c->stream));
+    score_row_gather_kernel<<<dim3(std::min(DivUpU32(pitch16, 256), 64u), cur), 256, 0, c->stream>>>(reinterpret_cast<const uint4*>(job->stage.d_raw.get()), reinterpret_cast<uint4*>(job->d_raw_grouped.get()), pitch16, job->d_perm);
+    ++c->launches;
+    PL2_CUDA_OK(cudaGetLastError());
+    // each class's block, in runs of one ploidy class, through the kernels and launch plan of the plain path
+    for (uint32_t k = 0; k < job->class_ct; ++k) {
+      for (uint32_t r0 = first[k]; r0 < first[k + 1];) {
+        uint32_t r1 = r0 + 1;
+        while (r1 < first[k + 1] && pcs[r1] == pcs[r0]) ++r1;
+        PL2_TRY(ScoreLaunchRun(job, job->d_raw_grouped.get() + static_cast<uint64_t>(r0) * job->stage.pitch, r1 - r0, job->d_w4 + w_row * r0, job->d_w4h ? job->d_w4h + w_row * r0 : nullptr, job->d_d4 + r0, pcs[r0], k));
+        r0 = r1;
+      }
+    }
+    PL2_CUDA_OK(cudaStreamSynchronize(c->stream));  // host tables and a host source may be reused by the caller
+    job->entries += cur;
+    done += cur;
+  }
+  return 0;
+}
+
+int pl2gpu_score_get_class(Pl2ScoreJob* job, uint32_t class_idx, double* score_sums, uint64_t* named_half_dosage_sums, uint32_t* missing_diploid_cts, uint32_t* missing_haploid_cts) {
+  if (!job || !score_sums || class_idx >= job->class_ct) {
+    set_error("pl2gpu_score_get_class: bad arguments");
+    return 1;
+  }
+  const uint32_t n = job->sample_ct;
+  const uint64_t acc = static_cast<uint64_t>(class_idx) * job->stage.sample_ct_padded;
+  std::vector<uint64_t> dos(n), hdos(n, 0);
+  Ctx* c = &job->ctx->c;
+  PL2_CUDA_OK(cudaSetDevice(c->device));
+  PL2_CUDA_OK(cudaMemcpyAsync(score_sums, job->d_acc_sum + acc * job->score_ct, 8ull * n * job->score_ct, cudaMemcpyDeviceToHost, c->stream));
+  PL2_CUDA_OK(cudaMemcpyAsync(dos.data(), job->d_acc_dos + acc, 8ull * n, cudaMemcpyDeviceToHost, c->stream));
+  if (missing_diploid_cts) PL2_CUDA_OK(cudaMemcpyAsync(missing_diploid_cts, job->d_acc_miss + acc, 4ull * n, cudaMemcpyDeviceToHost, c->stream));
+  if (job->d_acc_hdos) {
+    PL2_CUDA_OK(cudaMemcpyAsync(hdos.data(), job->d_acc_hdos + acc, 8ull * n, cudaMemcpyDeviceToHost, c->stream));
+    if (missing_haploid_cts) PL2_CUDA_OK(cudaMemcpyAsync(missing_haploid_cts, job->d_acc_miss_hap + acc, 4ull * n, cudaMemcpyDeviceToHost, c->stream));
+  } else if (missing_haploid_cts) {
+    std::fill(missing_haploid_cts, missing_haploid_cts + n, 0u);
+  }
+  PL2_CUDA_OK(cudaStreamSynchronize(c->stream));
+  if (named_half_dosage_sums)
+    for (uint32_t s = 0; s < n; ++s) named_half_dosage_sums[s] = 2 * dos[s] + hdos[s];
   return 0;
 }
 
@@ -666,20 +839,7 @@ int pl2gpu_score_get_ploidy(Pl2ScoreJob* job, double* score_sums, uint64_t* name
     set_error("pl2gpu_score_get_ploidy: bad arguments");
     return 1;
   }
-  const uint32_t n = job->sample_ct;
-  std::vector<uint64_t> dos(n), hdos(n, 0);
-  PL2_TRY(pl2gpu_score_get(job, score_sums, dos.data(), missing_diploid_cts));
-  Ctx* c = &job->ctx->c;
-  if (job->d_acc_hdos) {
-    PL2_CUDA_OK(cudaMemcpyAsync(hdos.data(), job->d_acc_hdos, 8ull * n, cudaMemcpyDeviceToHost, c->stream));
-    if (missing_haploid_cts) PL2_CUDA_OK(cudaMemcpyAsync(missing_haploid_cts, job->d_acc_miss_hap, 4ull * n, cudaMemcpyDeviceToHost, c->stream));
-    PL2_CUDA_OK(cudaStreamSynchronize(c->stream));
-  } else if (missing_haploid_cts) {
-    std::fill(missing_haploid_cts, missing_haploid_cts + n, 0u);
-  }
-  if (named_half_dosage_sums)
-    for (uint32_t s = 0; s < n; ++s) named_half_dosage_sums[s] = 2 * dos[s] + hdos[s];
-  return 0;
+  return pl2gpu_score_get_class(job, 0, score_sums, named_half_dosage_sums, missing_diploid_cts, missing_haploid_cts);
 }
 
 int pl2gpu_score_get(Pl2ScoreJob* job, double* score_sums, uint64_t* named_dosage_sums, uint32_t* missing_cts) {
