@@ -328,6 +328,14 @@ int pl2gpu_score_begin_classes(Pl2GpuCtx* ctx, uint32_t sample_ct, uint32_t scor
 int pl2gpu_score_add_variants_classes(Pl2ScoreJob* job, const void* genovecs, uint64_t variant_stride_bytes, uint32_t variant_ct, int src_is_device, const uint32_t* entry_classes, const uint8_t* ploidy_classes,
                                       const double* weights4_diploid, const double* weights4_haploid, const uint8_t* named_dosages);
 int pl2gpu_score_get_class(Pl2ScoreJob* job, uint32_t class_idx, double* score_sums, uint64_t* named_half_dosage_sums, uint32_t* missing_diploid_cts, uint32_t* missing_haploid_cts);
+/* Entries that share staged rows (--score-list: a variant scored by several files, one class per file and range set).
+ * genovecs holds row_ct rows; entry e reads row entry_rows[e] (non-decreasing, < row_ct; a row may have several
+ * entries, in any classes), and its class, ploidy class and tables are those of pl2gpu_score_add_variants_classes.
+ * Each row is uploaded once per call and copied on the device once per entry that reads it; a batch holds whole rows,
+ * at most 16,384 rows and as many entries, so one row may have at most that many entries.  A call with one entry per
+ * row (entry_rows[e] = e) does exactly the work of pl2gpu_score_add_variants_classes and gives bit-identical sums. */
+int pl2gpu_score_add_entries(Pl2ScoreJob* job, const void* genovecs, uint64_t variant_stride_bytes, uint32_t row_ct, int src_is_device, uint32_t entry_ct, const uint32_t* entry_rows, const uint32_t* entry_classes,
+                             const uint8_t* ploidy_classes, const double* weights4_diploid, const double* weights4_haploid, const uint8_t* named_dosages);
 
 /* ---- measured tensor peak: two warpgroups per SM issue back-to-back wgmmas with A fragments in registers and B in
  * shared memory, as the KING/GRM kernels use them, for at least min_seconds.  form 1: int8 (M = 64, N = n_cols in

@@ -94,8 +94,10 @@ struct Cmd {
   bool freq = false;                      // --freq
   std::string indep_preferred;            // --indep-preferred <file of variant IDs>
   std::string read_freq;                  // --read-freq <PLINK 2 --freq report>
-  // --score <file> [i] [j] [k] [header | header-read] [no-mean-imputation] [zs] [cols=]
+  // --score <file> [i] [j] [k] [header | header-read] [no-mean-imputation] [zs] [ignore-dup-ids] [cols=]; with
+  // --score-list, score_file names a list of score files (score_list)
   std::string score_file;
+  bool score_list = false, score_ignore_dup_ids = false;
   uint32_t score_id_col = 1, score_allele_col = 2, score_coef_col = 3, score_numeric_params = 0;
   std::vector<uint32_t> score_col_nums;   // --score-col-nums: 1-based coefficient columns, increasing, no duplicates
   // --q-score-range <range file> <data file> [i] [j] ['header'] ['min']: variant IDs from column i, p-values from j
@@ -425,10 +427,15 @@ int ParseArgs(int argc, char** argv, Cmd* c) {
         else return Usage("--freq modifiers other than 'zs' and 'counts' (cols=, bins) are not supported by plink2_b200.");
       }
       c->freq = true;
-    } else if (flag == "--score") {
-      // plink2.cc --score parsing: filename, up to three 1-based column numbers, then modifiers
-      if (nparam < 1) return Usage("--score requires a filename.");
+    } else if (flag == "--score" || flag == "--score-list") {
+      // plink2.cc --score / --score-list parsing (:11453-11570): filename, up to three 1-based column numbers, then
+      // modifiers.  --score-list keeps the reference's wording for its refusals.
+      const bool list = flag == "--score-list";
+      if (nparam < 1) return Usage(list ? "--score-list requires a filename." : "--score requires a filename.");
+      if (!c->score_file.empty() && list != c->score_list) return Usage("--score-list cannot be used with --score.");
       c->score_file = prm[0];
+      c->score_list = list;
+      if (list) c->sc_nallele = c->sc_dosagesum = false;  // kfScoreListColDefault: maybefid, maybesid, phenos, scoreavgs
       int k = 1;
       uint32_t nums[3], nnum = 0;
       while (k < nparam && nnum < 3 && ParseU32(prm[k], &nums[nnum]) && nums[nnum]) ++nnum, ++k;
@@ -436,17 +443,19 @@ int ParseArgs(int argc, char** argv, Cmd* c) {
       c->score_allele_col = nnum >= 2 ? nums[1] : c->score_id_col + 1;
       c->score_coef_col = nnum >= 3 ? nums[2] : c->score_allele_col + 1;
       c->score_numeric_params = nnum;
+      uint32_t model_bits = 0;  // center, variance-standardize, dominant, recessive
       for (; k < nparam; ++k) {
         const std::string m = prm[k];
         if (m == "header") c->score_header = true;
         else if (m == "header-read") c->score_header_read = true;
         else if (m == "no-mean-imputation") c->score_no_meanimpute = true;
-        else if (m == "center") c->score_center = true;
-        else if (m == "variance-standardize") c->score_center = c->score_varstd = true;
-        else if (m == "dominant") c->score_dominant = true;
-        else if (m == "recessive") c->score_recessive = true;
+        else if (m == "center") c->score_center = true, model_bits |= 1;
+        else if (m == "variance-standardize") c->score_center = c->score_varstd = true, model_bits |= 2;
+        else if (m == "dominant") c->score_dominant = true, model_bits |= 4;
+        else if (m == "recessive") c->score_recessive = true, model_bits |= 8;
         else if (m == "list-variants") c->score_list_variants = true;
         else if (m == "zs") c->score_zs = true;
+        else if (m == "ignore-dup-ids") c->score_ignore_dup_ids = true;
         else if (m.compare(0, 5, "cols=") == 0) {
           // column-set descriptor: a plain list replaces the default, +x / -x entries edit it
           const std::string spec = m.substr(5);
@@ -480,9 +489,17 @@ int ParseArgs(int argc, char** argv, Cmd* c) {
             else if (tok == "scoresums") c->sc_sums = on;
             else return Usage(("Invalid --score cols= entry '" + tok + "'.").c_str());
           }
+          if (list && (c->sc_nallele || c->sc_denom || c->sc_dosagesum)) return Usage("--score-list cannot be used with the nallele, denom, or dosagesum\ncolumn-sets.");
+        } else if (list) {
+          return Usage(("--score-list modifier '" + m + "' is not supported by plink2_b200 (supported: header, header-read, center, variance-standardize, dominant, recessive, no-mean-imputation, zs, ignore-dup-ids, cols=).").c_str());
         } else {
-          return Usage(("--score modifier '" + m + "' is not supported by plink2_b200 (supported: header, header-read, center, variance-standardize, dominant, recessive, no-mean-imputation, list-variants, zs, cols=).").c_str());
+          return Usage(("--score modifier '" + m + "' is not supported by plink2_b200 (supported: header, header-read, center, variance-standardize, dominant, recessive, no-mean-imputation, list-variants, zs, ignore-dup-ids, cols=).").c_str());
         }
+      }
+      if (list) {
+        if (c->score_header && c->score_header_read) return Usage("--score[-list] 'header' and 'header-read' modifiers cannot be used\ntogether.");
+        if (model_bits & (model_bits - 1)) return Usage("--score[-list] 'dominant', 'recessive', 'center', and\n'variance-standardize' modifiers are mutually exclusive.");
+        if (c->score_list_variants) return Usage("'list-variants[-zs]' modifier can only be used with --score, not\n--score-list.");
       }
       if (c->score_header && c->score_header_read) return Usage("--score 'header' and 'header-read' modifiers cannot be used together.");
       if ((c->score_dominant || c->score_recessive) && (c->score_center || (c->score_dominant && c->score_recessive))) return Usage("--score 'dominant' / 'recessive' cannot be combined with each other or with 'center' / 'variance-standardize'.");
@@ -2927,21 +2944,52 @@ int LoadQsr(const Cmd& c, const VariantInfo& V, const std::unordered_map<std::st
   return 0;
 }
 
-// `--score` (ScoreReport, 2.0/plink2_matrix_calc.cc:6892-9270) for hard calls: default report columns plus
-// denom / scoresums, 'header' / 'header-read', 'no-mean-imputation', and any number of coefficient columns
-// (--score-col-nums).  chrX, chrY and MT entries are scored with the reference's sex-dependent ploidy (--xchr-model 2:
-// chrX like an autosome; 1: chrX males haploid).  The per-sample sums of every column come from one device pass
-// (pl2gpu_score_*); the file parsing, allele matching, mean-imputation weights and the report are here.
+// --score-list (ScoreListLoad, 2.0/plink2_matrix_calc.cc:6332): the first token of each line names a score file, as
+// written; like the reference, the list ends at its first line without a token.
+int LoadScoreList(const std::string& list, std::vector<std::string>* files) {
+  std::vector<std::string> lines;
+  std::string err;
+  if (!ReadLines(list, &lines, &err)) {
+    logprintf("Error: %s\n", err.c_str());
+    return kRetOpenFail;
+  }
+  for (const std::string& ln : lines) {
+    const std::vector<std::string> t = SplitWs(ln);
+    if (t.empty()) break;
+    files->push_back(t[0]);
+  }
+  if (files->empty()) {
+    logprintf("Error: --score-list: %s is empty.\n", list.c_str());
+    return kRetMalformedInput;
+  }
+  return 0;
+}
+
+// `--score` and `--score-list` (ScoreReport, 2.0/plink2_matrix_calc.cc:6892-9270) for hard calls: default report
+// columns plus denom / scoresums, 'header' / 'header-read', 'no-mean-imputation', 'ignore-dup-ids', and any number of
+// coefficient columns (--score-col-nums).  chrX, chrY and MT entries are scored with the reference's sex-dependent
+// ploidy (--xchr-model 2: chrX like an autosome; 1: chrX males haploid).  The per-sample sums of every column come from
+// one device pass (pl2gpu_score_*); the file parsing, allele matching, mean-imputation weights and the report are here.
+// Each file of a --score-list has its own score columns and its own denominators (:7324, :8389): its entries form
+// classes of their own, and a variant several files score is staged once and gathered once per entry on the device.
 int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   const SampleInfo& S = ds->samples;
   const VariantInfo& V = ds->variants;
   const uint32_t n = S.size();
+  const char* flagname = c.score_list ? "--score-list" : "--score";
+  std::vector<std::string> files;
   std::vector<std::string> lines;
   std::string err;
-  if (!ReadLines(c.score_file, &lines, &err)) {
-    logprintf("Error: %s\n", err.c_str());
-    return kRetOpenFail;
+  if (c.score_list) {
+    if (int rc = LoadScoreList(c.score_file, &files)) return rc;
+  } else {
+    files.push_back(c.score_file);
+    if (!ReadLines(c.score_file, &lines, &err)) {
+      logprintf("Error: %s\n", err.c_str());
+      return kRetOpenFail;
+    }
   }
+  const uint32_t file_ct = static_cast<uint32_t>(files.size());
   std::unordered_map<std::string, uint32_t> by_id;
   std::unordered_map<std::string, uint32_t> dup;
   by_id.reserve(static_cast<size_t>(V.size()) * 2);
@@ -2959,105 +3007,146 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
     uint32_t v;
     uint8_t aidx;  // 0 = REF named, 1 = ALT named
     size_t coef_row;  // coefficients at coefs[coef_row * score_ct ...]
+    uint32_t file;    // index in the --score-list (0 for --score)
   };
   std::vector<Entry> entries;
   std::vector<double> coefs;
-  std::vector<uint8_t> seen(2ull * V.size(), 0);
+  std::vector<uint8_t> seen;
   const bool y_prohibited = !c.score_no_meanimpute && std::find(S.sex.begin(), S.sex.end(), 0) != S.sex.end();
-  uint64_t missing_id = 0, missing_allele = 0;
   // coefficient columns in file order (1-based); without --score-col-nums the one column --score names
   const std::vector<uint32_t> score_cols = c.score_col_nums.empty() ? std::vector<uint32_t>{c.score_coef_col} : c.score_col_nums;
   const uint32_t score_ct = static_cast<uint32_t>(score_cols.size());
   const uint32_t need_cols = std::max({c.score_id_col, c.score_allele_col, score_cols.back()});
-  // names: the header tokens with 'header-read', else SCORE1 .. by position in the column list (:7620-7672)
-  std::vector<std::string> score_names(score_ct);
-  for (uint32_t j = 0; j < score_ct; ++j) score_names[j] = "SCORE" + std::to_string(j + 1);
-  size_t li = 0;
-  if ((c.score_header || c.score_header_read) && !lines.empty()) {
-    if (c.score_header_read) {
-      const std::vector<std::string> h = SplitWs(lines[0]);
-      if (h.size() < need_cols) {
-        logprintf("Error: Line 1 of --score file has fewer tokens than expected.\n");
+  // names, file by file: the header tokens with 'header-read', else SCORE1 .. by position in all the files' columns
+  // (:7620-7672)
+  std::vector<std::string> score_names(static_cast<size_t>(file_ct) * score_ct);
+  for (size_t j = 0; j < score_names.size(); ++j) score_names[j] = "SCORE" + std::to_string(j + 1);
+  std::vector<size_t> file_processed(file_ct, 0);
+  for (uint32_t f = 0; f < file_ct; ++f) {
+    const std::string& fname = files[f];
+    // a --score file is described as such in messages, a --score-list file by its name (:8683)
+    const std::string fdesc = c.score_list ? fname : "--score file";
+    if (c.score_list) {
+      lines.clear();
+      if (!ReadLines(fname, &lines, &err)) {
+        logprintf("Error: %s\n", err.c_str());
+        return kRetOpenFail;
+      }
+      if (std::all_of(lines.begin(), lines.end(), [](const std::string& ln) { return SplitWs(ln).empty(); })) {
+        logprintf("Error: --score-list: %s is empty.\n", fname.c_str());
         return kRetMalformedInput;
       }
-      for (uint32_t j = 0; j < score_ct; ++j) score_names[j] = h[score_cols[j] - 1];
-      std::vector<std::string> sorted_names(score_names);
-      std::sort(sorted_names.begin(), sorted_names.end());
-      if (std::adjacent_find(sorted_names.begin(), sorted_names.end()) != sorted_names.end()) {
-        logprintf("Error: --score: Score IDs are not unique.\n");
+    }
+    seen.assign(2ull * V.size(), 0);
+    uint64_t missing_id = 0, missing_allele = 0, dup_id = 0;
+    const size_t file_first = entries.size();
+    size_t li = 0;
+    if ((c.score_header || c.score_header_read) && !lines.empty()) {
+      if (c.score_header_read) {
+        const std::vector<std::string> h = SplitWs(lines[0]);
+        if (h.size() < need_cols) {
+          logprintf("Error: Line 1 of %s has fewer tokens than expected.\n", fdesc.c_str());
+          return kRetMalformedInput;
+        }
+        for (uint32_t j = 0; j < score_ct; ++j) score_names[static_cast<size_t>(f) * score_ct + j] = h[score_cols[j] - 1];
+        // the reference checks the first file's names (:7655-7668)
+        std::vector<std::string> sorted_names(score_names.begin(), score_names.begin() + score_ct);
+        std::sort(sorted_names.begin(), sorted_names.end());
+        if (f == 0 && std::adjacent_find(sorted_names.begin(), sorted_names.end()) != sorted_names.end()) {
+          logprintf("Error: %s: Score IDs are not unique.\n", flagname);
+          return kRetMalformedInput;
+        }
+      }
+      li = 1;
+    }
+    for (; li < lines.size(); ++li) {
+      if (lines[li].empty()) continue;
+      const std::vector<std::string> t = SplitWs(lines[li]);
+      if (t.empty()) continue;
+      // the ID and allele tokens are needed first; the coefficients only on lines that are scored (:7712-7790)
+      if (t.size() < std::max(c.score_id_col, c.score_allele_col)) {
+        logprintf("Error: Line %zu of %s has fewer tokens than expected.\n", li + 1, fdesc.c_str());
         return kRetMalformedInput;
       }
-    }
-    li = 1;
-  }
-  for (; li < lines.size(); ++li) {
-    if (lines[li].empty()) continue;
-    const std::vector<std::string> t = SplitWs(lines[li]);
-    if (t.empty()) continue;
-    // the ID and allele tokens are needed first; the coefficients only on lines that are scored (:7712-7790)
-    if (t.size() < std::max(c.score_id_col, c.score_allele_col)) {
-      logprintf("Error: Line %zu of --score file has fewer tokens than expected.\n", li + 1);
-      return kRetMalformedInput;
-    }
-    const std::string& id = t[c.score_id_col - 1];
-    const auto it = by_id.find(id);
-    if (it == by_id.end()) {
-      ++missing_id;
-      continue;
-    }
-    if (dup.count(id)) {
-      logprintf("Error: --score variant ID '%s' appears multiple times in main dataset.\n", id.c_str());
-      return kRetInconsistentInput;
-    }
-    const uint32_t v = it->second;
-    const std::string& al = t[c.score_allele_col - 1];
-    uint8_t aidx;
-    if (al == V.ref[v]) aidx = 0;
-    else if (al == V.alt[v]) aidx = 1;
-    else {
-      ++missing_allele;
-      continue;
-    }
-    if (seen[2ull * v + aidx]) {
-      logprintf("Error: --score: %s allele for variant '%s' appears multiple times in %s file.\n", aidx ? "ALT1" : "REF", id.c_str(), c.score_file.c_str());
-      return kRetMalformedInput;
-    }
-    seen[2ull * v + aidx] = 1;
-    if (t.size() < need_cols) {
-      logprintf("Error: Line %zu of --score file has fewer tokens than expected.\n", li + 1);
-      return kRetMalformedInput;
-    }
-    for (const uint32_t col : score_cols) {
-      double coef;
-      if (!ParseDouble(t[col - 1].c_str(), &coef)) {
-        logprintf("Error: Line %zu of --score file has an invalid coefficient.\n", li + 1);
+      const std::string& id = t[c.score_id_col - 1];
+      const auto it = by_id.find(id);
+      if (it == by_id.end()) {
+        ++missing_id;
+        continue;
+      }
+      if (dup.count(id)) {
+        if (!c.score_ignore_dup_ids) {
+          logprintf("Error: %s variant ID '%s' appears multiple times in main dataset.\n", flagname, id.c_str());
+          return kRetInconsistentInput;
+        }
+        ++dup_id;  // 'ignore-dup-ids' (:7724)
+        continue;
+      }
+      const uint32_t v = it->second;
+      const std::string& al = t[c.score_allele_col - 1];
+      uint8_t aidx;
+      if (al == V.ref[v]) aidx = 0;
+      else if (al == V.alt[v]) aidx = 1;
+      else {
+        ++missing_allele;
+        continue;
+      }
+      if (seen[2ull * v + aidx]) {
+        logprintf("Error: %s: %s allele for variant '%s' appears multiple times in %s%s file.\n", flagname, aidx ? "ALT1" : "REF", id.c_str(), fname.c_str(), c.score_list ? "-list" : "");
         return kRetMalformedInput;
       }
-      coefs.push_back(coef);
+      seen[2ull * v + aidx] = 1;
+      if (t.size() < need_cols) {
+        logprintf("Error: Line %zu of %s has fewer tokens than expected.\n", li + 1, fdesc.c_str());
+        return kRetMalformedInput;
+      }
+      for (const uint32_t col : score_cols) {
+        double coef;
+        if (!ParseDouble(t[col - 1].c_str(), &coef)) {
+          logprintf("Error: Line %zu of %s has an invalid coefficient.\n", li + 1, fdesc.c_str());
+          return kRetMalformedInput;
+        }
+        coefs.push_back(coef);
+      }
+      // the reference's refusals for haploid chromosomes (:7794-7814)
+      const uint32_t chr = V.chr_code[v];
+      if ((chr == 23 || chr == 24 || chr == 26) && (c.score_dominant || c.score_recessive)) {
+        logprintf("Error: --score[-list] 'dominant' and 'recessive' modifiers cannot be used with\nhaploid chromosomes.\n");
+        return kRetInconsistentInput;
+      }
+      if ((chr == 23 || chr == 26) && c.score_varstd) {
+        logprintf("Error: --score[-list] 'variance-standardize' cannot be used with chrX or MT.\n");
+        return kRetInconsistentInput;
+      }
+      if (chr == 24 && y_prohibited) {
+        logprintf("Error: When both chrY variants and unknown-sex samples are present,\n--score[-list] can only be run with the 'no-mean-imputation' modifier.\n");
+        return kRetInconsistentInput;
+      }
+      entries.push_back({v, aidx, entries.size(), f});
     }
-    // the reference's refusals for haploid chromosomes (:7794-7814)
-    const uint32_t chr = V.chr_code[v];
-    if ((chr == 23 || chr == 24 || chr == 26) && (c.score_dominant || c.score_recessive)) {
-      logprintf("Error: --score[-list] 'dominant' and 'recessive' modifiers cannot be used with\nhaploid chromosomes.\n");
-      return kRetInconsistentInput;
+    if (!c.score_list) {
+      if (missing_id || missing_allele) {
+        logprintf("Warning: --score: %llu entr%s in %s %s skipped due to missing variant IDs, and %llu %s skipped due to mismatching allele codes.\n", static_cast<unsigned long long>(missing_id), missing_id == 1 ? "y" : "ies",
+                  c.score_file.c_str(), missing_id == 1 ? "was" : "were", static_cast<unsigned long long>(missing_allele), missing_allele == 1 ? "was" : "were");
+      }
+    } else if (missing_id && missing_allele) {  // the reference's three forms (:8239-8280)
+      logprintf("Warning: --score-list: %llu entr%s in %s %s skipped due to %s, and %llu %s skipped due to %s.\n", static_cast<unsigned long long>(missing_id), missing_id == 1 ? "y" : "ies", fname.c_str(), missing_id == 1 ? "was" : "were",
+                missing_id == 1 ? "a missing variant ID" : "missing variant IDs", static_cast<unsigned long long>(missing_allele), missing_allele == 1 ? "was" : "were", missing_allele == 1 ? "a mismatching allele code" : "mismatching allele codes");
+    } else if (missing_id || missing_allele) {
+      const uint64_t ct = missing_id + missing_allele;
+      logprintf("Warning: --score-list: %llu entr%s in %s %s skipped due to %s.\n", static_cast<unsigned long long>(ct), ct == 1 ? "y" : "ies", fname.c_str(), ct == 1 ? "was" : "were",
+                missing_id ? (ct == 1 ? "a missing variant ID" : "missing variant IDs") : (ct == 1 ? "a mismatching allele code" : "mismatching allele codes"));
     }
-    if ((chr == 23 || chr == 26) && c.score_varstd) {
-      logprintf("Error: --score[-list] 'variance-standardize' cannot be used with chrX or MT.\n");
-      return kRetInconsistentInput;
+    if (dup_id) {
+      logprintf("Warning: %s: %llu entr%s in %s %s skipped since %s multiple times in the main dataset.\n", flagname, static_cast<unsigned long long>(dup_id), dup_id == 1 ? "y" : "ies", fname.c_str(), dup_id == 1 ? "was" : "were",
+                dup_id == 1 ? "its variant ID appears" : "their variant IDs appear");
     }
-    if (chr == 24 && y_prohibited) {
-      logprintf("Error: When both chrY variants and unknown-sex samples are present,\n--score[-list] can only be run with the 'no-mean-imputation' modifier.\n");
-      return kRetInconsistentInput;
+    if (entries.size() == file_first) {
+      if (c.score_list) logprintf("Error: --score-list: No valid variants in %s.\n", fname.c_str());
+      else logprintf("Error: No valid variants in --score file.\n");
+      return kRetDegenerateData;
     }
-    entries.push_back({v, aidx, entries.size()});
-  }
-  if (missing_id || missing_allele) {
-    logprintf("Warning: --score: %llu entr%s in %s %s skipped due to missing variant IDs, and %llu %s skipped due to mismatching allele codes.\n", static_cast<unsigned long long>(missing_id), missing_id == 1 ? "y" : "ies",
-              c.score_file.c_str(), missing_id == 1 ? "was" : "were", static_cast<unsigned long long>(missing_allele), missing_allele == 1 ? "was" : "were");
-  }
-  if (entries.empty()) {
-    logprintf("Error: No valid variants in --score file.\n");
-    return kRetDegenerateData;
+    file_processed[f] = entries.size() - file_first;
   }
   // <out>.sscore.vars lists the variants in score-file order, each once (:7790-7800)
   std::vector<uint32_t> file_order;
@@ -3070,36 +3159,50 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
       }
     }
   }
-  // device passes run in variant order (sums are order-independent up to fp64 rounding; the device adds in a fixed order)
+  // device passes run in variant order (sums are order-independent up to fp64 rounding; the device adds in a fixed
+  // order); a variant's entries stay in list order
   std::stable_sort(entries.begin(), entries.end(), [](const Entry& a, const Entry& b) { return a.v < b.v; });
-  const size_t processed_ct = entries.size();
-  // --q-score-range classes: entries whose variant lies in the same set of ranges share a class (numbered in variant
-  // order); each range is the union of its classes.  Entries in no range are dropped here.
-  std::vector<uint32_t> entry_class;                // per entry
-  std::vector<std::vector<uint8_t>> class_ranges;  // per class: 1 for each range it lies in
-  if (qsr) {
-    std::map<std::vector<uint8_t>, uint32_t> class_of;
+  // classes: one per file, split further under --q-score-range into the entries whose variant lies in the same set of
+  // ranges (numbered in variant order); each range of a file is the union of its classes.  Entries in no range are
+  // dropped here.
+  std::vector<uint32_t> entry_class(entries.size(), 0);  // per entry
+  std::vector<uint32_t> class_file;                     // per class
+  std::vector<std::vector<uint8_t>> class_ranges;      // per class: 1 for each range it lies in
+  {
+    std::map<std::pair<uint32_t, std::vector<uint8_t>>, uint32_t> class_of;
     std::vector<Entry> kept;
+    std::vector<uint32_t> kept_class;
     for (const Entry& e : entries) {
-      if (!qsr_seen[e.v]) continue;
       std::vector<uint8_t> in(ranges.size(), 0);
-      bool any = false;
-      for (size_t r = 0; r < ranges.size(); ++r) {
-        in[r] = !(qsr_p[e.v] < ranges[r].lb || qsr_p[e.v] > ranges[r].ub);
-        any = any || in[r];
+      if (qsr) {
+        if (!qsr_seen[e.v]) continue;
+        bool any = false;
+        for (size_t r = 0; r < ranges.size(); ++r) {
+          in[r] = !(qsr_p[e.v] < ranges[r].lb || qsr_p[e.v] > ranges[r].ub);
+          any = any || in[r];
+        }
+        if (!any) continue;
       }
-      if (!any) continue;
-      const auto it = class_of.emplace(in, static_cast<uint32_t>(class_ranges.size()));
-      if (it.second) class_ranges.push_back(in);
-      entry_class.push_back(it.first->second);
+      const auto it = class_of.emplace(std::make_pair(e.file, in), static_cast<uint32_t>(class_ranges.size()));
+      if (it.second) {
+        class_ranges.push_back(in);
+        class_file.push_back(e.file);
+      }
+      kept_class.push_back(it.first->second);
       kept.push_back(e);
     }
     entries.swap(kept);
+    entry_class.swap(kept_class);
   }
-  const uint32_t class_ct = qsr ? std::max<uint32_t>(1, static_cast<uint32_t>(class_ranges.size())) : 1;
-  std::vector<uint32_t> vidx(entries.size());
-  for (size_t k = 0; k < entries.size(); ++k) vidx[k] = entries[k].v;
-  // named-allele frequencies for the mean imputation: founders (ComputeAlleleFreqs), --read-freq values first
+  const uint32_t class_ct = std::max<uint32_t>(1, static_cast<uint32_t>(class_ranges.size()));
+  const bool class_job = qsr || c.score_list;
+  // staged rows: one per entry for --score (the rows are the entries), one per variant for --score-list
+  std::vector<uint32_t> vidx, entry_row(entries.size());
+  for (size_t k = 0; k < entries.size(); ++k) {
+    if (!c.score_list || vidx.empty() || vidx.back() != entries[k].v) vidx.push_back(entries[k].v);
+    entry_row[k] = static_cast<uint32_t>(vidx.size() - 1);
+  }
+  // named-allele frequencies for the mean imputation (per row): founders (ComputeAlleleFreqs), --read-freq values first
   std::vector<double> ref_freqs;
   {
     int rc = 0;
@@ -3117,142 +3220,192 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   };
   bool ploidy_job = false;
   for (const Entry& e : entries) ploidy_job = ploidy_job || ploidy_class(e.v) != kPl2ScoreDiploid;
-  Pl2ScoreJob* job = nullptr;
-  if (qsr) {
-    if (pl2gpu_score_begin_classes(ctx, n, score_ct, class_ct, &job)) return GpuFail("pl2gpu_score_begin_classes");
-  } else if (score_ct == 1) {  // the one-column job (same device work as pl2gpu_score_begin_cols with one column)
-    if (pl2gpu_score_begin(ctx, n, &job)) return GpuFail("pl2gpu_score_begin");
-  } else if (pl2gpu_score_begin_cols(ctx, n, score_ct, &job)) {
-    return GpuFail("pl2gpu_score_begin_cols");
-  }
-  struct JobGuard {
-    Pl2ScoreJob* j;
-    ~JobGuard() { pl2gpu_score_end(j); }
-  } guard{job};
-  if (ploidy_job && pl2gpu_score_set_sex(job, S.sex.data())) return GpuFail("pl2gpu_score_set_sex");
-  BlockStreamer bs(ds, &vidx, n, 16384);
-  if (!bs.Init()) return GpuFail("pl2gpu_host_alloc");
-  std::vector<double> w4, w4h;  // diploid and haploid tables
-  std::vector<uint8_t> d4, cls;
-  std::vector<uint32_t> ecls;
-  std::vector<int64_t> repeat_miss(static_cast<uint64_t>(class_ct) * n, 0), repeat_miss_hap(static_cast<uint64_t>(class_ct) * n, 0);  // [class][sample]
-  size_t base = 0;
-  for (;;) {
-    const int got = bs.Next(&err);
-    if (got < 0) {
-      logprintf("Error: %s\n", err.c_str());
-      return kRetMalformedInput;
+  // class groups: the accumulators take class_ct x (8 score_ct + 24) bytes per padded sample.  When they do not all fit
+  // the device budget (free memory less 10 %, capped by --gpu-memory) next to the job's staging buffers, consecutive
+  // classes are scored in groups, one pass over the genotypes each.
+  std::vector<uint32_t> group_start{0, class_ct};
+  if (class_job && class_ct > 1) {
+    uint64_t free_b = 0, total_b = 0;
+    if (pl2gpu_ctx_mem_info(ctx, &free_b, &total_b)) return GpuFail("pl2gpu_ctx_mem_info");
+    uint64_t budget = free_b - free_b / 10;
+    if (c.gpu_memory_mib && (c.gpu_memory_mib << 20) < budget) budget = c.gpu_memory_mib << 20;
+    const uint64_t np = (n + 63) / 64 * 64;
+    const uint64_t staging = 2ull * 16384 * (np / 4) + np * 64 * (8ull * std::min(score_ct, 4u) + 12) + 16384ull * (64ull * score_ct + 5);
+    const uint64_t per_class = np * (8ull * score_ct + 24);
+    const uint64_t fit = budget > staging ? (budget - staging) / per_class : 0;
+    if (fit < class_ct) {
+      const uint32_t step = static_cast<uint32_t>(std::max<uint64_t>(fit, 1));
+      group_start.assign(1, 0);
+      for (uint32_t k = step; k < class_ct; k += step) group_start.push_back(k);
+      group_start.push_back(class_ct);
+      logprintf("%s: The accumulators of %u score classes do not fit in GPU memory together; scoring them in %zu passes over the genotypes.\n", flagname, class_ct, group_start.size() - 1);
     }
-    if (!got) break;
-    w4.resize(4ull * score_ct * got);
-    w4h.resize(4ull * score_ct * got);
-    d4.resize(got);
-    cls.resize(got);
-    ecls.resize(got);
-    for (int k = 0; k < got; ++k) {
-      const Entry& e = entries[base + k];
-      const uint64_t cbase = qsr ? static_cast<uint64_t>(ecls[k] = entry_class[base + k]) * n : 0;
-      const uint8_t pc = cls[k] = ploidy_class(e.v);
-      const double f_named = e.aidx ? (1.0 - ref_freqs[base + k]) : ref_freqs[base + k];
-      // genotype code = ALT allele count; named-allele dosage of codes 0, 1, 2.  The tables below do not depend on
-      // the column; each column scales them by its coefficient.  'center' / 'variance-standardize'
-      // (:8003-8033): dosage x slope + intercept with intercept = -p f slope and slope = 1 / sqrt(p / 2 x 2 f (1 - f))
-      // (0 when the variance is not above 2^-44), p the variant's ploidy: 1 on chrY and MT, else 2 (chrX too, whatever
-      // the model).  A missing call contributes (sample ploidy) f slope WITHOUT the intercept in the reference
-      // (missing_effect, :6756-6762, :6795-6836) - kept, since the outputs are compared with its files.
-      const uint32_t d0 = e.aidx ? 0 : 2, d2 = e.aidx ? 2 : 0;
-      const bool haploid_variant = pc == kPl2ScoreChrY || pc == kPl2ScoreHaploidAll;
-      double slope = 1.0, icpt = 0.0;
-      if (c.score_center) {
-        if (c.score_varstd) {
-          const double variance = (haploid_variant ? 0.5 : 1.0) * (2.0 * f_named * (1.0 - f_named));
-          if (!(variance > 1.0 / 17592186044416.0)) {
-            slope = 0.0;  // the reference additionally insists that such a variant is monomorphic (:8013-8027); a weight of 0 scores it the same
-          } else {
-            slope = 1.0 / sqrt(variance);
-          }
-        }
-        icpt = ((haploid_variant ? -1.0 : -2.0) * f_named) * slope;
-      }
-      // 'dominant' / 'recessive' (:6747-6762): copies -> min(copies, 1) / max(copies - 1, 0), a missing call -> ONE x f
-      uint32_t e0 = d0, e1 = 1, e2 = d2;
-      double miss_dosage = 2.0 * f_named;
-      if (c.score_dominant) {
-        e0 = d0 ? 1 : 0, e2 = d2 ? 1 : 0;
-        miss_dosage = f_named;
-      } else if (c.score_recessive) {
-        e0 = d0 ? 1 : 0, e1 = 0, e2 = d2 ? 1 : 0;
-        miss_dosage = f_named;
-      }
-      const double t0 = static_cast<double>(e0) * slope + icpt, t1 = static_cast<double>(e1) * slope + icpt, t2 = static_cast<double>(e2) * slope + icpt, t3 = miss_dosage * slope;
-      // a haploid sample (chrY nonfemales, MT, chrX males under --xchr-model 1) holds half the dosage of each code
-      const double h0 = (0.5 * e0) * slope + icpt, h1 = (0.5 * e1) * slope + icpt, h2 = (0.5 * e2) * slope + icpt, h3 = f_named * slope;
-      for (uint32_t j = 0; j < score_ct; ++j) {
-        const double coef = coefs[e.coef_row * score_ct + j];
-        double* w = &w4[4ull * (static_cast<uint64_t>(k) * score_ct + j)];
-        w[0] = coef * t0;
-        w[1] = coef * t1;
-        w[2] = coef * t2;
-        w[3] = c.score_no_meanimpute ? 0.0 : coef * t3;
-        if (pc == kPl2ScoreChrY) {  // the first table serves unknown-sex samples, whose chrY dosage the reference zeroes
-          w[0] = w[1] = w[2] = coef * icpt;
-          w[3] = c.score_no_meanimpute ? 0.0 : coef * h3;
-        }
-        double* wh = &w4h[4ull * (static_cast<uint64_t>(k) * score_ct + j)];
-        wh[0] = coef * h0;
-        wh[1] = coef * h1;
-        wh[2] = coef * h2;
-        wh[3] = c.score_no_meanimpute ? 0.0 : coef * h3;
-      }
-      d4[k] = static_cast<uint8_t>(e0 | (e1 << 2) | (e2 << 4));
-      // a file that names both alleles of a variant (PC projection with allele weights): the device counts the missing
-      // calls of both entries, the reference counts them once per variant (:7788), so the second entry's are taken
-      // back out here, from the diploid or haploid count the sample's class put them in
-      if (base + k > 0 && entries[base + k - 1].v == e.v) {
-        const uint64_t* row = bs.buf + static_cast<uint64_t>(k) * bs.words;
-        for (uint32_t w = 0; w < bs.words; ++w) {
-          uint64_t ms = row[w] & (row[w] >> 1) & 0x5555555555555555ull;
-          if (32ull * (w + 1) > n) ms &= (1ull << (2 * (n - 32 * w))) - 1;
-          for (; ms; ms &= ms - 1) {
-            const uint32_t s = 32 * w + __builtin_ctzll(ms) / 2;
-            const uint8_t sex = S.sex[s];
-            if (pc == kPl2ScoreDiploid || (pc == kPl2ScoreChrXMaleHaploid && sex != 1)) --repeat_miss[cbase + s];
-            else if (pc != kPl2ScoreChrY || sex != 2) --repeat_miss_hap[cbase + s];  // chrY females are not counted
-          }
-        }
-      }
-    }
-    if (qsr) {
-      if (pl2gpu_score_add_variants_classes(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0, ecls.data(), ploidy_job ? cls.data() : nullptr, w4.data(), w4h.data(), d4.data()))
-        return GpuFail("pl2gpu_score_add_variants_classes");
-    } else if (ploidy_job) {
-      if (pl2gpu_score_add_variants_ploidy(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0, cls.data(), w4.data(), w4h.data(), d4.data())) return GpuFail("pl2gpu_score_add_variants_ploidy");
-    } else if (pl2gpu_score_add_variants(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0, w4.data(), d4.data())) {
-      return GpuFail("pl2gpu_score_add_variants");
-    }
-    base += static_cast<size_t>(got);
   }
   // per class: score sums [sample][score_ct], named-allele dosage sums in half allele units, diploid and haploid
-  // missing calls (with the second entries of variants named by both alleles taken back out)
+  // missing calls (with the second entries of variants a file names by both alleles taken back out)
   std::vector<double> sums(static_cast<uint64_t>(class_ct) * n * score_ct);
   std::vector<uint64_t> hdos(static_cast<uint64_t>(class_ct) * n);
   std::vector<uint32_t> miss(static_cast<uint64_t>(class_ct) * n), miss_hap(static_cast<uint64_t>(class_ct) * n, 0);
-  if (qsr) {
-    for (uint32_t k = 0; k < class_ct; ++k) {
-      const uint64_t o = static_cast<uint64_t>(k) * n;
-      if (pl2gpu_score_get_class(job, k, sums.data() + o * score_ct, hdos.data() + o, miss.data() + o, miss_hap.data() + o)) return GpuFail("pl2gpu_score_get_class");
+  std::vector<int64_t> repeat_miss(static_cast<uint64_t>(class_ct) * n, 0), repeat_miss_hap(static_cast<uint64_t>(class_ct) * n, 0);  // [class][sample]
+  for (size_t g = 0; g + 1 < group_start.size(); ++g) {
+    const uint32_t k0 = group_start[g], k1 = group_start[g + 1];
+    // this group's entries (in entry order) and the rows they read
+    std::vector<size_t> gent;
+    std::vector<uint32_t> gvidx, grow;  // staged variants; per group entry, its row among them
+    for (size_t k = 0; k < entries.size(); ++k) {
+      if (entry_class[k] < k0 || entry_class[k] >= k1) continue;
+      if (gent.empty() || entry_row[k] != entry_row[gent.back()]) gvidx.push_back(entries[k].v);
+      gent.push_back(k);
+      grow.push_back(static_cast<uint32_t>(gvidx.size() - 1));
     }
-  } else if (ploidy_job) {
-    if (pl2gpu_score_get_ploidy(job, sums.data(), hdos.data(), miss.data(), miss_hap.data())) return GpuFail("pl2gpu_score_get_ploidy");
-  } else {
-    if (pl2gpu_score_get(job, sums.data(), hdos.data(), miss.data())) return GpuFail("pl2gpu_score_get");
-    for (uint64_t& d : hdos) d *= 2;
+    Pl2ScoreJob* job = nullptr;
+    if (class_job) {
+      if (pl2gpu_score_begin_classes(ctx, n, score_ct, k1 - k0, &job)) return GpuFail("pl2gpu_score_begin_classes");
+    } else if (score_ct == 1) {  // the one-column job (same device work as pl2gpu_score_begin_cols with one column)
+      if (pl2gpu_score_begin(ctx, n, &job)) return GpuFail("pl2gpu_score_begin");
+    } else if (pl2gpu_score_begin_cols(ctx, n, score_ct, &job)) {
+      return GpuFail("pl2gpu_score_begin_cols");
+    }
+    struct JobGuard {
+      Pl2ScoreJob* j;
+      ~JobGuard() { pl2gpu_score_end(j); }
+    } guard{job};
+    if (ploidy_job && pl2gpu_score_set_sex(job, S.sex.data())) return GpuFail("pl2gpu_score_set_sex");
+    BlockStreamer bs(ds, &gvidx, n, 16384);
+    if (!bs.Init()) return GpuFail("pl2gpu_host_alloc");
+    std::vector<double> w4, w4h;  // diploid and haploid tables
+    std::vector<uint8_t> d4, cls;
+    std::vector<uint32_t> ecls, erow;
+    size_t ge = 0;        // next group entry
+    uint32_t row0 = 0;    // first row of the block
+    for (;;) {
+      const int got = bs.Next(&err);
+      if (got < 0) {
+        logprintf("Error: %s\n", err.c_str());
+        return kRetMalformedInput;
+      }
+      if (!got) break;
+      size_t ge_end = ge;
+      while (ge_end < gent.size() && grow[ge_end] < row0 + static_cast<uint32_t>(got)) ++ge_end;
+      const uint32_t ecnt = static_cast<uint32_t>(ge_end - ge);
+      w4.resize(4ull * score_ct * ecnt);
+      w4h.resize(4ull * score_ct * ecnt);
+      d4.resize(ecnt);
+      cls.resize(ecnt);
+      ecls.resize(ecnt);
+      erow.resize(ecnt);
+      for (uint32_t k = 0; k < ecnt; ++k) {
+        const size_t ei = gent[ge + k];
+        const Entry& e = entries[ei];
+        erow[k] = grow[ge + k] - row0;
+        ecls[k] = entry_class[ei] - k0;
+        const uint64_t cbase = static_cast<uint64_t>(entry_class[ei]) * n;
+        const uint8_t pc = cls[k] = ploidy_class(e.v);
+        const double rf = ref_freqs[entry_row[ei]];
+        const double f_named = e.aidx ? (1.0 - rf) : rf;
+        // genotype code = ALT allele count; named-allele dosage of codes 0, 1, 2.  The tables below do not depend on
+        // the column; each column scales them by its coefficient.  'center' / 'variance-standardize'
+        // (:8003-8033): dosage x slope + intercept with intercept = -p f slope and slope = 1 / sqrt(p / 2 x 2 f (1 - f))
+        // (0 when the variance is not above 2^-44), p the variant's ploidy: 1 on chrY and MT, else 2 (chrX too, whatever
+        // the model).  A missing call contributes (sample ploidy) f slope WITHOUT the intercept in the reference
+        // (missing_effect, :6756-6762, :6795-6836) - kept, since the outputs are compared with its files.
+        const uint32_t d0 = e.aidx ? 0 : 2, d2 = e.aidx ? 2 : 0;
+        const bool haploid_variant = pc == kPl2ScoreChrY || pc == kPl2ScoreHaploidAll;
+        double slope = 1.0, icpt = 0.0;
+        if (c.score_center) {
+          if (c.score_varstd) {
+            const double variance = (haploid_variant ? 0.5 : 1.0) * (2.0 * f_named * (1.0 - f_named));
+            if (!(variance > 1.0 / 17592186044416.0)) {
+              slope = 0.0;  // the reference additionally insists that such a variant is monomorphic (:8013-8027); a weight of 0 scores it the same
+            } else {
+              slope = 1.0 / sqrt(variance);
+            }
+          }
+          icpt = ((haploid_variant ? -1.0 : -2.0) * f_named) * slope;
+        }
+        // 'dominant' / 'recessive' (:6747-6762): copies -> min(copies, 1) / max(copies - 1, 0), a missing call -> ONE x f
+        uint32_t e0 = d0, e1 = 1, e2 = d2;
+        double miss_dosage = 2.0 * f_named;
+        if (c.score_dominant) {
+          e0 = d0 ? 1 : 0, e2 = d2 ? 1 : 0;
+          miss_dosage = f_named;
+        } else if (c.score_recessive) {
+          e0 = d0 ? 1 : 0, e1 = 0, e2 = d2 ? 1 : 0;
+          miss_dosage = f_named;
+        }
+        const double t0 = static_cast<double>(e0) * slope + icpt, t1 = static_cast<double>(e1) * slope + icpt, t2 = static_cast<double>(e2) * slope + icpt, t3 = miss_dosage * slope;
+        // a haploid sample (chrY nonfemales, MT, chrX males under --xchr-model 1) holds half the dosage of each code
+        const double h0 = (0.5 * e0) * slope + icpt, h1 = (0.5 * e1) * slope + icpt, h2 = (0.5 * e2) * slope + icpt, h3 = f_named * slope;
+        for (uint32_t j = 0; j < score_ct; ++j) {
+          const double coef = coefs[e.coef_row * score_ct + j];
+          double* w = &w4[4ull * (static_cast<uint64_t>(k) * score_ct + j)];
+          w[0] = coef * t0;
+          w[1] = coef * t1;
+          w[2] = coef * t2;
+          w[3] = c.score_no_meanimpute ? 0.0 : coef * t3;
+          if (pc == kPl2ScoreChrY) {  // the first table serves unknown-sex samples, whose chrY dosage the reference zeroes
+            w[0] = w[1] = w[2] = coef * icpt;
+            w[3] = c.score_no_meanimpute ? 0.0 : coef * h3;
+          }
+          double* wh = &w4h[4ull * (static_cast<uint64_t>(k) * score_ct + j)];
+          wh[0] = coef * h0;
+          wh[1] = coef * h1;
+          wh[2] = coef * h2;
+          wh[3] = c.score_no_meanimpute ? 0.0 : coef * h3;
+        }
+        d4[k] = static_cast<uint8_t>(e0 | (e1 << 2) | (e2 << 4));
+        // a file that names both alleles of a variant (PC projection with allele weights): the device counts the missing
+        // calls of both entries, the reference counts them once per variant and file (:7788), so the second entry's are
+        // taken back out here, from the diploid or haploid count the sample's class put them in
+        if (ei > 0 && entries[ei - 1].v == e.v && entry_class[ei - 1] == entry_class[ei]) {
+          const uint64_t* row = bs.buf + static_cast<uint64_t>(erow[k]) * bs.words;
+          for (uint32_t w = 0; w < bs.words; ++w) {
+            uint64_t ms = row[w] & (row[w] >> 1) & 0x5555555555555555ull;
+            if (32ull * (w + 1) > n) ms &= (1ull << (2 * (n - 32 * w))) - 1;
+            for (; ms; ms &= ms - 1) {
+              const uint32_t s = 32 * w + __builtin_ctzll(ms) / 2;
+              const uint8_t sex = S.sex[s];
+              if (pc == kPl2ScoreDiploid || (pc == kPl2ScoreChrXMaleHaploid && sex != 1)) --repeat_miss[cbase + s];
+              else if (pc != kPl2ScoreChrY || sex != 2) --repeat_miss_hap[cbase + s];  // chrY females are not counted
+            }
+          }
+        }
+      }
+      if (c.score_list) {
+        if (pl2gpu_score_add_entries(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, static_cast<uint32_t>(got), 0, ecnt, erow.data(), ecls.data(), ploidy_job ? cls.data() : nullptr, w4.data(), w4h.data(), d4.data()))
+          return GpuFail("pl2gpu_score_add_entries");
+      } else if (qsr) {  // one entry per row
+        if (pl2gpu_score_add_variants_classes(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, ecnt, 0, ecls.data(), ploidy_job ? cls.data() : nullptr, w4.data(), w4h.data(), d4.data()))
+          return GpuFail("pl2gpu_score_add_variants_classes");
+      } else if (ploidy_job) {
+        if (pl2gpu_score_add_variants_ploidy(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, ecnt, 0, cls.data(), w4.data(), w4h.data(), d4.data())) return GpuFail("pl2gpu_score_add_variants_ploidy");
+      } else if (pl2gpu_score_add_variants(job, bs.buf, static_cast<uint64_t>(bs.words) * 8, ecnt, 0, w4.data(), d4.data())) {
+        return GpuFail("pl2gpu_score_add_variants");
+      }
+      ge = ge_end;
+      row0 += static_cast<uint32_t>(got);
+    }
+    if (class_job) {
+      for (uint32_t k = k0; k < k1; ++k) {
+        const uint64_t o = static_cast<uint64_t>(k) * n;
+        if (pl2gpu_score_get_class(job, k - k0, sums.data() + o * score_ct, hdos.data() + o, miss.data() + o, miss_hap.data() + o)) return GpuFail("pl2gpu_score_get_class");
+      }
+    } else if (ploidy_job) {
+      if (pl2gpu_score_get_ploidy(job, sums.data(), hdos.data(), miss.data(), miss_hap.data())) return GpuFail("pl2gpu_score_get_ploidy");
+    } else {
+      if (pl2gpu_score_get(job, sums.data(), hdos.data(), miss.data())) return GpuFail("pl2gpu_score_get");
+      for (uint64_t& d : hdos) d *= 2;
+    }
   }
   for (uint64_t k = 0; k < miss.size(); ++k) {
     miss[k] = static_cast<uint32_t>(miss[k] + repeat_miss[k]);
     miss_hap[k] = static_cast<uint32_t>(miss_hap[k] + repeat_miss_hap[k]);
   }
-  logprintf("--score: %zu variant%s processed.\n", processed_ct, processed_ct == 1 ? "" : "s");
+  if (c.score_list) {
+    for (uint32_t f = 0; f < file_ct; ++f) logprintf("--score-list file %u/%u: %zu variant%s processed.\n", f + 1, file_ct, file_processed[f], file_processed[f] == 1 ? "" : "s");
+  } else {
+    logprintf("--score: %zu variant%s processed.\n", file_processed[0], file_processed[0] == 1 ? "" : "s");
+  }
   if (c.score_list_variants) {
     OutFile fv;
     const std::string vname = c.out + ".sscore.vars";
@@ -3268,9 +3421,9 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   // diploid variant and 1 per MT variant.  Per class here; a range's terms are the sums over its classes (:8389).
   std::vector<uint32_t> denom_base(class_ct, 0), y_incr(class_ct, 0), x_decr(class_ct, 0);
   for (size_t k = 0; k < entries.size(); ++k) {
-    if (k && entries[k - 1].v == entries[k].v) continue;
+    if (k && entries[k - 1].v == entries[k].v && entry_class[k - 1] == entry_class[k]) continue;
     const uint8_t pc = ploidy_class(entries[k].v);
-    const uint32_t cl = qsr ? entry_class[k] : 0;
+    const uint32_t cl = entry_class[k];
     denom_base[cl] += pc == kPl2ScoreHaploidAll ? 1 : pc == kPl2ScoreChrY ? 0 : 2;
     y_incr[cl] += pc == kPl2ScoreChrY;
     x_decr[cl] += pc == kPl2ScoreChrXMaleHaploid;
@@ -3293,73 +3446,85 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
   if (c.sc_nallele) hdr += "\tALLELE_CT";
   if (c.sc_denom) hdr += "\tDENOM";
   if (c.sc_dosagesum) hdr += "\tNAMED_ALLELE_DOSAGE_SUM";
-  // every _AVG column, then every _SUM column (:8520-8539)
+  // every file's _AVG columns, then every file's _SUM columns (:8520-8539, :8595-8612)
   if (c.sc_avgs)
     for (const std::string& nm : score_names) hdr += "\t" + nm + "_AVG";
   if (c.sc_sums)
     for (const std::string& nm : score_names) hdr += "\t" + nm + "_SUM";
   hdr += "\n";
-  // one report: the classes with in_report[class] set, added in ascending class order
+  // one report: per file, the classes with in_report[class] set, added in ascending class order.  ALLELE_CT, DENOM and
+  // NAMED_ALLELE_DOSAGE_SUM exist for --score only (one file).
   auto write_report = [&](const std::string& name, const std::vector<uint8_t>& in_report) -> int {
-    std::vector<double> rs(static_cast<uint64_t>(n) * score_ct, 0.0);
-    std::vector<uint64_t> rhdos(n, 0);
-    std::vector<uint32_t> rmiss(n, 0), rmiss_hap(n, 0);
-    uint32_t rbase = 0, ry = 0, rx = 0;
+    std::vector<double> rs(static_cast<uint64_t>(file_ct) * n * score_ct, 0.0);  // [file][sample][score_ct]
+    std::vector<uint64_t> rhdos(static_cast<uint64_t>(file_ct) * n, 0);
+    std::vector<uint32_t> rmiss(static_cast<uint64_t>(file_ct) * n, 0), rmiss_hap(static_cast<uint64_t>(file_ct) * n, 0);
+    std::vector<uint32_t> rbase(file_ct, 0), ry(file_ct, 0), rx(file_ct, 0);
     for (uint32_t k = 0; k < class_ct; ++k) {
       if (!in_report[k]) continue;
-      const uint64_t o = static_cast<uint64_t>(k) * n;
-      for (uint64_t i = 0; i < rs.size(); ++i) rs[i] += sums[o * score_ct + i];
+      const uint32_t f = class_file.empty() ? 0 : class_file[k];
+      const uint64_t o = static_cast<uint64_t>(k) * n, fo = static_cast<uint64_t>(f) * n;
+      for (uint64_t i = 0; i < static_cast<uint64_t>(n) * score_ct; ++i) rs[fo * score_ct + i] += sums[o * score_ct + i];
       for (uint32_t s = 0; s < n; ++s) {
-        rhdos[s] += hdos[o + s];
-        rmiss[s] += miss[o + s];
-        rmiss_hap[s] += miss_hap[o + s];
+        rhdos[fo + s] += hdos[o + s];
+        rmiss[fo + s] += miss[o + s];
+        rmiss_hap[fo + s] += miss_hap[o + s];
       }
-      rbase += denom_base[k];
-      ry += y_incr[k];
-      rx += x_decr[k];
+      rbase[f] += denom_base[k];
+      ry[f] += y_incr[k];
+      rx[f] += x_decr[k];
     }
-    OutFile f;
-    if (!f.Open(name, c.score_zs)) return kRetOpenFail;
-    f.Puts(hdr.c_str());
+    OutFile out;
+    if (!out.Open(name, c.score_zs)) return kRetOpenFail;
+    out.Puts(hdr.c_str());
     char num[64];
+    std::vector<uint32_t> denom(file_ct);
     for (uint32_t k = 0; k < n; ++k) {
       std::string row = FmtId(S, k, idf);
       for (const PhenoOut& po : phenos) row += "\t" + po.text[k];
-      const uint32_t denom_full = rbase + (S.sex[k] != 2 ? ry : 0) - (S.sex[k] == 1 ? rx : 0);
-      const uint32_t nallele = denom_full - 2 * rmiss[k] - rmiss_hap[k];
-      const uint32_t denom = c.score_no_meanimpute ? nallele : denom_full;
-      if (c.sc_nallele) {
-        *u32toa(nallele, num) = '\0';
-        row += std::string("\t") + num;
-      }
-      if (c.sc_denom) {
-        *u32toa(denom, num) = '\0';
-        row += std::string("\t") + num;
-      }
-      if (c.sc_dosagesum) row += "\t" + std::to_string(rhdos[k] / 2) + ((rhdos[k] & 1) ? ".5" : "");
-      const double* ks = &rs[static_cast<uint64_t>(k) * score_ct];
-      if (c.sc_avgs) {
-        for (uint32_t j = 0; j < score_ct; ++j) {
-          *dtoa_g(ks[j] * (1.0 / static_cast<double>(denom)), num) = '\0';
+      for (uint32_t f = 0; f < file_ct; ++f) {
+        const uint64_t fk = static_cast<uint64_t>(f) * n + k;
+        const uint32_t denom_full = rbase[f] + (S.sex[k] != 2 ? ry[f] : 0) - (S.sex[k] == 1 ? rx[f] : 0);
+        const uint32_t nallele = denom_full - 2 * rmiss[fk] - rmiss_hap[fk];
+        denom[f] = c.score_no_meanimpute ? nallele : denom_full;
+        if (f) continue;
+        if (c.sc_nallele) {
+          *u32toa(nallele, num) = '\0';
           row += std::string("\t") + num;
+        }
+        if (c.sc_denom) {
+          *u32toa(denom[0], num) = '\0';
+          row += std::string("\t") + num;
+        }
+        if (c.sc_dosagesum) row += "\t" + std::to_string(rhdos[fk] / 2) + ((rhdos[fk] & 1) ? ".5" : "");
+      }
+      if (c.sc_avgs) {
+        for (uint32_t f = 0; f < file_ct; ++f) {
+          const double* ks = &rs[(static_cast<uint64_t>(f) * n + k) * score_ct];
+          for (uint32_t j = 0; j < score_ct; ++j) {
+            *dtoa_g(ks[j] * (1.0 / static_cast<double>(denom[f])), num) = '\0';
+            row += std::string("\t") + num;
+          }
         }
       }
       if (c.sc_sums) {
-        for (uint32_t j = 0; j < score_ct; ++j) {
-          *dtoa_g(ks[j], num) = '\0';
-          row += std::string("\t") + num;
+        for (uint32_t f = 0; f < file_ct; ++f) {
+          const double* ks = &rs[(static_cast<uint64_t>(f) * n + k) * score_ct];
+          for (uint32_t j = 0; j < score_ct; ++j) {
+            *dtoa_g(ks[j], num) = '\0';
+            row += std::string("\t") + num;
+          }
         }
       }
       row += "\n";
-      f.Write(row.data(), row.size());
+      out.Write(row.data(), row.size());
     }
-    return f.Close() ? 0 : kRetWriteFail;
+    return out.Close() ? 0 : kRetWriteFail;
   };
   const char* ext = c.score_zs ? ".sscore.zst" : ".sscore";
   if (!qsr) {
     const std::string name = c.out + ext;
-    if (int rc = write_report(name, std::vector<uint8_t>(1, 1))) return rc;
-    logprintf("--score: Results written to %s .\n", name.c_str());
+    if (int rc = write_report(name, std::vector<uint8_t>(class_ct, 1))) return rc;
+    logprintf("%s: Results written to %s .\n", flagname, name.c_str());
     return 0;
   }
   // one report per range, in range-file order; a range no entry lies in gets one of zero sums
@@ -3368,7 +3533,7 @@ int RunScore(const Cmd& c, Dataset* ds, Pl2GpuCtx* ctx) {
     for (uint32_t k = 0; k < class_ranges.size(); ++k) in_report[k] = class_ranges[k][r];
     if (int rc = write_report(c.out + "." + ranges[r].name + ext, in_report)) return rc;
   }
-  logprintf("--score + --q-score-range: Results written to %s.<range name>%s .\n", c.out.c_str(), ext);
+  logprintf("%s + --q-score-range: Results written to %s.<range name>%s .\n", flagname, c.out.c_str(), ext);
   return 0;
 }
 

@@ -12,7 +12,9 @@
 // allele units with diploid and haploid missing calls apart; runs of diploid entries keep score_kernel and its plan.
 // A job may keep several accumulator sets, one per class (--q-score-range: the entries whose p-values lie in the same
 // set of ranges): each staged batch is gathered into class-major order on the device (score_row_gather_kernel), and
-// each (class, ploidy class) run goes through the same kernels and launch plan into its class's accumulators.
+// each (class, ploidy class) run goes through the same kernels and launch plan into its class's accumulators.  With
+// pl2gpu_score_add_entries several entries (--score-list: one per file that scores the variant) read one staged row,
+// which the gather copies once per entry.
 //
 // Streaming: every 32-bit word of a variant row (16 samples) is read once.  A CTA covers 128 words x a chunk of
 // variants and writes per-chunk partial sums; a second kernel adds the partials in chunk order, so results do not
@@ -667,6 +669,113 @@ int ScoreAddPloidyRuns(Pl2ScoreJob* job, const uint8_t* src, uint64_t variant_st
   return 0;
 }
 
+// Entries of several classes, each reading one staged row (entry_rows NULL: entry e reads row e).  Each batch is as many
+// whole rows as fit the stage whose entries also fit the entry buffers (stage_variants each), so no row's entries are
+// split between batches.  A batch's rows are uploaded once; its entries are gathered on the device into class-major
+// order (a row is copied once per entry that reads it), stably, with their tables in the same order, and each class's
+// block runs, in runs of one ploidy class, through the kernels and launch plan of the plain path.  One class for every
+// entry with one entry per row: the ploidy runs of the plain path, into that class, with no gather.
+int ScoreAddEntries(Pl2ScoreJob* job, const void* genovecs, uint64_t variant_stride_bytes, uint32_t row_ct, int src_is_device, uint32_t entry_ct, const uint32_t* entry_rows, const uint32_t* entry_classes, const uint8_t* ploidy_classes,
+                    const double* weights4_diploid, const double* weights4_haploid, const uint8_t* named_dosages, const char* fn) {
+  if (!job || (entry_ct && (!genovecs || !entry_classes || !weights4_diploid || !named_dosages))) {
+    set_error("%s: bad arguments", fn);
+    return 1;
+  }
+  if (!ValidNamedDosages(named_dosages, entry_ct, fn)) return 1;
+  if (ploidy_classes && !ValidPloidyClasses(job, ploidy_classes, entry_ct, weights4_haploid, named_dosages, fn)) return 1;
+  for (uint32_t e = 0; e < entry_ct; ++e) {
+    if (entry_classes[e] >= job->class_ct) {
+      set_error("%s: entry %u has class %u of a job of %u classes", fn, e, entry_classes[e], job->class_ct);
+      return 1;
+    }
+  }
+  auto row_of = [&](uint32_t e) { return entry_rows ? entry_rows[e] : e; };
+  for (uint32_t e0 = 0; e0 < entry_ct;) {
+    uint32_t e1 = e0 + 1;
+    while (e1 < entry_ct && row_of(e1) == row_of(e0)) ++e1;
+    if (e1 - e0 > job->stage_variants) {
+      set_error("%s: row %u has %u entries, more than the %u of a staged batch", fn, row_of(e0), e1 - e0, job->stage_variants);
+      return 1;
+    }
+    e0 = e1;
+  }
+  PL2_CUDA_OK(cudaSetDevice(job->ctx->c.device));
+  const uint8_t* src = static_cast<const uint8_t*>(genovecs);
+  if (!entry_rows && std::all_of(entry_classes, entry_classes + entry_ct, [&](uint32_t k) { return k == entry_classes[0]; }))
+    return ScoreAddPloidyRuns(job, src, variant_stride_bytes, entry_ct, src_is_device, ploidy_classes, weights4_diploid, weights4_haploid, named_dosages, entry_ct ? entry_classes[0] : 0);
+  Ctx* c = &job->ctx->c;
+  if (ploidy_classes && std::any_of(ploidy_classes, ploidy_classes + entry_ct, [](uint8_t pc) { return pc != kPl2ScoreDiploid; }) && ScoreAllocPloidy(job)) return 1;
+  if (!job->d_raw_grouped) {  // the class-major copy holds a batch's entries (stage_variants rows of the stage's pitch)
+    DevArray<uint8_t> raw;
+    DevArray<uint32_t> perm;
+    if (raw.alloc(static_cast<uint64_t>(job->stage_variants) * job->stage.pitch, "%s: insufficient device memory for a class-major copy of the %u-sample genotype stage", fn, job->sample_ct) ||
+        perm.alloc(job->stage_variants, "%s: insufficient device memory", fn))
+      return 1;
+    job->d_raw_grouped = std::move(raw);
+    job->d_perm = std::move(perm);
+  }
+  const uint64_t w_row = 4ull * job->score_ct;
+  const uint32_t pitch16 = job->stage.pitch / 16;
+  std::vector<uint32_t> perm, first(job->class_ct + 1);
+  std::vector<double> w4, w4h;
+  std::vector<uint8_t> d4, pcs;
+  for (uint32_t done = 0; done < entry_ct;) {
+    // whole rows from the batch's first row while the rows fit the stage and their entries the entry buffers
+    const uint32_t r0 = row_of(done);
+    uint32_t end = done;
+    while (end < entry_ct && row_of(end) - r0 < job->stage_variants) {
+      uint32_t next = end + 1;
+      while (next < entry_ct && row_of(next) == row_of(end)) ++next;
+      if (next - done > job->stage_variants) break;
+      end = next;
+    }
+    const uint32_t cur = end - done, rows = row_of(end - 1) - r0 + 1;
+    const uint32_t* cls = entry_classes + done;
+    std::fill(first.begin(), first.end(), 0u);
+    for (uint32_t e = 0; e < cur; ++e) ++first[cls[e] + 1];
+    for (uint32_t k = 0; k < job->class_ct; ++k) first[k + 1] += first[k];
+    perm.resize(cur);
+    {
+      std::vector<uint32_t> next(first.begin(), first.end() - 1);
+      for (uint32_t e = 0; e < cur; ++e) perm[next[cls[e]]++] = done + e;
+    }
+    w4.resize(w_row * cur);
+    d4.resize(cur);
+    pcs.assign(cur, kPl2ScoreDiploid);
+    const bool any_hap = ploidy_classes && std::any_of(ploidy_classes + done, ploidy_classes + done + cur, [](uint8_t pc) { return pc != kPl2ScoreDiploid; });
+    if (any_hap) w4h.assign(w_row * cur, 0.0);
+    for (uint32_t r = 0; r < cur; ++r) {
+      const uint32_t e = perm[r];
+      std::copy_n(weights4_diploid + w_row * e, w_row, w4.data() + w_row * r);
+      d4[r] = named_dosages[e];
+      if (ploidy_classes) pcs[r] = ploidy_classes[e];
+      if (any_hap && pcs[r] != kPl2ScoreDiploid) std::copy_n(weights4_haploid + w_row * e, w_row, w4h.data() + w_row * r);
+      perm[r] = row_of(e) - r0;  // the entry's row in the staged batch
+    }
+    uint32_t padded = 0;
+    PL2_TRY(StageUpload(c, &job->stage, src + static_cast<uint64_t>(r0) * variant_stride_bytes, variant_stride_bytes, rows, src_is_device, &padded));
+    PL2_CUDA_OK(cudaMemcpyAsync(job->d_perm, perm.data(), 4ull * cur, cudaMemcpyHostToDevice, c->stream));
+    PL2_CUDA_OK(cudaMemcpyAsync(job->d_w4, w4.data(), 8 * w_row * cur, cudaMemcpyHostToDevice, c->stream));
+    if (any_hap) PL2_CUDA_OK(cudaMemcpyAsync(job->d_w4h, w4h.data(), 8 * w_row * cur, cudaMemcpyHostToDevice, c->stream));
+    PL2_CUDA_OK(cudaMemcpyAsync(job->d_d4, d4.data(), cur, cudaMemcpyHostToDevice, c->stream));
+    score_row_gather_kernel<<<dim3(std::min(DivUpU32(pitch16, 256), 64u), cur), 256, 0, c->stream>>>(reinterpret_cast<const uint4*>(job->stage.d_raw.get()), reinterpret_cast<uint4*>(job->d_raw_grouped.get()), pitch16, job->d_perm);
+    ++c->launches;
+    PL2_CUDA_OK(cudaGetLastError());
+    for (uint32_t k = 0; k < job->class_ct; ++k) {
+      for (uint32_t r0k = first[k]; r0k < first[k + 1];) {
+        uint32_t r1k = r0k + 1;
+        while (r1k < first[k + 1] && pcs[r1k] == pcs[r0k]) ++r1k;
+        PL2_TRY(ScoreLaunchRun(job, job->d_raw_grouped.get() + static_cast<uint64_t>(r0k) * job->stage.pitch, r1k - r0k, job->d_w4 + w_row * r0k, job->d_w4h ? job->d_w4h + w_row * r0k : nullptr, job->d_d4 + r0k, pcs[r0k], k));
+        r0k = r1k;
+      }
+    }
+    PL2_CUDA_OK(cudaStreamSynchronize(c->stream));  // host tables and a host source may be reused by the caller
+    job->entries += cur;
+    done = end;
+  }
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -724,89 +833,26 @@ int pl2gpu_score_add_variants_ploidy(Pl2ScoreJob* job, const void* genovecs, uin
 
 int pl2gpu_score_add_variants_classes(Pl2ScoreJob* job, const void* genovecs, uint64_t variant_stride_bytes, uint32_t variant_ct, int src_is_device, const uint32_t* entry_classes, const uint8_t* ploidy_classes,
                                       const double* weights4_diploid, const double* weights4_haploid, const uint8_t* named_dosages) {
-  const char* fn = "pl2gpu_score_add_variants_classes";
-  if (!job || (variant_ct && (!genovecs || !entry_classes || !weights4_diploid || !named_dosages))) {
+  return ScoreAddEntries(job, genovecs, variant_stride_bytes, variant_ct, src_is_device, variant_ct, nullptr, entry_classes, ploidy_classes, weights4_diploid, weights4_haploid, named_dosages, "pl2gpu_score_add_variants_classes");
+}
+
+int pl2gpu_score_add_entries(Pl2ScoreJob* job, const void* genovecs, uint64_t variant_stride_bytes, uint32_t row_ct, int src_is_device, uint32_t entry_ct, const uint32_t* entry_rows, const uint32_t* entry_classes,
+                             const uint8_t* ploidy_classes, const double* weights4_diploid, const double* weights4_haploid, const uint8_t* named_dosages) {
+  const char* fn = "pl2gpu_score_add_entries";
+  if (!job || (entry_ct && !entry_rows)) {
     set_error("%s: bad arguments", fn);
     return 1;
   }
-  if (!ValidNamedDosages(named_dosages, variant_ct, fn)) return 1;
-  if (ploidy_classes && !ValidPloidyClasses(job, ploidy_classes, variant_ct, weights4_haploid, named_dosages, fn)) return 1;
-  for (uint32_t v = 0; v < variant_ct; ++v) {
-    if (entry_classes[v] >= job->class_ct) {
-      set_error("%s: entry %u has class %u of a job of %u classes", fn, v, entry_classes[v], job->class_ct);
+  for (uint32_t e = 0; e < entry_ct; ++e) {
+    if (entry_rows[e] >= row_ct || (e && entry_rows[e] < entry_rows[e - 1])) {
+      set_error("%s: entry %u has row %u (rows must be < %u and non-decreasing)", fn, e, entry_rows[e], row_ct);
       return 1;
     }
   }
-  PL2_CUDA_OK(cudaSetDevice(job->ctx->c.device));
-  const uint8_t* src = static_cast<const uint8_t*>(genovecs);
-  // one class for every entry: the ploidy runs of the plain path, into that class
-  if (std::all_of(entry_classes, entry_classes + variant_ct, [&](uint32_t k) { return k == entry_classes[0]; }))
-    return ScoreAddPloidyRuns(job, src, variant_stride_bytes, variant_ct, src_is_device, ploidy_classes, weights4_diploid, weights4_haploid, named_dosages, variant_ct ? entry_classes[0] : 0);
-  Ctx* c = &job->ctx->c;
-  if (ploidy_classes && std::any_of(ploidy_classes, ploidy_classes + variant_ct, [](uint8_t pc) { return pc != kPl2ScoreDiploid; }) && ScoreAllocPloidy(job)) return 1;
-  if (!job->d_raw_grouped) {
-    DevArray<uint8_t> raw;
-    DevArray<uint32_t> perm;
-    if (raw.alloc(static_cast<uint64_t>(job->stage.variant_cap) * job->stage.pitch, "%s: insufficient device memory for a class-major copy of the %u-sample genotype stage", fn, job->sample_ct) ||
-        perm.alloc(job->stage_variants, "%s: insufficient device memory", fn))
-      return 1;
-    job->d_raw_grouped = std::move(raw);
-    job->d_perm = std::move(perm);
-  }
-  const uint64_t w_row = 4ull * job->score_ct;
-  const uint32_t pitch16 = job->stage.pitch / 16;
-  std::vector<uint32_t> perm, first(job->class_ct + 1);
-  std::vector<double> w4, w4h;
-  std::vector<uint8_t> d4, pcs;
-  for (uint32_t done = 0; done < variant_ct;) {
-    // one staged batch in the caller's order; its entries grouped by class on the device, stably, with the tables
-    // in the same order
-    const uint32_t cur = std::min(job->stage_variants, variant_ct - done);
-    const uint32_t* cls = entry_classes + done;
-    std::fill(first.begin(), first.end(), 0u);
-    for (uint32_t e = 0; e < cur; ++e) ++first[cls[e] + 1];
-    for (uint32_t k = 0; k < job->class_ct; ++k) first[k + 1] += first[k];
-    perm.resize(cur);
-    {
-      std::vector<uint32_t> next(first.begin(), first.end() - 1);
-      for (uint32_t e = 0; e < cur; ++e) perm[next[cls[e]]++] = done + e;
-    }
-    w4.resize(w_row * cur);
-    d4.resize(cur);
-    pcs.assign(cur, kPl2ScoreDiploid);
-    const bool any_hap = ploidy_classes && std::any_of(ploidy_classes + done, ploidy_classes + done + cur, [](uint8_t pc) { return pc != kPl2ScoreDiploid; });
-    if (any_hap) w4h.assign(w_row * cur, 0.0);
-    for (uint32_t r = 0; r < cur; ++r) {
-      const uint32_t e = perm[r];
-      std::copy_n(weights4_diploid + w_row * e, w_row, w4.data() + w_row * r);
-      d4[r] = named_dosages[e];
-      if (ploidy_classes) pcs[r] = ploidy_classes[e];
-      if (any_hap && pcs[r] != kPl2ScoreDiploid) std::copy_n(weights4_haploid + w_row * e, w_row, w4h.data() + w_row * r);
-      perm[r] = e - done;
-    }
-    uint32_t padded = 0;
-    PL2_TRY(StageUpload(c, &job->stage, src + static_cast<uint64_t>(done) * variant_stride_bytes, variant_stride_bytes, cur, src_is_device, &padded));
-    PL2_CUDA_OK(cudaMemcpyAsync(job->d_perm, perm.data(), 4ull * cur, cudaMemcpyHostToDevice, c->stream));
-    PL2_CUDA_OK(cudaMemcpyAsync(job->d_w4, w4.data(), 8 * w_row * cur, cudaMemcpyHostToDevice, c->stream));
-    if (any_hap) PL2_CUDA_OK(cudaMemcpyAsync(job->d_w4h, w4h.data(), 8 * w_row * cur, cudaMemcpyHostToDevice, c->stream));
-    PL2_CUDA_OK(cudaMemcpyAsync(job->d_d4, d4.data(), cur, cudaMemcpyHostToDevice, c->stream));
-    score_row_gather_kernel<<<dim3(std::min(DivUpU32(pitch16, 256), 64u), cur), 256, 0, c->stream>>>(reinterpret_cast<const uint4*>(job->stage.d_raw.get()), reinterpret_cast<uint4*>(job->d_raw_grouped.get()), pitch16, job->d_perm);
-    ++c->launches;
-    PL2_CUDA_OK(cudaGetLastError());
-    // each class's block, in runs of one ploidy class, through the kernels and launch plan of the plain path
-    for (uint32_t k = 0; k < job->class_ct; ++k) {
-      for (uint32_t r0 = first[k]; r0 < first[k + 1];) {
-        uint32_t r1 = r0 + 1;
-        while (r1 < first[k + 1] && pcs[r1] == pcs[r0]) ++r1;
-        PL2_TRY(ScoreLaunchRun(job, job->d_raw_grouped.get() + static_cast<uint64_t>(r0) * job->stage.pitch, r1 - r0, job->d_w4 + w_row * r0, job->d_w4h ? job->d_w4h + w_row * r0 : nullptr, job->d_d4 + r0, pcs[r0], k));
-        r0 = r1;
-      }
-    }
-    PL2_CUDA_OK(cudaStreamSynchronize(c->stream));  // host tables and a host source may be reused by the caller
-    job->entries += cur;
-    done += cur;
-  }
-  return 0;
+  // one entry per row, in row order: the rows are the entries
+  bool identity = entry_ct == row_ct;
+  for (uint32_t e = 0; identity && e < entry_ct; ++e) identity = entry_rows[e] == e;
+  return ScoreAddEntries(job, genovecs, variant_stride_bytes, row_ct, src_is_device, entry_ct, identity ? nullptr : entry_rows, entry_classes, ploidy_classes, weights4_diploid, weights4_haploid, named_dosages, fn);
 }
 
 int pl2gpu_score_get_class(Pl2ScoreJob* job, uint32_t class_idx, double* score_sums, uint64_t* named_half_dosage_sums, uint32_t* missing_diploid_cts, uint32_t* missing_haploid_cts) {

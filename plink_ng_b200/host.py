@@ -519,6 +519,48 @@ def score_sums_classes(ctx: GpuContext, genovecs: np.ndarray, sample_ct: int, cl
         lib.pl2gpu_score_end(h)
 
 
+def score_sums_entries(ctx: GpuContext, genovecs: np.ndarray, sample_ct: int, class_ct: int, entry_rows: np.ndarray, entry_classes: np.ndarray, weights4_diploid: np.ndarray, named_dosages: np.ndarray, sample_sex=None,
+                       ploidy_classes=None, weights4_haploid=None, batches=None):
+    """`--score` entries that share staged rows (pl2gpu_score_begin_classes / _add_entries / _get_class): genovecs
+    [rows, bytes]; entry_rows [entries] (non-decreasing row of each entry), entry_classes and the tables as
+    score_sums_classes, per entry.  batches: row counts of successive add calls, each with the entries of its rows
+    (default: one call).  -> per class (score sums [sample_ct, score_ct], named-allele dosage sums in half allele units,
+    diploid and haploid missing counts)."""
+    g = np.ascontiguousarray(genovecs)
+    wd = np.ascontiguousarray(weights4_diploid, dtype=np.float64)
+    er = np.ascontiguousarray(entry_rows, dtype=np.uint32)
+    ec = np.ascontiguousarray(entry_classes, dtype=np.uint32)
+    d = np.ascontiguousarray(named_dosages, dtype=np.uint8)
+    assert wd.ndim == 3 and wd.shape[0] == er.shape[0] and wd.shape[2] == 4 and d.shape == ec.shape == er.shape
+    pc = None if ploidy_classes is None else np.ascontiguousarray(ploidy_classes, dtype=np.uint8)
+    wh = None if weights4_haploid is None else np.ascontiguousarray(weights4_haploid, dtype=np.float64)
+    score_ct = wd.shape[1]
+    h = C.c_void_p()
+    check(lib.pl2gpu_score_begin_classes(ctx.handle, sample_ct, score_ct, class_ct, C.byref(h)), "pl2gpu_score_begin_classes")
+    try:
+        if sample_sex is not None:
+            sx = np.ascontiguousarray(sample_sex, dtype=np.uint8)
+            check(lib.pl2gpu_score_set_sex(h, sx.ctypes.data), "pl2gpu_score_set_sex")
+        r0 = 0
+        for cnt in (batches or [g.shape[0]]):
+            e0, e1 = np.searchsorted(er, r0), np.searchsorted(er, r0 + cnt)
+            rows = np.ascontiguousarray(er[e0:e1] - r0)
+            check(lib.pl2gpu_score_add_entries(h, g[r0:].ctypes.data, g.strides[0], cnt, 0, int(e1 - e0), rows.ctypes.data, ec[e0:].ctypes.data, None if pc is None else pc[e0:].ctypes.data, wd[e0:].ctypes.data,
+                                               None if wh is None else wh[e0:].ctypes.data, d[e0:].ctypes.data), "pl2gpu_score_add_entries")
+            r0 += cnt
+        out = []
+        for k in range(class_ct):
+            sums = np.empty((sample_ct, score_ct), dtype=np.float64)
+            hdos = np.empty(sample_ct, dtype=np.uint64)
+            miss_d = np.empty(sample_ct, dtype=np.uint32)
+            miss_h = np.empty(sample_ct, dtype=np.uint32)
+            check(lib.pl2gpu_score_get_class(h, k, sums.ctypes.data, hdos.ctypes.data, miss_d.ctypes.data, miss_h.ctypes.data), "pl2gpu_score_get_class")
+            out.append((sums, hdos, miss_d, miss_h))
+        return out
+    finally:
+        lib.pl2gpu_score_end(h)
+
+
 def variant_scores(ctx: GpuContext, genovecs: np.ndarray, sample_ct: int, weights: np.ndarray, ref_freqs=None) -> np.ndarray:
     """`--variant-score` sums (pl2gpu_pca_vscore) for an in-memory block: weights [sample_ct, cols] -> [variants, cols]."""
     g = np.ascontiguousarray(genovecs)
